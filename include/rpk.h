@@ -239,7 +239,8 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
              uint32_t stride, uint32_t* changed_idx, uint16_t* changed_code, uint32_t* n_changed);
 
 /* Device-resident variant on GPU `shard`: d_records N*stride bytes, d_hash_prev N uint64 updated in place
- * (caller-owned column; 0 = never seen), d_changed_idx capacity N, d_n_changed one uint32.  Enqueued on
+ * (caller-owned column; 0 = never seen; both 16-byte aligned, else RPK_EINVAL), d_changed_idx capacity N, d_n_changed
+ * one uint32.  Enqueued on
  * `stream`, no synchronisation.  The _device entry points of one shard share ctx-owned scratch: issue them from one
  * stream per shard (select) / one stream per shard (status) at a time. */
 int rpk_status_diff_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,

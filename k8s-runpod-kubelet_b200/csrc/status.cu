@@ -496,7 +496,9 @@ __global__ void __launch_bounds__(kStThreads) k_status_diff(StatusArgs a) {
     __shared__ uint32_t s_tile, s_excl, s_last;
     __shared__ uint32_t s_wcnt[ITEMS * (kStThreads / 32)];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) s_tile = atomicAdd(a.tile_counter, 1u);  // tile ids in scheduling order: look-back cannot starve
+    // reporting sweeps take tile ids from the ticket (scheduling order: the look-back cannot starve); a seed has no
+    // look-back and returns before the last-CTA cleanup below, so it must not touch the ticket (nobody would reset it)
+    if (tid == 0) s_tile = a.changed_idx != nullptr ? atomicAdd(a.tile_counter, 1u) : blockIdx.x;
     __syncthreads();
     const uint32_t tile = s_tile;
     constexpr uint32_t kTileRecs = kStThreads * ITEMS;

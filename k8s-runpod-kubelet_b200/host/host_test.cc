@@ -364,6 +364,60 @@ static void TestLongStatusStrings() {
     CHECK_EQ(notified.size(), 1u); CHECK_EQ(notified[0], "l2:Succeeded:");
 }
 
+// Statuses of 30 and 62 characters widen the table to 64 and 128 bytes: strides of the tiled kernel.  Each widening
+// seeds the whole table at the new stride right before the sweep at that stride (WidenRecords), so that sweep must
+// start from a clean context, not from whatever the seed's launch left behind.  125 characters (len byte 127, the most
+// a record holds) still fit 128 bytes; one more is compared on the host and the table stays at 128.
+static void TestWideStatusStrings() {
+    auto api = std::make_shared<FakeRunPod>();
+    api->types = KatTable();
+    Provider prov(api, 1, 600);  // more than one tile (512 slots at 64 bytes, 256 above) at every tiled stride
+    std::vector<std::string> notified;
+    prov.NotifyPods([&](const PodPtr& p) { notified.push_back(p->name + ":" + p->status.phase + ":" + p->status.container_message); });
+    for (int i = 0; i < 6; ++i) prov.CreatePod(MakePod("v" + std::to_string(i)));
+    prov.UpdateAllPodStatuses();
+    notified.clear();
+    uint64_t host = prov.HostCompares();
+    const struct { size_t len; uint32_t stride; char c; } kSteps[] = {{30, 64, 'A'}, {62, 128, 'B'}};
+    for (const auto& st : kSteps) {
+        const std::string s(st.len, st.c), t = std::string(st.len - 1, st.c) + "Z";
+        api->status["rp-1"].DesiredStatus = s;  // v0: does not fit, compared on the host this sweep, widened before the next
+        prov.UpdateAllPodStatuses();
+        CHECK_EQ(notified.size(), 1u); CHECK_EQ(notified[0], "v0:Unknown:Unknown RunPod status: " + s);
+        CHECK_EQ(prov.HostCompares(), ++host);
+        notified.clear();
+        prov.UpdateAllPodStatuses();  // WidenRecords(stride), then the sweep at the new stride: nothing changed
+        CHECK_EQ(prov.Stride(), st.stride); CHECK(notified.empty()); CHECK_EQ(prov.HostCompares(), host);
+        api->status["rp-2"].DesiredStatus = t;  // v1: same length, differs in the last byte -- exactly v1, through the kernel
+        prov.UpdateAllPodStatuses();
+        CHECK_EQ(notified.size(), 1u); CHECK_EQ(notified[0], "v1:Unknown:Unknown RunPod status: " + t);  // default: branch, :1971-1979
+        CHECK_EQ(prov.HostCompares(), host); CHECK_EQ(prov.Info("default", "v1")->Status, t);
+        notified.clear();
+        prov.UpdateAllPodStatuses();
+        CHECK(notified.empty());
+    }
+    const std::string s125(125, 'C'), s126(126, 'D');
+    api->status["rp-3"].DesiredStatus = s125;  // v2: fits the 128-byte slot
+    prov.UpdateAllPodStatuses();
+    CHECK_EQ(notified.size(), 1u); CHECK_EQ(notified[0], "v2:Unknown:Unknown RunPod status: " + s125);
+    CHECK_EQ(prov.HostCompares(), host); CHECK_EQ(prov.Stride(), 128u);
+    notified.clear();
+    api->status["rp-3"].DesiredStatus = s126;  // longer than any slot: host compare, no widening
+    prov.UpdateAllPodStatuses();
+    CHECK_EQ(notified.size(), 1u); CHECK_EQ(prov.HostCompares(), host + 1);
+    notified.clear();
+    prov.UpdateAllPodStatuses();
+    CHECK(notified.empty()); CHECK_EQ(prov.Stride(), 128u);
+    // back to a known status: Running (no ports requested, so they count as exposed)
+    for (const char* id : {"rp-1", "rp-2", "rp-3"}) api->status[id].DesiredStatus = "RUNNING";
+    prov.UpdateAllPodStatuses();
+    std::set<std::string> s(notified.begin(), notified.end());
+    CHECK_EQ(notified.size(), 3u); CHECK(s.count("v0:Running:") == 1); CHECK(s.count("v1:Running:") == 1); CHECK(s.count("v2:Running:") == 1);
+    notified.clear();
+    prov.UpdateAllPodStatuses();
+    CHECK(notified.empty());
+}
+
 // CreatePod / DeletePod on other threads while sweeps run (the reference: pod worker + two tickers + API handlers,
 // kubelet.go:374-376, 718): every status transition the fake API makes must reach notifyFunc exactly once, and device
 // and host state must agree afterwards (a final quiet sweep reports nothing).
@@ -566,6 +620,7 @@ int main(int argc, char** argv) {
         TestProviderStatusSweep();
         TestSweepNotFoundDoesNotAbsorbOtherChanges();
         TestLongStatusStrings();
+        TestWideStatusStrings();
         TestConcurrentCreateAndSweep();
         TestSelfTick();
     } else {

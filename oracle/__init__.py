@@ -120,19 +120,65 @@ def select(offers, pods, want_top5: bool = True, n_threads: int = 1):
 
 
 class StatusTable:
-    """Previous-state table of the reference's sweep (Provider.podStatus, kubelet.go:42)."""
+    """Previous-state table of the reference's sweep (Provider.podStatus, kubelet.go:42): per slot the decoded
+    (status, ports) pair, compared as string + bool (``rpk_oracle_status_diff``), or "never seen".
+
+    Records are canonical slots of any stride 16..256 (include/rpk.h).  Their prefix does not depend on the stride,
+    so one table follows the engine across stride changes: the state is kept at the widest stride seen so far
+    (``self.stride``), a wider table copies every slot's bytes into the new width, and narrower records are
+    zero-padded to the table's width before they are compared."""
 
     def __init__(self, N: int, stride: int = 32):
         self.N, self.stride = N, stride
         self.prev = np.zeros((N, stride), np.uint8)
         self.has_prev = np.zeros(N, np.uint8)
 
+    def _fit(self, records: np.ndarray) -> np.ndarray:
+        """``records`` at the table's width (the table widens first when the records are wider)"""
+        s = records.shape[1]
+        assert records.dtype == np.uint8 and records.ndim == 2 and 16 <= s <= 256 and s % 16 == 0
+        if s > self.stride:
+            wide = np.zeros((self.prev.shape[0], s), np.uint8)
+            wide[:, : self.stride] = self.prev
+            self.prev, self.stride = wide, s
+        if s < self.stride:
+            wide = np.zeros((records.shape[0], self.stride), np.uint8)
+            wide[:, :s] = records
+            return wide
+        return np.ascontiguousarray(records)
+
     def diff(self, records: np.ndarray) -> np.ndarray:
-        assert records.dtype == np.uint8 and records.shape == (self.N, self.stride) and records.flags.c_contiguous
+        """rpk_status_diff: ascending changed slots; their state is replaced (kubelet.go:875-880)"""
+        assert records.shape[0] == self.N
+        recs = self._fit(records)
         idx = np.empty(self.N, np.uint32)
-        n = lib().rpk_oracle_status_diff(C.c_uint32(self.N), C.c_uint32(self.stride), _p(records, C.c_uint8),
+        n = lib().rpk_oracle_status_diff(C.c_uint32(self.N), C.c_uint32(self.stride), _p(recs, C.c_uint8),
                                          _p(self.prev, C.c_uint8), _p(self.has_prev, C.c_uint8), _p(idx, C.c_uint32))
         return idx[:n].copy()
+
+    def seed(self, records: np.ndarray) -> None:
+        """rpk_status_seed: every slot's state := its record; nothing is reported"""
+        assert records.shape[0] == self.N
+        self.prev[:] = self._fit(records)
+        self.has_prev[:] = 1
+
+    def seed_slots(self, slots: np.ndarray, records: np.ndarray) -> None:
+        """rpk_status_seed_slots: state of slot slots[i] := records[i] (distinct slots); no other slot is touched"""
+        slots = np.asarray(slots, np.int64)
+        assert records.shape[0] == len(slots) and len(np.unique(slots)) == len(slots)
+        assert len(slots) == 0 or (slots.min() >= 0 and slots.max() < self.N)
+        self.prev[slots] = self._fit(records)
+        self.has_prev[slots] = 1
+
+    def reset(self, N: int) -> None:
+        """rpk_status_reset: N slots, none seen (every slot reports on the next diff)"""
+        self.N = N
+        self.prev = np.zeros((N, self.stride), np.uint8)
+        self.has_prev = np.zeros(N, np.uint8)
+
+    def prev_hashes(self) -> np.ndarray:
+        """the device's previous-hash column for this state: the record hash of a seen slot, 0 for a slot never seen"""
+        return np.where(self.has_prev != 0, record_hashes(self.prev), np.uint64(0))
 
 
 def record_hashes(records: np.ndarray) -> np.ndarray:

@@ -9,6 +9,7 @@ import pytest
 import np_restatement as npr
 import oracle
 import rpk
+import status_cases as sc
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 CLOUD = {"SECURE": oracle.CLOUD_SECURE, "COMMUNITY": oracle.CLOUD_COMMUNITY}
@@ -223,3 +224,121 @@ def test_translate_run_pod_status_table():
             for f in (False, True):
                 rec = rpk.synth.encode_record(s, p, 16, f)[None, :]
                 assert int(oracle.record_codes(rec)[0]) == oracle.translate(s.decode(), "it FAILed" if f else "", p)
+
+
+# ---- the sweep-state model (oracle.StatusTable) across calls and strides ----------------------------------------
+
+def _decoded(records):
+    return [npr.decode_record(r) for r in records]
+
+
+def test_status_table_seed_then_diff_reports_nothing():
+    lt = sc.LogicalTable(700, np.random.default_rng(1))
+    for stride in (16, 48, 256):
+        lt.step(stride, 0.5)
+        recs = lt.records(stride)
+        tab = oracle.StatusTable(700, stride)
+        tab.seed(recs)
+        assert len(tab.diff(recs)) == 0
+        lt.step(stride, 0.1)
+        nxt = lt.records(stride)
+        prev = _decoded(recs)
+        assert np.array_equal(tab.diff(nxt), npr.status_changed_set(nxt, prev))
+
+
+def test_status_table_seed_slots_touches_only_named_slots():
+    N = 500
+    lt = sc.LogicalTable(N, np.random.default_rng(2))
+    base = lt.records(32)
+    tab = oracle.StatusTable(N, 32)
+    tab.diff(base)
+    lt.step(32, 0.6)
+    nxt = lt.records(32)
+    moved = npr.status_changed_set(nxt, _decoded(base))
+    assert len(moved) > 100
+    quiet = moved[::4]
+    tab.seed_slots(quiet, nxt[quiet])
+    assert np.array_equal(tab.diff(nxt), np.setdiff1d(moved, quiet).astype(np.uint32))
+    # a seeded slot takes the seeded record as its state, whatever it held before
+    tab.seed_slots(np.array([3]), base[3:4])
+    assert tab.diff(nxt).tolist() == ([3] if npr.decode_record(base[3]) != npr.decode_record(nxt[3]) else [])
+    tab.seed_slots(np.array([], np.int64), nxt[:0])
+    assert len(tab.diff(nxt)) == 0
+
+
+def test_status_table_reset_makes_every_slot_report():
+    recs = rpk.synth.make_status_records(300, 0)
+    tab = oracle.StatusTable(300)
+    tab.seed(recs)
+    tab.reset(300)
+    assert np.array_equal(tab.diff(recs), np.arange(300, dtype=np.uint32))
+    tab.reset(120)
+    assert tab.N == 120 and (tab.prev_hashes() == 0).all()
+    assert np.array_equal(tab.diff(np.ascontiguousarray(recs[:120])), np.arange(120, dtype=np.uint32))
+    assert np.array_equal(tab.prev_hashes(), oracle.record_hashes(np.ascontiguousarray(recs[:120])))
+
+
+def test_status_table_restride_keeps_state():
+    """The same logical records at another stride are the same state: seeded at 16, they report nothing at 64 or 256,
+    and a long status seeded at 256 still differs from everything a 16-byte slot can hold -- until it is replaced."""
+    N = 400
+    lt = sc.LogicalTable(N, np.random.default_rng(3))
+    tab = oracle.StatusTable(N, 16)
+    tab.seed(lt.records(16))
+    for stride in (64, 256, 32, 16):
+        assert len(tab.diff(lt.records(stride))) == 0, stride
+    lt.step(256, 0.5)
+    wide = lt.records(256)
+    long_rows = np.nonzero(lt.lens[lt.ids] > sc.capacity(16))[0]
+    assert len(long_rows) > 20
+    tab.seed(wide)
+    assert tab.stride == 256 and len(tab.diff(lt.records(256))) == 0
+    assert np.array_equal(tab.prev_hashes(), oracle.record_hashes(wide))
+    lt.step(16, 0.0)  # only the slots whose status does not fit 16 bytes change
+    got = tab.diff(lt.records(16))
+    assert np.array_equal(got, long_rows.astype(np.uint32))
+    assert len(tab.diff(lt.records(128))) == 0
+
+
+def test_status_table_program_matches_numpy_restatement():
+    """Seeded programs of reset / seed / seed_slots / diff at every stride: the oracle's table equals the decoded
+    (status, ports) bookkeeping of np_restatement after every step."""
+    for seed in range(6):
+        rng = np.random.default_rng(100 + seed)
+        N = int(rng.choice([1, 63, 200, 513]))
+        lt = sc.LogicalTable(N, rng)
+        tab = oracle.StatusTable(N, 16)
+        prev = [None] * N
+        log = []
+        for step in range(40):
+            stride = int(rng.choice(sc.STRIDES))
+            lt.step(stride, float(rng.choice([0.0, 0.05, 0.5])))
+            recs = lt.records(stride)
+            op = rng.choice(["diff", "diff", "seed", "seed_slots", "reset"])
+            log.append((str(op), stride))
+            if op == "diff":
+                assert np.array_equal(tab.diff(recs), npr.status_changed_set(recs, prev)), (seed, log)
+            elif op == "seed":
+                tab.seed(recs)
+                prev = _decoded(recs)
+            elif op == "seed_slots":
+                slots = rng.choice(N, int(rng.integers(1, N + 1)), replace=False)
+                tab.seed_slots(slots, recs[slots])
+                for s in slots:
+                    prev[s] = npr.decode_record(recs[s])
+            else:
+                tab.reset(N)
+                prev = [None] * N
+            want = np.array([0 if p is None else 1 for p in prev], np.uint8)
+            assert np.array_equal(tab.has_prev, want), (seed, log)
+
+
+@pytest.mark.parametrize("stride", sc.STRIDES)
+def test_status_code_corpus_oracles_agree(stride):
+    """The adversarial corpus (near-misses of every known status) x ports x message flag: the record decoder of the
+    oracle (record_codes) and translateRunPodStatus on the decoded string agree -- so either can pin the kernels."""
+    recs, sts, ports, flags = sc.corpus_records(stride)
+    want = sc.translated_codes(sts, ports, flags)
+    assert np.array_equal(oracle.record_codes(recs), want)
+    # the corpus really reaches every branch: all six known statuses, both RUNNING forms, both EXITED forms, unknown
+    assert len(set(want.tolist())) == 8

@@ -8,6 +8,7 @@ import pytest
 import np_restatement as npr
 import oracle
 import rpk
+import status_cases as sc
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
@@ -180,3 +181,24 @@ def test_tick_matches_separate_calls():
             if P:
                 assert np.array_equal(best, ob[0]) and np.array_equal(top5, ob[1])
         eng.close()
+
+
+@pytest.mark.parametrize("stride", sc.STRIDES)
+def test_code_corpus_every_stride(stride):
+    """The adversarial corpus (each known status, each with one byte changed at every position, one byte short or
+    long, lower-cased; unknown strings of a known status's length; empty and one-character statuses) x ports x
+    message flag: the code of every slot equals translateRunPodStatus of the decoded string.  Strides 16 / 32 run it
+    through both streaming shapes (the corpus as it is, and tiled past the 4M-slot big-table boundary), the other
+    strides through the tiled kernel."""
+    recs, sts, ports, flags = sc.corpus_records(stride)
+    want = sc.translated_codes(sts, ports, flags)
+    shapes = [1] + ([-(-(4 << 20) // len(recs))] if stride <= 32 else [])
+    for reps in shapes:
+        tab = np.ascontiguousarray(np.tile(recs, (reps, 1)))
+        eng = make_engine()
+        idx, codes, hashes = eng.status_diff(tab, want_hashes=True, want_codes=True)
+        eng.close()
+        assert len(idx) == len(tab)  # a fresh table: every slot reports, with its code
+        assert np.array_equal(codes, np.tile(want, reps)), (stride, len(tab))
+        assert np.array_equal(codes, oracle.record_codes(tab)), (stride, len(tab))
+        assert np.array_equal(hashes, oracle.record_hashes(tab)), (stride, len(tab))
