@@ -352,10 +352,52 @@ struct PersistArgs {
     uint32_t S, per, qspan, n_groups, tickets_per_block, stage_cap_subs;
 };
 
+// The (cloud, stage) queue CTA `cta` of `grid` serves when every queue has at least one CTA.  Queue q = c * S + s
+// (q = s when cloud 0 has no rows) holds the cloud's weighted rows times the sub-ranges of stage s -- the walk covers
+// whole sub-ranges, the table's partial last one included, so the last stage can be the lighter one.  A CTA keeps its
+// queue for the whole call, so the call ends when the queue with the most work per CTA drains: CTAs are shared out in
+// proportion to the work, then single CTAs move between queues while a move lowers the largest work per CTA -- when
+// no move does, no split of `grid` CTAs has a smaller largest load.  Every CTA computes the same split from the same
+// totals.  n: npairs words of scratch.
+__host__ __device__ uint32_t persist_queue_of(uint32_t cta, uint32_t grid, uint32_t npairs, uint32_t S, uint32_t per, uint32_t nsub,
+                                     const uint32_t (&work)[2], uint32_t have0, uint32_t* n) {
+    using u64 = unsigned long long;
+    auto load = [&](uint32_t q) -> u64 {
+        const uint32_t c = have0 ? q / S : 1u, s = q % S;
+        return (u64)max(work[c], 1u) * min(per, nsub - s * per);
+    };
+    u64 tot = 0;
+    for (uint32_t q = 0; q < npairs; ++q) tot += load(q);
+    uint32_t sum = 0;
+    for (uint32_t q = 0; q < npairs; ++q) { n[q] = max(1u, (uint32_t)((u64)grid * load(q) / tot)); sum += n[q]; }
+    auto heaviest = [&]() {  // the largest load per CTA
+        uint32_t b = 0;
+        for (uint32_t q = 1; q < npairs; ++q) if (load(q) * n[b] > load(b) * n[q]) b = q;
+        return b;
+    };
+    auto cheapest = [&](uint32_t skip) {  // the smallest load per CTA after giving up one
+        uint32_t a = kNone;
+        for (uint32_t q = 0; q < npairs; ++q)
+            if (q != skip && n[q] > 1u && (a == kNone || load(q) * (n[a] - 1u) < load(a) * (n[q] - 1u))) a = q;
+        return a;
+    };
+    while (sum > grid) { --n[cheapest(kNone)]; --sum; }  // npairs <= grid: some queue has two
+    while (sum < grid) { ++n[heaviest()]; ++sum; }
+    for (uint32_t i = 0; i < 4u * npairs; ++i) {  // every move shrinks the set of queues at the largest load
+        const uint32_t b = heaviest(), a = cheapest(b);
+        if (a == kNone || load(a) * n[b] >= load(b) * (n[a] - 1u)) break;
+        --n[a]; ++n[b];
+    }
+    uint32_t q = 0;
+    for (uint32_t acc = n[0]; acc <= cta; acc += n[++q]) {}
+    return q;
+}
+
 template <int RPL, int MINB>
 __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const PersistArgs& pa) {
     extern __shared__ __align__(128) uint32_t s_stage[];
     __shared__ __align__(8) uint64_t s_bar[kCopyGroups];
+    __shared__ uint32_t s_first;
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     constexpr uint32_t RPI = 32 * RPL;  // rows per item
     if (tid == 0) {
@@ -373,20 +415,19 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
     const uint32_t S = pa.S, W = a.pk.bm_words, w68 = W * kSubWords;
     const uint32_t have0 = rows[0] ? 1u : 0u, have1 = rows[1] ? 1u : 0u;
     const uint32_t npairs = S * (have0 + have1);  // 0: every row was final in the scatter kernel (neither cloud); only the push is left
-    // which (cloud, segment) stages this CTA serves: with at least as many CTAs as stages the CTAs are shared out in
-    // proportion to the clouds' mask-word work and every CTA keeps one stage for the whole call; otherwise CTA b serves
-    // stages b, b + grid, ... one after the other
-    uint32_t first, step, ctas0 = 0;
+    // which (cloud, segment) stages this CTA serves: with at least as many CTAs as stages the CTAs are shared out over
+    // the stages in proportion to their work (persist_queue_of) and every CTA keeps one stage for the whole call;
+    // otherwise CTA b serves stages b, b + grid, ... one after the other
+    uint32_t first, step;
     const bool shared_out = npairs <= gridDim.x;
     if (npairs == 0) {
         first = 0; step = 1;
     } else if (shared_out) {
-        const unsigned long long tot = (unsigned long long)work[0] + work[1];
-        ctas0 = tot ? (uint32_t)(((unsigned long long)gridDim.x * work[0] + tot / 2) / tot) : gridDim.x / 2;
-        ctas0 = max(ctas0, S * have0);
-        ctas0 = min(ctas0, gridDim.x - S * have1);
-        if (!have0) ctas0 = 0;
-        first = blockIdx.x < ctas0 ? blockIdx.x % S : S * have0 + (blockIdx.x - ctas0) % S;
+        // the stage memory is free until this CTA's copies are issued: thread 0 keeps the per-queue CTA counts there
+        if (tid == 0) s_first = persist_queue_of(blockIdx.x, gridDim.x, npairs, S, pa.per, a.nsub, work, have0, s_stage);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the bulk copies below overwrite those words
+        __syncthreads();
+        first = s_first;
         step = npairs;  // one stage only
     } else {
         first = blockIdx.x; step = gridDim.x;
@@ -663,7 +704,10 @@ int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream
         tickets += (nsubs + pl.qspan - 1) / pl.qspan;
     }
     pa.tickets_per_block = tickets;
-    // K0: one wave of CTAs (four per SM), each looping over 512-row chunks
+    // K0: one wave of CTAs (four per SM), each looping over 512-row chunks.  Four fill an SM's threads, so a status
+    // sweep enqueued beside the select waits for K0 and then runs beside K1.  Three per SM would let the sweep in
+    // beside K0, but the two then share HBM and K0 is on the select's critical path: with a 1M-slot sweep beside it, a
+    // 1M-row select took 383 us that way against 376 us with four (H100 SXM, 400 W, profiles/h100_step_sweep.json).
     const uint32_t chunks = (a.P + kPThreads - 1) / kPThreads;
     const uint32_t k0ctas = t.k0ctas > 0 ? (uint32_t)t.k0ctas : 4u * (uint32_t)pl.sm_count;
     const uint32_t blocks = chunks < k0ctas ? (chunks ? chunks : 1u) : k0ctas;

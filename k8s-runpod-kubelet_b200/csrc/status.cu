@@ -202,9 +202,11 @@ __device__ __forceinline__ uint32_t sum_before(volatile u64* st, uint32_t id, ui
 constexpr int kStreamItems = 2;                          // slots per lane per unit
 constexpr uint32_t kUnit = 32 * kStreamItems;            // slots per warp per unit
 // Two launch shapes of the same kernel.  1024-thread CTAs, one per SM: the CTA's 32 warps read one long sequential
-// stream -- the shape for a sweep that has the GPU to itself over a large table (HBM-bound regime).  256-thread CTAs, up to four per SM: 16K registers each, so ONE of them still fits
-// beside the 96-register persistent select kernel and the sweep of a tick runs next to the selection instead of in
-// front of it; used for tables below kBigTable slots (latency regime).
+// stream -- the shape for a sweep that has the GPU to itself over a large table (HBM-bound regime).  256-thread CTAs,
+// at most one per SM: 16K registers, exactly what the 96-register persistent select kernel leaves free, so the sweep of
+// a tick runs next to the selection instead of in front of it; used for tables below kBigTable slots (latency regime).
+// A second or third sweep CTA on an SM would keep the select's CTA off that SM until they leave; alone on the GPU, one
+// CTA per SM is also faster at 1M slots than four (fewer look-back entries and copy rounds).
 constexpr uint32_t kBigTable = 4u << 20;
 // control words (StatusArgs::tile_counter): [0] scheduling ticket, [1] finished CTAs
 template <int STRIDE> struct SlotData { uint4 lo; uint4 hi; u64 prev; };
@@ -615,8 +617,8 @@ int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
         RPK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         const uint32_t n_units = (a.N + kUnit - 1) / kUnit;
         const bool big = a.N >= kBigTable;
-        const uint32_t warps = big ? 32u : 8u, max_grid = (uint32_t)(big ? sms : 4 * sms);
-        // one unit per warp until every SM has its CTA(s), then longer runs per warp
+        const uint32_t warps = big ? 32u : 8u, max_grid = (uint32_t)sms;
+        // one unit per warp until every SM has its CTA, then longer runs per warp
         uint32_t grid = (n_units + warps - 1) / warps;
         if (grid > max_grid) grid = max_grid;
         if (grid == 0) grid = 1;

@@ -1,0 +1,80 @@
+"""GPU tests of the streaming status sweep (strides 16 and 32) on both sides of its two launch boundaries, each call
+checked against oracle.StatusTable.
+
+Below the big-table threshold the sweep runs one 8-warp CTA per SM (so that it fits beside the persistent select), and
+every warp takes one 64-slot unit until SMs * 8 * 64 slots; past that point the warps take longer runs.  At 4M slots
+the sweep switches to 1024-thread CTAs.  Each size runs a host-entry sequence (seed, diff with codes and hashes, an
+unchanged diff, reset, diff), a device-entry diff of a caller-owned hash column, and an rpk_tick."""
+import numpy as np
+import pytest
+
+import oracle
+import rpk
+
+pytestmark = pytest.mark.gpu
+
+BIG = 4 << 20  # kBigTable (status.cu)
+
+
+def sm_count() -> int:
+    import torch
+
+    return torch.cuda.get_device_properties(0).multi_processor_count
+
+
+def resolve(size: str) -> int:
+    """sizes that depend on the device are named at collection time (no GPU there) and resolved here"""
+    sat = sm_count() * 8 * 64  # one CTA per SM x 8 warps x one 64-slot unit
+    base, _, off = size.partition("+") if "+" in size else size.partition("-")
+    n = {"sat": sat, "big": BIG}[base]
+    return n + int(off) if "+" in size else n - int(off or 0)
+
+
+@pytest.mark.parametrize("stride", [16, 32])
+@pytest.mark.parametrize("size", ["sat-1", "sat", "sat+1", "big-1", "big", "big+1"])
+def test_sweep_at_launch_boundary(size, stride):
+    import torch
+
+    N = resolve(size)
+    base = rpk.synth.make_status_records(N, 0, stride=stride)
+    nxt = rpk.synth.make_status_records(N, 3, 0.2, stride=stride)
+    tab = oracle.StatusTable(N, stride)
+    with rpk.Engine(1) as eng:
+        eng.status_reset(N)
+        eng.status_seed(base)
+        tab.seed(base)
+        got, codes, hashes = eng.status_diff(nxt, want_codes=True, want_hashes=True)
+        want = tab.diff(nxt)
+        assert len(want) > N // 20
+        assert np.array_equal(got, want), f"N {N}: changed list"
+        assert np.array_equal(codes, oracle.record_codes(nxt)[want]), f"N {N}: codes"
+        assert np.array_equal(hashes, oracle.record_hashes(nxt)), f"N {N}: hash column"
+        got, _ = eng.status_diff(nxt)
+        assert np.array_equal(got, tab.diff(nxt)) and len(got) == 0, f"N {N}: unchanged sweep"
+        eng.status_reset(N)
+        tab.reset(N)
+        got, codes, _ = eng.status_diff(base, want_codes=True)
+        want = tab.diff(base)
+        assert len(want) == N and np.array_equal(got, want), f"N {N}: sweep after reset"
+        assert np.array_equal(codes, oracle.record_codes(base)), f"N {N}: codes after reset"
+
+        # device entry point: a caller-owned column holding the hashes of `base`
+        col_tab = oracle.StatusTable(N, stride)
+        col_tab.seed(base)
+        col = torch.from_numpy(oracle.record_hashes(base).view(np.int64)).cuda()
+        d_idx = torch.empty(N, dtype=torch.int32, device="cuda")
+        d_code = torch.empty(N, dtype=torch.int16, device="cuda")
+        d_n = torch.zeros(1, dtype=torch.int32, device="cuda")
+        eng.status_diff_device(torch.from_numpy(nxt).cuda(), stride, col, d_idx, d_n, d_changed_code=d_code)
+        torch.cuda.synchronize()
+        n = int(d_n.item())
+        want = col_tab.diff(nxt)
+        assert np.array_equal(d_idx[:n].cpu().numpy().view(np.uint32), want), f"N {N}: device changed list"
+        assert np.array_equal(d_code[:n].cpu().numpy().view(np.uint16), oracle.record_codes(nxt)[want]), f"N {N}: device codes"
+        assert np.array_equal(col.cpu().numpy().view(np.uint64), col_tab.prev_hashes()), f"N {N}: device column"
+
+        # rpk_tick (P = 0): the same kernel behind the tick entry point
+        _, _, got, codes = eng.tick(None, nxt)
+        want = tab.diff(nxt)
+        assert np.array_equal(got, want), f"N {N}: tick changed list"
+        assert np.array_equal(codes, oracle.record_codes(nxt)[want]), f"N {N}: tick codes"
