@@ -202,6 +202,24 @@ __global__ void __launch_bounds__(256) k_offer_bitmap(BitmapArgs a) {
     }
 }
 
+// Per-mem-threshold view for the persistent kernel: every pod row ANDs its mem threshold's row with at most one vcpu and
+// one ram row, so the products are stored instead -- slice m of sub-range s holds mem[m] & vcpu[v] (v = 0..D_vcpu), then
+// mem[m] & ram[r] (r = 0..D_ram), with the transposed view's row pitch.  mem[m] implies "available", so
+// mem[m] & vcpu[0] is mem[m] itself: a row whose vcpu and ram requests constrain nothing reads one word per chunk, and so
+// does a row where only one of them constrains.  One thread per output word.
+__global__ void k_offer_slices(const uint32_t* __restrict__ bmT, uint32_t* __restrict__ bmM, uint32_t nsub, uint32_t words,
+                               uint32_t dm1, uint32_t off_vcpu, uint32_t off_ram, uint32_t rows) {
+    const uint32_t per_slice = nsub * rows * kSubStride;
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= (size_t)dm1 * per_slice) return;
+    const uint32_t m = (uint32_t)(i / per_slice), rest = (uint32_t)(i % per_slice);
+    const uint32_t k = rest % kSubStride, row = (rest / kSubStride) % rows, sub = rest / (kSubStride * rows);
+    const uint32_t dv1 = off_ram - off_vcpu;
+    const uint32_t other = row < dv1 ? off_vcpu + row : off_ram + (row - dv1);
+    const uint32_t* sp = bmT + (size_t)sub * words * kSubStride + k;
+    bmM[i] = sp[m * kSubStride] & sp[other * kSubStride];
+}
+
 static uint32_t bitlen(uint32_t x) { uint32_t b = 0; while (x) { ++b; x >>= 1; } return b ? b : 1; }
 
 int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st) {
@@ -251,7 +269,8 @@ int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st)
         pk.bm_words = bm_words; pk.bm_off_vcpu = D[0] + 1; pk.bm_off_ram = D[0] + 1 + D[1] + 1;
         pk.bm_stride = bm_words <= 32 ? 32 : 64;
     }
-    if (ds.force_kind == 5 || ds.force_kind == 6) pk.no_fused = 1;
+    if (ds.force_kind >= 5) pk.no_fused = 1;
+    if (ds.force_kind == 7) pk.no_slice = 1;
     if (ds.force_kind == 6) pk.no_persist = 1;
     if (ds.force_kind == 1) { pk.bits = 0; pk.pos_bits = 0; pk.bm_words = 0; }
     if (ds.force_kind == 2) { pk.pos_bits = 0; pk.bm_words = 0; }
@@ -274,6 +293,18 @@ int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st)
             RPK_CUDA(cudaMemsetAsync(ds.v_bitmapT[c].p, 0, (size_t)(ds.nsub ? ds.nsub : 1) * pk.bm_words * kSubStride * sizeof(uint32_t), st));
         }
         k_offer_bitmap<<<dim3((ba.nchunks * 32 + 255) / 256, 2), 256, 0, st>>>(ba); ++launches;
+        // the per-mem-threshold view needs the mem threshold in the pod class key (select_persist.cu, class_dims)
+        const uint32_t dm1 = D[0] + 1, dv1 = D[1] + 1, dr1 = D[2] + 1;
+        if (ds.nsub && 2u * dm1 * dv1 * dr1 <= kMaxClasses) {
+            pk.slice_rows = dv1 + dr1;
+            const size_t n_words = (size_t)dm1 * ds.nsub * pk.slice_rows * kSubStride;
+            for (int c = 0; c < 2; ++c) {
+                ds.v_bitmapM[c].reserve(n_words);
+                k_offer_slices<<<(unsigned)((n_words + 255) / 256), 256, 0, st>>>(ds.v_bitmapT[c].p, ds.v_bitmapM[c].p, ds.nsub, pk.bm_words,
+                                                                               dm1, pk.bm_off_vcpu, pk.bm_off_ram, pk.slice_rows);
+                ++launches;
+            }
+        }
     }
     PackArgs pa;
     pa.G = G; pa.Gpad = Gpad; pa.n = n; pa.keys = keys; pa.vals = vals;

@@ -117,7 +117,8 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
 
 void fill_offer_args(const DeviceState& ds, SelectArgs& a) {
     for (int c = 0; c < 2; ++c) {
-        a.view[c].packed = ds.v_packed[c].p; a.view[c].bitmap = ds.v_bitmap[c].p; a.view[c].bitmapT = ds.v_bitmapT[c].p; a.view[c].wide = ds.v_wide[c].p;
+        a.view[c].packed = ds.v_packed[c].p; a.view[c].bitmap = ds.v_bitmap[c].p; a.view[c].bitmapT = ds.v_bitmapT[c].p;
+        a.view[c].bitmapM = ds.pk.slice_rows ? ds.v_bitmapM[c].p : nullptr; a.view[c].wide = ds.v_wide[c].p;
         a.view[c].price = ds.v_price[c].p; a.view[c].perm = ds.v_perm[c].p;
     }
     a.G = ds.G; a.Gpad = ds.Gpad; a.pk = ds.pk; a.nsub = ds.nsub;
@@ -130,7 +131,8 @@ int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, S
     const int R = ds.pk.bm_words ? 32 * pick_rows_per_lane(P, ds.G, ds.sm_count) : pick_rows_per_warp(P, ds.sm_count);
     const uint32_t tiles = select_tiles_max(P, R);
     ln.rw.reserve(P); ln.order.reserve((size_t)kGroups * P); ln.pos.reserve(P);
-    const size_t need = std::max<size_t>((size_t)2 * kGroups + tiles, (size_t)P / 8 + 3 * kGroups);  // worst case (1 row per warp): never regrown mid-pipeline
+    // worst case (1 row per warp; the persistent kernel's row blocks: one partial block per row group): never regrown mid-pipeline
+    const size_t need = std::max<size_t>((size_t)2 * kGroups + tiles, (size_t)P / 8 + 3 * kGroups + kMaxGroups);
     if (need > ln.ctrs.cap || ln.ctrs_dirty) {
         // the counters are zero between calls by construction (finish_tile); a fresh or suspect buffer is zeroed here
         ln.ctrs.reserve(need);
@@ -144,7 +146,7 @@ int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, S
     *use_persist = ds.pk.bm_words && (P > kFusedRowsMax || ds.pk.no_fused) && !ds.pk.no_persist && persist_plan(a, ds.sm_count, pl);
     if (*use_persist) {
         ln.key.reserve(P); ln.ord_rw.reserve(P);
-        const size_t hdr_words = persist_hdr_words(ds.G, ds.pk.bm_words);
+        const size_t hdr_words = persist_hdr_words(*pl);
         const bool fresh = !ln.hist.p || hdr_words > ln.hdr.cap;
         ln.hist.reserve(2 * kMaxClasses); ln.cursor.reserve(2 * kMaxClasses); ln.hdr.reserve(hdr_words);
         if (fresh || ln.persist_dirty) {  // zero between calls by construction (k_pod_classify's last block, the pushers)
@@ -484,6 +486,7 @@ int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int
                 else if (!strcmp(fk, "packed_pos")) ds.force_kind = 3; else if (!strcmp(fk, "bitmap")) ds.force_kind = 4;
                 else if (!strcmp(fk, "bitmap_grouped")) ds.force_kind = 5;  // every batch size through the persistent kernel
                 else if (!strcmp(fk, "bitmap_grid")) ds.force_kind = 6;     // ... through the first-generation grid kernel
+                else if (!strcmp(fk, "bitmap_price")) ds.force_kind = 7;    // ... through the persistent kernel, table staged by price
             }
             const size_t n = G ? G : 1;
             ds.raw_mem.reserve(n); ds.raw_vcpu.reserve(n); ds.raw_ram.reserve(n); ds.raw_sp.reserve(n); ds.raw_cp.reserve(n); ds.raw_flags.reserve(n);

@@ -42,6 +42,8 @@ struct PackLayout {
     uint32_t bm_stride; // words per chunk row: 32 (conflict-free) or 64 (up to 64 thresholds; words 32 apart share a bank)
     uint32_t no_fused;  // test hook (RPK_FORCE_KERNEL=bitmap_grouped): small batches also take the three-launch path
     uint32_t no_persist; // test hook (RPK_FORCE_KERNEL=bitmap_grid): the first-generation (tile x segment) grid kernel
+    uint32_t slice_rows; // rows per sub-range of the per-mem-threshold view bitmapM (D_vcpu+1 + D_ram+1); 0 = not built
+    uint32_t no_slice;   // test hook (RPK_FORCE_KERNEL=bitmap_price): the persistent kernel stages the table by price
 };
 constexpr uint32_t kBmMaxStride = 64;
 constexpr uint32_t kBmSegBytes = 65536;      // bit-sliced rows staged per CTA: 512 chunks (stride 32) or 256 (stride 64)
@@ -54,16 +56,19 @@ constexpr uint32_t kSmallBatch = 4096;       // rows: the host entry point's sin
 constexpr uint32_t kSubChunks = 64;
 constexpr uint32_t kSubStride = 68;
 constexpr uint32_t kMaxClasses = 4096;       // row classes (cloud x thresholds) the pod-side counting sort distinguishes
+constexpr uint32_t kMaxGroups = 2 * kBmMaxStride;  // row groups of the persistent select: cloud, or (cloud, mem threshold)
 // control words of the persistent select (Lane::hdr)
-// (words 0..3 are written before the grid kernel starts; RowsDone is polled while it runs and sits on a cache line of
-// its own; Pushed counts CTAs in the push tail; the queue cursors start on the next line)
-enum : uint32_t { kHdrRows0 = 0, kHdrRows1 = 1, kHdrWork0 = 2, kHdrWork1 = 3, kHdrRowsDone = 32, kHdrPushed = 64,
-                  kHdrCursors = 96 };
+// (RowsDone is polled while the grid kernel runs and sits on a cache line of its own; Pushed counts CTAs in the push
+// tail; the per-group row / work totals are written before the grid kernel starts; the queue cursors follow them)
+enum : uint32_t { kHdrRowsDone = 32, kHdrPushed = 64, kHdrGroupRows = 96, kHdrGroupWork = kHdrGroupRows + kMaxGroups,
+                  kHdrCursors = kHdrGroupWork + kMaxGroups };
 
 struct OfferView {       // one per cloud, all arrays in price-sorted order, length Gpad
     uint32_t* packed = nullptr;
     uint32_t* bitmap = nullptr;  // [Gpad/32][bm_stride]
     uint32_t* bitmapT = nullptr; // [nsub][bm_words][kSubStride] (transposed, see kSubChunks)
+    uint32_t* bitmapM = nullptr; // [D_mem+1][nsub][slice_rows][kSubStride]: per mem threshold m, rows mem[m] & vcpu[v]
+                                 // (v = 0..D_vcpu), then mem[m] & ram[r] (r = 0..D_ram); null when not built
     int4* wide = nullptr;     // (mem_gb, vcpu, ram_gb, offer index)
     double* price = nullptr;  // NaN when the offer is not available in this cloud / padding
     int32_t* perm = nullptr;  // offer index, -1 when unavailable / padding
@@ -109,6 +114,7 @@ struct SelectArgs {
     int n_flags, my_rank;
     int inline_wait;     // the signalling warp also waits for every peer's signal (rpk_peer_inline_wait)
     uint32_t tune_natural_order;  // tuning hook (RPK_TUNE=order=natural): row tiles in group order instead of heaviest first
+    uint32_t slice;      // persistent select: rows grouped and the table staged per (cloud, mem threshold) on bitmapM
 };
 
 struct StatusArgs {
@@ -158,9 +164,9 @@ int launch_peer_fence(const PeerFenceArgs& a, cudaStream_t st);
 int launch_peer_signal(const PeerFenceArgs& a, uint32_t word0, cudaStream_t st);
 int launch_peer_wait(const PeerFenceArgs& a, uint32_t what, cudaStream_t st);
 // persistent bit-sliced select (select_persist.cu)
-struct PersistPlan { uint32_t cap_subs, S, per, qspan, Qi, grid, smem_bytes; int rpl, minb, sm_count; };
+struct PersistPlan { uint32_t cap_subs, S, per, qspan, Qi, grid, smem_bytes, slice, n_cursors; int rpl, minb, sm_count; };
 bool persist_plan(const SelectArgs& a, int sm_count, PersistPlan* pl);
-uint32_t persist_hdr_words(uint32_t G, uint32_t bm_words);
+uint32_t persist_hdr_words(const PersistPlan& pl);
 int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream_t st);
 uint32_t status_tiles(uint32_t N, uint32_t stride);
 uint32_t status_state_words(uint32_t N, uint32_t stride, int sm_count);
@@ -192,11 +198,12 @@ struct DeviceState {
     bool offers_ready = false;
     DevBuf<int32_t> raw_mem, raw_vcpu, raw_ram; DevBuf<double> raw_sp, raw_cp; DevBuf<uint8_t> raw_flags;
     DevBuf<unsigned long long> sort_keys; DevBuf<uint32_t> sort_vals;
-    DevBuf<uint32_t> v_packed[2]; DevBuf<uint32_t> v_bitmap[2]; DevBuf<uint32_t> v_bitmapT[2]; uint32_t nsub = 0; DevBuf<int4> v_wide[2]; DevBuf<double> v_price[2]; DevBuf<int32_t> v_perm[2];
+    DevBuf<uint32_t> v_packed[2]; DevBuf<uint32_t> v_bitmap[2]; DevBuf<uint32_t> v_bitmapT[2]; DevBuf<uint32_t> v_bitmapM[2]; uint32_t nsub = 0; DevBuf<int4> v_wide[2]; DevBuf<double> v_price[2]; DevBuf<int32_t> v_perm[2];
     DevBuf<int32_t> distinct[3]; DevBuf<uint32_t> dcount;
     uint32_t D[3] = {0, 0, 0};
     PackLayout pk = {};
-    int force_kind = 0;  // RPK_FORCE_KERNEL (tests): 0 auto, 1 generic, 2 packed+select, 3 packed+pos, 4 bit-sliced
+    int force_kind = 0;  // RPK_FORCE_KERNEL (tests): 0 auto, 1 generic, 2 packed+select, 3 packed+pos, 4 bit-sliced,
+                         // 5 / 6 / 7 every batch through the persistent / first-generation / price-staged persistent kernel
     // select scratch.  The host entry point pipelines row sub-batches over four lanes (stream + staging +
     // scratch each) so that the H2D of one sub-batch, the kernels of another and the D2H of a third overlap;
     // the device entry points use lane 0's scratch on the caller's stream.

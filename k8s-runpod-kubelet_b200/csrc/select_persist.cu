@@ -2,28 +2,32 @@
 // fused kernel's size).  Same predicate and tie rule as select.cu (reference runpod_client.go:465-509); what changes
 // is how the mask words reach the lanes and who owns a stage of the offer table:
 //
-//   k_pod_classify   row -> rank thresholds -> class key (cloud, vcpu threshold, ram threshold, mem threshold); one wave of
+//   k_pod_classify   row -> rank thresholds -> class key (cloud, thresholds; see class_key for the order); one wave of
 //                    CTAs, each looping over 512-row chunks: shared-memory histogram -> global class counts; fills
 //                    pos[] = none; block 0 resets the queue state of the grid kernel.
 //   k_pod_scatter    counting-sort scatter, same CTA shape: every CTA scans the class counts itself, reserves its rows
 //                    per class with one atomic per non-empty class and writes ONE {row, thresholds} pair per row in
-//                    class order (ord_rw[]); block 0 publishes per-cloud row / work totals.  Rows of neither cloud
-//                    are final here (-1, runpod_client.go:469-475).
-//   k_select_persist persistent CTAs (512 threads, as many per SM as the stage allows).  A CTA loads ONE stage of one
-//                    cloud view -- `per` 64-chunk sub-ranges of the transposed view, 8 bulk async copies on 8 mbarriers,
-//                    so the first items start before the whole stage has landed -- and keeps it for the whole call.
-//                    Its warps pull items (64 consecutive rows of the class order x a range of sub-ranges) from the
-//                    stage's queue with one atomic each.  A lane owns RPL rows and reads its rows' threshold words for
-//                    FOUR chunks with one LDS.128 (the view is [threshold][chunk]-major); rows of a warp share their
-//                    thresholds after the sort, so the 32 lanes read at most a few distinct 16-byte addresses and the
-//                    load costs 2 LSU cycles instead of the ~5 that four LDS.32 cost (tools/microbench/lds_probe.cu on
-//                    H100: LDS.128 with <= 8 distinct addresses = 2.0 cycles/warp, LDS.32 = 1.2).  Every (row, chunk) mask is
-//                    still loaded and ANDed -- bit j of it IS the predicate of runpod_client.go:478 (minus the price
-//                    bound) for offer j; eight chunks are OR-folded before the "any hit" test, the cheapest hit's block
-//                    is re-read once at the end for the bit position.
-//                    Segments merge with atomicMin; the warp that takes a row block's last ticket applies
-//                    price < maxPrice to the winner (strict, :478; the bound is a prefix of the price order) and stores
-//                    the offer index.
+//                    class order (ord_rw[]); block 0 publishes per-group row / work totals (a group is a cloud, or a
+//                    (cloud, mem threshold) pair on the per-mem-threshold view).  Rows of neither cloud are final here
+//                    (-1, runpod_client.go:469-475).
+//   k_select_persist persistent CTAs (512 threads, as many per SM as the stage allows).  A CTA loads ONE stage -- `per`
+//                    64-chunk sub-ranges, 8 bulk async copies on 8 mbarriers, so the first items start before the whole
+//                    stage has landed -- and keeps it for the whole call.  A stage is, where the table allows it, the
+//                    slice of one mem threshold m over the whole price range (bitmapM: rows mem[m] & vcpu[v] and
+//                    mem[m] & ram[r]; a row reads ONE word per chunk, two when both its vcpu and ram requests
+//                    constrain), else a price range of the per-threshold view (bitmapT: one word for mem plus one per
+//                    constraining column).  Its warps pull items (64 consecutive rows of one group x a range of
+//                    sub-ranges) from the stage's queue with one atomic each.  A lane owns RPL rows and reads its rows'
+//                    mask words for FOUR chunks with one LDS.128 (the views are [row][chunk]-major); rows of a warp
+//                    share their thresholds after the sort, so the 32 lanes read at most a few distinct 16-byte
+//                    addresses and the load costs 2 LSU cycles instead of the ~5 that four LDS.32 cost
+//                    (tools/microbench/lds_probe.cu on H100: LDS.128 with <= 8 distinct addresses = 2.0 cycles/warp,
+//                    LDS.32 = 1.2).  Every (row, chunk) mask is still loaded and ANDed -- bit j of it IS the predicate
+//                    of runpod_client.go:478 (minus the price bound) for offer j; eight chunks are OR-folded before the
+//                    "any hit" test, the cheapest hit's block is re-read once at the end for the bit position.
+//                    An item that spans the whole table is final after its walk: price < maxPrice on the winner (strict,
+//                    :478; the bound is a prefix of the price order) and the offer index is stored at once.  Otherwise
+//                    segments merge with atomicMin and the warp that takes a row block's last ticket does that.
 //   fused all-gather every retired row block adds its rows to one counter; a CTA that has run out of items waits until the
 //                    counter reaches the row count (one polling thread per CTA), then EVERY warp of the grid copies an
 //                    equal share of the slice to every peer with 16-byte NVLink stores; the CTA that finishes last
@@ -48,26 +52,44 @@ constexpr uint32_t kSubWords = kSubStride;
 // ---------------------------------------------------------------------------------------------------------
 // row classes
 // ---------------------------------------------------------------------------------------------------------
-struct ClassDims { uint32_t Dm1, Dv1, Dr1, use_mem, C; };
-__host__ __device__ __forceinline__ ClassDims class_dims(const uint32_t (&D)[3]) {
+struct ClassDims { uint32_t Dm1, Dv1, Dr1, use_mem, C, slice; };
+__host__ __device__ __forceinline__ ClassDims class_dims(const uint32_t (&D)[3], uint32_t slice) {
     ClassDims cd;
     cd.Dm1 = D[0] + 1; cd.Dv1 = D[1] + 1; cd.Dr1 = D[2] + 1;
     // bm_words = Dm1 + Dv1 + Dr1 <= 64, so 2 * Dv1 * Dr1 <= 1922 always fits; the mem threshold joins the key when it fits too
+    // (bitmapM is only built, and `slice` only set, when it does)
     cd.use_mem = 2u * cd.Dm1 * cd.Dv1 * cd.Dr1 <= kMaxClasses ? 1u : 0u;
     cd.C = 2u * cd.Dv1 * cd.Dr1 * (cd.use_mem ? cd.Dm1 : 1u);
+    cd.slice = slice;
     return cd;
 }
-// Class order = processing order: cloud, then vcpu threshold DEscending, ram threshold descending (rows whose requests
-// constrain nothing -- one mask word per chunk -- come last, so the warps that finish the grid are the light ones),
-// then the mem threshold.
+// Class order = processing order.  Table staged by price: cloud, then vcpu threshold DEscending, ram threshold
+// descending (rows whose requests constrain nothing -- one mask word per chunk -- come last, so the warps that finish
+// the grid are the light ones), then the mem threshold.  Table staged per mem threshold (slice): cloud, mem threshold,
+// vcpu threshold descending, ram threshold descending -- each (cloud, mem threshold) group is one run of the order.
 __device__ __forceinline__ uint32_t class_key(const ClassDims& cd, uint32_t c, uint32_t tm1, uint32_t tv, uint32_t tr) {
+    if (cd.slice) return ((c * cd.Dm1 + tm1) * cd.Dv1 + (cd.Dv1 - 1 - tv)) * cd.Dr1 + (cd.Dr1 - 1 - tr);
     uint32_t k = (c * cd.Dv1 + (cd.Dv1 - 1 - tv)) * cd.Dr1 + (cd.Dr1 - 1 - tr);
     return cd.use_mem ? k * cd.Dm1 + tm1 : k;
 }
 __device__ __forceinline__ uint32_t class_weight(const ClassDims& cd, uint32_t key) {  // mask words per (row, chunk)
-    const uint32_t k = cd.use_mem ? key / cd.Dm1 : key;
-    const uint32_t tr_rev = k % cd.Dr1, tv_rev = (k / cd.Dr1) % cd.Dv1;
-    return 1u + (tv_rev != cd.Dv1 - 1 ? 1u : 0u) + (tr_rev != cd.Dr1 - 1 ? 1u : 0u);
+    const uint32_t k = cd.use_mem && !cd.slice ? key / cd.Dm1 : key;
+    const bool nv = k / cd.Dr1 % cd.Dv1 != cd.Dv1 - 1, nr = k % cd.Dr1 != cd.Dr1 - 1;
+    if (cd.slice) return nv && nr ? 2u : 1u;  // mem & vcpu and mem & ram are stored: the one or two that constrain
+    return 1u + (nv ? 1u : 0u) + (nr ? 1u : 0u);
+}
+// row group = K1's unit of queues: the cloud, or (cloud, mem threshold) on the per-mem-threshold view
+__device__ __forceinline__ uint32_t class_group(const ClassDims& cd, uint32_t key) {
+    return cd.slice ? key / (cd.Dv1 * cd.Dr1) : key / (cd.C / 2);
+}
+
+// The grid kernel's threshold word on the per-mem-threshold view: the row's mask rows inside its mem threshold's slice --
+// mem & vcpu[tv] or mem & ram[tr] (mem itself when neither constrains) first, then mem & ram[tr] when both constrain,
+// else the first again (ANDing it twice changes nothing).  rw: the row's bitmap words.
+__device__ __forceinline__ uint32_t slice_rw(const ClassDims& cd, const PackLayout& pk, uint32_t rw) {
+    const uint32_t tv = ((rw >> 8) & 0xFFu) - pk.bm_off_vcpu, tr = ((rw >> 16) & 0xFFu) - pk.bm_off_ram;
+    const uint32_t i1 = tv ? tv : tr ? cd.Dv1 + tr : 0u, i2 = tv && tr ? cd.Dv1 + tr : i1;
+    return i1 | (i2 << 8) | (i1 << 16);
 }
 
 __device__ __forceinline__ uint32_t lb_smem(const int32_t* a, uint32_t n, int32_t x) {
@@ -195,7 +217,7 @@ __global__ void __launch_bounds__(kPThreads) k_pod_classify(SelectArgs a, uint32
     __shared__ int32_t s_dist[3][64];
     __shared__ uint32_t s_hist[kMaxClasses];
     const uint32_t tid = threadIdx.x;
-    const ClassDims cd = class_dims(a.D);
+    const ClassDims cd = class_dims(a.D, a.slice);
     uint32_t* hist = a.hist;
     for (uint32_t i = tid; i < 192; i += kPThreads) {
         const uint32_t d = i >> 6, k = i & 63;
@@ -213,7 +235,7 @@ __global__ void __launch_bounds__(kPThreads) k_pod_classify(SelectArgs a, uint32
         const uint32_t tm1 = lb_smem(s_dist[0], a.D[0], a.req_mem[p]);
         const uint32_t tv = lb_smem(s_dist[1], a.D[1], a.req_vcpu ? a.req_vcpu[p] : 0);
         const uint32_t tr = lb_smem(s_dist[2], a.D[2], a.req_ram ? a.req_ram[p] : 0);
-        a.rw[p] = tm1 | ((a.pk.bm_off_vcpu + tv) << 8) | ((a.pk.bm_off_ram + tr) << 16);
+        a.rw[p] = tm1 | ((a.pk.bm_off_vcpu + tv) << 8) | ((a.pk.bm_off_ram + tr) << 16);  // bitmap words (the top-5 kernel reads these)
         uint32_t key = 0xFFFFu;  // neither SECURE nor COMMUNITY: nothing is feasible (runpod_client.go:469-475)
         if (c <= 1) { key = class_key(cd, c, tm1, tv, tr); atomicAdd(&s_hist[key], 1u); }
         a.key[p] = (uint16_t)key;
@@ -229,18 +251,19 @@ __global__ void __launch_bounds__(kPThreads) k_pod_classify(SelectArgs a, uint32
 // itself (<= 4096 words: cheaper than a serial "last block" phase in the kernel before) and adds its counts to the
 // global class cursors with one atomic per non-empty class, which turns its shared table into "next free position per
 // class"; pass 2 re-reads the keys (L2 hits) and hands every row its position.  The per-CTA cost of the 4096-bin
-// tables is paid once per CTA, not once per 512 rows.  Block 0 also publishes the per-cloud row / work totals the grid
+// tables is paid once per CTA, not once per 512 rows.  Block 0 also publishes the per-group row / work totals the grid
 // kernel shares its CTAs out by.
 // ---------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
     __shared__ uint32_t s_cnt[kMaxClasses], s_base[kMaxClasses];
     __shared__ uint32_t s_warp[kPWarps];
-    __shared__ unsigned long long s_work[2];
-    __shared__ uint32_t s_rows[2];
+    __shared__ unsigned long long s_work[kMaxGroups];
+    __shared__ uint32_t s_rows[kMaxGroups];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    const ClassDims cd = class_dims(a.D);
+    const ClassDims cd = class_dims(a.D, a.slice);
+    const uint32_t n_groups = cd.slice ? 2u * cd.Dm1 : 2u;
     for (uint32_t i = tid; i < cd.C; i += kPThreads) s_cnt[i] = 0u;
-    if (tid < 2) { s_work[tid] = 0ull; s_rows[tid] = 0u; }
+    if (tid < kMaxGroups) { s_work[tid] = 0ull; s_rows[tid] = 0u; }
     __syncthreads();
     pdl_wait();     // k_pod_classify has completed: keys, rw, class counts
     pdl_trigger();  // the grid kernel may be scheduled; it waits before it reads anything written here
@@ -260,14 +283,8 @@ __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
         const uint32_t key = (uint32_t)a.key[p];
         if (key != 0xFFFFu) atomicAdd(&s_cnt[key], 1u);
     }
-    unsigned long long work[2] = {0ull, 0ull};
-    uint32_t rows[2] = {0u, 0u};
 #pragma unroll
-    for (uint32_t k = 0; k < kPer; ++k) {
-        const uint32_t i = tid * kPer + k;
-        sum += v[k];
-        if (blockIdx.x == 0 && v[k]) { const uint32_t c = i >= cd.C / 2 ? 1u : 0u; rows[c] += v[k]; work[c] += (unsigned long long)v[k] * class_weight(cd, i); }
-    }
+    for (uint32_t k = 0; k < kPer; ++k) sum += v[k];
     uint32_t inc = sum;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) { const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, inc, d); if ((int)lane >= d) inc += n; }
@@ -275,8 +292,18 @@ __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
     __syncthreads();  // s_warp, and every row of pass 1 is counted
     uint32_t run = inc - sum;
     for (uint32_t w = 0; w < warp; ++w) run += s_warp[w];
-    if (blockIdx.x == 0) {
-        for (int c = 0; c < 2; ++c) if (rows[c]) { atomicAdd(&s_rows[c], rows[c]); atomicAdd(&s_work[c], work[c]); }
+    if (blockIdx.x == 0) {  // this thread's classes, one run per group
+        uint32_t g_run = 0, rows = 0;
+        unsigned long long work = 0ull;
+#pragma unroll
+        for (uint32_t k = 0; k < kPer; ++k) {
+            const uint32_t i = tid * kPer + k;
+            if (!v[k]) continue;
+            const uint32_t g = class_group(cd, i);
+            if (rows && g != g_run) { atomicAdd(&s_rows[g_run], rows); atomicAdd(&s_work[g_run], work); rows = 0; work = 0ull; }
+            g_run = g; rows += v[k]; work += (unsigned long long)v[k] * class_weight(cd, i);
+        }
+        if (rows) { atomicAdd(&s_rows[g_run], rows); atomicAdd(&s_work[g_run], work); }
     }
     // class start + this CTA's share of the class = the first position this CTA may use
 #pragma unroll
@@ -286,9 +313,9 @@ __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
         run += v[k];
     }
     __syncthreads();
-    if (blockIdx.x == 0 && tid == 0) {
-        a.hdr[kHdrRows0] = s_rows[0]; a.hdr[kHdrRows1] = s_rows[1];
-        a.hdr[kHdrWork0] = (uint32_t)min(s_work[0] >> 2, 0xFFFFFFFFull); a.hdr[kHdrWork1] = (uint32_t)min(s_work[1] >> 2, 0xFFFFFFFFull);
+    if (blockIdx.x == 0 && tid < n_groups) {
+        a.hdr[kHdrGroupRows + tid] = s_rows[tid];
+        a.hdr[kHdrGroupWork + tid] = (uint32_t)min(s_work[tid] >> 2, 0xFFFFFFFFull);
     }
     // pass 2: positions (the order inside a class is arbitrary -- results go back by row id)
     uint32_t n_neither = 0;
@@ -298,7 +325,8 @@ __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
         const bool neither = p < a.P && key == 0xFFFFu;
         if (p < a.P && !neither) {
             const uint32_t dst = atomicAdd(&s_base[key], 1u);
-            a.ord_rw[dst] = make_uint2(p, a.rw[p]);  // the one scattered store of the sort
+            const uint32_t w = a.rw[p];
+            a.ord_rw[dst] = make_uint2(p, cd.slice ? slice_rw(cd, a.pk, w) : w);  // the one scattered store of the sort
         }
         if (neither) {
             store_best_local(a, p, -1);
@@ -350,54 +378,60 @@ __device__ __forceinline__ void walk(const uint32_t* __restrict__ stage, uint32_
 
 struct PersistArgs {
     uint32_t S, per, qspan, n_groups, tickets_per_block, stage_cap_subs;
+    uint32_t slice, groups, groups_per_cloud;  // slice: stages are cut from bitmapM; row groups in all / per cloud
 };
 
-// The (cloud, stage) queue CTA `cta` of `grid` serves when every queue has at least one CTA.  Queue q = c * S + s
-// (q = s when cloud 0 has no rows) holds the cloud's weighted rows times the sub-ranges of stage s -- the walk covers
-// whole sub-ranges, the table's partial last one included, so the last stage can be the lighter one.  A CTA keeps its
-// queue for the whole call, so the call ends when the queue with the most work per CTA drains: CTAs are shared out in
-// proportion to the work, then single CTAs move between queues while a move lowers the largest work per CTA -- when
-// no move does, no split of `grid` CTAs has a smaller largest load.  Every CTA computes the same split from the same
-// totals.  n: npairs words of scratch.
-__host__ __device__ uint32_t persist_queue_of(uint32_t cta, uint32_t grid, uint32_t npairs, uint32_t S, uint32_t per, uint32_t nsub,
-                                     const uint32_t (&work)[2], uint32_t have0, uint32_t* n) {
-    using u64 = unsigned long long;
-    auto load = [&](uint32_t q) -> u64 {
-        const uint32_t c = have0 ? q / S : 1u, s = q % S;
-        return (u64)max(work[c], 1u) * min(per, nsub - s * per);
+// The (group, stage) queue CTA `cta` of `grid` serves when every queue has at least one CTA.  Queue q = (non-empty row
+// group q / S, stage q % S) holds the group's weighted rows times the sub-ranges of the stage -- the walk covers whole
+// sub-ranges, the table's partial last one included, so the last stage can be the lighter one.  A CTA keeps its queue
+// for the whole call, so the call ends when the queue with the most work per CTA drains: the split minimises that.
+// Bisection finds (to float precision) the least load per CTA T for which max(1, ceil(load / T)) CTAs per queue add
+// up to at most `grid`; each queue gets that many, and any CTAs left over join queues 0, 1, ... one each.  Whole warp
+// (lane l owns a run of queues: 32 halvings of a few divisions each); every CTA computes the same split from the same
+// totals.  work: per non-empty group.
+__device__ uint32_t persist_queue_of(uint32_t cta, uint32_t grid, uint32_t npairs, uint32_t S, uint32_t per, uint32_t nsub,
+                                     const uint32_t* work) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t k = (npairs + 31) / 32, q0 = min(npairs, lane * k), q1 = min(npairs, q0 + k);
+    auto load = [&](uint32_t q) { return (float)max(work[q / S], 1u) * (float)min(per, nsub - q % S * per); };
+    auto ctas = [&](uint32_t q, float T) { return (uint32_t)fmaxf(1.f, ceilf(load(q) / T)); };
+    auto need = [&](float T) {
+        uint32_t n = 0;
+        for (uint32_t q = q0; q < q1; ++q) n += ctas(q, T);
+#pragma unroll
+        for (int d = 16; d; d >>= 1) n += __shfl_xor_sync(0xFFFFFFFFu, n, d);
+        return n;
     };
-    u64 tot = 0;
-    for (uint32_t q = 0; q < npairs; ++q) tot += load(q);
-    uint32_t sum = 0;
-    for (uint32_t q = 0; q < npairs; ++q) { n[q] = max(1u, (uint32_t)((u64)grid * load(q) / tot)); sum += n[q]; }
-    auto heaviest = [&]() {  // the largest load per CTA
-        uint32_t b = 0;
-        for (uint32_t q = 1; q < npairs; ++q) if (load(q) * n[b] > load(b) * n[q]) b = q;
-        return b;
-    };
-    auto cheapest = [&](uint32_t skip) {  // the smallest load per CTA after giving up one
-        uint32_t a = kNone;
-        for (uint32_t q = 0; q < npairs; ++q)
-            if (q != skip && n[q] > 1u && (a == kNone || load(q) * (n[a] - 1u) < load(a) * (n[q] - 1u))) a = q;
-        return a;
-    };
-    while (sum > grid) { --n[cheapest(kNone)]; --sum; }  // npairs <= grid: some queue has two
-    while (sum < grid) { ++n[heaviest()]; ++sum; }
-    for (uint32_t i = 0; i < 4u * npairs; ++i) {  // every move shrinks the set of queues at the largest load
-        const uint32_t b = heaviest(), a = cheapest(b);
-        if (a == kNone || load(a) * n[b] >= load(b) * (n[a] - 1u)) break;
-        --n[a]; ++n[b];
+    float tot = 0.f, hi = 0.f;
+    for (uint32_t q = q0; q < q1; ++q) { tot += load(q); hi = fmaxf(hi, load(q)); }
+#pragma unroll
+    for (int d = 16; d; d >>= 1) { tot += __shfl_down_sync(0xFFFFFFFFu, tot, d); hi = fmaxf(hi, __shfl_xor_sync(0xFFFFFFFFu, hi, d)); }
+    float lo = __shfl_sync(0xFFFFFFFFu, tot, 0) / (float)grid;  // no split does better; hi (one CTA each) fits: npairs <= grid
+    for (int i = 0; i < 32; ++i) {
+        const float mid = 0.5f * (lo + hi);
+        if (need(mid) <= grid) hi = mid; else lo = mid;
     }
-    uint32_t q = 0;
-    for (uint32_t acc = n[0]; acc <= cta; acc += n[++q]) {}
-    return q;
+    uint32_t mine = 0;
+    for (uint32_t q = q0; q < q1; ++q) mine += ctas(q, hi);
+    uint32_t incl = mine;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) { const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, incl, d); if ((int)lane >= d) incl += n; }
+    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+    if (cta >= total) return (cta - total) % npairs;
+    uint32_t found = kNone;
+    if (incl - mine <= cta && cta < incl)
+        for (uint32_t q = q0, acc = incl - mine; q < q1 && found == kNone; ++q) { acc += ctas(q, hi); if (cta < acc) found = q; }
+    const uint32_t owner = __ffs(__ballot_sync(0xFFFFFFFFu, found != kNone)) - 1;
+    return __shfl_sync(0xFFFFFFFFu, found, owner);
 }
 
 template <int RPL, int MINB>
 __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const PersistArgs& pa) {
     extern __shared__ __align__(128) uint32_t s_stage[];
     __shared__ __align__(8) uint64_t s_bar[kCopyGroups];
-    __shared__ uint32_t s_first;
+    __shared__ uint32_t s_first, s_ng;
+    // the non-empty row groups in class order: group id, rows, first row (of the class order), first row block, work
+    __shared__ uint32_t s_grp[kMaxGroups], s_rows[kMaxGroups], s_start[kMaxGroups], s_blk0[kMaxGroups], s_work[kMaxGroups];
     const uint32_t tid = threadIdx.x, lane = tid & 31;
     constexpr uint32_t RPI = 32 * RPL;  // rows per item
     if (tid == 0) {
@@ -409,33 +443,52 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
     // the scatter kernel is done with the class counts and cursors: zero them for the next call (all kMaxClasses words --
     // the table, and with it the class count, may change between calls)
     if (blockIdx.x == 0) for (uint32_t i = tid; i < kMaxClasses; i += kPThreads) { a.hist[i] = 0u; a.cursor[i] = 0u; }
+    if (tid < 32) {
+        uint32_t row_run = 0, blk_run = 0, n_ne = 0;
+        for (uint32_t g0 = 0; g0 < pa.groups; g0 += 32) {
+            const uint32_t g = g0 + lane;
+            const uint32_t r = g < pa.groups ? __ldcg(a.hdr + kHdrGroupRows + g) : 0u, b = (r + RPI - 1) / RPI;
+            uint32_t ir = r, ib = b;
+#pragma unroll
+            for (int d = 1; d < 32; d <<= 1) {
+                const uint32_t xr = __shfl_up_sync(0xFFFFFFFFu, ir, d), xb = __shfl_up_sync(0xFFFFFFFFu, ib, d);
+                if ((int)lane >= d) { ir += xr; ib += xb; }
+            }
+            const uint32_t ne = __ballot_sync(0xFFFFFFFFu, r != 0);
+            if (r) {
+                const uint32_t j = n_ne + __popc(ne & ((1u << lane) - 1u));
+                s_grp[j] = g; s_rows[j] = r; s_start[j] = row_run + ir - r; s_blk0[j] = blk_run + ib - b;
+                s_work[j] = __ldcg(a.hdr + kHdrGroupWork + g);
+            }
+            row_run += __shfl_sync(0xFFFFFFFFu, ir, 31); blk_run += __shfl_sync(0xFFFFFFFFu, ib, 31); n_ne += __popc(ne);
+        }
+        if (lane == 0) s_ng = n_ne;
+    }
     __syncthreads();
-    const uint32_t rows[2] = {__ldcg(a.hdr + kHdrRows0), __ldcg(a.hdr + kHdrRows1)};
-    const uint32_t work[2] = {__ldcg(a.hdr + kHdrWork0), __ldcg(a.hdr + kHdrWork1)};
-    const uint32_t S = pa.S, W = a.pk.bm_words, w68 = W * kSubWords;
-    const uint32_t have0 = rows[0] ? 1u : 0u, have1 = rows[1] ? 1u : 0u;
-    const uint32_t npairs = S * (have0 + have1);  // 0: every row was final in the scatter kernel (neither cloud); only the push is left
-    // which (cloud, segment) stages this CTA serves: with at least as many CTAs as stages the CTAs are shared out over
-    // the stages in proportion to their work (persist_queue_of) and every CTA keeps one stage for the whole call;
-    // otherwise CTA b serves stages b, b + grid, ... one after the other
+    const uint32_t S = pa.S, w68 = (pa.slice ? a.pk.slice_rows : a.pk.bm_words) * kSubWords;
+    const uint32_t npairs = S * s_ng;  // 0: every row was final in the scatter kernel (neither cloud); only the push is left
+    // which (group, stage) queues this CTA serves: with at least as many CTAs as queues the CTAs are shared out over
+    // the queues in proportion to their work (persist_queue_of) and every CTA keeps one queue for the whole call;
+    // otherwise CTA b serves queues b, b + grid, ... one after the other
     uint32_t first, step;
-    const bool shared_out = npairs <= gridDim.x;
     if (npairs == 0) {
         first = 0; step = 1;
-    } else if (shared_out) {
-        // the stage memory is free until this CTA's copies are issued: thread 0 keeps the per-queue CTA counts there
-        if (tid == 0) s_first = persist_queue_of(blockIdx.x, gridDim.x, npairs, S, pa.per, a.nsub, work, have0, s_stage);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // the bulk copies below overwrite those words
+    } else if (npairs <= gridDim.x) {
+        if (tid < 32) { const uint32_t q = persist_queue_of(blockIdx.x, gridDim.x, npairs, S, pa.per, a.nsub, s_work); if (lane == 0) s_first = q; }
         __syncthreads();
         first = s_first;
-        step = npairs;  // one stage only
+        step = npairs;  // one queue only
     } else {
         first = blockIdx.x; step = gridDim.x;
     }
-    const uint32_t nblk0 = (rows[0] + RPI - 1) / RPI;
+    const uint32_t w_none = pa.slice ? 0u : (a.pk.bm_off_vcpu << 8) | (a.pk.bm_off_ram << 16);  // padding rows: no constraint
+    // an item that covers the whole table (one stage, one item per row block) leaves its rows final: no merge
+    const bool direct = pa.tickets_per_block == 1;
     uint32_t it = 0, phase_bits = 0;  // bit g: parity of copy group g's next completion (groups are not all used by every stage)
     for (uint32_t pair = first; pair < npairs; pair += step, ++it) {
-        const uint32_t c = have0 ? pair / S : 1u, s = pair % S;
+        const uint32_t gi = pair / S, s = pair % S, grp = s_grp[gi];
+        const uint32_t c = grp / pa.groups_per_cloud;
+        const uint32_t* src = pa.slice ? a.view[c].bitmapM + (size_t)(grp % pa.groups_per_cloud) * a.nsub * w68 : a.view[c].bitmapT;
         const uint32_t sub0 = s * pa.per, nsubs = min(pa.per, a.nsub - sub0);
         const uint32_t gs = (nsubs + pa.n_groups - 1) / pa.n_groups;  // subs per copy group
         if (it) __syncthreads();  // every warp is done with the previous stage
@@ -445,31 +498,40 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
             if (tid == 0) {
                 const uint32_t g0 = g * gs, gn = min(gs, nsubs - g0);
                 mbar_expect_tx(&s_bar[g], gn * w68 * 4u);
-                bulk_g2s(s_stage + (size_t)g0 * w68, a.view[c].bitmapT + ((size_t)sub0 + g0) * w68, gn * w68 * 4u, &s_bar[g]);
+                bulk_g2s(s_stage + (size_t)g0 * w68, src + ((size_t)sub0 + g0) * w68, gn * w68 * 4u, &s_bar[g]);
             }
         }
         const uint32_t parity = phase_bits;
         phase_bits ^= used;
         uint32_t ready = 0;  // copy groups this warp has seen complete
-        const uint32_t n_c = rows[c], c_start = c ? rows[0] : 0u;
+        const uint32_t n_c = s_rows[gi], c_start = s_start[gi];
         const uint32_t nblk = (n_c + RPI - 1) / RPI;
         const uint32_t Qi = (nsubs + pa.qspan - 1) / pa.qspan;
         const uint32_t n_items = nblk * Qi;
-        uint32_t* cursor = a.hdr + kHdrCursors + c * S + s;
-        uint32_t* tickets = a.tile_ctr + (c ? nblk0 : 0u);
+        uint32_t* cursor = a.hdr + kHdrCursors + grp * S + s;
+        uint32_t* tickets = a.tile_ctr + s_blk0[gi];
         uint32_t item = 0;
         if (lane == 0) item = atomicAdd(cursor, 1u);
         item = __shfl_sync(0xFFFFFFFFu, item, 0);
-        const uint32_t w_none = (a.pk.bm_off_vcpu << 8) | (a.pk.bm_off_ram << 16);  // padding rows: threshold 0 everywhere
         uint32_t w_cur[RPL];
 #pragma unroll
         for (int r = 0; r < RPL; ++r) {
             const uint32_t local = (item / Qi) * RPI + (uint32_t)r * 32 + lane;
             w_cur[r] = item < n_items && local < n_c ? __ldcg(a.ord_rw + c_start + local).y : w_none;
         }
+        // the offer at sorted position p wins row `row` if it is under the row's price bound (strict, runpod_client.go:478)
+        auto finish = [&](uint32_t row, uint32_t p) {
+            int32_t b = -1;
+            if (p != kNone) {
+                const double pr = a.view[c].price[p];
+                const double mx = a.max_price ? a.max_price[row] : RPK_DEFAULT_MAX_PRICE;
+                if (pr < mx) b = a.view[c].perm[p];
+            }
+            store_best_local(a, row, b);
+        };
         uint32_t pend1_blk = kNone, pend2_blk = kNone, pend2_ticket = 0;  // merge pipeline (see below)
         // the row block whose ticket was taken one iteration ago: if that was its last ticket, every segment of its rows
-        // has been merged -- price < maxPrice on the winner (strict, runpod_client.go:478), position -> offer index
+        // has been merged -- price < maxPrice on the winner, position -> offer index
         auto retire = [&](uint32_t rblk, uint32_t ticket) {
             if (rblk == kNone) return;
             if (__shfl_sync(0xFFFFFFFFu, ticket, 0) != pa.tickets_per_block - 1) return;
@@ -481,18 +543,7 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
                 const uint32_t local = rblk * RPI + (uint32_t)r * 32 + lane;
                 const bool ok = local < n_c;
                 n_final += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, ok));
-                uint32_t row = 0;
-                if (ok) {
-                    row = a.ord_rw[c_start + local].x;
-                    const uint32_t p = __ldcg(a.pos + c_start + local);
-                    int32_t b = -1;
-                    if (p != kNone) {
-                        const double pr = a.view[c].price[p];
-                        const double mx = a.max_price ? a.max_price[row] : RPK_DEFAULT_MAX_PRICE;
-                        if (pr < mx) b = a.view[c].perm[p];
-                    }
-                    store_best_local(a, row, b);
-                }
+                if (ok) finish(a.ord_rw[c_start + local].x, __ldcg(a.pos + c_start + local));
             }
             count_rows_done(a, n_final);
             if (a.n_out > 1 && a.self_out < 0) __threadfence_system();  // direct peer stores: performed before the grid completes
@@ -513,14 +564,16 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
                 const uint32_t w = w_cur[r];
                 const uint32_t i1 = w & 0xFFu, i2 = (w >> 8) & 0xFFu, i3 = (w >> 16) & 0xFFu;
                 o1[r] = i1 * kSubWords; o2[r] = i2 * kSubWords; o3[r] = i3 * kSubWords;
-                nv |= i2 != a.pk.bm_off_vcpu; nr |= i3 != a.pk.bm_off_ram;
+                // slice: a second word only when both vcpu and ram constrain (i3 = i1 never adds one)
+                if (pa.slice) nv |= i2 != i1;
+                else { nv |= i2 != a.pk.bm_off_vcpu; nr |= i3 != a.pk.bm_off_ram; }
                 bb[r] = kNone;
             }
             nv = __any_sync(0xFFFFFFFFu, nv); nr = __any_sync(0xFFFFFFFFu, nr);
             for (uint32_t g = (uint32_t)sub_lo / gs; g * gs < (uint32_t)sub_hi; ++g)
                 if (!(ready >> g & 1u)) { mbar_wait(&s_bar[g], parity >> g & 1u); ready |= 1u << g; }
-            // rows of an item share the "column constrains" flags except at class boundaries; a non-constraining column's
-            // threshold-0 word is all-available, so reading it for a row that does not need it is harmless
+            // rows of an item share the "column constrains" flags except at class boundaries; a word a row does not
+            // need is all-available for it (price stages: the column's threshold 0; slice: its own first word)
             if (!nv && !nr) walk<RPL, false, false>(s_stage, w68, sub_lo, sub_hi, o1, o2, o3, bb);
             else if (nv && !nr) walk<RPL, true, false>(s_stage, w68, sub_lo, sub_hi, o1, o2, o3, bb);
             else if (!nv && nr) walk<RPL, false, true>(s_stage, w68, sub_lo, sub_hi, o1, o2, o3, bb);
@@ -529,7 +582,7 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
             // taken, and the ticket's return value says whether these rows are final), so it is pipelined over the
             // NEXT items' walks: here the item walked one iteration ago takes its ticket (its atomicMin's were issued a
             // whole walk ago: the fence returns at once), and the item before that reads its ticket and, if it was the
-            // last one of its row block, runs the epilogue.
+            // last one of its row block, runs the epilogue.  Direct items never enter the pipeline.
             retire(pend2_blk, pend2_ticket);
             pend2_blk = pend1_blk; pend2_ticket = 0;
             if (pend1_blk != kNone) {
@@ -543,8 +596,10 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
                 const uint32_t local = (item_next / Qi) * RPI + (uint32_t)r * 32 + lane;
                 w_cur[r] = item_next < n_items && local < n_c ? __ldcg(a.ord_rw + c_start + local).y : w_none;
             }
+            uint32_t n_final = 0;
 #pragma unroll
             for (int r = 0; r < RPL; ++r) {
+                uint32_t p = kNone;
                 if (valid[r] && bb[r] != kNone) {  // re-read the cheapest block with a hit: first chunk, first bit
                     const uint32_t sub = bb[r] >> 3, b8 = bb[r] & 7u;
                     const uint32_t* sp = s_stage + (size_t)sub * w68 + b8 * 8;
@@ -554,10 +609,20 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
                         const uint32_t mk = sp[o1[r] + k] & sp[o2[r] + k] & sp[o3[r] + k];
                         if (mk) { j = (uint32_t)k; m = mk; }
                     }
-                    atomicMin(&a.pos[idx[r]], (((sub0 + sub) * kSubChunks + b8 * 8 + j) << 5) + (uint32_t)__ffs(m) - 1u);
+                    p = (((sub0 + sub) * kSubChunks + b8 * 8 + j) << 5) + (uint32_t)__ffs(m) - 1u;
+                }
+                if (direct) {
+                    n_final += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, valid[r]));
+                    if (valid[r]) finish(a.ord_rw[idx[r]].x, p);
+                } else if (p != kNone) {
+                    atomicMin(&a.pos[idx[r]], p);
                 }
             }
-            pend1_blk = blk;
+            if (direct) {
+                count_rows_done(a, n_final);
+                if (a.n_out > 1 && a.self_out < 0) __threadfence_system();
+            }
+            pend1_blk = direct ? kNone : blk;
             item = item_next;
         }
         // drain the pipeline: the last two items of this stage
@@ -618,7 +683,7 @@ __global__ void k_peer_wait(PeerFenceArgs a, uint32_t what) {
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-struct PTune { int rpl = 0; int stage_kb = 0; int items_per_warp = 0; int ctas = 0; int minb = 0; int regs = 0; int k0ctas = 0; bool pdl = true; };  // k0ctas 0: four per SM
+struct PTune { int rpl = 0; int stage_kb = 0; int items_per_warp = 0; int ctas = 0; int minb = 0; int regs = 0; int k0ctas = 0; bool pdl = true; bool price = false; };  // k0ctas 0: four per SM
 static PTune parse_ptune();
 static PTune read_ptune() {  // read once per process unless RPK_TUNE_RELOAD is set (see select.cu)
     static const bool reload = getenv("RPK_TUNE_RELOAD") != nullptr;
@@ -638,24 +703,27 @@ static PTune parse_ptune() {
     if (const char* p = strstr(e, "regs=")) t.regs = atoi(p + 5);
     if (const char* p = strstr(e, "k0ctas=")) { const int v = atoi(p + 7); if (v > 0) t.k0ctas = v; }
     t.pdl = strstr(e, "pdl=off") == nullptr;
+    t.price = strstr(e, "k1=price") != nullptr;  // stage the table by price even where the per-mem-threshold view exists (A/B)
     return t;
 }
 
-uint32_t persist_hdr_words(uint32_t G, uint32_t bm_words) {
-    (void)bm_words;
-    const uint32_t nsub = ((G + 31) / 32 + kSubChunks - 1) / kSubChunks;
-    return kHdrCursors + 2 * (nsub ? nsub : 1) + 8;  // S <= nsub
-}
+uint32_t persist_hdr_words(const PersistPlan& pl) { return kHdrCursors + pl.n_cursors + 8; }
 
 bool persist_plan(const SelectArgs& a, int sm_count, PersistPlan* pl) {
     if (!a.pk.bm_words || !a.nsub) return false;
     const PTune t = read_ptune();
-    const uint32_t sub_bytes = a.pk.bm_words * kSubWords * 4u;
     // minb = 2: two CTAs of 512 threads per SM share the 227 KB (stage up to ~110 KB, 64 registers per thread);
     // minb = 1: one CTA per SM with the whole shared memory and up to 128 registers per thread (deeper load pipelining)
     pl->minb = t.minb == 2 ? 2 : 1;
     uint32_t max_stage = (uint32_t)(t.stage_kb > 0 ? t.stage_kb : (pl->minb == 1 ? 220 : 110)) * 1024u;
     if (max_stage > 220u * 1024u) max_stage = 220u * 1024u;
+    // Stages per mem threshold (bitmapM) when the view exists and one of its sub-ranges fits a stage: a row then reads
+    // one mask word per chunk, two when both its vcpu and ram requests constrain, instead of one per constraining
+    // column plus mem.  A queue is (cloud, mem threshold, stage), and at the usual table sizes one stage holds the whole
+    // slice.  Otherwise a stage is a price range of the per-threshold view bitmapT and a queue is (cloud, stage).
+    const uint32_t slice_bytes = a.pk.slice_rows * kSubWords * 4u;
+    pl->slice = a.pk.slice_rows && !a.pk.no_slice && !t.price && slice_bytes <= max_stage ? 1u : 0u;
+    const uint32_t sub_bytes = pl->slice ? slice_bytes : a.pk.bm_words * kSubWords * 4u;
     uint32_t cap = max_stage / sub_bytes;
     if (cap == 0) cap = 1;
     const uint32_t S = (a.nsub + cap - 1) / cap;
@@ -679,6 +747,7 @@ bool persist_plan(const SelectArgs& a, int sm_count, PersistPlan* pl) {
     if (Qi > per) Qi = per;
     pl->qspan = (uint32_t)((per + Qi - 1) / Qi);
     pl->Qi = (per + pl->qspan - 1) / pl->qspan;
+    pl->n_cursors = (pl->slice ? 2u * (a.D[0] + 1u) : 2u) * pl->S;
     return true;
 }
 
@@ -693,10 +762,13 @@ static void launch_pdl_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t
     RPK_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
 }
 
-int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream_t st) {
+int launch_select_persist(const SelectArgs& args, const PersistPlan& pl, cudaStream_t st) {
     const PTune t = read_ptune();
+    SelectArgs a = args;
+    a.slice = pl.slice;
     PersistArgs pa;
     pa.S = pl.S; pa.per = pl.per; pa.qspan = pl.qspan; pa.stage_cap_subs = pl.cap_subs;
+    pa.slice = pl.slice; pa.groups_per_cloud = pl.slice ? a.D[0] + 1u : 1u; pa.groups = 2u * pa.groups_per_cloud;
     pa.n_groups = pl.per < (uint32_t)kCopyGroups ? pl.per : (uint32_t)kCopyGroups;
     uint32_t tickets = 0;
     for (uint32_t s = 0; s < pl.S; ++s) {
@@ -711,7 +783,7 @@ int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream
     const uint32_t chunks = (a.P + kPThreads - 1) / kPThreads;
     const uint32_t k0ctas = t.k0ctas > 0 ? (uint32_t)t.k0ctas : 4u * (uint32_t)pl.sm_count;
     const uint32_t blocks = chunks < k0ctas ? (chunks ? chunks : 1u) : k0ctas;
-    k_pod_classify<<<blocks, kPThreads, 0, st>>>(a, 2 * pl.S);
+    k_pod_classify<<<blocks, kPThreads, 0, st>>>(a, pl.n_cursors);
     launch_pdl_k(k_pod_scatter, dim3(blocks), dim3(kPThreads), 0, st, t.pdl, a);
     static thread_local int attr_dev[5] = {-1, -1, -1, -1, -1};
     int dev = 0;
