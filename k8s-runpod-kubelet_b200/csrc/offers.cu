@@ -270,8 +270,7 @@ int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st)
         pk.bm_stride = bm_words <= 32 ? 32 : 64;
     }
     if (ds.force_kind >= 5) pk.no_fused = 1;
-    if (ds.force_kind == 7) pk.no_slice = 1;
-    if (ds.force_kind == 6) pk.no_persist = 1;
+    if (ds.force_kind == 6) pk.no_slice = 1;
     if (ds.force_kind == 1) { pk.bits = 0; pk.pos_bits = 0; pk.bm_words = 0; }
     if (ds.force_kind == 2) { pk.pos_bits = 0; pk.bm_words = 0; }
     if (ds.force_kind == 3) pk.bm_words = 0;

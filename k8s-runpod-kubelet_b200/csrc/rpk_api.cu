@@ -125,11 +125,12 @@ void fill_offer_args(const DeviceState& ds, SelectArgs& a) {
     for (int d = 0; d < 3; ++d) { a.distinct[d] = ds.distinct[d].p; a.D[d] = ds.D[d]; }
 }
 
-// scratch for one select over P rows on ds (in lane ln); returns rows-per-warp.  *use_persist: the batch takes the
-// persistent bit-sliced kernel (plan in *pl).
+// scratch for one select over P rows on ds (in lane ln); returns rows-per-warp of the packed / wide kernels (0 on a
+// bit-sliced table).  *use_persist: the batch takes the persistent bit-sliced kernel (plan in *pl); a bit-sliced table
+// otherwise takes the fused kernel, which also serves an empty table at any batch size.
 int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, SelectArgs& a, PersistPlan* pl, bool* use_persist) {
-    const int R = ds.pk.bm_words ? 32 * pick_rows_per_lane(P, ds.G, ds.sm_count) : pick_rows_per_warp(P, ds.sm_count);
-    const uint32_t tiles = select_tiles_max(P, R);
+    const int R = ds.pk.bm_words ? 0 : pick_rows_per_warp(P, ds.sm_count);
+    const uint32_t tiles = R ? select_tiles_max(P, R) : 0u;
     ln.rw.reserve(P); ln.order.reserve((size_t)kGroups * P); ln.pos.reserve(P);
     // worst case (1 row per warp; the persistent kernel's row blocks: one partial block per row group): never regrown mid-pipeline
     const size_t need = std::max<size_t>((size_t)2 * kGroups + tiles, (size_t)P / 8 + 3 * kGroups + kMaxGroups);
@@ -143,8 +144,9 @@ int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, S
     a.rw = ln.rw.p; a.order = ln.order.p; a.pos = ln.pos.p;
     a.counts = ln.ctrs.p; a.done = ln.ctrs.p + kGroups; a.tile_ctr = ln.ctrs.p + 2 * kGroups;
     a.P = P;
-    *use_persist = ds.pk.bm_words && (P > kFusedRowsMax || ds.pk.no_fused) && !ds.pk.no_persist && persist_plan(a, ds.sm_count, pl);
+    *use_persist = ds.pk.bm_words && ds.nsub && (P > kFusedRowsMax || ds.pk.no_fused);
     if (*use_persist) {
+        *pl = persist_plan(a, ds.sm_count);
         ln.key.reserve(P); ln.ord_rw.reserve(P);
         const size_t hdr_words = persist_hdr_words(*pl);
         const bool fresh = !ln.hist.p || hdr_words > ln.hdr.cap;
@@ -485,8 +487,7 @@ int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int
                 if (!strcmp(fk, "generic")) ds.force_kind = 1; else if (!strcmp(fk, "packed")) ds.force_kind = 2;
                 else if (!strcmp(fk, "packed_pos")) ds.force_kind = 3; else if (!strcmp(fk, "bitmap")) ds.force_kind = 4;
                 else if (!strcmp(fk, "bitmap_grouped")) ds.force_kind = 5;  // every batch size through the persistent kernel
-                else if (!strcmp(fk, "bitmap_grid")) ds.force_kind = 6;     // ... through the first-generation grid kernel
-                else if (!strcmp(fk, "bitmap_price")) ds.force_kind = 7;    // ... through the persistent kernel, table staged by price
+                else if (!strcmp(fk, "bitmap_price")) ds.force_kind = 6;    // ... through the persistent kernel, table staged by price
             }
             const size_t n = G ? G : 1;
             ds.raw_mem.reserve(n); ds.raw_vcpu.reserve(n); ds.raw_ram.reserve(n); ds.raw_sp.reserve(n); ds.raw_cp.reserve(n); ds.raw_flags.reserve(n);

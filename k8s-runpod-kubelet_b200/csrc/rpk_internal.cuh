@@ -40,8 +40,7 @@ struct PackLayout {
     uint32_t bm_words; // D_mem+1 + D_vcpu+1 + D_ram+1 if that fits 64 words, else 0
     uint32_t bm_off_vcpu, bm_off_ram;
     uint32_t bm_stride; // words per chunk row: 32 (conflict-free) or 64 (up to 64 thresholds; words 32 apart share a bank)
-    uint32_t no_fused;  // test hook (RPK_FORCE_KERNEL=bitmap_grouped): small batches also take the three-launch path
-    uint32_t no_persist; // test hook (RPK_FORCE_KERNEL=bitmap_grid): the first-generation (tile x segment) grid kernel
+    uint32_t no_fused;  // test hook (RPK_FORCE_KERNEL=bitmap_grouped): small batches also take the persistent kernel
     uint32_t slice_rows; // rows per sub-range of the per-mem-threshold view bitmapM (D_vcpu+1 + D_ram+1); 0 = not built
     uint32_t no_slice;   // test hook (RPK_FORCE_KERNEL=bitmap_price): the persistent kernel stages the table by price
 };
@@ -117,6 +116,13 @@ struct SelectArgs {
     uint32_t slice;      // persistent select: rows grouped and the table staged per (cloud, mem threshold) on bitmapM
 };
 
+// One row's result.  With several output vectors (the all-gather) only the local one is written here -- scattered
+// 4-byte stores over NVLink are far slower than 16-byte ones -- and the finished slice is pushed to the peers after.
+__device__ __forceinline__ void store_best(const SelectArgs& a, uint32_t row, int32_t b) {
+    if (a.self_out >= 0) { a.best_out[a.self_out][a.row0 + row] = b; return; }
+    for (int o = 0; o < a.n_out; ++o) a.best_out[o][a.row0 + row] = b;
+}
+
 struct StatusArgs {
     const uint8_t* records;
     uint32_t stride;
@@ -145,6 +151,32 @@ struct StatusArgs {
 struct CudaError { cudaError_t err; const char* what; const char* file; int line; };
 #define RPK_CUDA(x) do { cudaError_t e__ = (x); if (e__ != cudaSuccess) throw ::rpk::CudaError{e__, #x, __FILE__, __LINE__}; } while (0)
 
+// RPK_TUNE="pdl=off,order=natural,stagekb=<KB>,ipw=<n>,k0ctas=<n>" -- measurement hooks for tools/k1_tune.py; unset =
+// the defaults chosen from those measurements.  The environment is read ONCE per process (this sits on the
+// tens-of-microseconds latency path of production callers); tools that sweep settings inside one process set
+// RPK_TUNE_RELOAD=1 before the first call.
+struct Tune {
+    bool pdl = true;             // pdl=off: launch without programmatic dependent launch
+    bool natural_order = false;  // order=natural: row tiles in group order instead of heaviest first (packed / wide kernels)
+    int stage_kb = 0;            // stagekb=: persistent select's stage cap (0: 220 KB)
+    int items_per_warp = 0;      // ipw=: persistent select's items per warp (0: 4)
+    int k0ctas = 0;              // k0ctas=: CTAs of the persistent select's class sort (0: four per SM)
+};
+Tune read_tune();
+
+// Launch with the programmatic-serialization attribute (PDL, rpk_device.cuh): the kernel may start before its stream
+// predecessor has finished and synchronises with griddepcontrol.wait itself.
+template <typename... KArgs, typename... Args>
+void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
+    RPK_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
+}
+
 struct OfferIngest {   // raw device columns in, views out
     uint32_t G;
     const int32_t* mem; const int32_t* vcpu; const int32_t* ram;  // vcpu/ram never null here (zero-filled)
@@ -157,15 +189,14 @@ struct PersistPlan;
 int launch_select(const SelectArgs& a, int rows_per_warp, const PersistPlan* pl, cudaStream_t st);
 uint32_t select_tiles_max(uint32_t P, int rows_per_warp);
 int pick_rows_per_warp(uint32_t P, int sm_count);
-int pick_rows_per_lane(uint32_t P, uint32_t G, int sm_count);
 int launch_status_diff(const StatusArgs& a, cudaStream_t st);
 struct PeerFenceArgs { uint32_t* flags[RPK_MAX_GPUS]; int n; int my_rank; uint32_t epoch; };
 int launch_peer_fence(const PeerFenceArgs& a, cudaStream_t st);
 int launch_peer_signal(const PeerFenceArgs& a, uint32_t word0, cudaStream_t st);
 int launch_peer_wait(const PeerFenceArgs& a, uint32_t what, cudaStream_t st);
 // persistent bit-sliced select (select_persist.cu)
-struct PersistPlan { uint32_t cap_subs, S, per, qspan, Qi, grid, smem_bytes, slice, n_cursors; int rpl, minb, sm_count; };
-bool persist_plan(const SelectArgs& a, int sm_count, PersistPlan* pl);
+struct PersistPlan { uint32_t S, per, qspan, grid, smem_bytes, slice, n_cursors; int sm_count; };
+PersistPlan persist_plan(const SelectArgs& a, int sm_count);  // a.pk.bm_words and a.nsub non-zero
 uint32_t persist_hdr_words(const PersistPlan& pl);
 int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream_t st);
 uint32_t status_tiles(uint32_t N, uint32_t stride);
@@ -203,7 +234,7 @@ struct DeviceState {
     uint32_t D[3] = {0, 0, 0};
     PackLayout pk = {};
     int force_kind = 0;  // RPK_FORCE_KERNEL (tests): 0 auto, 1 generic, 2 packed+select, 3 packed+pos, 4 bit-sliced,
-                         // 5 / 6 / 7 every batch through the persistent / first-generation / price-staged persistent kernel
+                         // 5 / 6 every batch of a non-empty table through the persistent / price-staged persistent kernel
     // select scratch.  The host entry point pipelines row sub-batches over four lanes (stream + staging +
     // scratch each) so that the H2D of one sub-batch, the kernels of another and the D2H of a third overlap;
     // the device entry points use lane 0's scratch on the caller's stream.

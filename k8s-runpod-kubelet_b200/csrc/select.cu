@@ -2,18 +2,16 @@
 // (reference runpod_client.go:465-509, called per pod from :1281).
 //
 // Data flow per call (all on one stream):
-//   k_pod_prep        pod columns -> per-row threshold word (rank compression), rows grouped by (cloud view,
-//                     vcpu constrains, ram constrains), pos[] = none
-//   k_select_bitmap   kind 4: grid = (row tile) x (offer segment).  The segment of the price-sorted, bit-sliced
-//                     view (one 32-bit mask per column threshold per 32-offer chunk) is staged in shared
-//                     memory with one bulk async copy (TMA, mbarrier completion); each lane owns RPL rows and
-//                     ANDs its masks: one LOP3 = 32 (pod, offer) pairs.  Every pair is evaluated.
+//   k_select_fused    kind 4 (bit-sliced view), batches up to kFusedRowsMax rows and empty tables: one launch, one
+//                     lane per row; larger batches take the persistent kernel (select_persist.cu).
+//   k_pod_prep        kinds 3..1: pod columns -> per-row threshold word (rank compression), rows grouped by (cloud
+//                     view, vcpu constrains, ram constrains), pos[] = none
 //   k_select_packed   kinds 3/2: one u32 of rank fields per offer, R rows per warp in registers, lanes stride
 //                     over offers, row argmin by redux.sync.min over lanes.
 //   k_select_wide     kind 1: int32 compares on (mem, vcpu, ram) for tables that do not rank-pack.
-//   (all grid kernels) atomicMin merges segments; the last CTA of a row tile applies price < maxPrice to the
-//                     winner (the bound is a prefix of the sorted order) and stores the offer index into
-//                     every peer's assignment vector (the fused all-gather).
+//   (packed / wide)   grid = (row tile) x (offer segment); atomicMin merges segments; the last CTA of a row tile
+//                     applies price < maxPrice to the winner (the bound is a prefix of the sorted order) and stores
+//                     the offer index into every peer's assignment vector (the fused all-gather).
 //   k_select_top5*    optional: the whole <=5 gpuTypeIds list per row (runpod_client.go:502-509).
 //   k_peer_fence      one warp: signal / wait across GPUs after the fused gather.
 #include <math_constants.h>
@@ -21,29 +19,16 @@
 #include <cstdlib>
 #include <cstring>
 
+#include "rpk_device.cuh"
 #include "rpk_internal.cuh"
 
 namespace rpk {
+using namespace dev;
 
 __device__ __forceinline__ uint32_t lower_bound_i32(const int32_t* __restrict__ a, uint32_t n, int32_t x) {
     uint32_t lo = 0, hi = n;
     while (lo < hi) { uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
     return lo;
-}
-
-// Programmatic dependent launch (PDL): a kernel launched with the programmatic-serialization attribute may start
-// while its predecessor in the stream is still running; pdl_wait() blocks until the predecessor has completed and
-// its writes are visible, pdl_trigger() in the predecessor lets the dependent start early.  Both are no-ops for
-// launches without the attribute.  Used so that the grid kernel's launch latency hides behind k_pod_prep, and the
-// fence kernel's behind the grid kernel's last wave.
-__device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
-__device__ __forceinline__ void pdl_trigger() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
-
-// One row's result.  With several output vectors (the all-gather) only the local one is written here -- scattered
-// 4-byte stores over NVLink are far slower than 16-byte ones -- and k_gather_push forwards the finished slice.
-__device__ __forceinline__ void store_best(const SelectArgs& a, uint32_t row, int32_t b) {
-    if (a.self_out >= 0) { a.best_out[a.self_out][a.row0 + row] = b; return; }
-    for (int o = 0; o < a.n_out; ++o) a.best_out[o][a.row0 + row] = b;
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -63,15 +48,12 @@ __global__ void __launch_bounds__(1024) k_pod_prep(SelectArgs a) {
         uint8_t c = a.cloud ? a.cloud[p] : (uint8_t)RPK_CLOUD_SECURE;
         a.pos[p] = kNone;
         uint32_t need = 3;  // kernels without rank thresholds always test both extension columns
-        if (a.pk.bits || a.pk.bm_words) {
+        if (a.pk.bits) {
             uint32_t tm = lower_bound_i32(a.distinct[0], a.D[0], a.req_mem[p]) + 1;
             uint32_t tv = lower_bound_i32(a.distinct[1], a.D[1], a.req_vcpu ? a.req_vcpu[p] : 0);
             uint32_t tr = lower_bound_i32(a.distinct[2], a.D[2], a.req_ram ? a.req_ram[p] : 0);
             need = (tv != 0 ? 2u : 0u) | (tr != 0 ? 1u : 0u);
-            if (a.pk.bm_words)  // bit-sliced view: the three mask-word indices of this row inside a chunk
-                a.rw[p] = (tm - 1) | ((a.pk.bm_off_vcpu + tv) << 8) | ((a.pk.bm_off_ram + tr) << 16);
-            else
-                a.rw[p] = (tm << a.pk.sh_mem) | (tv << a.pk.sh_vcpu) | (tr << a.pk.sh_ram);
+            a.rw[p] = (tm << a.pk.sh_mem) | (tv << a.pk.sh_vcpu) | (tr << a.pk.sh_ram);
         }
         if (c <= 1) {
             grp = c * 4u + need;
@@ -105,38 +87,7 @@ __global__ void __launch_bounds__(1024) k_pod_prep(SelectArgs a) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// bulk async copy global -> shared with mbarrier completion (cp.async.bulk, SASS UBLKCP)
-// ---------------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(dst)),
-                 "l"(src), "r"(bytes), "r"(smem_u32(bar))
-                 : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_%=:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra DONE_%=;\n"
-        "bra WAIT_%=;\n"
-        "DONE_%=:\n"
-        "}\n" ::"r"(smem_u32(bar)),
-        "r"(parity)
-        : "memory");
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// row-tile decoding shared by both grid kernels
+// row-tile decoding shared by the packed and wide kernels
 // ---------------------------------------------------------------------------------------------------------
 struct TileInfo { int cloud; uint32_t group; uint32_t row_base; uint32_t nrows; uint32_t total_tiles; bool valid; };
 
@@ -226,7 +177,7 @@ __global__ void __launch_bounds__(kCtaThreads, 3) k_select_packed(SelectArgs a, 
     const uint32_t Gc = ((a.G + kChunk - 1) / kChunk) * kChunk;
     const uint32_t g0 = seg * seg_len;
     const uint32_t len = g0 < Gc ? min(seg_len, Gc - g0) : 0;
-    if (threadIdx.x == 0) mbar_init(&s_bar, 1);
+    if (threadIdx.x == 0) { mbar_init(&s_bar, 1); mbar_fence_init(); }
     __syncthreads();
     if (threadIdx.x == 0) {
         mbar_expect_tx(&s_bar, len * 4u);
@@ -319,60 +270,11 @@ __device__ __forceinline__ void bitmap_walk(const uint32_t* s_off, int n, const 
     }
 }
 
-template <int RPL, int STRIDE>
-__global__ void __launch_bounds__(kCtaThreads, 3) k_select_bitmap(SelectArgs a, uint32_t S, uint32_t seg_chunks) {
-    constexpr uint32_t kBmStride = STRIDE;
-    extern __shared__ __align__(128) uint32_t s_off[];
-    __shared__ __align__(8) uint64_t s_bar;
-    __shared__ int s_last;
-    constexpr uint32_t RPC = kCtaThreads * RPL;
-    const uint32_t tile = blockIdx.x / S, seg = blockIdx.x - tile * S;
-    pdl_wait();     // k_pod_prep (counts, order, rw, pos) has completed
-    pdl_trigger();  // a dependent (the peer fence) may be scheduled; it waits for this grid to complete
-    const TileInfo t = decode_tile(a, tile, RPC);
-    if (!t.valid) return;
-    const uint32_t total_chunks = (a.G + 31) / 32;
-    const uint32_t c0 = seg * seg_chunks;
-    const uint32_t n = c0 < total_chunks ? min(seg_chunks, total_chunks - c0) : 0;
-    if (threadIdx.x == 0) mbar_init(&s_bar, 1);
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        mbar_expect_tx(&s_bar, n * kBmStride * 4u);
-        if (n) bulk_g2s(s_off, a.view[t.cloud].bitmap + (size_t)c0 * kBmStride, n * kBmStride * 4u, &s_bar);
-    }
-    uint32_t o1[RPL], o2[RPL], o3[RPL], bc[RPL];
-#pragma unroll
-    for (int r = 0; r < RPL; ++r) {
-        const uint32_t slot = (uint32_t)r * kCtaThreads + threadIdx.x;
-        const uint32_t w = slot < t.nrows ? a.rw[tile_row(a, t, slot)] : 0u;
-        o1[r] = w & 0xFFu; o2[r] = (w >> 8) & 0xFFu; o3[r] = (w >> 16) & 0xFFu;
-        bc[r] = kNone;
-    }
-    mbar_wait(&s_bar, 0);
-    // the tile's rows all share the two "column constrains" flags: masks of a non-constraining column are never read
-    switch (t.group & 3u) {
-        case 0: bitmap_walk<RPL, STRIDE, false, false>(s_off, (int)n, o1, o2, o3, bc); break;
-        case 1: bitmap_walk<RPL, STRIDE, false, true>(s_off, (int)n, o1, o2, o3, bc); break;
-        case 2: bitmap_walk<RPL, STRIDE, true, false>(s_off, (int)n, o1, o2, o3, bc); break;
-        default: bitmap_walk<RPL, STRIDE, true, true>(s_off, (int)n, o1, o2, o3, bc); break;
-    }
-#pragma unroll
-    for (int r = 0; r < RPL; ++r) {
-        const uint32_t slot = (uint32_t)r * kCtaThreads + threadIdx.x;
-        if (slot < t.nrows && bc[r] != kNone) {
-            const uint32_t* p = s_off + (size_t)bc[r] * kBmStride;
-            const uint32_t m = p[o1[r]] & p[o2[r]] & p[o3[r]];  // a non-constraining column's word is all-available: harmless here
-            atomicMin(&a.pos[tile_row(a, t, slot)], (c0 + bc[r]) * 32u + (uint32_t)__ffs(m) - 1u);
-        }
-    }
-    finish_tile(a, t, tile, S, &s_last);
-}
-
 // ---------------------------------------------------------------------------------------------------------
-// K1 (bit-sliced, fused, small batches): one launch does what k_pod_prep + k_select_bitmap + the epilogue do,
-// for batches too small to fill the GPU anyway (micro-batches of the streaming path, BASELINE config 2).  One
-// lane per pod row in arrival order, no grouping, no atomics, no counters to clear: the CTA walks every segment
-// of the view(s) its rows use, so each row's result is final when its loop ends.
+// K1 (bit-sliced, fused, small batches): one launch does what a row sort, a grid kernel and its epilogue would do,
+// for batches too small to fill the GPU anyway (micro-batches of the streaming path, BASELINE config 2), and for
+// an empty table at any batch size.  One lane per pod row in arrival order, no grouping, no atomics, no counters
+// to clear: the CTA walks every segment of the view(s) its rows use, so each row's result is final when its loop ends.
 // ---------------------------------------------------------------------------------------------------------
 template <int STRIDE>
 __global__ void __launch_bounds__(kCtaThreads) k_select_fused(SelectArgs a, uint32_t seg_chunks) {
@@ -395,7 +297,7 @@ __global__ void __launch_bounds__(kCtaThreads) k_select_fused(SelectArgs a, uint
         if (cls == 2 && a.top5) for (int k = 0; k < RPK_TOPK; ++k) a.top5[(size_t)p * RPK_TOPK + k] = -1;
     }
     const bool wv = __any_sync(0xFFFFFFFFu, needv), wr = __any_sync(0xFFFFFFFFu, needr);  // warp-uniform
-    if (threadIdx.x == 0) mbar_init(&s_bar, 1);
+    if (threadIdx.x == 0) { mbar_init(&s_bar, 1); mbar_fence_init(); }
     __syncthreads();
     const uint32_t total_chunks = (a.G + 31) / 32;
     const uint32_t S = total_chunks ? (total_chunks + seg_chunks - 1) / seg_chunks : 0;
@@ -455,7 +357,7 @@ __global__ void __launch_bounds__(kCtaThreads, 2) k_select_wide(SelectArgs a, ui
     const uint32_t Gc = ((a.G + kChunk - 1) / kChunk) * kChunk;
     const uint32_t g0 = seg * seg_len;
     const uint32_t len = g0 < Gc ? min(seg_len, Gc - g0) : 0;
-    if (threadIdx.x == 0) mbar_init(&s_bar, 1);
+    if (threadIdx.x == 0) { mbar_init(&s_bar, 1); mbar_fence_init(); }
     __syncthreads();
     if (threadIdx.x == 0) {
         mbar_expect_tx(&s_bar, len * 16u);
@@ -621,72 +523,27 @@ __global__ void k_peer_fence(PeerFenceArgs a) {
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-// RPK_TUNE="rpl=<1|2|4>,order=natural,seg=full,segmul=<1..8>,pdl=off" -- measurement hooks for tools/k1_tune.py (read per call, so one
-// process can sweep them); unset = the defaults chosen from those measurements.
-struct Tune { int rpl = 0; int segmul = 1; bool natural_order = false; bool full_segments = false; bool pdl = true; bool grid_kernel = false; };
-// The environment is read ONCE per process (this sits on the tens-of-microseconds latency path of production callers); measurement
-// tools that sweep settings inside one process set RPK_TUNE_RELOAD=1 before the first call.
-static bool tune_reload() { static const bool r = getenv("RPK_TUNE_RELOAD") != nullptr; return r; }
-static Tune parse_tune();
-static Tune read_tune() {
-    if (tune_reload()) return parse_tune();
-    static const Tune cached = parse_tune();
-    return cached;
-}
 static Tune parse_tune() {
     Tune t;
     const char* e = getenv("RPK_TUNE");
     if (!e) return t;
-    if (const char* p = strstr(e, "rpl=")) t.rpl = atoi(p + 4);
-    t.natural_order = strstr(e, "order=natural") != nullptr;
-    t.full_segments = strstr(e, "seg=full") != nullptr;
     t.pdl = strstr(e, "pdl=off") == nullptr;
-    t.grid_kernel = strstr(e, "k1=grid") != nullptr;  // the first-generation (tile x segment) bit-sliced kernel, for A/B runs
-    if (const char* p = strstr(e, "segmul=")) { t.segmul = atoi(p + 7); if (t.segmul < 1 || t.segmul > 8) t.segmul = 1; }
+    t.natural_order = strstr(e, "order=natural") != nullptr;
+    if (const char* p = strstr(e, "stagekb=")) t.stage_kb = atoi(p + 8);
+    if (const char* p = strstr(e, "ipw=")) t.items_per_warp = atoi(p + 4);
+    if (const char* p = strstr(e, "k0ctas=")) { const int v = atoi(p + 7); if (v > 0) t.k0ctas = v; }
     return t;
+}
+Tune read_tune() {
+    static const bool reload = getenv("RPK_TUNE_RELOAD") != nullptr;
+    if (reload) return parse_tune();
+    static const Tune cached = parse_tune();
+    return cached;
 }
 
 uint32_t select_tiles_max(uint32_t P, int rows_per_warp) {
-    const uint32_t rpc = (uint32_t)(kWarpsPerCta * rows_per_warp);  // bit-sliced kernel: rows_per_warp = 32 * RPL
+    const uint32_t rpc = (uint32_t)(kWarpsPerCta * rows_per_warp);
     return (P + rpc - 1) / rpc + kGroups;  // every row group can end in one partial tile
-}
-
-int pick_rows_per_lane(uint32_t P, uint32_t G, int sm_count) {  // bit-sliced kernel
-    // CTAs = row tiles x offer segments (RPK_TUNE rpl=1|2|4 and tools/k1_tune.py compare the choices): many small
-    // CTAs beat few large ones until the grid is tens of waves deep (the tail of the last wave outweighs the extra
-    // segment loads).
-    const int forced = read_tune().rpl;
-    if (forced == 1 || forced == 2 || forced == 4) return forced;
-    const uint64_t want = (uint64_t)sm_count * 3 * 24;  // >= 24 waves of 3 CTAs/SM at 2 rows per lane
-    const uint64_t total_chunks = (G + 31) / 32;
-    const uint64_t kBmSegChunks = kBmSegBytes / (32 * 4);
-    uint64_t S = (total_chunks + kBmSegChunks - 1) / kBmSegChunks;
-    if (S == 0) S = 1;
-    if ((P + (uint64_t)kCtaThreads * 2 - 1) / ((uint64_t)kCtaThreads * 2) * S >= want) return 2;
-    return 1;
-}
-
-template <int RPL, int STRIDE>
-static void launch_bitmap(const SelectArgs& a, cudaStream_t st) {
-    const uint32_t tiles = select_tiles_max(a.P, 32 * RPL);
-    const uint32_t total_chunks = (a.G + 31) / 32;
-    constexpr uint32_t kBmSegChunks = kBmSegBytes / (STRIDE * 4);
-    const Tune tune = read_tune();
-    uint32_t S = (total_chunks + kBmSegChunks - 1) / kBmSegChunks * (uint32_t)tune.segmul;
-    if (S == 0) S = 1;
-    // equal segments (ceil(chunks / S) each) instead of S-1 full ones and a short one: every CTA of a row group
-    // then costs the same, and the stage is no larger than the table needs
-    uint32_t seg_chunks = tune.full_segments ? kBmSegChunks : (total_chunks + S - 1) / S;
-    if (seg_chunks == 0) seg_chunks = 1;
-    const size_t smem = (size_t)seg_chunks * STRIDE * 4;
-    static thread_local int attr_dev = -1;  // the attribute is per device: set it once per (thread, device)
-    int dev = 0;
-    RPK_CUDA(cudaGetDevice(&dev));
-    if (attr_dev != dev) {
-        RPK_CUDA(cudaFuncSetAttribute(k_select_bitmap<RPL, STRIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBmSegBytes));
-        attr_dev = dev;
-    }
-    launch_pdl(k_select_bitmap<RPL, STRIDE>, dim3(tiles * S), dim3(kCtaThreads), smem, st, tune.pdl, a, S, seg_chunks);
 }
 
 static void seg_plan(uint32_t G, uint32_t seg_cap, uint32_t* S, uint32_t* seg_len) {
@@ -705,19 +562,6 @@ int pick_rows_per_warp(uint32_t P, int sm_count) {
         if (tiles >= want) return r;
     }
     return 1;
-}
-
-// Launch with the programmatic-serialization attribute (see pdl_wait): the kernel may start before its stream
-// predecessor has finished and synchronises with griddepcontrol.wait itself.
-template <typename... KArgs, typename... Args>
-static void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    RPK_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
 }
 
 static int device_sm_count() {
@@ -763,8 +607,6 @@ static void launch_grid(const SelectArgs& a, cudaStream_t st) {
         launch_pdl(k_select_wide<R>, dim3(tiles * S), dim3(kCtaThreads), smem, st, pdl, a, S, seg_len);
     }
 }
-
-constexpr uint32_t kFusedMaxRows = kFusedRowsMax;  // below this a batch cannot fill the GPU: one fused launch beats three
 
 template <int STRIDE>
 static void launch_fused(const SelectArgs& a, cudaStream_t st) {
@@ -814,21 +656,14 @@ int launch_select(const SelectArgs& args, int R, const PersistPlan* pl, cudaStre
 
 static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* pl, cudaStream_t st, bool* fused_push) {
     int launches = 0;
-    if (a.pk.bm_words && a.P <= kFusedMaxRows && !a.pk.no_fused) {
-        const bool wide_rows = a.pk.bm_stride == 64;
-        if (wide_rows) launch_fused<64>(a, st); else launch_fused<32>(a, st);
-        ++launches;
-        if (a.top5) {
-            if (wide_rows) k_select_top5_bitmap<64><<<(a.P + 255) / 256, 256, 0, st>>>(a);
-            else k_select_top5_bitmap<32><<<(a.P + 255) / 256, 256, 0, st>>>(a);
+    if (a.pk.bm_words) {
+        if (pl) {  // persistent kernel on the transposed view: sorts, selects, pushes, signals
+            launches += launch_select_persist(a, *pl, st);
+            *fused_push = true;
+        } else {
+            if (a.pk.bm_stride == 64) launch_fused<64>(a, st); else launch_fused<32>(a, st);
             ++launches;
         }
-        RPK_CUDA(cudaGetLastError());
-        return launches;
-    }
-    if (a.pk.bm_words && pl && !read_tune().grid_kernel) {  // persistent kernel on the transposed view: sorts, selects, pushes, signals
-        launches += launch_select_persist(a, *pl, st);
-        *fused_push = true;
         if (a.top5) {
             if (a.pk.bm_stride == 64) k_select_top5_bitmap<64><<<(a.P + 255) / 256, 256, 0, st>>>(a);
             else k_select_top5_bitmap<32><<<(a.P + 255) / 256, 256, 0, st>>>(a);
@@ -839,22 +674,6 @@ static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* 
     }
     // counts / done / tile tickets are zero here: zeroed when allocated, and every grid kernel leaves them zero
     k_pod_prep<<<(a.P + 1023) / 1024, 1024, 0, st>>>(a); ++launches;
-    if (a.pk.bm_words) {  // R = 32 * rows-per-lane
-        const bool wide_rows = a.pk.bm_stride == 64;
-        switch (R / 32) {
-            case 4: if (wide_rows) launch_bitmap<4, 64>(a, st); else launch_bitmap<4, 32>(a, st); break;
-            case 2: if (wide_rows) launch_bitmap<2, 64>(a, st); else launch_bitmap<2, 32>(a, st); break;
-            default: if (wide_rows) launch_bitmap<1, 64>(a, st); else launch_bitmap<1, 32>(a, st); break;
-        }
-        ++launches;
-        if (a.top5) {
-            if (wide_rows) k_select_top5_bitmap<64><<<(a.P + 255) / 256, 256, 0, st>>>(a);
-            else k_select_top5_bitmap<32><<<(a.P + 255) / 256, 256, 0, st>>>(a);
-            ++launches;
-        }
-        RPK_CUDA(cudaGetLastError());
-        return launches;
-    }
     switch (R) {
         case 16: launch_grid<16>(a, st); break;
         case 8: launch_grid<8>(a, st); break;

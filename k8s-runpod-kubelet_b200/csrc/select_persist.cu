@@ -10,14 +10,14 @@
 //                    class order (ord_rw[]); block 0 publishes per-group row / work totals (a group is a cloud, or a
 //                    (cloud, mem threshold) pair on the per-mem-threshold view).  Rows of neither cloud are final here
 //                    (-1, runpod_client.go:469-475).
-//   k_select_persist persistent CTAs (512 threads, as many per SM as the stage allows).  A CTA loads ONE stage -- `per`
+//   k_select_persist persistent CTAs (512 threads, one per SM).  A CTA loads ONE stage -- `per`
 //                    64-chunk sub-ranges, 8 bulk async copies on 8 mbarriers, so the first items start before the whole
 //                    stage has landed -- and keeps it for the whole call.  A stage is, where the table allows it, the
 //                    slice of one mem threshold m over the whole price range (bitmapM: rows mem[m] & vcpu[v] and
 //                    mem[m] & ram[r]; a row reads ONE word per chunk, two when both its vcpu and ram requests
 //                    constrain), else a price range of the per-threshold view (bitmapT: one word for mem plus one per
 //                    constraining column).  Its warps pull items (64 consecutive rows of one group x a range of
-//                    sub-ranges) from the stage's queue with one atomic each.  A lane owns RPL rows and reads its rows'
+//                    sub-ranges) from the stage's queue with one atomic each.  A lane owns two rows and reads its rows'
 //                    mask words for FOUR chunks with one LDS.128 (the views are [row][chunk]-major); rows of a warp
 //                    share their thresholds after the sort, so the 32 lanes read at most a few distinct 16-byte
 //                    addresses and the load costs 2 LSU cycles instead of the ~5 that four LDS.32 cost
@@ -35,9 +35,6 @@
 //                    No drain, no copy kernel, no signal kernel, no wait kernel.
 #include <math_constants.h>
 
-#include <cstdlib>
-#include <cstring>
-
 #include "rpk_device.cuh"
 #include "rpk_internal.cuh"
 
@@ -47,6 +44,7 @@ using namespace dev;
 constexpr int kPThreads = 512;
 constexpr int kPWarps = kPThreads / 32;
 constexpr int kCopyGroups = 8;
+constexpr int kRpl = 2;  // pod rows per lane
 constexpr uint32_t kSubWords = kSubStride;
 
 // ---------------------------------------------------------------------------------------------------------
@@ -203,11 +201,6 @@ __device__ __forceinline__ void push_tail(const SelectArgs& a) {
     }
 }
 
-__device__ __forceinline__ void store_best_local(const SelectArgs& a, uint32_t row, int32_t b) {
-    if (a.self_out >= 0) { a.best_out[a.self_out][a.row0 + row] = b; return; }
-    for (int o = 0; o < a.n_out; ++o) a.best_out[o][a.row0 + row] = b;
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // K0a: classify.  No block waits for another one: the class counts are only added to here (the grid kernel of the
 // previous call zeroed them once the scatter kernel was done with them); block 0 resets the grid kernel's queue cursors.
@@ -329,7 +322,7 @@ __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
             a.ord_rw[dst] = make_uint2(p, cd.slice ? slice_rw(cd, a.pk, w) : w);  // the one scattered store of the sort
         }
         if (neither) {
-            store_best_local(a, p, -1);
+            store_best(a, p, -1);
             if (a.top5) for (int k = 0; k < RPK_TOPK; ++k) a.top5[(size_t)p * RPK_TOPK + k] = -1;
         }
         n_neither += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, neither));
@@ -377,7 +370,7 @@ __device__ __forceinline__ void walk(const uint32_t* __restrict__ stage, uint32_
 }
 
 struct PersistArgs {
-    uint32_t S, per, qspan, n_groups, tickets_per_block, stage_cap_subs;
+    uint32_t S, per, qspan, n_groups, tickets_per_block;
     uint32_t slice, groups, groups_per_cloud;  // slice: stages are cut from bitmapM; row groups in all / per cloud
 };
 
@@ -425,8 +418,12 @@ __device__ uint32_t persist_queue_of(uint32_t cta, uint32_t grid, uint32_t npair
     return __shfl_sync(0xFFFFFFFFu, found, owner);
 }
 
-template <int RPL, int MINB>
-__device__ __forceinline__ void select_persist_body(const SelectArgs& a, const PersistArgs& pa) {
+// 96 registers: the CTA owns the SM's shared memory, and 16K registers stay free -- exactly one 256-thread CTA of the
+// status sweep kernel, so a sweep enqueued beside the select (other stream) really runs side by side with it, one kernel
+// bound by shared memory, the other by HBM and integer multiplies.  With the whole register file (128 per thread) the
+// sweep could not start on the SM until the select is over -- or, if it got there first, would delay it.
+__global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
+    constexpr int RPL = kRpl;
     extern __shared__ __align__(128) uint32_t s_stage[];
     __shared__ __align__(8) uint64_t s_bar[kCopyGroups];
     __shared__ uint32_t s_first, s_ng;
@@ -527,7 +524,7 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
                 const double mx = a.max_price ? a.max_price[row] : RPK_DEFAULT_MAX_PRICE;
                 if (pr < mx) b = a.view[c].perm[p];
             }
-            store_best_local(a, row, b);
+            store_best(a, row, b);
         };
         uint32_t pend1_blk = kNone, pend2_blk = kNone, pend2_ticket = 0;  // merge pipeline (see below)
         // the row block whose ticket was taken one iteration ago: if that was its last ticket, every segment of its rows
@@ -638,16 +635,6 @@ __device__ __forceinline__ void select_persist_body(const SelectArgs& a, const P
     push_tail(a);
 }
 
-// Register budgets.  <RPL, 2>: two CTAs per SM, 64 registers.  <RPL, 1>: one CTA per SM; 128 registers give the deepest
-// load pipelining, but then the CTA owns the SM's whole register file and a status sweep enqueued beside the select
-// (other stream) cannot start on that SM until the select is over -- or, if it got there first, delays it.  With 96
-// registers (k_select_persist96) 16K registers stay free: exactly one 256-thread CTA of the sweep kernel, so the two
-// kernels -- one bound by shared memory, the other by HBM and integer multiplies -- really run side by side.
-template <int RPL, int MINB>
-__global__ void __launch_bounds__(kPThreads, MINB) k_select_persist(SelectArgs a, PersistArgs pa) { select_persist_body<RPL, MINB>(a, pa); }
-template <int RPL>
-__global__ void __maxnreg__(96) k_select_persist96(SelectArgs a, PersistArgs pa) { select_persist_body<RPL, 1>(a, pa); }
-
 // ---------------------------------------------------------------------------------------------------------
 // peer signal / wait (flags bound with rpk_peer_bind).  The persistent kernel signals from its last pusher; the
 // other select paths launch k_peer_signal behind their copy kernel; k_peer_wait is what remains of the fence.
@@ -683,91 +670,46 @@ __global__ void k_peer_wait(PeerFenceArgs a, uint32_t what) {
 // ---------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------
-struct PTune { int rpl = 0; int stage_kb = 0; int items_per_warp = 0; int ctas = 0; int minb = 0; int regs = 0; int k0ctas = 0; bool pdl = true; bool price = false; };  // k0ctas 0: four per SM
-static PTune parse_ptune();
-static PTune read_ptune() {  // read once per process unless RPK_TUNE_RELOAD is set (see select.cu)
-    static const bool reload = getenv("RPK_TUNE_RELOAD") != nullptr;
-    if (reload) return parse_ptune();
-    static const PTune cached = parse_ptune();
-    return cached;
-}
-static PTune parse_ptune() {
-    PTune t;
-    const char* e = getenv("RPK_TUNE");
-    if (!e) return t;
-    if (const char* p = strstr(e, "prpl=")) t.rpl = atoi(p + 5);
-    if (const char* p = strstr(e, "stagekb=")) t.stage_kb = atoi(p + 8);
-    if (const char* p = strstr(e, "ipw=")) t.items_per_warp = atoi(p + 4);
-    if (const char* p = strstr(e, "pctas=")) t.ctas = atoi(p + 6);
-    if (const char* p = strstr(e, "minb=")) t.minb = atoi(p + 5);
-    if (const char* p = strstr(e, "regs=")) t.regs = atoi(p + 5);
-    if (const char* p = strstr(e, "k0ctas=")) { const int v = atoi(p + 7); if (v > 0) t.k0ctas = v; }
-    t.pdl = strstr(e, "pdl=off") == nullptr;
-    t.price = strstr(e, "k1=price") != nullptr;  // stage the table by price even where the per-mem-threshold view exists (A/B)
-    return t;
-}
-
 uint32_t persist_hdr_words(const PersistPlan& pl) { return kHdrCursors + pl.n_cursors + 8; }
 
-bool persist_plan(const SelectArgs& a, int sm_count, PersistPlan* pl) {
-    if (!a.pk.bm_words || !a.nsub) return false;
-    const PTune t = read_ptune();
-    // minb = 2: two CTAs of 512 threads per SM share the 227 KB (stage up to ~110 KB, 64 registers per thread);
-    // minb = 1: one CTA per SM with the whole shared memory and up to 128 registers per thread (deeper load pipelining)
-    pl->minb = t.minb == 2 ? 2 : 1;
-    uint32_t max_stage = (uint32_t)(t.stage_kb > 0 ? t.stage_kb : (pl->minb == 1 ? 220 : 110)) * 1024u;
+PersistPlan persist_plan(const SelectArgs& a, int sm_count) {
+    const Tune t = read_tune();
+    PersistPlan pl;
+    uint32_t max_stage = (uint32_t)(t.stage_kb > 0 ? t.stage_kb : 220) * 1024u;
     if (max_stage > 220u * 1024u) max_stage = 220u * 1024u;
     // Stages per mem threshold (bitmapM) when the view exists and one of its sub-ranges fits a stage: a row then reads
     // one mask word per chunk, two when both its vcpu and ram requests constrain, instead of one per constraining
     // column plus mem.  A queue is (cloud, mem threshold, stage), and at the usual table sizes one stage holds the whole
     // slice.  Otherwise a stage is a price range of the per-threshold view bitmapT and a queue is (cloud, stage).
     const uint32_t slice_bytes = a.pk.slice_rows * kSubWords * 4u;
-    pl->slice = a.pk.slice_rows && !a.pk.no_slice && !t.price && slice_bytes <= max_stage ? 1u : 0u;
-    const uint32_t sub_bytes = pl->slice ? slice_bytes : a.pk.bm_words * kSubWords * 4u;
+    pl.slice = a.pk.slice_rows && !a.pk.no_slice && slice_bytes <= max_stage ? 1u : 0u;
+    const uint32_t sub_bytes = pl.slice ? slice_bytes : a.pk.bm_words * kSubWords * 4u;
     uint32_t cap = max_stage / sub_bytes;
     if (cap == 0) cap = 1;
     const uint32_t S = (a.nsub + cap - 1) / cap;
     const uint32_t per = (a.nsub + S - 1) / S;
-    pl->cap_subs = cap; pl->S = (a.nsub + per - 1) / per; pl->per = per;
-    pl->smem_bytes = per * sub_bytes;
-    uint32_t ctas = (227u * 1024u) / (pl->smem_bytes + 1024u + 128u);
-    if (ctas > 2048u / kPThreads) ctas = 2048u / kPThreads;
-    if (ctas == 0) ctas = 1;
-    if (t.ctas > 0 && (uint32_t)t.ctas < ctas) ctas = (uint32_t)t.ctas;
-    if (pl->minb == 1) ctas = 1;
-    pl->grid = (uint32_t)sm_count * ctas;
-    pl->sm_count = sm_count;
-    pl->rpl = t.rpl == 1 ? 1 : t.rpl == 4 && pl->minb == 1 ? 4 : 2;
-    const uint64_t warps = (uint64_t)pl->grid * kPWarps;
-    const uint64_t nblk = ((uint64_t)a.P + 32u * pl->rpl - 1) / (32u * pl->rpl);
+    pl.S = (a.nsub + per - 1) / per; pl.per = per;
+    pl.smem_bytes = per * sub_bytes;
+    pl.grid = (uint32_t)sm_count;  // one CTA per SM: the stage takes the SM's shared memory
+    pl.sm_count = sm_count;
+    const uint64_t warps = (uint64_t)pl.grid * kPWarps;
+    const uint64_t nblk = ((uint64_t)a.P + 32u * kRpl - 1) / (32u * kRpl);
     const uint64_t want = (uint64_t)(t.items_per_warp > 0 ? t.items_per_warp : 4) * warps;  // items per warp: the tail is one item long
-    const uint64_t visits = nblk * pl->S > 0 ? nblk * pl->S : 1;  // (row block, stage) visits
+    const uint64_t visits = nblk * pl.S > 0 ? nblk * pl.S : 1;  // (row block, stage) visits
     uint64_t Qi = (want + visits - 1) / visits;
     if (Qi < 1) Qi = 1;
     if (Qi > per) Qi = per;
-    pl->qspan = (uint32_t)((per + Qi - 1) / Qi);
-    pl->Qi = (per + pl->qspan - 1) / pl->qspan;
-    pl->n_cursors = (pl->slice ? 2u * (a.D[0] + 1u) : 2u) * pl->S;
-    return true;
-}
-
-template <typename... KArgs, typename... Args>
-static void launch_pdl_k(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, bool pdl, Args... args) {
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = 1;
-    cfg.attrs = attr; cfg.numAttrs = pdl ? 1 : 0;
-    RPK_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
+    pl.qspan = (uint32_t)((per + Qi - 1) / Qi);
+    pl.n_cursors = (pl.slice ? 2u * (a.D[0] + 1u) : 2u) * pl.S;
+    return pl;
 }
 
 int launch_select_persist(const SelectArgs& args, const PersistPlan& pl, cudaStream_t st) {
-    const PTune t = read_ptune();
+    const Tune t = read_tune();
     SelectArgs a = args;
     a.slice = pl.slice;
     PersistArgs pa;
-    pa.S = pl.S; pa.per = pl.per; pa.qspan = pl.qspan; pa.stage_cap_subs = pl.cap_subs;
+    pa.S = pl.S; pa.per = pl.per; pa.qspan = pl.qspan;
     pa.slice = pl.slice; pa.groups_per_cloud = pl.slice ? a.D[0] + 1u : 1u; pa.groups = 2u * pa.groups_per_cloud;
     pa.n_groups = pl.per < (uint32_t)kCopyGroups ? pl.per : (uint32_t)kCopyGroups;
     uint32_t tickets = 0;
@@ -784,33 +726,24 @@ int launch_select_persist(const SelectArgs& args, const PersistPlan& pl, cudaStr
     const uint32_t k0ctas = t.k0ctas > 0 ? (uint32_t)t.k0ctas : 4u * (uint32_t)pl.sm_count;
     const uint32_t blocks = chunks < k0ctas ? (chunks ? chunks : 1u) : k0ctas;
     k_pod_classify<<<blocks, kPThreads, 0, st>>>(a, pl.n_cursors);
-    launch_pdl_k(k_pod_scatter, dim3(blocks), dim3(kPThreads), 0, st, t.pdl, a);
-    static thread_local int attr_dev[5] = {-1, -1, -1, -1, -1};
+    launch_pdl(k_pod_scatter, dim3(blocks), dim3(kPThreads), 0, st, t.pdl, a);
+    static thread_local int attr_dev = -1;  // the attribute is per device: set it once per (thread, device)
     int dev = 0;
     RPK_CUDA(cudaGetDevice(&dev));
-    auto go = [&](auto kernel, int slot) {
-        if (attr_dev[slot] != dev) { RPK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024)); attr_dev[slot] = dev; }
-        launch_pdl_k(kernel, dim3(pl.grid), dim3(kPThreads), pl.smem_bytes, st, t.pdl, a, pa);
-    };
-    if (pl.minb == 1) {
-        if (pl.rpl == 4) go(k_select_persist<4, 1>, 3);
-        else if (t.regs == 128) go(k_select_persist<2, 1>, 2);
-        else go(k_select_persist96<2>, 4);
-    } else {
-        if (pl.rpl == 1) go(k_select_persist<1, 2>, 0); else go(k_select_persist<2, 2>, 1);
-    }
+    if (attr_dev != dev) { RPK_CUDA(cudaFuncSetAttribute(k_select_persist, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024)); attr_dev = dev; }
+    launch_pdl(k_select_persist, dim3(pl.grid), dim3(kPThreads), pl.smem_bytes, st, t.pdl, a, pa);
     RPK_CUDA(cudaGetLastError());
     return 3;
 }
 
 int launch_peer_signal(const PeerFenceArgs& a, uint32_t word0, cudaStream_t st) {
-    launch_pdl_k(k_peer_signal, dim3(1), dim3(32), 0, st, read_ptune().pdl, a, word0, word0 == kFlagSelect ? kFlagSelectCtr : kFlagStatusCtr);
+    launch_pdl(k_peer_signal, dim3(1), dim3(32), 0, st, read_tune().pdl, a, word0, word0 == kFlagSelect ? kFlagSelectCtr : kFlagStatusCtr);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }
 
 int launch_peer_wait(const PeerFenceArgs& a, uint32_t what, cudaStream_t st) {
-    launch_pdl_k(k_peer_wait, dim3(1), dim3(32), 0, st, read_ptune().pdl, a, what);
+    launch_pdl(k_peer_wait, dim3(1), dim3(32), 0, st, read_tune().pdl, a, what);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

@@ -13,7 +13,8 @@
 // not hashed; it only selects the EXITED branch of the code.
 //
 // Kernels:
-//   k_status_stream<STRIDE>  strides 16 and 32: HBM-bound scan.  Persistent CTAs; every WARP owns a contiguous run of
+//   k_status_stream<STRIDE, THREADS>
+//                            strides 16 and 32: HBM-bound scan.  Persistent CTAs; every WARP owns a contiguous run of
 //                            slots and streams it with 16-byte global loads, the next unit's loads in flight while
 //                            the current one is hashed; changed slots are staged in slot order in the warp's own
 //                            part of a staging array -- no CTA barrier in the loop.  At the end each CTA publishes
@@ -22,9 +23,6 @@
 //                            ascending position (and, for the sharded sweep, into every peer's exchange buffer).
 //   k_status_diff<ITEMS>     the other strides (48..256): padded shared-memory tile + look-back per tile.
 //   k_status_seed_slots      previous state of individual slots (CreatePod writes ONE InstanceInfo, kubelet.go:391-401).
-#include <cstdlib>
-#include <cstring>
-
 #include "rpk_device.cuh"
 #include "rpk_internal.cuh"
 
@@ -226,30 +224,9 @@ __device__ __forceinline__ void load_unit(const StatusArgs& a, uint32_t base, ui
     }
 }
 
-// RING (big tables): every warp owns a ring of kRingDepth<STRIDE> shared-memory stages, each one unit (64 records + their
-// 64 previous hashes), filled by bulk async copies (TMA, one elected lane, one mbarrier per stage).  A stage is
-// refilled as soon as the warp has moved it into registers, so while a unit is hashed the warp has depth units
-// (5 KB at stride 32) in flight without holding a register for them -- the register double buffer has one unit in
-// flight for about half of the time, which is what held that build at 0.70 of the HBM peak.
-constexpr int kModeUnits = 0;  // two register sets of one unit each (small tables: fewest instructions)
-constexpr int kModeRing = 1;   // per-warp shared-memory ring filled by bulk copies (no clear gain: kept as an experiment, k2=ring)
-constexpr int kModeBeats = 2;  // three register sets of half a unit each: two loads in flight behind the one being hashed
-constexpr int kModeBeats4 = 3; // four sets: three loads in flight (k2=beats4)
-template <int STRIDE> struct RingCfg {
-    static constexpr uint32_t kDepth = STRIDE == 32 ? 2u : 3u;
-    static constexpr uint32_t kRecBytes = kUnit * (uint32_t)STRIDE, kStageBytes = kRecBytes + kUnit * 8u;
-};
-constexpr uint32_t ring_smem_bytes(int stride, int warps) {
-    return (uint32_t)warps * (stride == 32 ? RingCfg<32>::kDepth * RingCfg<32>::kStageBytes : RingCfg<16>::kDepth * RingCfg<16>::kStageBytes);
-}
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-
-template <int STRIDE, int THREADS, int MODE>
+template <int STRIDE, int THREADS>
 __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(StatusArgs a, uint32_t n_units) {
     constexpr int kSThreads = THREADS, kSWarps = THREADS / 32;
-    constexpr bool RING = MODE == kModeRing;
-    extern __shared__ __align__(128) unsigned char s_ring[];
-    __shared__ __align__(8) uint64_t s_full[RING ? kSWarps : 1][RING ? RingCfg<STRIDE>::kDepth : 1];
     __shared__ uint32_t s_warp[kSWarps];
     __shared__ uint32_t s_id, s_excl, s_last, s_carry;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -287,114 +264,6 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
         }
         if (report && lane == 0) a.unit_cnt[u] = running;
     };
-    if (RING) {
-        using R = RingCfg<STRIDE>;
-        unsigned char* my = s_ring + (size_t)warp * R::kDepth * R::kStageBytes;
-        uint64_t* bar = &s_full[RING ? warp : 0][0];
-        if (lane == 0) {
-            for (uint32_t d = 0; d < R::kDepth; ++d) mbar_init(&bar[d], 1);
-            mbar_fence_init();
-        }
-        __syncwarp();
-        // whole units only (the table's last unit may be ragged: that one is loaded the plain way)
-        auto whole = [&](uint32_t unit) { return (unit + 1u) * kUnit <= a.N; };
-        auto issue = [&](uint32_t unit, uint32_t stage) {  // lane 0
-            unsigned char* dst = my + stage * R::kStageBytes;
-            mbar_expect_tx(&bar[stage], R::kStageBytes);
-            bulk_g2s(dst, a.records + (size_t)unit * R::kRecBytes, R::kRecBytes, &bar[stage]);
-            bulk_g2s(dst + R::kRecBytes, a.hash_prev + (size_t)unit * kUnit, kUnit * 8u, &bar[stage]);
-        };
-        uint32_t u = c_lo + warp;
-        if (lane == 0)
-            for (uint32_t d = 0; d < R::kDepth; ++d) { const uint32_t v = u + d * kSWarps; if (v < c_hi && whole(v)) issue(v, d); }
-        uint32_t stage = 0, parity = 0;
-        for (; u < c_hi; u += kSWarps) {
-            SlotData<STRIDE> r[kStreamItems];
-            if (whole(u)) {
-                mbar_wait(&bar[stage], parity);
-                const unsigned char* sp = my + stage * R::kStageBytes;
-#pragma unroll
-                for (int k = 0; k < kStreamItems; ++k) {
-                    const uint32_t slot = (uint32_t)k * 32 + lane;
-                    r[k].lo = *reinterpret_cast<const uint4*>(sp + slot * STRIDE);
-                    if (STRIDE == 32) r[k].hi = *reinterpret_cast<const uint4*>(sp + slot * STRIDE + 16);
-                    else r[k].hi = make_uint4(0, 0, 0, 0);
-                    r[k].prev = *reinterpret_cast<const u64*>(sp + R::kRecBytes + slot * 8);
-                }
-                __syncwarp();  // every lane has its copy: the stage may be overwritten
-                if (lane == 0) {
-                    fence_proxy_async();
-                    const uint32_t v = u + R::kDepth * kSWarps;
-                    if (v < c_hi && whole(v)) issue(v, stage);
-                }
-            } else {
-                load_unit<STRIDE>(a, u * kUnit, lane, r);
-            }
-            process(u, r);
-            if (++stage == R::kDepth) { stage = 0; parity ^= 1u; }
-        }
-    } else if (MODE == kModeBeats || MODE == kModeBeats4) {
-        // Half units ("beats": 32 slots, one per lane) through three register sets: while beat b is hashed the loads of
-        // beats b + 1 and b + 2 are in flight -- the same registers as two whole-unit sets, but the memory system
-        // always has at least one beat per warp outstanding (with whole units it is idle while the second set is hashed
-        // and the first one has not been re-issued yet).
-        const uint32_t first = c_lo + warp;
-        const uint32_t n_beats = first < c_hi ? 2u * ((c_hi - first + kSWarps - 1) / kSWarps) : 0u;
-        SlotData<STRIDE> q0[1], q1[1], q2[1];
-        uint32_t running = 0;
-        auto ld = [&](uint32_t b, SlotData<STRIDE> (&q)[1]) {
-            if (b >= n_beats) return;
-            const uint32_t s = (first + (b >> 1) * kSWarps) * kUnit + (b & 1u) * 32u + lane;
-            q[0].lo = make_uint4(0, 0, 0, 0); q[0].hi = q[0].lo; q[0].prev = 0;
-            if (s < a.N) {
-                const uint4* p = reinterpret_cast<const uint4*>(a.records + (size_t)s * STRIDE);
-                q[0].lo = __ldg(p);
-                if (STRIDE == 32) q[0].hi = __ldg(p + 1);
-                q[0].prev = a.hash_prev[s];
-            }
-        };
-        auto pr = [&](uint32_t b, SlotData<STRIDE> (&q)[1]) {
-            if (b >= n_beats) return;
-            const uint32_t u = first + (b >> 1) * kSWarps;
-            if ((b & 1u) == 0u) running = 0;
-            const uint32_t s = u * kUnit + (b & 1u) * 32u + lane;
-            const uint32_t len = min(q[0].lo.x & 0x7Fu, (uint32_t)STRIDE - 1u);
-            const uint32_t nl = (len + 8u) >> 3;
-            const u64 l0 = mk64(q[0].lo.x & ~0x80u, q[0].lo.y), l1 = mk64(q[0].lo.z, q[0].lo.w);
-            u64 h;
-            if (STRIDE == 16) h = xxh64_lanes2(l0, l1, nl);
-            else h = xxh64_lanes4(l0, l1, mk64(q[0].hi.x, q[0].hi.y), mk64(q[0].hi.z, q[0].hi.w), nl);
-            bool changed = false;
-            if (s < a.N) {
-                changed = (q[0].prev == 0ull) || (h != q[0].prev);
-                if (changed) a.hash_prev[s] = h;
-                if (a.hash_out) a.hash_out[s] = h;
-            }
-            if (report) {
-                const uint32_t bal = __ballot_sync(0xFFFFFFFFu, changed);
-                if (changed) a.stage_idx[u * kUnit + running + (uint32_t)__popc(bal & ((1u << lane) - 1u))] = s;
-                running += (uint32_t)__popc(bal);
-                if ((b & 1u) && lane == 0) a.unit_cnt[u] = running;
-            }
-        };
-        if (MODE == kModeBeats) {
-            ld(0, q0); ld(1, q1);
-            for (uint32_t b = 0; b < n_beats; b += 3) {
-                ld(b + 2, q2); pr(b, q0);
-                ld(b + 3, q0); pr(b + 1, q1);
-                ld(b + 4, q1); pr(b + 2, q2);
-            }
-        } else {
-            SlotData<STRIDE> q3[1];
-            ld(0, q0); ld(1, q1); ld(2, q2);
-            for (uint32_t b = 0; b < n_beats; b += 4) {
-                ld(b + 3, q3); pr(b, q0);
-                ld(b + 4, q0); pr(b + 1, q1);
-                ld(b + 5, q1); pr(b + 2, q2);
-                ld(b + 6, q2); pr(b + 3, q3);
-            }
-        }
-    } else {
     // two register sets, used alternately: the next unit's loads are in flight while the current one is hashed
     SlotData<STRIDE> ra[kStreamItems], rb[kStreamItems];
     uint32_t u = c_lo + warp;
@@ -407,7 +276,6 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
         if (u + kSWarps < c_hi) load_unit<STRIDE>(a, (u + kSWarps) * kUnit, lane, ra);
         process(u, rb);
         u += kSWarps;
-    }
     }
     if (!report) return;  // seed: state only
     // ---- CTA count -> offset among the CTAs (look-back) -> final, ascending position ----
@@ -624,42 +492,15 @@ int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
         if (grid == 0) grid = 1;
         StatusArgs b = a;
         if (a.changed_idx == nullptr && a.n_out == 0) { b.stage_idx = nullptr; b.stage_code = nullptr; }
-        // big tables: the streaming loop is "beats" at stride 32 and "units" at stride 16.  On an H100 SXM (700 W) at 16.8M
-        // slots with codes, the modes are within 4 % of each other (stride 32: 281 us beats / 278 units / 273 ring; stride 16:
-        // 182 beats / 178 units / 186 ring; tools/k2_tune.py); RPK_TUNE k2=units|ring|beats forces one.  The ring build
-        // needs 16-byte aligned tables (bulk copies).
-        static const int mode_forced = [] {
-            const char* e = getenv("RPK_TUNE");
-            if (e && strstr(e, "k2=units")) return kModeUnits;
-            if (e && strstr(e, "k2=ring")) return kModeRing;
-            if (e && strstr(e, "k2=beats4")) return kModeBeats4;
-            if (e && strstr(e, "k2=beats")) return kModeBeats;
-            return -1;
-        }();
-        const int mode_big = mode_forced >= 0 ? mode_forced : (a.stride == 32 ? kModeBeats : kModeUnits);
-        const bool ring = big && mode_big == kModeRing && (reinterpret_cast<uintptr_t>(a.records) & 15u) == 0 && (reinterpret_cast<uintptr_t>(a.hash_prev) & 15u) == 0;
-        if (ring) {
-            static thread_local int ring_dev[2] = {-1, -1};
-            const uint32_t smem = ring_smem_bytes((int)a.stride, 32);
-            if (a.stride == 16) {
-                if (ring_dev[0] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_stream<16, 1024, kModeRing>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); ring_dev[0] = dev; }
-                k_status_stream<16, 1024, kModeRing><<<grid, 1024, smem, st>>>(b, n_units);
-            } else {
-                if (ring_dev[1] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_stream<32, 1024, kModeRing>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); ring_dev[1] = dev; }
-                k_status_stream<32, 1024, kModeRing><<<grid, 1024, smem, st>>>(b, n_units);
-            }
-        } else if (big && mode_big == kModeBeats4) {
-            if (a.stride == 16) k_status_stream<16, 1024, kModeBeats4><<<grid, 1024, 0, st>>>(b, n_units);
-            else k_status_stream<32, 1024, kModeBeats4><<<grid, 1024, 0, st>>>(b, n_units);
-        } else if (big && mode_big != kModeUnits) {
-            if (a.stride == 16) k_status_stream<16, 1024, kModeBeats><<<grid, 1024, 0, st>>>(b, n_units);
-            else k_status_stream<32, 1024, kModeBeats><<<grid, 1024, 0, st>>>(b, n_units);
-        } else if (big) {
-            if (a.stride == 16) k_status_stream<16, 1024, kModeUnits><<<grid, 1024, 0, st>>>(b, n_units);
-            else k_status_stream<32, 1024, kModeUnits><<<grid, 1024, 0, st>>>(b, n_units);
+        // one loop, two launch shapes (see kBigTable).  Other loops -- three or four half-unit register sets, a per-warp
+        // shared-memory ring filled by bulk copies -- were within 4 % of it at 16.8M slots on an H100 SXM (700 W) and
+        // none was faster at both strides (DESIGN §4, profiles/h100_k2_tune.json)
+        if (big) {
+            if (a.stride == 16) k_status_stream<16, 1024><<<grid, 1024, 0, st>>>(b, n_units);
+            else k_status_stream<32, 1024><<<grid, 1024, 0, st>>>(b, n_units);
         } else {
-            if (a.stride == 16) k_status_stream<16, 256, kModeUnits><<<grid, 256, 0, st>>>(b, n_units);
-            else k_status_stream<32, 256, kModeUnits><<<grid, 256, 0, st>>>(b, n_units);
+            if (a.stride == 16) k_status_stream<16, 256><<<grid, 256, 0, st>>>(b, n_units);
+            else k_status_stream<32, 256><<<grid, 256, 0, st>>>(b, n_units);
         }
         RPK_CUDA(cudaGetLastError());
         return 1;

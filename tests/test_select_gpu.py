@@ -14,8 +14,8 @@ pytestmark = pytest.mark.gpu
 
 
 # "bitmap": the natural choice (fused kernel up to 16k rows, persistent kernel above); "bitmap_grouped": every size
-# through the persistent kernel; "bitmap_grid": every size through the first-generation (tile x segment) kernel
-KINDS = {"generic": 1, "packed": 2, "packed_pos": 3, "bitmap": 4, "bitmap_grouped": 4, "bitmap_grid": 4}
+# through the persistent kernel (an empty table: the fused kernel at every size)
+KINDS = {"generic": 1, "packed": 2, "packed_pos": 3, "bitmap": 4, "bitmap_grouped": 4}
 
 
 def upload_forced(engine, offers, force):
@@ -36,7 +36,7 @@ def check(engine, offers, pods, top5=True, expect_kind=None, all_kernels=True):
     choice first, then each lower kind forced)."""
     ob, ot = oracle.select(offers, pods, want_top5=True, n_threads=8)
     best0 = None
-    for force in ([None, "bitmap_grouped", "bitmap_grid", "packed_pos", "packed", "generic"] if all_kernels else [None]):
+    for force in ([None, "bitmap_grouped", "packed_pos", "packed", "generic"] if all_kernels else [None]):
         upload_forced(engine, offers, force)
         kind = engine.stats()["select_kernel_kind"]
         if force is None and expect_kind is not None:
@@ -209,6 +209,9 @@ def test_edge_cases(engine):
     assert (best == -1).all() and (t5 == -1).all()
     b0, _ = engine.select({"req_mem_gb": np.zeros(0, np.int32)})
     assert b0.size == 0
+    # empty offer table and a batch above the fused kernel's size, through every kernel
+    best = check(engine, empty, rpk.synth.make_pods(20_000))
+    assert (best == -1).all()
     # nothing feasible at all / everything tied
     offers2 = rpk.synth.make_offers(300)
     offers2["secure_price"][:] = 0.25

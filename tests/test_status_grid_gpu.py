@@ -78,3 +78,51 @@ def test_sweep_at_launch_boundary(size, stride):
         want = tab.diff(nxt)
         assert np.array_equal(got, want), f"N {N}: tick changed list"
         assert np.array_equal(codes, oracle.record_codes(nxt)[want]), f"N {N}: tick codes"
+
+
+@pytest.mark.parametrize("stride", [16, 32])
+def test_big_table_boundary(stride):
+    """One context over the big-table boundary (4M - 1 slots: the largest 256-thread table; 4M; 4M + 37: a ragged last
+    unit), host entry point; then the device entry point on a caller-owned column, and a misaligned column refused."""
+    import torch
+
+    M = BIG + 37
+    base_all = rpk.synth.make_status_records(M, 0, stride=stride)
+    next_all = rpk.synth.make_status_records(M, 2, 0.37, stride=stride)
+    with rpk.Engine(1) as eng:
+        for N in (BIG - 1, BIG, BIG + 37):
+            base, nxt = base_all[:N], next_all[:N]
+            tab = oracle.StatusTable(N, stride)
+            eng.status_reset(N)
+            eng.status_seed(base)
+            tab.seed(base)
+            got, codes, hashes = eng.status_diff(nxt, want_codes=True, want_hashes=True)
+            want = tab.diff(nxt)
+            assert len(want) > N // 10, f"N {N}: the tables barely differ"
+            assert np.array_equal(got, want), f"N {N}: changed list"
+            assert np.array_equal(codes, oracle.record_codes(nxt)[want]), f"N {N}: codes"
+            assert np.array_equal(hashes, oracle.record_hashes(nxt)), f"N {N}: hash column"
+            got, _ = eng.status_diff(nxt)
+            assert len(got) == 0, f"N {N}: second sweep reported {len(got)} slots"
+        # device entry point, caller-owned column seeded by the caller with the reference hashes of `base_all`
+        col_tab = oracle.StatusTable(M, stride)
+        col_tab.seed(base_all)
+        d_recs = torch.from_numpy(next_all).cuda()
+        col = torch.from_numpy(oracle.record_hashes(base_all).view(np.int64)).cuda()
+        d_idx = torch.empty(M, dtype=torch.int32, device="cuda")
+        d_code = torch.empty(M, dtype=torch.int16, device="cuda")
+        d_n = torch.zeros(1, dtype=torch.int32, device="cuda")
+        eng.status_diff_device(d_recs, stride, col, d_idx, d_n, d_changed_code=d_code)
+        torch.cuda.synchronize()
+        n = int(d_n.item())
+        want = col_tab.diff(next_all)
+        assert np.array_equal(d_idx[:n].cpu().numpy().view(np.uint32), want), "device changed list"
+        assert np.array_equal(d_code[:n].cpu().numpy().view(np.uint16), oracle.record_codes(next_all)[want]), "device codes"
+        assert np.array_equal(col.cpu().numpy().view(np.uint64), oracle.record_hashes(next_all)), "device column"
+        # a column that starts 8 bytes off a 16-byte boundary is refused before anything is launched
+        buf = torch.zeros(M + 1, dtype=torch.int64, device="cuda")
+        with pytest.raises(rpk.RpkError) as ei:
+            eng.status_diff_device(d_recs, stride, buf[1:], d_idx, d_n)
+        assert ei.value.code == rpk._ffi.RPK_EINVAL
+        torch.cuda.synchronize()
+        assert int(buf.count_nonzero().item()) == 0, "the refused call wrote the column"

@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""K1 tuning sweep (1 GPU): time rpk_select_device (memset + k_pod_prep + grid kernel) for several row counts and
-RPK_TUNE settings -- the per-GPU work of the N-GPU strong-scaling bench is P/N rows, so P = 125k here is what
-each GPU does at N = 8.
+"""K1 tuning sweep (1 GPU): time rpk_select_device (k_pod_classify + k_pod_scatter + the persistent k_select_persist)
+for several row counts and RPK_TUNE settings -- the per-GPU work of the N-GPU strong-scaling bench is P/N rows, so
+P = 125k here is what each GPU does at N = 8.  --variants is a '|'-separated list of RPK_TUNE values (spaces become
+commas), e.g. "|stagekb=110|ipw=8 pdl=off"; the default times the defaults only.
 
-    python tools/k1_tune.py [--iters 20] [--out results/k1_tune.json]
+    python tools/k1_tune.py [--iters 20] [--variants ""] [--out results/k1_tune.json]
 """
 import argparse
 import importlib
@@ -21,7 +22,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--offers", type=int, default=100_000)
     ap.add_argument("--pods", default="125000,250000,1000000")
-    ap.add_argument("--variants", default="k1=grid|")
+    ap.add_argument("--variants", default="")
     ap.add_argument("--status-slots", type=int, default=0, help="run a status sweep of this many slots on a side stream alongside")
     ap.add_argument("--prio", action="store_true", help="select on a high-priority stream, the sweep on a low-priority one")
     ap.add_argument("--out", default=os.path.join(ROOT, "results", "k1_tune.json"))

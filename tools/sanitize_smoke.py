@@ -14,7 +14,7 @@ import rpk  # noqa: E402
 ONLY_MULTI = os.environ.get("RPK_SANITIZE_ONLY_MULTI") == "1"  # the 2-GPU part alone (a 2-GPU box is charged twice)
 eng = rpk.Engine(1)
 offers = rpk.synth.make_offers(20_000, correlated=True)
-for force in () if ONLY_MULTI else (None, "bitmap_grouped", "bitmap_grid", "packed_pos", "packed", "generic"):
+for force in () if ONLY_MULTI else (None, "bitmap_grouped", "packed_pos", "packed", "generic"):
     os.environ.pop("RPK_FORCE_KERNEL", None)
     if force:
         os.environ["RPK_FORCE_KERNEL"] = force
