@@ -246,6 +246,26 @@ func (e *Engine) StatusSeedSlots(slots []uint32, records []byte, stride int) err
 	return nil
 }
 
+// StatusDiffSlots compares only the listed slots (strictly ascending, < N of the tracked table; records holds
+// len(slots) packed slots, records[i] this sweep's state of slots[i]): the pods updateAllPodStatuses fetched this
+// cycle (kubelet.go:836-864).  Returns the changed slot ids ascending and their codes.  Unlisted slots are not touched.
+func (e *Engine) StatusDiffSlots(slots []uint32, records []byte, stride int) ([]uint32, []StatusCode, error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if len(slots) == 0 {
+		return nil, nil, nil
+	}
+	changed := make([]uint32, len(slots))
+	codes := make([]StatusCode, len(slots))
+	var cnt C.uint32_t
+	rc := C.rpk_status_diff_slots(e.ctx, C.uint32_t(len(slots)), (*C.uint32_t)(unsafe.Pointer(&slots[0])), u8p(records),
+		C.uint32_t(stride), (*C.uint32_t)(unsafe.Pointer(&changed[0])), (*C.uint16_t)(unsafe.Pointer(&codes[0])), &cnt)
+	if rc != C.RPK_OK {
+		return nil, nil, lastError(e.ctx, rc)
+	}
+	return changed[:int(cnt)], codes[:int(cnt)], nil
+}
+
 // Tick runs the pending-pod selection and the status sweep of one kubelet tick together (rpk_tick): the two
 // are independent, so their copies and kernels overlap and the call synchronises once.  p may be nil.
 func (e *Engine) Tick(p *Pods, wantTop5 bool, records []byte, stride int) (best, top5 []int32, changed []uint32, codes []StatusCode, err error) {

@@ -3,7 +3,7 @@
 // whose two data-parallel loop bodies go through the rpk engine instead of per-pod Go loops:
 //
 //	processPendingPods  (kubelet.go:747-814)  one Engine.Select over ALL pending pods per tick
-//	updateAllPodStatuses (kubelet.go:816-974) one Engine.StatusDiffCodes over ALL tracked slots per tick
+//	updateAllPodStatuses (kubelet.go:816-974) one Engine.StatusDiffSlots over the slots fetched this tick
 //
 // NOT BUILT IN THIS REPOSITORY: the image has no Go toolchain and the reference's dependencies (client-go,
 // virtual-kubelet v1.9.0) are not vendored (SURVEY.md 8c).  The executable twin of this file is the C++ mirror
@@ -14,6 +14,7 @@ package vk
 import (
 	"context"
 	"fmt"
+	"sort"
 	"strings"
 	"sync"
 	"time"
@@ -299,9 +300,9 @@ func (p *Provider) updateAllPodStatuses() {
 	type fresh struct {
 		key, status string
 		ports       bool
+		rec         []byte
 	}
 	p.podsMutex.RLock()
-	staged := append([]byte(nil), p.records...)
 	type target struct {
 		key  string
 		pod  *v1.Pod
@@ -330,11 +331,21 @@ func (p *Provider) updateAllPodStatuses() {
 		ports := checkPortsExposed(ds.PortMappings, t.info.RequestedPorts) // :867
 		low := strings.ToLower(t.info.StatusMessage)
 		flag := strings.Contains(low, "error") || strings.Contains(low, "fail")
-		if rpk.EncodeStatusRecord(staged[int(t.info.slot)*stride:int(t.info.slot+1)*stride], ds.DesiredStatus, ports, flag) == nil {
-			bySlot[t.info.slot] = fresh{t.key, ds.DesiredStatus, ports}
+		rec := make([]byte, stride)
+		if rpk.EncodeStatusRecord(rec, ds.DesiredStatus, ports, flag) == nil {
+			bySlot[t.info.slot] = fresh{t.key, ds.DesiredStatus, ports, rec}
 		}
 	}
-	changed, codes, err := p.engine.StatusDiffCodes(staged, stride) // :870-873 for every slot + the decision per changed slot
+	slots := make([]uint32, 0, len(bySlot)) // the fetched slots, ascending, and their records packed in that order
+	for s := range bySlot {
+		slots = append(slots, s)
+	}
+	sort.Slice(slots, func(i, j int) bool { return slots[i] < slots[j] })
+	recs := make([]byte, 0, len(slots)*stride)
+	for _, s := range slots {
+		recs = append(recs, bySlot[s].rec...)
+	}
+	changed, codes, err := p.engine.StatusDiffSlots(slots, recs, stride) // :870-873 for the fetched slots + the decision per changed slot
 	if err != nil {
 		return
 	}
@@ -345,11 +356,11 @@ func (p *Provider) updateAllPodStatuses() {
 		info, tracked := p.podStatus[f.key]
 		if !ok || !tracked || info.slot != slot {
 			p.podsMutex.Unlock()
-			reseed = append(reseed, slot) // reported but not applied: device state must follow records, not the staged copy
+			reseed = append(reseed, slot) // reported but not applied: device state must follow records, not the fetched one
 			continue
 		}
 		info.Status, info.PortsExposed = f.status, f.ports // :875-880
-		copy(p.records[int(slot)*stride:int(slot+1)*stride], staged[int(slot)*stride:int(slot+1)*stride])
+		copy(p.records[int(slot)*stride:int(slot+1)*stride], f.rec)
 		np := p.pods[f.key].DeepCopy()
 		np.Status = *podStatusFromCode(codes[i], f.status, info.StatusMessage) // translateRunPodStatus, :883
 		p.pods[f.key] = np

@@ -227,6 +227,25 @@ int rpk_status_seed(rpk_ctx* ctx, uint32_t N, const uint8_t* records, uint32_t s
  * of slot slots[i] (CreatePod writes ONE InstanceInfo, kubelet.go:391-401; handleMissingRunPodInstance rewrites one,
  * :976-1040).  Nothing else is touched, so a sweep whose records are already staged loses nothing. */
 int rpk_status_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* records, uint32_t stride);
+/* Diff of individual slots of the tracked table: records holds n_slots packed slots of `stride` bytes, records[i]
+ * is this sweep's state of slot slots[i] (updateAllPodStatuses compares only the pods it fetched this cycle,
+ * kubelet.go:836-864).  slots must be strictly ascending and < N of the tracked table (else RPK_EINVAL, nothing
+ * changed; no tracked table: RPK_ESTATE).  Same predicate, state update and codes as rpk_status_diff_codes restricted
+ * to the listed slots: changed_idx (capacity n_slots) receives the changed SLOT ids ascending, changed_code
+ * (nullable) their codes.  Slots not listed are neither compared nor touched.  n_slots == 0: *n_changed = 0.
+ * Counts n_slots records in rpk_stats.status_records. */
+int rpk_status_diff_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* records,
+                          uint32_t stride, uint32_t* changed_idx, uint16_t* changed_code, uint32_t* n_changed);
+/* Device variant on a caller-owned column: d_hash_prev holds global slots [idx_base, idx_base + N).  An entry whose
+ * slot lies outside that range is skipped (never read, written or reported), so the ranks of a sharded table can
+ * all be handed the same global list.  Enqueued on `stream`, no synchronisation, graph-capturable after one call
+ * of the size.  d_records and d_hash_prev 16-byte aligned (else RPK_EINVAL); d_changed_idx capacity n_slots.  Order
+ * is a precondition here (not checked): with a list that is not strictly ascending the changed list is unspecified,
+ * but no memory outside d_hash_prev[0, N) and the outputs is touched. */
+int rpk_status_diff_slots_device(rpk_ctx* ctx, int shard, uint32_t N, uint32_t idx_base, uint32_t n_slots,
+                                 const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride,
+                                 uint64_t* d_hash_prev, uint32_t* d_changed_idx, uint16_t* d_changed_code,
+                                 uint32_t* d_n_changed, void* stream);
 /* Forget all previous hashes and (re)size the table to N slots: every slot reports changed next time. */
 int rpk_status_reset(rpk_ctx* ctx, uint32_t N);
 

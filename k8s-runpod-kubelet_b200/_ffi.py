@@ -21,7 +21,8 @@ SYMBOLS = [
     "rpk_status_diff", "rpk_status_seed", "rpk_status_reset", "rpk_status_diff_device", "rpk_stats_get",
     "rpk_launch_count", "rpk_ipc_alloc", "rpk_ipc_open", "rpk_ipc_close", "rpk_ipc_free", "rpk_peer_fence",
     "rpk_peer_bind", "rpk_peer_wait", "rpk_peer_inline_wait", "rpk_status_diff_codes", "rpk_status_seed_slots", "rpk_tick",
-    "rpk_status_diff_device_codes", "rpk_xchg_bytes", "rpk_status_diff_device_gather",
+    "rpk_status_diff_device_codes", "rpk_xchg_bytes", "rpk_status_diff_device_gather", "rpk_status_diff_slots",
+    "rpk_status_diff_slots_device",
 ]
 
 
@@ -97,6 +98,10 @@ def load():
     L.rpk_xchg_bytes.argtypes = [C.c_int, u32]
     L.rpk_status_diff_device_gather.restype = C.c_int
     L.rpk_status_diff_device_gather.argtypes = [vp, C.c_int, u32, u8p, u32, u64p, u32, C.c_int, C.POINTER(vp), u32, C.c_int, u32p, vp]
+    L.rpk_status_diff_slots.restype = C.c_int
+    L.rpk_status_diff_slots.argtypes = [vp, u32, u32p, u8p, u32, u32p, vp, u32p]
+    L.rpk_status_diff_slots_device.restype = C.c_int
+    L.rpk_status_diff_slots_device.argtypes = [vp, C.c_int, u32, u32, u32, u32p, u8p, u32, u64p, u32p, vp, u32p, vp]
     L.rpk_stats_get.restype = C.c_int
     L.rpk_stats_get.argtypes = [vp, C.POINTER(RpkStats)]
     for name in ("rpk_ipc_alloc", "rpk_ipc_open", "rpk_ipc_close", "rpk_ipc_free"):

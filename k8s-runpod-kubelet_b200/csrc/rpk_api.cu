@@ -750,18 +750,34 @@ void reserve_status_state(DeviceState& ds, uint32_t N, uint32_t stride) {
 struct StatusHostArgs {
     uint32_t N; const uint8_t* records; uint32_t stride;
     uint32_t* changed_idx; uint16_t* changed_code; uint32_t* n_changed; uint64_t* hashes_out; bool report;
+    const uint32_t* slots; uint32_t n_slots;  // rpk_status_diff_slots: records holds the n_slots listed slots (ascending)
 };
+
+// Shard s of a host sweep: its hash column holds global slots [lo, hi); its records are [p0, p1) of the caller's table
+// (the same range) or, for a slot list, the entries whose slot lies in [lo, hi) -- two binary searches, since the list
+// is ascending.
+struct ShardPart { uint32_t lo, hi, p0, p1; };
+ShardPart shard_part(const rpk_ctx* ctx, int s, const StatusHostArgs& h) {
+    ShardPart p;
+    shard_range(h.N, (int)ctx->devs.size(), s, &p.lo, &p.hi);
+    p.p0 = p.lo; p.p1 = p.hi;
+    if (h.slots) {
+        p.p0 = (uint32_t)(std::lower_bound(h.slots, h.slots + h.n_slots, p.lo) - h.slots);
+        p.p1 = (uint32_t)(std::lower_bound(h.slots, h.slots + h.n_slots, p.hi) - h.slots);
+    }
+    return p;
+}
 
 // Sizes one shard's buffers (calling thread).  The changed list comes back through mapped pinned memory -- the kernel's
 // final copy writes indices, codes and the count straight into it, so the host needs ONE stream synchronise and no
 // device-to-host copy whose size it would first have to learn.
 void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
-    const int n = (int)ctx->devs.size();
     DeviceState& ds = ctx->devs[(size_t)s];
-    uint32_t lo, hi; shard_range(h.N, n, s, &lo, &hi);
-    const uint32_t Ns = hi - lo, cap = Ns ? Ns : 1;
+    const ShardPart sp = shard_part(ctx, s, h);
+    const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
     RPK_CUDA(cudaSetDevice(ds.dev));
     ds.s_records.reserve((size_t)cap * h.stride);
+    if (h.slots) ds.s_seed_slots.reserve(cap);
     ds.s_stage_idx.reserve(cap + 64); ds.s_unit_cnt.reserve(cap / 32 + 2);
     if (h.changed_code) ds.s_stage_code.reserve(cap + 64);
     if (h.hashes_out) ds.s_hash_out.reserve(cap);
@@ -779,13 +795,13 @@ void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
 
 // One shard's half of a host sweep, enqueued on ds.stream (ds.ev[0..2] bracket copy and kernel); the caller synchronises.
 void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint64_t* launches) {
-    const int n = (int)ctx->devs.size();
     DeviceState& ds = ctx->devs[(size_t)s];
-    uint32_t lo, hi; shard_range(h.N, n, s, &lo, &hi);
-    const uint32_t Ns = hi - lo, cap = Ns ? Ns : 1;
+    const ShardPart sp = shard_part(ctx, s, h);
+    const uint32_t lo = sp.lo, Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
     RPK_CUDA(cudaSetDevice(ds.dev));
     RPK_CUDA(cudaEventRecord(ds.ev[0], ds.stream));
-    if (Ns) RPK_CUDA(cudaMemcpyAsync(ds.s_records.p, h.records + (size_t)lo * h.stride, (size_t)Ns * h.stride, cudaMemcpyHostToDevice, ds.stream));
+    if (Ns) RPK_CUDA(cudaMemcpyAsync(ds.s_records.p, h.records + (size_t)sp.p0 * h.stride, (size_t)Ns * h.stride, cudaMemcpyHostToDevice, ds.stream));
+    if (Ns && h.slots) RPK_CUDA(cudaMemcpyAsync(ds.s_seed_slots.p, h.slots + sp.p0, (size_t)Ns * 4, cudaMemcpyHostToDevice, ds.stream));
     RPK_CUDA(cudaEventRecord(ds.ev[1], ds.stream));
     // mapped block: [count : 64 bytes][indices : cap u32][codes : cap u16]
     uint32_t* m_count = reinterpret_cast<uint32_t*>(ds.d_changed_map);
@@ -799,6 +815,7 @@ void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint64_t
     a.changed_code = h.report && h.changed_code ? m_code : nullptr;
     a.idx_base = lo; a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
     a.stage_idx = ds.s_stage_idx.p; a.stage_code = h.changed_code ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
+    if (h.slots) { a.slots = ds.s_seed_slots.p; a.col_n = sp.hi - sp.lo; }
     ds.status_dirty = true;
     if (Ns) *launches += (uint64_t)launch_status_diff(a, ds.stream);
     ds.status_dirty = false;
@@ -808,16 +825,17 @@ void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint64_t
 
 // after the shard's stream has been synchronised: this shard's part of the caller's arrays (ascending over shards)
 uint32_t collect_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint32_t out_at) {
-    const int n = (int)ctx->devs.size();
     DeviceState& ds = ctx->devs[(size_t)s];
-    uint32_t lo, hi; shard_range(h.N, n, s, &lo, &hi);
-    const uint32_t Ns = hi - lo, cap = Ns ? Ns : 1;
+    const ShardPart sp = shard_part(ctx, s, h);
+    const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
     if (!h.report || !Ns) return 0;
     const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(ds.h_changed);
     memcpy(h.changed_idx + out_at, ds.h_changed + 64, (size_t)cnt * 4);
     if (h.changed_code) memcpy(h.changed_code + out_at, ds.h_changed + 64 + (size_t)cap * 4, (size_t)cnt * 2);
     return cnt;
 }
+
+int run_status_host(rpk_ctx* ctx, const StatusHostArgs& h);
 
 int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
     if (!ctx) return RPK_EINVAL;
@@ -826,6 +844,11 @@ int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
     if (h.report && (!h.n_changed || (h.N > 0 && !h.changed_idx))) return fail(ctx, RPK_EINVAL, "rpk_status_diff: changed_idx and n_changed are required");
     if (!ctx->devs[0].status_sized) { if (int rc = rpk_status_reset(ctx, h.N)) return rc; }
     if (ctx->devs[0].statusN != h.N) return fail(ctx, RPK_ESTATE, "rpk_status_diff: N differs from the tracked table (call rpk_status_reset to resize)");
+    return run_status_host(ctx, h);
+}
+
+// a host sweep whose arguments have been checked: every shard uploads its part, sweeps it and synchronises once
+int run_status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
     return guarded(ctx, [&]() -> int {
         const int n = (int)ctx->devs.size();
         for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, h);
@@ -848,7 +871,7 @@ int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
         }
         if (h.report) *h.n_changed = total;
         ctx->stats.last_status_kernel_ms = kmax; ctx->stats.last_status_total_ms = tmax;
-        ctx->stats.status_calls += 1; ctx->stats.status_records += h.N;
+        ctx->stats.status_calls += 1; ctx->stats.status_records += h.slots ? h.n_slots : h.N;
         return RPK_OK;
     });
 }
@@ -894,6 +917,24 @@ int rpk_status_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
         }
         return RPK_OK;
     });
+}
+
+int rpk_status_diff_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* records, uint32_t stride,
+                          uint32_t* changed_idx, uint16_t* changed_code, uint32_t* n_changed) {
+    if (!ctx) return RPK_EINVAL;
+    if (int rc = check_stride(ctx, stride)) return rc;
+    if (!n_changed) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: n_changed is required");
+    if (n_slots == 0) { *n_changed = 0; return RPK_OK; }
+    if (!slots || !records || !changed_idx) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slots, records and changed_idx are required");
+    if (!ctx->devs[0].status_sized) return fail(ctx, RPK_ESTATE, "rpk_status_diff_slots: no tracked table (call rpk_status_reset first)");
+    const uint32_t N = ctx->devs[0].statusN;
+    for (uint32_t i = 0; i < n_slots; ++i) {
+        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slot index outside the tracked table");
+        if (i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slots must be strictly ascending");
+    }
+    StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
+    h.slots = slots; h.n_slots = n_slots;
+    return run_status_host(ctx, h);
 }
 
 // One tick of the kubelet: the pending-pod selection (processPendingPods, kubelet.go:747-814) and the status sweep
@@ -942,7 +983,8 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
 namespace {
 int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride, uint64_t* d_hash_prev,
                   uint32_t idx_base, uint32_t* d_changed_idx, uint16_t* d_changed_code, uint32_t* d_n_changed, int n_out,
-                  uint32_t* const* d_xchg, uint32_t cap, int my_rank, void* stream) {
+                  uint32_t* const* d_xchg, uint32_t cap, int my_rank, void* stream, const uint32_t* d_slots = nullptr, uint32_t col_n = 0) {
+    // d_slots: N is the list's length, and the column (col_n rows) holds global slots [idx_base, idx_base + col_n)
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: shard out of range");
     if (int rc = check_stride(ctx, stride)) return rc;
@@ -953,6 +995,8 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
     if (n_out < 0 || n_out > RPK_MAX_GPUS || (n_out > 0 && (!d_xchg || my_rank < 0 || my_rank >= n_out || N > cap)))
         return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: bad exchange arguments (N must fit the per-rank capacity)");
     if (n_out > 0 && stride != 16 && stride != 32) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: strides 16 and 32 only");
+    if (d_slots == nullptr && col_n != 0) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: d_slots is NULL");
+    if ((uint64_t)idx_base + col_n > (1ull << 32)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: idx_base + N exceeds the slot range");
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
@@ -965,6 +1009,7 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
         a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
         a.stage_idx = ds.s_stage_idx.p; a.stage_code = (d_changed_code || n_out > 0) ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
         a.n_out = n_out; a.my_rank = my_rank;
+        a.slots = d_slots; a.col_n = col_n;
         for (int o = 0; o < n_out; ++o) {  // rank o's buffer: [counts : 8 words][n_out index regions of cap][n_out code regions of cap u16]
             uint32_t* base = d_xchg[o];
             a.out_count[o] = base;
@@ -996,6 +1041,14 @@ int rpk_status_diff_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d
 int rpk_status_diff_device_codes(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                                  uint64_t* d_hash_prev, uint32_t* d_changed_idx, uint16_t* d_changed_code, uint32_t* d_n_changed, void* stream) {
     return status_device(ctx, shard, N, d_records, stride, d_hash_prev, 0, d_changed_idx, d_changed_code, d_n_changed, 0, nullptr, 0, 0, stream);
+}
+
+int rpk_status_diff_slots_device(rpk_ctx* ctx, int shard, uint32_t N, uint32_t idx_base, uint32_t n_slots,
+                                 const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* d_hash_prev,
+                                 uint32_t* d_changed_idx, uint16_t* d_changed_code, uint32_t* d_n_changed, void* stream) {
+    if (ctx && n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: d_slots is NULL");
+    return status_device(ctx, shard, n_slots, d_records, stride, d_hash_prev, idx_base, d_changed_idx, d_changed_code, d_n_changed,
+                         0, nullptr, 0, 0, stream, n_slots > 0 ? d_slots : nullptr, n_slots > 0 ? N : 0);
 }
 
 size_t rpk_xchg_bytes(int n_ranks, uint32_t cap) { return (size_t)(8 + (size_t)n_ranks * cap) * 4 + (size_t)n_ranks * cap * 2 + 16; }

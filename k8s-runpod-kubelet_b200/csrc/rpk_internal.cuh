@@ -145,6 +145,10 @@ struct StatusArgs {
     uint32_t* out_count[RPK_MAX_GPUS];  // rank o's count words (one per source rank)
     uint32_t* flags[RPK_MAX_GPUS];      // bound peer flags: the CTA that finishes last signals (n_flags = 0: none)
     int n_flags, inline_wait;
+    // slot-list sweep (rpk_status_diff_slots): records[i] is the state of global slot slots[i] (ascending), whose previous
+    // hash is hash_prev[slots[i] - idx_base]; entries outside [idx_base, idx_base + col_n) are skipped.  N = list length.
+    const uint32_t* slots;  // null: whole-table sweep
+    uint32_t col_n;
 };
 
 // launchers (each returns the number of kernels it launched, or throws CudaError)
@@ -261,7 +265,7 @@ struct DeviceState {
     // status
     DevBuf<uint8_t> s_records; DevBuf<uint64_t> s_hash_prev, s_hash_out; DevBuf<uint32_t> s_changed, s_misc;
     DevBuf<unsigned long long> s_tile_state; DevBuf<uint32_t> s_stage_idx; DevBuf<uint16_t> s_stage_code, s_changed_code; DevBuf<uint32_t> s_unit_cnt;
-    DevBuf<uint32_t> s_seed_slots; DevBuf<uint8_t> s_seed_recs;
+    DevBuf<uint32_t> s_seed_slots; DevBuf<uint8_t> s_seed_recs;  // slot lists of rpk_status_seed_slots and rpk_status_diff_slots
     unsigned char* h_changed = nullptr; unsigned char* d_changed_map = nullptr; size_t h_changed_cap = 0;  // mapped pinned: count, indices, codes
     cudaStream_t status_stream = nullptr;  // rpk_tick: the sweep next to the selection
     // device entry points: the stream that last used the select / status scratch, and its completion event

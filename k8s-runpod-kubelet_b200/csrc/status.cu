@@ -23,6 +23,9 @@
 //                            ascending position (and, for the sharded sweep, into every peer's exchange buffer).
 //   k_status_diff<ITEMS>     the other strides (48..256): padded shared-memory tile + look-back per tile.
 //   k_status_seed_slots      previous state of individual slots (CreatePod writes ONE InstanceInfo, kubelet.go:391-401).
+// The first two also sweep a list of slots (template flag SLOTS, rpk_status_diff_slots): the listed slots' packed
+// records are a table of their own, streamed the same way; only the hash row (slots[i] - idx_base) and the id
+// reported (slots[i]) differ.  updateAllPodStatuses compares only the pods it fetched this cycle (kubelet.go:836-864).
 #include "rpk_device.cuh"
 #include "rpk_internal.cuh"
 
@@ -207,24 +210,32 @@ constexpr uint32_t kUnit = 32 * kStreamItems;            // slots per warp per u
 // CTA per SM is also faster at 1M slots than four (fewer look-back entries and copy rounds).
 constexpr uint32_t kBigTable = 4u << 20;
 // control words (StatusArgs::tile_counter): [0] scheduling ticket, [1] finished CTAs
-template <int STRIDE> struct SlotData { uint4 lo; uint4 hi; u64 prev; };
+// col (SLOTS only): the entry's row of hash_prev, kNone when the slot lies outside the column
+template <int STRIDE> struct SlotData { uint4 lo; uint4 hi; u64 prev; uint32_t col; };
 
-template <int STRIDE>
+template <int STRIDE, bool SLOTS>
 __device__ __forceinline__ void load_unit(const StatusArgs& a, uint32_t base, uint32_t lane, SlotData<STRIDE> (&d)[kStreamItems]) {
 #pragma unroll
     for (int k = 0; k < kStreamItems; ++k) {
         const uint32_t s = base + (uint32_t)k * 32 + lane;
         d[k].lo = make_uint4(0, 0, 0, 0); d[k].hi = d[k].lo; d[k].prev = 0;
+        if constexpr (SLOTS) d[k].col = kNone;
         if (s < a.N) {
             const uint4* p = reinterpret_cast<const uint4*>(a.records + (size_t)s * STRIDE);
             d[k].lo = __ldg(p);  // the two halves of a 32-byte slot share a sector: the second load hits L1
             if (STRIDE == 32) d[k].hi = __ldg(p + 1);
-            d[k].prev = a.hash_prev[s];
+            if constexpr (SLOTS) {
+                const uint32_t c = __ldg(a.slots + s) - a.idx_base;  // below idx_base wraps around: outside
+                if (c < a.col_n) { d[k].col = c; d[k].prev = a.hash_prev[c]; }
+            } else {
+                d[k].prev = a.hash_prev[s];
+            }
         }
     }
 }
 
-template <int STRIDE, int THREADS>
+// SLOTS: the table is a packed slot list (StatusArgs::slots); the exchange outputs (n_out, flags) are not used
+template <int STRIDE, int THREADS, bool SLOTS = false>
 __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(StatusArgs a, uint32_t n_units) {
     constexpr int kSThreads = THREADS, kSWarps = THREADS / 32;
     __shared__ uint32_t s_warp[kSWarps];
@@ -251,7 +262,12 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
             if (STRIDE == 16) h = xxh64_lanes2(l0, l1, nl);
             else h = xxh64_lanes4(l0, l1, mk64(d[k].hi.x, d[k].hi.y), mk64(d[k].hi.z, d[k].hi.w), nl);
             bool changed = false;
-            if (s < a.N) {
+            if constexpr (SLOTS) {
+                if (s < a.N && d[k].col != kNone) {
+                    changed = (d[k].prev == 0ull) || (h != d[k].prev);
+                    if (changed) a.hash_prev[d[k].col] = h;
+                }
+            } else if (s < a.N) {
                 changed = (d[k].prev == 0ull) || (h != d[k].prev);  // 0 = never seen
                 if (changed) a.hash_prev[s] = h;                     // kubelet.go:875-880
                 if (a.hash_out) a.hash_out[s] = h;
@@ -267,13 +283,13 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
     // two register sets, used alternately: the next unit's loads are in flight while the current one is hashed
     SlotData<STRIDE> ra[kStreamItems], rb[kStreamItems];
     uint32_t u = c_lo + warp;
-    if (u < c_hi) load_unit<STRIDE>(a, u * kUnit, lane, ra);
+    if (u < c_hi) load_unit<STRIDE, SLOTS>(a, u * kUnit, lane, ra);
     while (u < c_hi) {
-        if (u + kSWarps < c_hi) load_unit<STRIDE>(a, (u + kSWarps) * kUnit, lane, rb);
+        if (u + kSWarps < c_hi) load_unit<STRIDE, SLOTS>(a, (u + kSWarps) * kUnit, lane, rb);
         process(u, ra);
         u += kSWarps;
         if (u >= c_hi) break;
-        if (u + kSWarps < c_hi) load_unit<STRIDE>(a, (u + kSWarps) * kUnit, lane, ra);
+        if (u + kSWarps < c_hi) load_unit<STRIDE, SLOTS>(a, (u + kSWarps) * kUnit, lane, ra);
         process(u, rb);
         u += kSWarps;
     }
@@ -295,12 +311,12 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
             s_excl = excl; s_carry = 0;
             if (cid == n_ctas - 1) {  // the last CTA in slot order owns the count
                 *a.n_changed = excl + total;
-                for (int o = 0; o < a.n_out; ++o) a.out_count[o][a.my_rank] = excl + total;
+                for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_count[o][a.my_rank] = excl + total;
             }
         }
     }
     __syncthreads();
-    const bool want_codes = a.changed_code != nullptr || (a.n_out > 0 && a.out_code[0] != nullptr);
+    const bool want_codes = a.changed_code != nullptr || (!SLOTS && a.n_out > 0 && a.out_code[0] != nullptr);
     // exclusive scan of the unit counts in unit order, 1024 units per round; thread t copies unit t's staged entries
     for (uint32_t r0 = c_lo; r0 < c_hi; r0 += kSThreads) {
         const uint32_t v = r0 + tid;
@@ -315,9 +331,9 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
         const uint32_t off = s_excl + s_carry + wbase + inc - c;
         for (uint32_t i = 0; i < c; ++i) {
             const uint32_t slot = a.stage_idx[v * kUnit + i];
-            const uint32_t x = a.idx_base + slot;
+            const uint32_t x = SLOTS ? __ldg(a.slots + slot) : a.idx_base + slot;  // SLOTS: slot is the list position
             if (a.changed_idx) a.changed_idx[off + i] = x;
-            for (int o = 0; o < a.n_out; ++o) a.out_idx[o][off + i] = x;
+            for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_idx[o][off + i] = x;
             if (want_codes) {  // translateRunPodStatus's decision, for the changed slots only: their records are read once more
                 const uint4 r = __ldg(reinterpret_cast<const uint4*>(a.records + (size_t)slot * STRIDE));
                 bool ports;
@@ -325,14 +341,14 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
                 const uint32_t kind = classify_status(mk64(r.x & ~0x80u, r.y), mk64(r.z, r.w), len, &ports);
                 const uint16_t cc = (uint16_t)status_code(kind, ports, (r.x & 0x80u) != 0u);
                 if (a.changed_code) a.changed_code[off + i] = cc;
-                for (int o = 0; o < a.n_out; ++o) if (a.out_code[o]) a.out_code[o][off + i] = cc;
+                for (int o = 0; !SLOTS && o < a.n_out; ++o) if (a.out_code[o]) a.out_code[o][off + i] = cc;
             }
         }
         __syncthreads();
         if (tid == kSThreads - 1) s_carry += wbase + inc;  // this round's total
         __syncthreads();
     }
-    if (a.n_out > 0) __threadfence_system();  // peer stores are performed system-wide before this CTA counts as finished
+    if (!SLOTS && a.n_out > 0) __threadfence_system();  // peer stores are performed system-wide before this CTA counts as finished
     else __threadfence();
     __syncthreads();
     if (tid == 0) s_last = atomicAdd(a.tile_counter + 1, 1u) == n_ctas - 1 ? 1u : 0u;
@@ -341,7 +357,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
     // last CTA to finish: every look-back is over -- clean the state for the next call, then tell the peers
     for (uint32_t i = tid; i < n_ctas; i += kSThreads) a.tile_state[i] = 0ull;
     if (tid == 0) { a.tile_counter[0] = 0u; a.tile_counter[1] = 0u; }
-    if (a.n_flags > 0 && warp == 0) {
+    if (!SLOTS && a.n_flags > 0 && warp == 0) {
         uint32_t e = 0;
         if (lane == 0) { e = a.flags[a.my_rank][33] + 1u; a.flags[a.my_rank][33] = e; }  // status epoch counter
         e = __shfl_sync(0xFFFFFFFFu, e, 0);
@@ -360,7 +376,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
 // ---------------------------------------------------------------------------------------------------------
 // other strides: padded shared-memory tile, decoupled look-back per tile
 // ---------------------------------------------------------------------------------------------------------
-template <int ITEMS>
+template <int ITEMS, bool SLOTS = false>  // SLOTS: as k_status_stream
 __global__ void __launch_bounds__(kStThreads) k_status_diff(StatusArgs a) {
     extern __shared__ __align__(16) uint32_t s_rec[];  // tile_recs rows of (stride/4 + 1) words
     __shared__ uint32_t s_tile, s_excl, s_last;
@@ -393,16 +409,18 @@ __global__ void __launch_bounds__(kStThreads) k_status_diff(StatusArgs a) {
     for (int k = 0; k < ITEMS; ++k) {
         const uint32_t lr = (uint32_t)k * kStThreads + tid;
         changed[k] = false; code[k] = 0;
-        if (lr < nrec) {
+        // SLOTS: row slots[i] - idx_base of hash_prev, and nothing for a slot outside the column
+        const uint32_t col = SLOTS && lr < nrec ? a.slots[rec0 + lr] - a.idx_base : kNone;
+        if (lr < nrec && (!SLOTS || col < a.col_n)) {
             const uint32_t* w = s_rec + lr * row;
             const uint32_t b0 = w[0] & 0xFFu;
             const uint32_t len = min(b0 & 0x7Fu, a.stride - 1);
             const uint32_t nbytes = min(((len + 8u) >> 3) << 3, a.stride);
             const u64 h = xxh64_words(w, nbytes, w[0] & ~0x80u);
-            const u64 prev = a.hash_prev[rec0 + lr];
+            const u64 prev = a.hash_prev[SLOTS ? col : rec0 + lr];
             changed[k] = (prev == 0ull) || (h != prev);  // 0 = never seen (after reset)
-            if (changed[k]) a.hash_prev[rec0 + lr] = h;  // kubelet.go:875-880: state replaced only on change
-            if (a.hash_out) a.hash_out[rec0 + lr] = h;
+            if (changed[k]) a.hash_prev[SLOTS ? col : rec0 + lr] = h;  // kubelet.go:875-880: state replaced only on change
+            if (!SLOTS && a.hash_out) a.hash_out[rec0 + lr] = h;
             if (changed[k] && a.changed_code) {
                 bool ports;
                 const uint32_t kind = classify_status(mk64(w[0] & ~0x80u, w[1]), mk64(w[2], w[3]), len, &ports);
@@ -434,7 +452,8 @@ __global__ void __launch_bounds__(kStThreads) k_status_diff(StatusArgs a) {
     for (int k = 0; k < ITEMS; ++k) {
         if (changed[k]) {
             const uint32_t posn = excl + s_wcnt[k * (kStThreads / 32) + warp] + __popc(bal[k] & ((1u << lane) - 1));
-            a.changed_idx[posn] = a.idx_base + rec0 + (uint32_t)k * kStThreads + tid;
+            if constexpr (SLOTS) a.changed_idx[posn] = a.slots[rec0 + (uint32_t)k * kStThreads + tid];
+            else a.changed_idx[posn] = a.idx_base + rec0 + (uint32_t)k * kStThreads + tid;
             if (a.changed_code) a.changed_code[posn] = (uint16_t)code[k];
         }
     }
@@ -473,7 +492,9 @@ uint32_t status_state_words(uint32_t N, uint32_t stride, int sm_count) {  // u64
     return (a > b ? a : b) + 8;
 }
 
-int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
+// SLOTS: a slot-list sweep, whose launch shape follows from the list length (a.N) exactly as a table's does from N
+template <bool SLOTS>
+static int launch_status(const StatusArgs& a, cudaStream_t st) {
     if (a.N == 0) {
         if (a.n_changed) RPK_CUDA(cudaMemsetAsync(a.n_changed, 0, sizeof(uint32_t), st));
         // an empty shard of a sharded sweep still has to publish its (zero) count and signal: one tiny CTA does it
@@ -496,11 +517,11 @@ int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
         // shared-memory ring filled by bulk copies -- were within 4 % of it at 16.8M slots on an H100 SXM (700 W) and
         // none was faster at both strides (DESIGN §4, profiles/h100_k2_tune.json)
         if (big) {
-            if (a.stride == 16) k_status_stream<16, 1024><<<grid, 1024, 0, st>>>(b, n_units);
-            else k_status_stream<32, 1024><<<grid, 1024, 0, st>>>(b, n_units);
+            if (a.stride == 16) k_status_stream<16, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
+            else k_status_stream<32, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
         } else {
-            if (a.stride == 16) k_status_stream<16, 256><<<grid, 256, 0, st>>>(b, n_units);
-            else k_status_stream<32, 256><<<grid, 256, 0, st>>>(b, n_units);
+            if (a.stride == 16) k_status_stream<16, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
+            else k_status_stream<32, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
         }
         RPK_CUDA(cudaGetLastError());
         return 1;
@@ -512,21 +533,27 @@ int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
     int dev = 0;
     RPK_CUDA(cudaGetDevice(&dev));
     switch (items) {
-        case 4:
-            if (attr_dev[0] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[0] = dev; }
-            k_status_diff<4><<<tiles, kStThreads, smem, st>>>(a);
+        case 4:  // strides 16 / 32 take the streaming kernel above
+            if constexpr (!SLOTS) {
+                if (attr_dev[0] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[0] = dev; }
+                k_status_diff<4><<<tiles, kStThreads, smem, st>>>(a);
+            }
             break;
         case 2:
-            if (attr_dev[1] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[1] = dev; }
-            k_status_diff<2><<<tiles, kStThreads, smem, st>>>(a);
+            if (attr_dev[1] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<2, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[1] = dev; }
+            k_status_diff<2, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
             break;
         default:
-            if (attr_dev[2] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[2] = dev; }
-            k_status_diff<1><<<tiles, kStThreads, smem, st>>>(a);
+            if (attr_dev[2] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<1, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[2] = dev; }
+            k_status_diff<1, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
             break;
     }
     RPK_CUDA(cudaGetLastError());
     return 1;
+}
+
+int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
+    return a.slots ? launch_status<true>(a, st) : launch_status<false>(a, st);
 }
 
 }  // namespace rpk

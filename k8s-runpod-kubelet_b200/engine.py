@@ -206,6 +206,19 @@ class Engine:
         self._check(self._lib.rpk_status_seed_slots(self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"),
                                                     _np_ptr(records, np.uint8, n * stride, "records"), stride))
 
+    def status_diff_slots(self, slots: np.ndarray, records: np.ndarray, want_codes: bool = False):
+        """Diff of the listed slots only (records[i] is this sweep's state of slot slots[i]; slots strictly ascending):
+        -> (changed slot ids ascending, codes | None).  Slots not listed are neither compared nor touched."""
+        n, stride = records.shape
+        slots = np.ascontiguousarray(slots, np.uint32)  # keep the converted array alive across the call
+        idx = np.empty(max(n, 1), np.uint32)
+        codes = np.empty(max(n, 1), np.uint16) if want_codes else None
+        cnt = C.c_uint32(0)
+        self._check(self._lib.rpk_status_diff_slots(
+            self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(records, np.uint8, n * stride, "records"), stride,
+            C.c_void_p(idx.ctypes.data), C.c_void_p(codes.ctypes.data) if want_codes else None, C.cast(C.byref(cnt), C.c_void_p)))
+        return idx[: cnt.value].copy(), (codes[: cnt.value].copy() if want_codes else None)
+
     def tick(self, pods: dict | None, records: np.ndarray, want_top5: bool = False, want_codes: bool = True, out_best=None):
         """One kubelet tick: selection over ``pods`` (None: none pending) and the status sweep over ``records`` enqueued
         together (rpk_tick).  -> (best | None, top5 | None, changed_idx, codes | None)"""
@@ -234,6 +247,22 @@ class Engine:
             self._ctx, shard, N, _dev_ptr(d_records, "uint8", N * stride), stride, C.c_void_p(d_hash_prev.data_ptr()),
             C.c_void_p(d_changed_idx.data_ptr()), C.c_void_p(d_changed_code.data_ptr()) if d_changed_code is not None else None,
             C.c_void_p(d_n_changed.data_ptr()), C.c_void_p(st)))
+
+    def status_diff_slots_device(self, d_slots, d_records, stride: int, d_hash_prev, d_changed_idx, d_n_changed, idx_base: int = 0,
+                                 d_changed_code=None, shard: int = 0, stream=None):
+        """Diff of the listed slots against a caller-owned hash column holding global slots [idx_base, idx_base + N)
+        (N = d_hash_prev.numel()); entries outside that range are skipped.  Enqueued on ``stream``."""
+        import torch
+
+        N, n = int(d_hash_prev.numel()), int(d_slots.numel())
+        st = stream if stream is not None else (torch.cuda.current_stream().cuda_stream or 1)  # 0 -> cudaStreamLegacy
+        if not d_slots.is_cuda or d_slots.dtype not in (torch.int32, torch.uint32) or not d_slots.is_contiguous():
+            raise TypeError("d_slots: expected a contiguous CUDA tensor of int32 / uint32")
+        self._check(self._lib.rpk_status_diff_slots_device(
+            self._ctx, shard, N, idx_base, n, C.c_void_p(d_slots.data_ptr()), _dev_ptr(d_records, "uint8", n * stride), stride,
+            C.c_void_p(d_hash_prev.data_ptr()), C.c_void_p(d_changed_idx.data_ptr()),
+            C.c_void_p(d_changed_code.data_ptr()) if d_changed_code is not None else None, C.c_void_p(d_n_changed.data_ptr()),
+            C.c_void_p(st)))
 
     def xchg_bytes(self, n_ranks: int, cap: int) -> int:
         return int(self._lib.rpk_xchg_bytes(n_ranks, cap))

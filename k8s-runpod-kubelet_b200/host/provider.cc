@@ -631,27 +631,27 @@ void Provider::WidenRecords(uint32_t stride) {
 }
 
 // updateAllPodStatuses -- kubelet.go:816-974.  The per-pod fetches stay sequential host I/O (out of scope);
-// the compare of (status, portsExposed) against InstanceInfo for ALL tracked slots is one rpk_status_diff_codes,
-// which also returns translateRunPodStatus's decision for every changed slot.
+// the compare of (status, portsExposed) against InstanceInfo for the slots fetched this cycle is one
+// rpk_status_diff_slots, which also returns translateRunPodStatus's decision for every changed slot.  Pods the
+// reference skips (terminal, no RunPod id, failed fetch, NOT_FOUND: kubelet.go:836-864) are not in the list.
 //
 // Concurrency (the reference reaches this from two tickers while CreatePod / DeletePod run on other goroutines):
-// fresh records are staged in a buffer private to the sweep -- a copy of records_ (what InstanceInfo says) with this
-// sweep's fetches on top -- and records_ / InstanceInfo are updated per changed slot afterwards, under pods_mutex_,
+// fresh records are encoded into a buffer private to the sweep -- one packed record per fetched slot -- and
+// records_ / InstanceInfo are updated per changed slot afterwards, under pods_mutex_,
 // only if the slot still belongs to the pod the sweep fetched.  A changed slot whose update is not applied (the pod
 // was created, deleted or re-created meanwhile) gets its device state re-seeded from records_, so device and host
 // cannot drift apart.
 void Provider::UpdateAllPodStatuses() {
     std::lock_guard<std::mutex> sweep_guard(sweep_mutex_);
     if (want_stride_ > stride_) WidenRecords(want_stride_);
-    struct Fresh { std::string key, status, message; bool ports; uint32_t slot; bool host_compare; };
+    struct Fresh { std::string key, status, message; bool ports; uint32_t slot; bool host_compare; size_t at; };
     std::vector<Fresh> fresh;
     std::vector<std::string> keys;
-    std::vector<uint8_t> staged;
+    std::vector<uint8_t> fetched;  // fresh[i]'s record at [fresh[i].at, + stride)
     uint32_t stride;
     {
         std::lock_guard<std::mutex> g(pods_mutex_);
         for (auto& kv : pods_) keys.push_back(kv.first);  // :818-823
-        staged = records_;
         stride = stride_;
     }
     for (const auto& key : keys) {
@@ -679,15 +679,15 @@ void Provider::UpdateAllPodStatuses() {
                 it->second.pod = np;
                 it->second.info.ID.clear(); it->second.info.Status = PodExited; it->second.info.StatusMessage = "RunPod instance not found";
                 EncodeStatusRecord(&records_[(size_t)slot * stride_], stride_, it->second.info.Status, it->second.info.PortsExposed);
-                if (stride_ == stride) std::memcpy(&staged[(size_t)slot * stride], &records_[(size_t)slot * stride], stride);
             }
             SeedSlot(slot);  // InstanceInfo was rewritten: so is the previous state -- of this slot, nothing else
             Notify(np);
             continue;
         }
         const bool ports = CheckPortsExposed(ds.PortMappings, info.RequestedPorts);         // :867
-        Fresh f{key, ds.DesiredStatus, info.StatusMessage, ports, slot, false};
-        if (!EncodeStatusRecord(&staged[(size_t)slot * stride], stride, ds.DesiredStatus, ports, MessageHasError(info.StatusMessage))) {
+        Fresh f{key, ds.DesiredStatus, info.StatusMessage, ports, slot, false, fetched.size()};
+        fetched.resize(fetched.size() + stride);
+        if (!EncodeStatusRecord(&fetched[f.at], stride, ds.DesiredStatus, ports, MessageHasError(info.StatusMessage))) {
             // does not fit this table's slots: compare it the way the reference does (:870-873) this cycle, and widen
             // the table before the next sweep if any slot size can hold it
             f.host_compare = true;
@@ -696,24 +696,32 @@ void Provider::UpdateAllPodStatuses() {
         }
         fresh.push_back(std::move(f));
     }
-    // ---- the diff: statusChanged || portsExposureChanged for every slot at once (:870-873) + the decision per changed slot ----
-    std::vector<uint32_t> changed(max_pods_);
-    std::vector<uint16_t> codes(max_pods_);
+    // ---- the diff: statusChanged || portsExposureChanged for every fetched slot at once (:870-873) + the decision per
+    // changed slot.  A slot fetched twice (its pod was re-created under another key during the sweep) keeps the later fetch.
+    std::map<uint32_t, const Fresh*> by_slot;
+    for (const auto& f : fresh) by_slot[f.slot] = &f;
+    std::vector<uint32_t> slots;
+    std::vector<uint8_t> recs;
+    for (const auto& kv : by_slot) {  // ascending slots; statuses no slot holds are compared on the host below
+        if (kv.second->host_compare) continue;
+        slots.push_back(kv.first);
+        recs.insert(recs.end(), fetched.begin() + (long)kv.second->at, fetched.begin() + (long)(kv.second->at + stride));
+    }
+    std::vector<uint32_t> changed(slots.size() + 1);
+    std::vector<uint16_t> codes(slots.size() + 1);
     uint32_t n_changed = 0;
     {
         std::lock_guard<std::mutex> g(engine_mutex_);
-        if (rpk_status_diff_codes(ctx_, max_pods_, staged.data(), stride, changed.data(), codes.data(), &n_changed, nullptr) != RPK_OK) return;
+        if (rpk_status_diff_slots(ctx_, (uint32_t)slots.size(), slots.data(), recs.data(), stride, changed.data(), codes.data(), &n_changed) != RPK_OK) return;
         ++status_calls_;
     }
-    std::map<uint32_t, const Fresh*> by_slot;
-    for (const auto& f : fresh) by_slot[f.slot] = &f;
     auto apply = [&](const Fresh& f, const PodStatusView& view) -> PodPtr {  // :875-880, 883, 927-929 under podsMutex
         std::lock_guard<std::mutex> g(pods_mutex_);
         auto it = pods_.find(f.key);
         if (it == pods_.end() || it->second.slot != f.slot || slot_key_[f.slot] != f.key) return nullptr;
         it->second.info.Status = f.status;
         it->second.info.PortsExposed = f.ports;
-        if (!f.host_compare && stride_ == stride) std::memcpy(&records_[(size_t)f.slot * stride], &staged[(size_t)f.slot * stride], stride);
+        if (!f.host_compare && stride_ == stride) std::memcpy(&records_[(size_t)f.slot * stride], &fetched[f.at], stride);
         auto np = std::make_shared<Pod>(*it->second.pod);
         np->status = view;
         it->second.pod = np;
@@ -727,7 +735,7 @@ void Provider::UpdateAllPodStatuses() {
         if (ft != by_slot.end() && !ft->second->host_compare)
             np = apply(*ft->second, StatusFromCode(codes[i], ft->second->status, ft->second->message));
         if (np) Notify(np);  // :936-954 (the k8s PATCH of :915 is out of scope; the callback path is the PodNotifier contract)
-        else reseed.push_back(slot);  // reported but not applied: the device must not keep the staged record as "previous"
+        else reseed.push_back(slot);  // reported but not applied: the device must not keep the fetched record as "previous"
     }
     for (const auto& f : fresh) {  // statuses longer than any slot: string + bool compare on the host (:870-873)
         if (!f.host_compare) continue;

@@ -35,6 +35,10 @@ for stride in () if ONLY_MULTI else (16, 32, 64):
         assert np.array_equal(got, want) and np.array_equal(hashes, oracle.record_hashes(recs))
         assert np.array_equal(codes, oracle.record_codes(recs)[want])
     e2.status_seed_slots(np.array([5, 77], np.uint32), np.ascontiguousarray(recs[[5, 77]]))
+    sl = np.arange(3, 30_000, 7, dtype=np.uint32)  # the slot-list sweep: only the listed slots are compared
+    nxt = rpk.synth.make_status_records(30_000, 3, 0.5, stride=stride)[sl]
+    got, codes = e2.status_diff_slots(sl, nxt, want_codes=True)
+    assert np.array_equal(got, sl[oracle.record_hashes(nxt) != oracle.record_hashes(np.ascontiguousarray(recs[sl]))])
     e2.close()
 # the big-table build of the stream kernel (>= 4M slots), ragged last unit
 for stride in () if ONLY_MULTI else (32, 16):
