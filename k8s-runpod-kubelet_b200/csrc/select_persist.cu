@@ -482,6 +482,7 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
     // an item that covers the whole table (one stage, one item per row block) leaves its rows final: no merge
     const bool direct = pa.tickets_per_block == 1;
     uint32_t it = 0, phase_bits = 0;  // bit g: parity of copy group g's next completion (groups are not all used by every stage)
+    uint32_t last_used = 0, last_parity = 0;  // the copy groups of the stage loaded last, and the parity they complete with
     for (uint32_t pair = first; pair < npairs; pair += step, ++it) {
         const uint32_t gi = pair / S, s = pair % S, grp = s_grp[gi];
         const uint32_t c = grp / pa.groups_per_cloud;
@@ -500,6 +501,7 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
         }
         const uint32_t parity = phase_bits;
         phase_bits ^= used;
+        last_used = used; last_parity = parity;
         uint32_t ready = 0;  // copy groups this warp has seen complete
         const uint32_t n_c = s_rows[gi], c_start = s_start[gi];
         const uint32_t nblk = (n_c + RPI - 1) / RPI;
@@ -632,6 +634,13 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
         retire(pend2_blk, pend2_ticket);
         pend2_blk = kNone;
     }
+    // A warp waits only on the copy groups its items cover, so a CTA that found its queue already drained has waited on
+    // none of its stage's bulk copies.  Shared memory lives as long as its CTA, and nothing in the PTX ISA makes the
+    // CTA's exit wait for asynchronous writes into it: drain the last stage's copies before this CTA can exit (a group
+    // some warp already waited on returns at once; earlier stages were drained by their items before the next load).
+    if (tid == 0)
+        for (uint32_t g = 0; g < (uint32_t)kCopyGroups; ++g)
+            if (last_used >> g & 1u) mbar_wait(&s_bar[g], last_parity >> g & 1u);
     push_tail(a);
 }
 

@@ -1,0 +1,104 @@
+"""Restatement of the persistent select's launch plan: ``class_dims`` and ``persist_plan`` in
+k8s-runpod-kubelet_b200/csrc/select_persist.cu, with the constants of rpk_internal.cuh, the bitmapM condition of
+``launch_offer_ingest`` (offers.cu) and the host entry point's row sub-batches (``sub_batch_rows``, rpk_api.cu).
+
+The GPU tests assert through it which regime each case reaches, so a change to a constant that moves a case off its
+regime fails the case instead of quietly testing something else."""
+from types import SimpleNamespace
+
+import numpy as np
+
+SUB_CHUNKS, SUB_STRIDE = 64, 68       # kSubChunks, kSubStride: 64 chunks of 32 offers per sub-range, 68-word rows
+MAX_CLASSES, BM_MAX_STRIDE = 4096, 64  # kMaxClasses, kBmMaxStride
+PWARPS, RPI = 16, 64                   # warps per 512-thread CTA; rows per item (32 lanes x kRpl)
+STAGE_MAX = 220 * 1024                 # persist_plan's stage cap
+FUSED_ROWS_MAX, SMALL_BATCH = 16384, 4096  # kFusedRowsMax, kSmallBatch
+SUB_BATCH_ROWS = 131072                # kSubBatchRows (x1, x2, x3, then x4)
+
+
+def cdiv(a, b):
+    return -(-a // b)
+
+
+def distinct(offers):
+    """the sorted distinct values of mem / vcpu / ram (a missing column is all zero)"""
+    G = len(offers["mem_gb"])
+    return [np.unique(offers[k]) if offers.get(k) is not None else np.zeros(min(G, 1), np.int32)
+            for k in ("mem_gb", "vcpu", "ram_gb")]
+
+
+def class_dims(D):
+    """-> (Dm1, Dv1, Dr1, use_mem, C): the mem threshold joins the class key (and bitmapM exists) when it fits"""
+    Dm1, Dv1, Dr1 = D[0] + 1, D[1] + 1, D[2] + 1
+    use_mem = 2 * Dm1 * Dv1 * Dr1 <= MAX_CLASSES
+    return Dm1, Dv1, Dr1, use_mem, 2 * Dv1 * Dr1 * (Dm1 if use_mem else 1)
+
+
+def plan(G, P, D, sm_count, stage_kb=0, items_per_warp=0, no_slice=False, k0ctas=0):
+    """persist_plan for a table of G offers with distinct counts D and a batch of P rows (RPK_TUNE stagekb / ipw /
+    k0ctas when non-zero; no_slice: RPK_FORCE_KERNEL=bitmap_price)"""
+    Dm1, Dv1, Dr1, use_mem, C = class_dims(D)
+    bm_words = Dm1 + Dv1 + Dr1
+    assert bm_words <= BM_MAX_STRIDE, "no bit-sliced view: the table takes the packed or generic kernels"
+    nsub = cdiv(cdiv(G, 32), SUB_CHUNKS)
+    slice_rows = Dv1 + Dr1 if nsub and use_mem else 0
+    max_stage = min(stage_kb if stage_kb > 0 else 220, 220) * 1024
+    slice_bytes = slice_rows * SUB_STRIDE * 4
+    sl = bool(slice_rows) and not no_slice and slice_bytes <= max_stage
+    sub_bytes = slice_bytes if sl else bm_words * SUB_STRIDE * 4
+    cap = max(max_stage // sub_bytes, 1)
+    per = cdiv(nsub, cdiv(nsub, cap))
+    S = cdiv(nsub, per)
+    visits = max(cdiv(P, RPI) * S, 1)
+    Qi = min(max(cdiv((items_per_warp if items_per_warp > 0 else 4) * sm_count * PWARPS, visits), 1), per)
+    qspan = cdiv(per, Qi)
+    tickets = sum(cdiv(min(per, nsub - s * per), qspan) for s in range(S))
+    k0 = k0ctas if k0ctas > 0 else 4 * sm_count
+    return SimpleNamespace(slice=sl, nsub=nsub, S=S, per=per, qspan=qspan, tickets_per_block=tickets,
+                           direct=tickets == 1, classes=C, smem_bytes=per * sub_bytes, grid=sm_count,
+                           k0_blocks=max(min(cdiv(P, 512), k0), 1), groups_per_cloud=Dm1 if sl else 1)
+
+
+def queues(pl, dist, pods):
+    """non-empty (row group, stage) queues of one call: a row group is the cloud, or (cloud, mem threshold) when the
+    stages are slices of bitmapM; rows of neither cloud have no group"""
+    P = len(pods["req_mem_gb"])
+    cloud = pods.get("cloud")
+    cloud = np.zeros(P, np.int64) if cloud is None else cloud.astype(np.int64)
+    keep = cloud <= 1
+    grp = cloud[keep]
+    if pl.slice:
+        grp = grp * pl.groups_per_cloud + np.searchsorted(dist[0], pods["req_mem_gb"][keep], side="left")
+    return len(np.unique(grp)) * pl.S
+
+
+def host_sub_batches(P):
+    """row counts of the host entry point's sub-batches on one GPU (sub_batch_rows); P <= SMALL_BATCH is one call"""
+    out, j = [], 0
+    while P > 0:
+        want = SUB_BATCH_ROWS * min(j + 1, 4)
+        nb = P if P < want + SUB_BATCH_ROWS // 2 else want
+        out.append(nb)
+        P -= nb
+        j += 1
+    return out
+
+
+def persistent(P, no_fused=False):
+    """a bit-sliced, non-empty table takes the persistent kernel above the fused kernel's size (or when forced)"""
+    return P > FUSED_ROWS_MAX or no_fused
+
+
+def tune_from_env(env):
+    """(stage_kb, items_per_warp, k0ctas) of an RPK_TUNE string, parsed like parse_tune (select.cu)"""
+    def num(key):
+        i = env.find(key)
+        if i < 0:
+            return 0
+        digits = ""
+        for ch in env[i + len(key):]:
+            if not ch.isdigit():
+                break
+            digits += ch
+        return int(digits or 0)
+    return num("stagekb="), num("ipw="), num("k0ctas=")
