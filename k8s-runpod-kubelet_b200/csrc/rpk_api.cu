@@ -76,14 +76,32 @@ struct ShardWorkers {
 };
 
 struct rpk_ctx {
-    std::vector<DeviceState> devs;
+    std::vector<DeviceState> devs;  // one per shard, never resized: a DeviceState is neither copied nor moved
     std::vector<PeerBinding> bind;  // per shard: flag arrays bound with rpk_peer_bind
-    ShardWorkers workers;
+    ShardWorkers workers;           // stopped (rpk_destroy) before devs is destroyed
     std::vector<std::pair<int, void*>> ipc_owned, ipc_mapped;  // (shard, ptr)
     std::string err;
     rpk_stats stats;
     uint64_t launches = 0;
+    explicit rpk_ctx(int n_gpus) : devs((size_t)n_gpus), bind((size_t)n_gpus) {}
 };
+
+rpk::DeviceState::~DeviceState() {
+    if (dev < 0 || cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); return; }  // creation failed before this GPU
+    if (stream) cudaStreamSynchronize(stream);
+    if (status_stream) cudaStreamSynchronize(status_stream);
+    for (auto& ln : lane) if (ln.stream) cudaStreamSynchronize(ln.stream);
+    for (auto& ln : lane) {
+        if (ln.done) cudaEventDestroy(ln.done);
+        if (ln.stream) cudaStreamDestroy(ln.stream);
+    }
+    for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
+    if (ev_sel) cudaEventDestroy(ev_sel);
+    if (ev_st) cudaEventDestroy(ev_st);
+    if (status_stream) cudaStreamDestroy(status_stream);
+    if (stream) cudaStreamDestroy(stream);
+    cudaGetLastError();
+}
 
 static thread_local std::string g_create_err;
 
@@ -115,7 +133,13 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
     *hi = (uint32_t)((uint64_t)total * (uint64_t)(s + 1) / (uint64_t)n);
 }
 
-void fill_offer_args(const DeviceState& ds, SelectArgs& a) {
+// The pod columns of a host select (rpk_select, rpk_tick); the optional ones are null when not passed.
+struct PodCols { const int32_t* req_mem; const int32_t* req_vcpu; const int32_t* req_ram; const double* max_price; const uint8_t* cloud; };
+
+// One select on ds in lane ln's scratch: `a` holds the pod columns, P and the outputs; this adds the offer views and the
+// scratch and launches on st.  A bit-sliced table takes the persistent kernel above the fused kernel's batch size and
+// the fused kernel otherwise (which also serves an empty table at any batch size).  Returns the kernels launched.
+int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaStream_t st) {
     for (int c = 0; c < 2; ++c) {
         a.view[c].packed = ds.v_packed[c].p; a.view[c].bitmap = ds.v_bitmap[c].p; a.view[c].bitmapT = ds.v_bitmapT[c].p;
         a.view[c].bitmapM = ds.pk.slice_rows ? ds.v_bitmapM[c].p : nullptr; a.view[c].wide = ds.v_wide[c].p;
@@ -123,13 +147,8 @@ void fill_offer_args(const DeviceState& ds, SelectArgs& a) {
     }
     a.G = ds.G; a.Gpad = ds.Gpad; a.pk = ds.pk; a.nsub = ds.nsub;
     for (int d = 0; d < 3; ++d) { a.distinct[d] = ds.distinct[d].p; a.D[d] = ds.D[d]; }
-}
-
-// scratch for one select over P rows on ds (in lane ln); returns rows-per-warp of the packed / wide kernels (0 on a
-// bit-sliced table).  *use_persist: the batch takes the persistent bit-sliced kernel (plan in *pl); a bit-sliced table
-// otherwise takes the fused kernel, which also serves an empty table at any batch size.
-int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, SelectArgs& a, PersistPlan* pl, bool* use_persist) {
-    const int R = ds.pk.bm_words ? 0 : pick_rows_per_warp(P, ds.sm_count);
+    const uint32_t P = a.P;
+    const int R = ds.pk.bm_words ? 0 : pick_rows_per_warp(P, ds.sm_count);  // rows per warp of the packed / wide kernels
     const uint32_t tiles = R ? select_tiles_max(P, R) : 0u;
     ln.rw.reserve(P); ln.order.reserve((size_t)kGroups * P); ln.pos.reserve(P);
     // worst case (1 row per warp; the persistent kernel's row blocks: one partial block per row group): never regrown mid-pipeline
@@ -143,12 +162,12 @@ int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, S
     }
     a.rw = ln.rw.p; a.order = ln.order.p; a.pos = ln.pos.p;
     a.counts = ln.ctrs.p; a.done = ln.ctrs.p + kGroups; a.tile_ctr = ln.ctrs.p + 2 * kGroups;
-    a.P = P;
-    *use_persist = ds.pk.bm_words && ds.nsub && (P > kFusedRowsMax || ds.pk.no_fused);
-    if (*use_persist) {
-        *pl = persist_plan(a, ds.sm_count);
+    const bool persist = ds.pk.bm_words && ds.nsub && (P > kFusedRowsMax || ds.pk.no_fused);
+    PersistPlan pl;
+    if (persist) {
+        pl = persist_plan(a, ds.sm_count);
         ln.key.reserve(P); ln.ord_rw.reserve(P);
-        const size_t hdr_words = persist_hdr_words(*pl);
+        const size_t hdr_words = persist_hdr_words(pl);
         const bool fresh = !ln.hist.p || hdr_words > ln.hdr.cap;
         ln.hist.reserve(2 * kMaxClasses); ln.cursor.reserve(2 * kMaxClasses); ln.hdr.reserve(hdr_words);
         if (fresh || ln.persist_dirty) {  // zero between calls by construction (k_pod_classify's last block, the pushers)
@@ -160,7 +179,16 @@ int prepare_select_scratch(DeviceState& ds, DeviceState::Lane& ln, uint32_t P, S
         }
         a.key = ln.key.p; a.ord_rw = ln.ord_rw.p; a.hist = ln.hist.p; a.cursor = ln.cursor.p; a.hdr = ln.hdr.p;
     }
-    return R;
+    // the lane's counters are suspect until every launch of the call was accepted
+    ln.ctrs_dirty = true; ln.persist_dirty = true;
+    const int n = launch_select(a, R, persist ? &pl : nullptr, st);
+    ln.ctrs_dirty = false; ln.persist_dirty = false;
+    return n;
+}
+
+void count_select(rpk_ctx* ctx, uint32_t P, uint32_t G) {
+    ctx->stats.select_calls += 1;
+    ctx->stats.offer_scores += (uint64_t)P * G;
 }
 
 // The device entry points of a shard share ctx-owned scratch (tickets, queue cursors, look-back state).  Calls on ONE
@@ -184,8 +212,6 @@ struct ScratchGuard {
 };
 
 void bind_flags(const rpk_ctx* ctx, int shard, SelectArgs& a) {
-    a.n_flags = 0; a.my_rank = 0;
-    if ((size_t)shard >= ctx->bind.size()) return;
     const PeerBinding& b = ctx->bind[(size_t)shard];
     for (int r = 0; r < b.n; ++r) a.flags[r] = b.flags[r];
     a.n_flags = b.n; a.my_rank = b.my_rank; a.inline_wait = b.inline_wait;
@@ -210,14 +236,6 @@ int find_local_vector(const rpk_ctx* ctx, int shard, int dev, int n_out, int32_t
     return -1;
 }
 
-// launch_select with the lane's counters marked suspect until every launch of the call was accepted
-int run_select(DeviceState::Lane& ln, const SelectArgs& a, int R, const PersistPlan* pl, cudaStream_t st) {
-    ln.ctrs_dirty = true; ln.persist_dirty = true;
-    const int n = launch_select(a, R, pl, st);
-    ln.ctrs_dirty = false; ln.persist_dirty = false;
-    return n;
-}
-
 // Row sub-batches of the host entry point.  The first one is small, so that the first kernel starts after ~3 MB of
 // H2D; the following ones grow (128k, 256k, 384k, 512k, 512k ... rows), because every select call pays a fixed cost
 // (class sort, stage load, queue tail) that eight equal sub-batches paid eight times: with growing sizes each kernel
@@ -235,43 +253,38 @@ inline uint32_t sub_batch_cap(uint32_t Ps) {  // largest sub-batch a shard of Ps
 }
 
 // Latency path of the host entry point (micro-batches, one GPU): the five pod columns are packed into one
-// pinned block -> ONE H2D; best and top5 come back in ONE D2H; one stream synchronise.  Same kernels.
-int select_small(rpk_ctx* ctx, DeviceState& ds, uint32_t P, const int32_t* req_mem_gb, const int32_t* req_vcpu,
-                 const int32_t* req_ram_gb, const double* max_price, const uint8_t* cloud, int32_t* best, int32_t* top5,
-                 uint64_t* launches) {
-    (void)ctx;
+// pinned block -> ONE H2D; best and top5 come back in ONE D2H; one stream synchronise.  Same kernels.  Returns the
+// kernels launched.
+int select_small(DeviceState& ds, uint32_t P, const PodCols& pods, int32_t* best, int32_t* top5) {
     RPK_CUDA(cudaSetDevice(ds.dev));
     const size_t in_cap = (size_t)kSmallBatch * 24, out_cap = (size_t)kSmallBatch * 6 * 4;
-    if (!ds.h_small) RPK_CUDA(cudaHostAlloc((void**)&ds.h_small, in_cap + out_cap, cudaHostAllocPortable));
+    ds.h_small.reserve(in_cap + out_cap);
     ds.d_small_in.reserve(in_cap); ds.d_small_out.reserve((size_t)kSmallBatch * 6);
     const size_t o_mem = 0, o_vcpu = (size_t)P * 4, o_ram = (size_t)P * 8, o_price = ((size_t)P * 12 + 7) & ~(size_t)7,
                  o_cloud = o_price + (size_t)P * 8, total = o_cloud + P;
-    unsigned char* h = ds.h_small;
-    memcpy(h + o_mem, req_mem_gb, (size_t)P * 4);
-    if (req_vcpu) memcpy(h + o_vcpu, req_vcpu, (size_t)P * 4);
-    if (req_ram_gb) memcpy(h + o_ram, req_ram_gb, (size_t)P * 4);
-    if (max_price) memcpy(h + o_price, max_price, (size_t)P * 8);
-    if (cloud) memcpy(h + o_cloud, cloud, P);
+    unsigned char* h = ds.h_small.h;
+    memcpy(h + o_mem, pods.req_mem, (size_t)P * 4);
+    if (pods.req_vcpu) memcpy(h + o_vcpu, pods.req_vcpu, (size_t)P * 4);
+    if (pods.req_ram) memcpy(h + o_ram, pods.req_ram, (size_t)P * 4);
+    if (pods.max_price) memcpy(h + o_price, pods.max_price, (size_t)P * 8);
+    if (pods.cloud) memcpy(h + o_cloud, pods.cloud, P);
     DeviceState::Lane& ln = ds.lane[0];
     cudaStream_t st = ln.stream;
     unsigned char* d = ds.d_small_in.p;
     RPK_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, st));
     SelectArgs a{};
-    a.req_mem = (const int32_t*)(d + o_mem); a.req_vcpu = req_vcpu ? (const int32_t*)(d + o_vcpu) : nullptr;
-    a.req_ram = req_ram_gb ? (const int32_t*)(d + o_ram) : nullptr; a.max_price = max_price ? (const double*)(d + o_price) : nullptr;
-    a.cloud = cloud ? (const uint8_t*)(d + o_cloud) : nullptr;
+    a.req_mem = (const int32_t*)(d + o_mem); a.req_vcpu = pods.req_vcpu ? (const int32_t*)(d + o_vcpu) : nullptr;
+    a.req_ram = pods.req_ram ? (const int32_t*)(d + o_ram) : nullptr; a.max_price = pods.max_price ? (const double*)(d + o_price) : nullptr;
+    a.cloud = pods.cloud ? (const uint8_t*)(d + o_cloud) : nullptr;
     a.P = P;
-    fill_offer_args(ds, a);
-    PersistPlan pl; bool persist = false;
-    const int R = prepare_select_scratch(ds, ln, P, a, &pl, &persist);
     a.best_out[0] = ds.d_small_out.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = top5 ? ds.d_small_out.p + P : nullptr;
-    *launches += (uint64_t)run_select(ln, a, R, persist ? &pl : nullptr, st);
-    int32_t* hout = (int32_t*)(ds.h_small + in_cap);
+    const int launches = enqueue_select(ds, ln, a, st);
+    int32_t* hout = (int32_t*)(h + in_cap);
     RPK_CUDA(cudaMemcpyAsync(hout, ds.d_small_out.p, (size_t)P * 4 * (top5 ? 6 : 1), cudaMemcpyDeviceToHost, st));
     RPK_CUDA(cudaStreamSynchronize(st));
     memcpy(best, hout, (size_t)P * 4);
     if (top5) memcpy(top5, hout + P, (size_t)P * 4 * RPK_TOPK);
-    return RPK_OK;
+    return launches;
 }
 
 bool has_int32_max(const int32_t* col, uint32_t n) {
@@ -284,7 +297,7 @@ bool has_int32_max(const int32_t* col, uint32_t n) {
 // Buffers of the pipelined host select, sized from the calling thread (peers write into each other's best_full, so
 // every GPU's vector must exist before any shard is enqueued).  After the first call of a size this only compares
 // capacities.
-void reserve_select(rpk_ctx* ctx, uint32_t P, bool vcpu, bool ram, bool price, bool cloud, bool top5) {
+void reserve_select(rpk_ctx* ctx, uint32_t P, const PodCols& pods, bool top5) {
     const int n = (int)ctx->devs.size();
     for (int s = 0; s < n; ++s) {
         DeviceState& ds = ctx->devs[(size_t)s];
@@ -293,8 +306,9 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, bool vcpu, bool ram, bool price, b
         const uint32_t cap = sub_batch_cap(Ps);
         bool grow = P > ds.best_full.cap;
         for (auto& ln : ds.lane) {
-            grow = grow || cap > ln.p_req_mem.cap || (vcpu && cap > ln.p_req_vcpu.cap) || (ram && cap > ln.p_req_ram.cap) ||
-                   (price && cap > ln.p_max_price.cap) || (cloud && cap > ln.p_cloud.cap) || (top5 && (size_t)cap * RPK_TOPK > ln.top5.cap);
+            grow = grow || cap > ln.p_req_mem.cap || (pods.req_vcpu && cap > ln.p_req_vcpu.cap) || (pods.req_ram && cap > ln.p_req_ram.cap) ||
+                   (pods.max_price && cap > ln.p_max_price.cap) || (pods.cloud && cap > ln.p_cloud.cap) ||
+                   (top5 && (size_t)cap * RPK_TOPK > ln.top5.cap);
             if (cap == Ps) break;  // a single sub-batch uses lane 0 only
         }
         if (!grow) continue;
@@ -302,21 +316,20 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, bool vcpu, bool ram, bool price, b
         ds.best_full.reserve(P);
         for (auto& ln : ds.lane) {
             ln.p_req_mem.reserve(cap);
-            if (vcpu) ln.p_req_vcpu.reserve(cap);
-            if (ram) ln.p_req_ram.reserve(cap);
-            if (price) ln.p_max_price.reserve(cap);
-            if (cloud) ln.p_cloud.reserve(cap);
+            if (pods.req_vcpu) ln.p_req_vcpu.reserve(cap);
+            if (pods.req_ram) ln.p_req_ram.reserve(cap);
+            if (pods.max_price) ln.p_max_price.reserve(cap);
+            if (pods.cloud) ln.p_cloud.reserve(cap);
             if (top5) ln.top5.reserve((size_t)cap * RPK_TOPK);
             if (cap == Ps) break;
         }
     }
 }
 
-// One shard's half of the host select: row sub-batches alternate between two lanes; within a lane everything is stream
+// One shard's half of the host select: row sub-batches rotate over the lanes; within a lane everything is stream
 // ordered (H2D -> kernels -> D2H), across lanes copies and kernels overlap.  ds.ev[0] / ds.ev[3] bracket it on ds.stream;
 // the caller synchronises ds.stream.
-void enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const int32_t* req_mem_gb, const int32_t* req_vcpu, const int32_t* req_ram_gb,
-                          const double* max_price, const uint8_t* cloud, int32_t* best, int32_t* top5, uint64_t* launches) {
+void enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodCols& pods, int32_t* best, int32_t* top5, uint64_t* launches) {
     const int n = (int)ctx->devs.size();
     DeviceState& ds = ctx->devs[(size_t)s];
     uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
@@ -328,22 +341,21 @@ void enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const int32_t* req_me
         nb = sub_batch_rows(j, hi - b0);
         DeviceState::Lane& ln = ds.lane[j % DeviceState::kLanes];
         cudaStream_t st = ln.stream;
-        RPK_CUDA(cudaMemcpyAsync(ln.p_req_mem.p, req_mem_gb + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
-        if (req_vcpu) RPK_CUDA(cudaMemcpyAsync(ln.p_req_vcpu.p, req_vcpu + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
-        if (req_ram_gb) RPK_CUDA(cudaMemcpyAsync(ln.p_req_ram.p, req_ram_gb + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
-        if (max_price) RPK_CUDA(cudaMemcpyAsync(ln.p_max_price.p, max_price + b0, (size_t)nb * 8, cudaMemcpyHostToDevice, st));
-        if (cloud) RPK_CUDA(cudaMemcpyAsync(ln.p_cloud.p, cloud + b0, (size_t)nb, cudaMemcpyHostToDevice, st));
+        // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
+        auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
+            if (!col) return nullptr;
+            RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
+            return buf.p;
+        };
         SelectArgs a{};
-        a.req_mem = ln.p_req_mem.p; a.req_vcpu = req_vcpu ? ln.p_req_vcpu.p : nullptr; a.req_ram = req_ram_gb ? ln.p_req_ram.p : nullptr;
-        a.max_price = max_price ? ln.p_max_price.p : nullptr; a.cloud = cloud ? ln.p_cloud.p : nullptr;
+        a.req_mem = upload(ln.p_req_mem, pods.req_mem); a.req_vcpu = upload(ln.p_req_vcpu, pods.req_vcpu);
+        a.req_ram = upload(ln.p_req_ram, pods.req_ram); a.max_price = upload(ln.p_max_price, pods.max_price);
+        a.cloud = upload(ln.p_cloud, pods.cloud);
         a.P = nb;
-        fill_offer_args(ds, a);
-        PersistPlan pl; bool persist = false;
-        const int R = prepare_select_scratch(ds, ln, nb, a, &pl, &persist);
         for (int o = 0; o < n; ++o) a.best_out[o] = ctx->devs[(size_t)o].best_full.p;
         a.n_out = n; a.row0 = b0; a.top5 = top5 ? ln.top5.p : nullptr;
         a.self_out = s;  // own vector; finished push blocks / sub-batches are forwarded to the peers
-        *launches += (uint64_t)run_select(ln, a, R, persist ? &pl : nullptr, st);
+        *launches += (uint64_t)enqueue_select(ds, ln, a, st);
         RPK_CUDA(cudaMemcpyAsync(best + b0, ds.best_full.p + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, st));
         if (top5) RPK_CUDA(cudaMemcpyAsync(top5 + (size_t)b0 * RPK_TOPK, ln.top5.p, (size_t)nb * RPK_TOPK * 4, cudaMemcpyDeviceToHost, st));
     }
@@ -379,11 +391,10 @@ int rpk_create(int n_gpus, const int* device_ids, rpk_ctx** out) {
         cudaGetLastError();
         return fail(nullptr, RPK_ENODEV, std::string("rpk_create: no CUDA device (") + cudaGetErrorString(e) + "); there is no CPU fallback");
     }
-    rpk_ctx* ctx = new (std::nothrow) rpk_ctx();
-    if (!ctx) return fail(nullptr, RPK_ENOMEM, "rpk_create: host allocation failed");
+    rpk_ctx* ctx = nullptr;
+    try { ctx = new rpk_ctx(n_gpus); } catch (const std::bad_alloc&) { return fail(nullptr, RPK_ENOMEM, "rpk_create: host allocation failed"); }
     memset(&ctx->stats, 0, sizeof(ctx->stats));
     int rc = guarded(nullptr, [&]() -> int {
-        ctx->devs.resize((size_t)n_gpus);
         for (int i = 0; i < n_gpus; ++i) {
             const int dev = device_ids ? device_ids[i] : i;
             if (dev < 0 || dev >= count) return fail(nullptr, RPK_EINVAL, "rpk_create: device id out of range");
@@ -438,35 +449,8 @@ void rpk_destroy(rpk_ctx* ctx) {
     ctx->workers.stop();
     for (auto& m : ctx->ipc_mapped) if (cudaSetDevice(ctx->devs[(size_t)m.first].dev) == cudaSuccess) cudaIpcCloseMemHandle(m.second);
     for (auto& m : ctx->ipc_owned) if (cudaSetDevice(ctx->devs[(size_t)m.first].dev) == cudaSuccess) { cudaDeviceSynchronize(); cudaFree(m.second); }
+    delete ctx;  // every DeviceState synchronises its streams and frees what it holds
     cudaGetLastError();
-    for (auto& ds : ctx->devs) {
-        if (ds.dev < 0) continue;
-        if (cudaSetDevice(ds.dev) != cudaSuccess) { cudaGetLastError(); continue; }
-        if (ds.stream) cudaStreamSynchronize(ds.stream);
-        ds.raw_mem.release(); ds.raw_vcpu.release(); ds.raw_ram.release(); ds.raw_sp.release(); ds.raw_cp.release(); ds.raw_flags.release();
-        ds.sort_keys.release(); ds.sort_vals.release();
-        for (int c = 0; c < 2; ++c) { ds.v_bitmap[c].release(); ds.v_packed[c].release(); ds.v_wide[c].release(); ds.v_price[c].release(); ds.v_perm[c].release(); }
-        for (int d = 0; d < 3; ++d) ds.distinct[d].release();
-        ds.dcount.release();
-        for (auto& ln : ds.lane) {
-            if (ln.stream) cudaStreamSynchronize(ln.stream);
-            ln.release();
-            if (ln.done) cudaEventDestroy(ln.done);
-            if (ln.stream) cudaStreamDestroy(ln.stream);
-        }
-        ds.best_full.release(); ds.d_small_in.release(); ds.d_small_out.release();
-        if (ds.h_small) { cudaFreeHost(ds.h_small); ds.h_small = nullptr; }
-        ds.s_records.release(); ds.s_hash_prev.release(); ds.s_hash_out.release(); ds.s_changed.release(); ds.s_misc.release(); ds.s_tile_state.release(); ds.s_stage_idx.release();
-        ds.s_stage_code.release(); ds.s_unit_cnt.release(); ds.s_seed_slots.release(); ds.s_seed_recs.release();
-        if (ds.h_changed) { cudaFreeHost(ds.h_changed); ds.h_changed = nullptr; }
-        if (ds.status_stream) { cudaStreamSynchronize(ds.status_stream); cudaStreamDestroy(ds.status_stream); }
-        for (auto& ev : ds.ev) if (ev) cudaEventDestroy(ev);
-        if (ds.ev_sel) cudaEventDestroy(ds.ev_sel);
-        if (ds.ev_st) cudaEventDestroy(ds.ev_st);
-        if (ds.stream) cudaStreamDestroy(ds.stream);
-        cudaGetLastError();
-    }
-    delete ctx;
 }
 
 int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu, const int32_t* ram_gb,
@@ -528,19 +512,15 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
         SelectArgs a{};
         a.req_mem = d_req_mem_gb; a.req_vcpu = d_req_vcpu; a.req_ram = d_req_ram_gb; a.max_price = d_max_price; a.cloud = d_cloud;
         a.P = P;
-        fill_offer_args(ds, a);
-        PersistPlan pl; bool persist = false;
-        const int R = prepare_select_scratch(ds, ds.lane[0], P, a, &pl, &persist);
         for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
         a.n_out = n_out; a.row0 = row0; a.top5 = d_top5;
         a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
         if (n_out > 1) bind_flags(ctx, shard, a);
         cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
         ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);
-        ctx->launches += (uint64_t)run_select(ds.lane[0], a, R, persist ? &pl : nullptr, st);
+        ctx->launches += (uint64_t)enqueue_select(ds, ds.lane[0], a, st);
         guard.done();
-        ctx->stats.select_calls += 1;
-        ctx->stats.offer_scores += (uint64_t)P * ds.G;
+        count_select(ctx, P, ds.G);
         return RPK_OK;
     });
 }
@@ -559,29 +539,26 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
     if (!req_mem_gb || !best) return fail(ctx, RPK_EINVAL, "rpk_select: req_mem_gb and best are required");
     for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
     return guarded(ctx, [&]() -> int {
+        const PodCols pods{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud};
         const int n = (int)ctx->devs.size();
-        if (n == 1 && P <= kSmallBatch) {
-            int rc = select_small(ctx, ctx->devs[0], P, req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud, best, top5, &ctx->launches);
-            ctx->stats.last_select_kernel_ms = 0.f; ctx->stats.last_select_total_ms = 0.f;
-            ctx->stats.select_calls += 1;
-            ctx->stats.offer_scores += (uint64_t)P * ctx->devs[0].G;
-            return rc;
-        }
-        std::vector<uint64_t> launches((size_t)n, 0);
-        std::vector<float> ms((size_t)n, 0.f);
-        reserve_select(ctx, P, req_vcpu != nullptr, req_ram_gb != nullptr, max_price != nullptr, cloud != nullptr, top5 != nullptr);
-        ctx->workers.run(n, [&](int s) {
-            enqueue_select_shard(ctx, s, P, req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud, best, top5, &launches[(size_t)s]);
-            DeviceState& ds = ctx->devs[(size_t)s];
-            RPK_CUDA(cudaStreamSynchronize(ds.stream));
-            RPK_CUDA(cudaEventElapsedTime(&ms[(size_t)s], ds.ev[0], ds.ev[3]));
-        });
         float tmax = 0.f;
-        for (int s = 0; s < n; ++s) { ctx->launches += launches[(size_t)s]; tmax = ms[(size_t)s] > tmax ? ms[(size_t)s] : tmax; }
+        if (n == 1 && P <= kSmallBatch) {
+            ctx->launches += (uint64_t)select_small(ctx->devs[0], P, pods, best, top5);
+        } else {
+            std::vector<uint64_t> launches((size_t)n, 0);
+            std::vector<float> ms((size_t)n, 0.f);
+            reserve_select(ctx, P, pods, top5 != nullptr);
+            ctx->workers.run(n, [&](int s) {
+                enqueue_select_shard(ctx, s, P, pods, best, top5, &launches[(size_t)s]);
+                DeviceState& ds = ctx->devs[(size_t)s];
+                RPK_CUDA(cudaStreamSynchronize(ds.stream));
+                RPK_CUDA(cudaEventElapsedTime(&ms[(size_t)s], ds.ev[0], ds.ev[3]));
+            });
+            for (int s = 0; s < n; ++s) { ctx->launches += launches[(size_t)s]; tmax = ms[(size_t)s] > tmax ? ms[(size_t)s] : tmax; }
+        }
         ctx->stats.last_select_kernel_ms = 0.f;  // copies and kernels overlap in the pipelined host path: only the total is meaningful
-        ctx->stats.last_select_total_ms = tmax;
-        ctx->stats.select_calls += 1;
-        ctx->stats.offer_scores += (uint64_t)P * ctx->devs[0].G;
+        ctx->stats.last_select_total_ms = tmax;  // 0 on the single-copy path
+        count_select(ctx, P, ctx->devs[0].G);
         return RPK_OK;
     });
 }
@@ -669,7 +646,6 @@ int rpk_peer_bind(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int 
     if (shard < 0 || (size_t)shard >= ctx->devs.size() || n < 0 || n > RPK_MAX_GPUS || (n > 0 && (!d_flags || my_rank < 0 || my_rank >= n)))
         return fail(ctx, RPK_EINVAL, "rpk_peer_bind: bad argument");
     for (int r = 0; r < n; ++r) if (!d_flags[r]) return fail(ctx, RPK_EINVAL, "rpk_peer_bind: NULL flag array");
-    if (ctx->bind.size() < ctx->devs.size()) ctx->bind.resize(ctx->devs.size());
     PeerBinding& b = ctx->bind[(size_t)shard];
     const int keep = b.inline_wait;
     b = PeerBinding{};
@@ -681,7 +657,6 @@ int rpk_peer_bind(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int 
 int rpk_peer_inline_wait(rpk_ctx* ctx, int shard, int on) {
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_peer_inline_wait: shard out of range");
-    if (ctx->bind.size() < ctx->devs.size()) ctx->bind.resize(ctx->devs.size());
     ctx->bind[(size_t)shard].inline_wait = on ? 1 : 0;
     return RPK_OK;
 }
@@ -689,7 +664,7 @@ int rpk_peer_inline_wait(rpk_ctx* ctx, int shard, int on) {
 int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream) {
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size() || (what & ~3u) || !what) return fail(ctx, RPK_EINVAL, "rpk_peer_wait: bad argument");
-    if ((size_t)shard >= ctx->bind.size() || ctx->bind[(size_t)shard].n == 0) return fail(ctx, RPK_ESTATE, "rpk_peer_wait: no flags bound (rpk_peer_bind)");
+    if (ctx->bind[(size_t)shard].n == 0) return fail(ctx, RPK_ESTATE, "rpk_peer_wait: no flags bound (rpk_peer_bind)");
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
@@ -734,9 +709,12 @@ int rpk_status_reset(rpk_ctx* ctx, uint32_t N) {
 
 namespace {
 
-// look-back state / tickets of the status kernels: zero between calls by construction; zeroed here when (re)allocated
-void reserve_status_state(DeviceState& ds, uint32_t N, uint32_t stride) {
-    const size_t need = status_state_words(N, stride, ds.sm_count);
+// Scratch of a sweep over N records (or list entries) on ds: the look-back state and tickets -- zero between calls by
+// construction, zeroed here when (re)allocated -- and the per-warp index stage, its code stage (`codes`) and the
+// per-unit counts.
+void reserve_sweep_scratch(DeviceState& ds, uint32_t N, uint32_t stride, bool codes) {
+    const uint32_t cap = N ? N : 1;
+    const size_t need = status_state_words(cap, stride, ds.sm_count);
     if (need > ds.s_tile_state.cap || !ds.s_misc.p || ds.status_dirty) {
         ds.s_tile_state.reserve(need);
         ds.s_misc.reserve(64);
@@ -745,6 +723,14 @@ void reserve_status_state(DeviceState& ds, uint32_t N, uint32_t stride) {
         RPK_CUDA(cudaDeviceSynchronize());
         ds.status_dirty = false;
     }
+    ds.s_stage_idx.reserve(cap + 64); ds.s_unit_cnt.reserve(cap / 32 + 2);
+    if (codes) ds.s_stage_code.reserve(cap + 64);
+}
+
+// the StatusArgs fields of the scratch reserve_sweep_scratch sized
+void sweep_scratch_args(const DeviceState& ds, bool codes, StatusArgs& a) {
+    a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
+    a.stage_idx = ds.s_stage_idx.p; a.stage_code = codes ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
 }
 
 struct StatusHostArgs {
@@ -778,49 +764,39 @@ void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
     RPK_CUDA(cudaSetDevice(ds.dev));
     ds.s_records.reserve((size_t)cap * h.stride);
     if (h.slots) ds.s_seed_slots.reserve(cap);
-    ds.s_stage_idx.reserve(cap + 64); ds.s_unit_cnt.reserve(cap / 32 + 2);
-    if (h.changed_code) ds.s_stage_code.reserve(cap + 64);
     if (h.hashes_out) ds.s_hash_out.reserve(cap);
-    reserve_status_state(ds, cap, h.stride);
-    const size_t need = h.report ? (size_t)cap * (h.changed_code ? 6 : 4) + 64 : 64;
-    if (need > ds.h_changed_cap) {
-        if (ds.h_changed) RPK_CUDA(cudaFreeHost(ds.h_changed));
-        ds.h_changed = nullptr; ds.h_changed_cap = 0;
-        const size_t want = need + need / 4;
-        RPK_CUDA(cudaHostAlloc((void**)&ds.h_changed, want, cudaHostAllocMapped | cudaHostAllocPortable));
-        RPK_CUDA(cudaHostGetDevicePointer((void**)&ds.d_changed_map, ds.h_changed, 0));
-        ds.h_changed_cap = want;
-    }
+    reserve_sweep_scratch(ds, Ns, h.stride, h.changed_code != nullptr);
+    ds.h_changed.reserve(h.report ? (size_t)cap * (h.changed_code ? 6 : 4) + 64 : 64);
 }
 
-// One shard's half of a host sweep, enqueued on ds.stream (ds.ev[0..2] bracket copy and kernel); the caller synchronises.
-void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint64_t* launches) {
+// One shard's half of a host sweep, enqueued on st (ds.ev[0..2] bracket copy and kernel); the caller synchronises.
+void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, cudaStream_t st, uint64_t* launches) {
     DeviceState& ds = ctx->devs[(size_t)s];
     const ShardPart sp = shard_part(ctx, s, h);
     const uint32_t lo = sp.lo, Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
     RPK_CUDA(cudaSetDevice(ds.dev));
-    RPK_CUDA(cudaEventRecord(ds.ev[0], ds.stream));
-    if (Ns) RPK_CUDA(cudaMemcpyAsync(ds.s_records.p, h.records + (size_t)sp.p0 * h.stride, (size_t)Ns * h.stride, cudaMemcpyHostToDevice, ds.stream));
-    if (Ns && h.slots) RPK_CUDA(cudaMemcpyAsync(ds.s_seed_slots.p, h.slots + sp.p0, (size_t)Ns * 4, cudaMemcpyHostToDevice, ds.stream));
-    RPK_CUDA(cudaEventRecord(ds.ev[1], ds.stream));
+    RPK_CUDA(cudaEventRecord(ds.ev[0], st));
+    if (Ns) RPK_CUDA(cudaMemcpyAsync(ds.s_records.p, h.records + (size_t)sp.p0 * h.stride, (size_t)Ns * h.stride, cudaMemcpyHostToDevice, st));
+    if (Ns && h.slots) RPK_CUDA(cudaMemcpyAsync(ds.s_seed_slots.p, h.slots + sp.p0, (size_t)Ns * 4, cudaMemcpyHostToDevice, st));
+    RPK_CUDA(cudaEventRecord(ds.ev[1], st));
     // mapped block: [count : 64 bytes][indices : cap u32][codes : cap u16]
-    uint32_t* m_count = reinterpret_cast<uint32_t*>(ds.d_changed_map);
-    uint32_t* m_idx = reinterpret_cast<uint32_t*>(ds.d_changed_map + 64);
-    uint16_t* m_code = reinterpret_cast<uint16_t*>(ds.d_changed_map + 64 + (size_t)cap * 4);
-    *reinterpret_cast<volatile uint32_t*>(ds.h_changed) = 0u;
+    uint32_t* m_count = reinterpret_cast<uint32_t*>(ds.h_changed.d);
+    uint32_t* m_idx = reinterpret_cast<uint32_t*>(ds.h_changed.d + 64);
+    uint16_t* m_code = reinterpret_cast<uint16_t*>(ds.h_changed.d + 64 + (size_t)cap * 4);
+    *reinterpret_cast<volatile uint32_t*>(ds.h_changed.h) = 0u;
     StatusArgs a{};
     a.records = ds.s_records.p; a.stride = h.stride; a.N = Ns; a.hash_prev = ds.s_hash_prev.p;
     a.hash_out = h.hashes_out ? ds.s_hash_out.p : nullptr;
     a.changed_idx = h.report ? m_idx : nullptr; a.n_changed = h.report ? m_count : nullptr;
     a.changed_code = h.report && h.changed_code ? m_code : nullptr;
-    a.idx_base = lo; a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
-    a.stage_idx = ds.s_stage_idx.p; a.stage_code = h.changed_code ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
+    a.idx_base = lo;
+    sweep_scratch_args(ds, h.changed_code != nullptr, a);
     if (h.slots) { a.slots = ds.s_seed_slots.p; a.col_n = sp.hi - sp.lo; }
     ds.status_dirty = true;
-    if (Ns) *launches += (uint64_t)launch_status_diff(a, ds.stream);
+    if (Ns) *launches += (uint64_t)launch_status_diff(a, st);
     ds.status_dirty = false;
-    RPK_CUDA(cudaEventRecord(ds.ev[2], ds.stream));
-    if (h.hashes_out && Ns) RPK_CUDA(cudaMemcpyAsync(h.hashes_out + lo, ds.s_hash_out.p, (size_t)Ns * 8, cudaMemcpyDeviceToHost, ds.stream));
+    RPK_CUDA(cudaEventRecord(ds.ev[2], st));
+    if (h.hashes_out && Ns) RPK_CUDA(cudaMemcpyAsync(h.hashes_out + lo, ds.s_hash_out.p, (size_t)Ns * 8, cudaMemcpyDeviceToHost, st));
 }
 
 // after the shard's stream has been synchronised: this shard's part of the caller's arrays (ascending over shards)
@@ -829,22 +805,22 @@ uint32_t collect_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint
     const ShardPart sp = shard_part(ctx, s, h);
     const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
     if (!h.report || !Ns) return 0;
-    const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(ds.h_changed);
-    memcpy(h.changed_idx + out_at, ds.h_changed + 64, (size_t)cnt * 4);
-    if (h.changed_code) memcpy(h.changed_code + out_at, ds.h_changed + 64 + (size_t)cap * 4, (size_t)cnt * 2);
+    const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(ds.h_changed.h);
+    memcpy(h.changed_idx + out_at, ds.h_changed.h + 64, (size_t)cnt * 4);
+    if (h.changed_code) memcpy(h.changed_code + out_at, ds.h_changed.h + 64 + (size_t)cap * 4, (size_t)cnt * 2);
     return cnt;
 }
 
-int run_status_host(rpk_ctx* ctx, const StatusHostArgs& h);
-
-int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
-    if (!ctx) return RPK_EINVAL;
+// The argument checks of a whole-table host sweep (rpk_status_diff*, rpk_status_seed, rpk_tick; `who` names the entry
+// point in the messages).  The first sweep of a ctx sizes the tracked table to its N.
+int check_sweep(rpk_ctx* ctx, const StatusHostArgs& h, const char* who) {
+    const std::string w(who);
     if (int rc = check_stride(ctx, h.stride)) return rc;
-    if (h.N > 0 && !h.records) return fail(ctx, RPK_EINVAL, "rpk_status_diff: records is NULL");
-    if (h.report && (!h.n_changed || (h.N > 0 && !h.changed_idx))) return fail(ctx, RPK_EINVAL, "rpk_status_diff: changed_idx and n_changed are required");
+    if (h.N > 0 && !h.records) return fail(ctx, RPK_EINVAL, w + ": records is NULL");
+    if (h.report && (!h.n_changed || (h.N > 0 && !h.changed_idx))) return fail(ctx, RPK_EINVAL, w + ": changed_idx and n_changed are required");
     if (!ctx->devs[0].status_sized) { if (int rc = rpk_status_reset(ctx, h.N)) return rc; }
-    if (ctx->devs[0].statusN != h.N) return fail(ctx, RPK_ESTATE, "rpk_status_diff: N differs from the tracked table (call rpk_status_reset to resize)");
-    return run_status_host(ctx, h);
+    if (ctx->devs[0].statusN != h.N) return fail(ctx, RPK_ESTATE, w + ": N differs from the tracked table (call rpk_status_reset to resize)");
+    return RPK_OK;
 }
 
 // a host sweep whose arguments have been checked: every shard uploads its part, sweeps it and synchronises once
@@ -855,8 +831,8 @@ int run_status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
         std::vector<uint64_t> launches((size_t)n, 0);
         std::vector<float> km((size_t)n, 0.f), tm((size_t)n, 0.f);
         ctx->workers.run(n, [&](int s) {
-            enqueue_status_shard(ctx, s, h, &launches[(size_t)s]);
             DeviceState& ds = ctx->devs[(size_t)s];
+            enqueue_status_shard(ctx, s, h, ds.stream, &launches[(size_t)s]);
             RPK_CUDA(cudaEventRecord(ds.ev[3], ds.stream));
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
             RPK_CUDA(cudaEventElapsedTime(&km[(size_t)s], ds.ev[1], ds.ev[2]));
@@ -874,6 +850,12 @@ int run_status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
         ctx->stats.status_calls += 1; ctx->stats.status_records += h.slots ? h.n_slots : h.N;
         return RPK_OK;
     });
+}
+
+int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
+    if (!ctx) return RPK_EINVAL;
+    if (int rc = check_sweep(ctx, h, "rpk_status_diff")) return rc;
+    return run_status_host(ctx, h);
 }
 
 }  // namespace
@@ -945,29 +927,23 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
              const double* max_price, const uint8_t* cloud, int32_t* best, int32_t* top5, uint32_t N, const uint8_t* records,
              uint32_t stride, uint32_t* changed_idx, uint16_t* changed_code, uint32_t* n_changed) {
     if (!ctx) return RPK_EINVAL;
-    const StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
-    if (int rc = check_stride(ctx, stride)) return rc;
     if (P > 0 && (!req_mem_gb || !best)) return fail(ctx, RPK_EINVAL, "rpk_tick: req_mem_gb and best are required");
-    if (N > 0 && !records) return fail(ctx, RPK_EINVAL, "rpk_tick: records is NULL");
-    if (!n_changed || (N > 0 && !changed_idx)) return fail(ctx, RPK_EINVAL, "rpk_tick: changed_idx and n_changed are required");
     if (P > 0) for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_tick: no offer table uploaded (call rpk_offers_upload first)");
-    if (!ctx->devs[0].status_sized) { if (int rc = rpk_status_reset(ctx, N)) return rc; }
-    if (ctx->devs[0].statusN != N) return fail(ctx, RPK_ESTATE, "rpk_tick: N differs from the tracked table (call rpk_status_reset to resize)");
+    const StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
+    if (int rc = check_sweep(ctx, h, "rpk_tick")) return rc;
     return guarded(ctx, [&]() -> int {
+        const PodCols pods{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud};
         const int n = (int)ctx->devs.size();
-        if (P > 0) reserve_select(ctx, P, req_vcpu != nullptr, req_ram_gb != nullptr, max_price != nullptr, cloud != nullptr, top5 != nullptr);
+        if (P > 0) reserve_select(ctx, P, pods, top5 != nullptr);
         for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, h);
         std::vector<uint64_t> launches((size_t)n, 0);
         ctx->workers.run(n, [&](int s) {
             DeviceState& ds = ctx->devs[(size_t)s];
             // the selection goes first: its kernels are the long pole and start after the first 128k-row sub-batch has
-            // landed; the sweep's records follow on the status stream and its kernel runs under the selection's tail
-            if (P > 0) enqueue_select_shard(ctx, s, P, req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud, best, top5, &launches[(size_t)s]);
-            RPK_CUDA(cudaSetDevice(ds.dev));
-            cudaStream_t keep = ds.stream;
-            ds.stream = ds.status_stream;  // the sweep's copies and kernel: its own stream, concurrent with the lanes
-            try { enqueue_status_shard(ctx, s, h, &launches[(size_t)s]); } catch (...) { ds.stream = keep; throw; }
-            ds.stream = keep;
+            // landed; the sweep's records follow on the status stream, concurrent with the lanes, and its kernel runs
+            // under the selection's tail
+            if (P > 0) enqueue_select_shard(ctx, s, P, pods, best, top5, &launches[(size_t)s]);
+            enqueue_status_shard(ctx, s, h, ds.status_stream, &launches[(size_t)s]);
             RPK_CUDA(cudaStreamSynchronize(ds.status_stream));
             if (P > 0) RPK_CUDA(cudaStreamSynchronize(ds.stream));
         });
@@ -975,7 +951,7 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
         for (int s = 0; s < n; ++s) { total += collect_status_shard(ctx, s, h, total); ctx->launches += launches[(size_t)s]; }
         *n_changed = total;
         ctx->stats.status_calls += 1; ctx->stats.status_records += N;
-        if (P > 0) { ctx->stats.select_calls += 1; ctx->stats.offer_scores += (uint64_t)P * ctx->devs[0].G; }
+        if (P > 0) count_select(ctx, P, ctx->devs[0].G);
         return RPK_OK;
     });
 }
@@ -1000,14 +976,12 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
-        reserve_status_state(ds, N ? N : 1, stride);
-        ds.s_stage_idx.reserve((N ? N : 1) + 64); ds.s_unit_cnt.reserve(N / 32 + 2);
-        if (d_changed_code || n_out > 0) ds.s_stage_code.reserve((N ? N : 1) + 64);
+        const bool codes = d_changed_code || n_out > 0;
+        reserve_sweep_scratch(ds, N, stride, codes);
         StatusArgs a{};
         a.records = d_records; a.stride = stride; a.N = N; a.hash_prev = d_hash_prev; a.hash_out = nullptr;
         a.changed_idx = d_changed_idx; a.changed_code = d_changed_code; a.n_changed = d_n_changed; a.idx_base = idx_base;
-        a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
-        a.stage_idx = ds.s_stage_idx.p; a.stage_code = (d_changed_code || n_out > 0) ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
+        sweep_scratch_args(ds, codes, a);
         a.n_out = n_out; a.my_rank = my_rank;
         a.slots = d_slots; a.col_n = col_n;
         for (int o = 0; o < n_out; ++o) {  // rank o's buffer: [counts : 8 words][n_out index regions of cap][n_out code regions of cap u16]
@@ -1016,7 +990,7 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
             a.out_idx[o] = base + 8 + (size_t)my_rank * cap;
             a.out_code[o] = reinterpret_cast<uint16_t*>(base + 8 + (size_t)n_out * cap) + (size_t)my_rank * cap;
         }
-        if (n_out > 0 && (size_t)shard < ctx->bind.size()) {
+        if (n_out > 0) {
             const PeerBinding& b = ctx->bind[(size_t)shard];
             for (int r = 0; r < b.n; ++r) a.flags[r] = b.flags[r];
             a.n_flags = b.n; a.inline_wait = b.inline_wait;

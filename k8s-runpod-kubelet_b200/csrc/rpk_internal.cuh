@@ -209,9 +209,13 @@ int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t*
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
 template <typename T>
-struct DevBuf {  // grow-only device buffer
+struct DevBuf {  // grow-only device buffer, freed by its destructor
     T* p = nullptr;
     size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { if (p) cudaFree(p); }
     void reserve(size_t n) {
         if (n <= cap) return;
         if (p) RPK_CUDA(cudaFree(p));
@@ -220,9 +224,29 @@ struct DevBuf {  // grow-only device buffer
         RPK_CUDA(cudaMalloc(&p, want * sizeof(T)));
         cap = want;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
+struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches it at d
+    unsigned char* h = nullptr;
+    unsigned char* d = nullptr;
+    size_t cap = 0;
+    PinnedBuf() = default;
+    PinnedBuf(const PinnedBuf&) = delete;
+    PinnedBuf& operator=(const PinnedBuf&) = delete;
+    ~PinnedBuf() { if (h) cudaFreeHost(h); }
+    void reserve(size_t n) {
+        if (n <= cap) return;
+        if (h) RPK_CUDA(cudaFreeHost(h));
+        h = d = nullptr; cap = 0;
+        const size_t want = n + n / 4;
+        RPK_CUDA(cudaHostAlloc((void**)&h, want, cudaHostAllocMapped | cudaHostAllocPortable));
+        RPK_CUDA(cudaHostGetDevicePointer((void**)&d, h, 0));
+        cap = want;
+    }
+};
+
+// One GPU of a ctx.  Built once at its final place (never copied or moved); the destructor synchronises the streams
+// and destroys them and the events, then the members free the buffers with this device still current.
 struct DeviceState {
     int dev = -1;
     int sm_count = 132;
@@ -251,28 +275,24 @@ struct DeviceState {
         DevBuf<uint16_t> key; DevBuf<uint2> ord_rw; DevBuf<uint32_t> hist, cursor, hdr;  // persistent path
         bool ctrs_dirty = false;  // a select on this lane failed between its launches: re-zero the counters before the next one
         bool persist_dirty = false;
-        void release() {
-            p_req_mem.release(); p_req_vcpu.release(); p_req_ram.release(); p_max_price.release(); p_cloud.release();
-            top5.release(); rw.release(); order.release(); pos.release(); ctrs.release();
-            key.release(); ord_rw.release(); hist.release(); cursor.release(); hdr.release();
-        }
     };
     static constexpr int kLanes = 4;  // one per sub-batch of a 1M-row call: no upload ever waits for a kernel to free its buffers
     Lane lane[kLanes];
     DevBuf<int32_t> best_full;
     // small-batch (latency) path: one pinned staging block in, one out
-    unsigned char* h_small = nullptr; DevBuf<unsigned char> d_small_in; DevBuf<int32_t> d_small_out;
+    PinnedBuf h_small; DevBuf<unsigned char> d_small_in; DevBuf<int32_t> d_small_out;
     // status
-    DevBuf<uint8_t> s_records; DevBuf<uint64_t> s_hash_prev, s_hash_out; DevBuf<uint32_t> s_changed, s_misc;
-    DevBuf<unsigned long long> s_tile_state; DevBuf<uint32_t> s_stage_idx; DevBuf<uint16_t> s_stage_code, s_changed_code; DevBuf<uint32_t> s_unit_cnt;
+    DevBuf<uint8_t> s_records; DevBuf<uint64_t> s_hash_prev, s_hash_out; DevBuf<uint32_t> s_misc;
+    DevBuf<unsigned long long> s_tile_state; DevBuf<uint32_t> s_stage_idx; DevBuf<uint16_t> s_stage_code; DevBuf<uint32_t> s_unit_cnt;
     DevBuf<uint32_t> s_seed_slots; DevBuf<uint8_t> s_seed_recs;  // slot lists of rpk_status_seed_slots and rpk_status_diff_slots
-    unsigned char* h_changed = nullptr; unsigned char* d_changed_map = nullptr; size_t h_changed_cap = 0;  // mapped pinned: count, indices, codes
+    PinnedBuf h_changed;                   // the host sweep's changed list: count, indices, codes
     cudaStream_t status_stream = nullptr;  // rpk_tick: the sweep next to the selection
     // device entry points: the stream that last used the select / status scratch, and its completion event
     cudaStream_t sel_last_stream = nullptr, st_last_stream = nullptr;
     cudaEvent_t ev_sel = nullptr, ev_st = nullptr;
     bool status_dirty = false;             // a status launch failed midway: re-zero the look-back state before the next one
     uint32_t statusN = 0; bool status_sized = false;
+    ~DeviceState();
 };
 
 }  // namespace rpk
