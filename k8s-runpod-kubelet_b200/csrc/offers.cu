@@ -119,12 +119,6 @@ __global__ void __launch_bounds__(1024) k_unique(const u64* __restrict__ keys, u
 }
 
 // ---- pack the views ------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t lower_bound_i32(const int32_t* __restrict__ a, uint32_t n, int32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { uint32_t mid = (lo + hi) >> 1; if (a[mid] < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
-
 struct PackArgs {
     uint32_t G, Gpad, n;
     const u64* keys; const uint32_t* vals;  // [2n] sorted, cloud c at c*n

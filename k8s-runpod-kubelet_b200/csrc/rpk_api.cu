@@ -18,8 +18,6 @@
 
 using namespace rpk;
 
-struct PeerBinding { int n = 0, my_rank = 0, inline_wait = 0; uint32_t* flags[RPK_MAX_GPUS] = {}; };
-
 // One host thread per extra GPU of a multi-GPU ctx: the per-shard halves of rpk_select / rpk_status_diff / rpk_tick
 // (a dozen cudaMemcpyAsync + launches each) are issued in parallel instead of one shard after the other -- with 8
 // GPUs behind one caller thread the serial issue, not PCIe, was the end-to-end bound.
@@ -77,7 +75,7 @@ struct ShardWorkers {
 
 struct rpk_ctx {
     std::vector<DeviceState> devs;  // one per shard, never resized: a DeviceState is neither copied nor moved
-    std::vector<PeerBinding> bind;  // per shard: flag arrays bound with rpk_peer_bind
+    std::vector<PeerGroup> bind;    // per shard: flag arrays bound with rpk_peer_bind (value-initialised: none)
     ShardWorkers workers;           // stopped (rpk_destroy) before devs is destroyed
     std::vector<std::pair<int, void*>> ipc_owned, ipc_mapped;  // (shard, ptr)
     std::string err;
@@ -181,7 +179,7 @@ int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaSt
     }
     // the lane's counters are suspect until every launch of the call was accepted
     ln.ctrs_dirty = true; ln.persist_dirty = true;
-    const int n = launch_select(a, R, persist ? &pl : nullptr, st);
+    const int n = launch_select(a, R, persist ? &pl : nullptr, ds.sm_count, st);
     ln.ctrs_dirty = false; ln.persist_dirty = false;
     return n;
 }
@@ -210,12 +208,6 @@ struct ScratchGuard {
         *last = st;
     }
 };
-
-void bind_flags(const rpk_ctx* ctx, int shard, SelectArgs& a) {
-    const PeerBinding& b = ctx->bind[(size_t)shard];
-    for (int r = 0; r < b.n; ++r) a.flags[r] = b.flags[r];
-    a.n_flags = b.n; a.my_rank = b.my_rank; a.inline_wait = b.inline_wait;
-}
 
 // Which of the output vectors lives on GPU `shard` (the others are peers' memory); -1 if none does.  Vectors this ctx
 // allocated (rpk_ipc_alloc) or mapped from a peer (rpk_ipc_open) are known exactly; anything else is asked of the driver.
@@ -502,10 +494,21 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
                              int n_out, int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device: shard out of range");
-    if (P == 0) return RPK_OK;
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    const PeerGroup& peers = ctx->bind[(size_t)shard];
+    cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+    if (P == 0) {  // nothing to select, but a bound gather still tells its peers that this (empty) shard is done
+        if (n_out <= 1 || peers.n == 0) return RPK_OK;
+        return guarded(ctx, [&]() -> int {
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);  // orders the epoch counter after the last gather's
+            ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
+            guard.done();
+            return RPK_OK;
+        });
+    }
     if (!d_req_mem_gb || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
     for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device: NULL output vector");
-    DeviceState& ds = ctx->devs[(size_t)shard];
     if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
@@ -515,8 +518,7 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
         for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
         a.n_out = n_out; a.row0 = row0; a.top5 = d_top5;
         a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
-        if (n_out > 1) bind_flags(ctx, shard, a);
-        cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+        if (n_out > 1) a.peers = peers;
         ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);
         ctx->launches += (uint64_t)enqueue_select(ds, ds.lane[0], a, st);
         guard.done();
@@ -633,10 +635,10 @@ int rpk_peer_fence(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
-        PeerFenceArgs a{};
-        for (int r = 0; r < n; ++r) a.flags[r] = d_flags[r];
-        a.n = n; a.my_rank = my_rank; a.epoch = epoch;
-        ctx->launches += (uint64_t)launch_peer_fence(a, stream ? (cudaStream_t)stream : ds.stream);
+        PeerGroup g{};
+        for (int r = 0; r < n; ++r) g.flags[r] = d_flags[r];
+        g.n = n; g.my_rank = my_rank;
+        ctx->launches += (uint64_t)launch_peer_signal(g, epoch, true, stream ? (cudaStream_t)stream : ds.stream);
         return RPK_OK;
     });
 }
@@ -646,9 +648,9 @@ int rpk_peer_bind(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int 
     if (shard < 0 || (size_t)shard >= ctx->devs.size() || n < 0 || n > RPK_MAX_GPUS || (n > 0 && (!d_flags || my_rank < 0 || my_rank >= n)))
         return fail(ctx, RPK_EINVAL, "rpk_peer_bind: bad argument");
     for (int r = 0; r < n; ++r) if (!d_flags[r]) return fail(ctx, RPK_EINVAL, "rpk_peer_bind: NULL flag array");
-    PeerBinding& b = ctx->bind[(size_t)shard];
+    PeerGroup& b = ctx->bind[(size_t)shard];
     const int keep = b.inline_wait;
-    b = PeerBinding{};
+    b = PeerGroup{};
     for (int r = 0; r < n; ++r) b.flags[r] = d_flags[r];
     b.n = n; b.my_rank = my_rank; b.inline_wait = keep;
     return RPK_OK;
@@ -668,11 +670,7 @@ int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream) {
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
-        const PeerBinding& b = ctx->bind[(size_t)shard];
-        PeerFenceArgs a{};
-        for (int r = 0; r < b.n; ++r) a.flags[r] = b.flags[r];
-        a.n = b.n; a.my_rank = b.my_rank; a.epoch = 0;
-        ctx->launches += (uint64_t)launch_peer_wait(a, what, stream ? (cudaStream_t)stream : ds.stream);
+        ctx->launches += (uint64_t)launch_peer_wait(ctx->bind[(size_t)shard], what, stream ? (cudaStream_t)stream : ds.stream);
         return RPK_OK;
     });
 }
@@ -793,7 +791,7 @@ void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, cudaStre
     sweep_scratch_args(ds, h.changed_code != nullptr, a);
     if (h.slots) { a.slots = ds.s_seed_slots.p; a.col_n = sp.hi - sp.lo; }
     ds.status_dirty = true;
-    if (Ns) *launches += (uint64_t)launch_status_diff(a, st);
+    if (Ns) *launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
     ds.status_dirty = false;
     RPK_CUDA(cudaEventRecord(ds.ev[2], st));
     if (h.hashes_out && Ns) RPK_CUDA(cudaMemcpyAsync(h.hashes_out + lo, ds.s_hash_out.p, (size_t)Ns * 8, cudaMemcpyDeviceToHost, st));
@@ -982,7 +980,7 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
         a.records = d_records; a.stride = stride; a.N = N; a.hash_prev = d_hash_prev; a.hash_out = nullptr;
         a.changed_idx = d_changed_idx; a.changed_code = d_changed_code; a.n_changed = d_n_changed; a.idx_base = idx_base;
         sweep_scratch_args(ds, codes, a);
-        a.n_out = n_out; a.my_rank = my_rank;
+        a.n_out = n_out;
         a.slots = d_slots; a.col_n = col_n;
         for (int o = 0; o < n_out; ++o) {  // rank o's buffer: [counts : 8 words][n_out index regions of cap][n_out code regions of cap u16]
             uint32_t* base = d_xchg[o];
@@ -990,15 +988,12 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
             a.out_idx[o] = base + 8 + (size_t)my_rank * cap;
             a.out_code[o] = reinterpret_cast<uint16_t*>(base + 8 + (size_t)n_out * cap) + (size_t)my_rank * cap;
         }
-        if (n_out > 0) {
-            const PeerBinding& b = ctx->bind[(size_t)shard];
-            for (int r = 0; r < b.n; ++r) a.flags[r] = b.flags[r];
-            a.n_flags = b.n; a.inline_wait = b.inline_wait;
-        }
+        if (n_out > 0) a.peers = ctx->bind[(size_t)shard];
+        a.peers.my_rank = my_rank;  // the sweep fills and signals under the rank its call names
         cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
         ScratchGuard guard(&ds.st_last_stream, ds.ev_st, st);
         ds.status_dirty = true;
-        ctx->launches += (uint64_t)launch_status_diff(a, st);
+        ctx->launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
         ds.status_dirty = false;
         guard.done();
         ctx->stats.status_calls += 1; ctx->stats.status_records += N;

@@ -62,6 +62,39 @@ constexpr uint32_t kMaxGroups = 2 * kBmMaxStride;  // row groups of the persiste
 enum : uint32_t { kHdrRowsDone = 32, kHdrPushed = 64, kHdrGroupRows = 96, kHdrGroupWork = kHdrGroupRows + kMaxGroups,
                   kHdrCursors = kHdrGroupWork + kMaxGroups };
 
+// A peer group's flag arrays (rpk_peer_bind, rpk_peer_fence): flags[r] is rank r's array of >= 64 words; n = 0: none.
+// Word layout (rpk.h): a rank's epochs as seen by rank r sit at word kFlagSelect + my_rank / kFlagStatus + my_rank of
+// r's array; each rank counts its own epochs in kFlagSelectCtr / kFlagStatusCtr of its own array.
+struct PeerGroup {
+    uint32_t* flags[RPK_MAX_GPUS];
+    int n, my_rank;
+    int inline_wait;  // the signalling warp also waits for every peer's signal (rpk_peer_inline_wait)
+};
+enum : uint32_t { kFlagSelect = 0, kFlagStatus = 8, kFlagSelectCtr = 32, kFlagStatusCtr = 33 };
+
+// One warp signals the group: epoch 0 bumps the rank's own counter word `ctr` and uses the new value (the launch then
+// carries no per-call value and can be replayed from a CUDA graph), any other epoch is used as given and leaves `ctr`
+// alone.  After a system-scope fence (everything this grid and its stream did before, peer stores included, is visible
+// first) lane r stores the epoch into word `word0 + my_rank` of rank r's array; with `wait` it then spins until word
+// `word0 + r` of the own array has reached the same epoch.
+__device__ __forceinline__ void signal_peers(const PeerGroup& g, uint32_t word0, uint32_t ctr, uint32_t epoch, bool wait) {
+    const uint32_t lane = threadIdx.x & 31;
+    uint32_t e = epoch;
+    if (epoch == 0) {
+        if (lane == 0) { e = g.flags[g.my_rank][ctr] + 1u; g.flags[g.my_rank][ctr] = e; }
+        e = __shfl_sync(0xFFFFFFFFu, e, 0);
+    }
+    __threadfence_system();
+    if ((int)lane < g.n) {
+        *reinterpret_cast<volatile uint32_t*>(g.flags[lane] + word0 + g.my_rank) = e;
+        if (wait) {
+            const volatile uint32_t* mine = g.flags[g.my_rank] + word0 + lane;
+            while ((int32_t)(*mine - e) < 0) __nanosleep(32);
+            __threadfence_system();
+        }
+    }
+}
+
 struct OfferView {       // one per cloud, all arrays in price-sorted order, length Gpad
     uint32_t* packed = nullptr;
     uint32_t* bitmap = nullptr;  // [Gpad/32][bm_stride]
@@ -108,10 +141,7 @@ struct SelectArgs {
     uint32_t* hist;      // [kMaxClasses] rows per class       } zero between calls (k_pod_classify's last block)
     uint32_t* cursor;    // [kMaxClasses] class write cursors
     uint32_t* hdr;       // control words, kHdr*
-    // peer flags bound with rpk_peer_bind: the warp that finishes the last push signals every peer (n_flags = 0: none)
-    uint32_t* flags[RPK_MAX_GPUS];
-    int n_flags, my_rank;
-    int inline_wait;     // the signalling warp also waits for every peer's signal (rpk_peer_inline_wait)
+    PeerGroup peers;     // bound with rpk_peer_bind: the gather signals every peer once its slice has landed
     uint32_t tune_natural_order;  // tuning hook (RPK_TUNE=order=natural): row tiles in group order instead of heaviest first
     uint32_t slice;      // persistent select: rows grouped and the table staged per (cloud, mem threshold) on bitmapM
 };
@@ -121,6 +151,32 @@ struct SelectArgs {
 __device__ __forceinline__ void store_best(const SelectArgs& a, uint32_t row, int32_t b) {
     if (a.self_out >= 0) { a.best_out[a.self_out][a.row0 + row] = b; return; }
     for (int o = 0; o < a.n_out; ++o) a.best_out[o][a.row0 + row] = b;
+}
+
+// The result of a row whose cheapest feasible offer sits at sorted position p of its cloud's view v (kNone: none): the
+// offer index if its price is under the row's bound (strict, runpod_client.go:478; the bound is a prefix of the price
+// order), else -1.
+__device__ __forceinline__ void finish_row(const SelectArgs& a, const OfferView& v, uint32_t row, uint32_t p) {
+    int32_t b = -1;
+    if (p != kNone) {
+        const double pr = v.price[p];
+        const double mx = a.max_price ? a.max_price[row] : RPK_DEFAULT_MAX_PRICE;
+        if (pr < mx) b = v.perm[p];
+    }
+    store_best(a, row, b);
+}
+
+// A row of neither SECURE nor COMMUNITY cloud: nothing is feasible (runpod_client.go:469-475)
+__device__ __forceinline__ void finish_row_no_cloud(const SelectArgs& a, uint32_t row) {
+    store_best(a, row, -1);
+    if (a.top5) for (int k = 0; k < RPK_TOPK; ++k) a.top5[(size_t)row * RPK_TOPK + k] = -1;
+}
+
+// first position of the ascending array a[0, n) whose value is >= x (read-only data: the .nc path)
+__device__ __forceinline__ uint32_t lower_bound_i32(const int32_t* __restrict__ a, uint32_t n, int32_t x) {
+    uint32_t lo = 0, hi = n;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
+    return lo;
 }
 
 struct StatusArgs {
@@ -138,13 +194,12 @@ struct StatusArgs {
     uint32_t* stage_idx;             // [N] per-warp ordered index segments (strides 16/32)
     uint16_t* stage_code;            // [N] codes staged alongside
     uint32_t* unit_cnt;              // [N / 64 + 1] changed slots per 64-slot unit (strides 16/32)
-    // sharded sweep: the changed list also goes into region `my_rank` of every rank's exchange buffer
-    int n_out, my_rank;
+    // sharded sweep: the changed list also goes into region `peers.my_rank` of every rank's exchange buffer
+    int n_out;
     uint32_t* out_idx[RPK_MAX_GPUS];    // start of this rank's index region in rank o's buffer
     uint16_t* out_code[RPK_MAX_GPUS];   // ... code region (nullable)
     uint32_t* out_count[RPK_MAX_GPUS];  // rank o's count words (one per source rank)
-    uint32_t* flags[RPK_MAX_GPUS];      // bound peer flags: the CTA that finishes last signals (n_flags = 0: none)
-    int n_flags, inline_wait;
+    PeerGroup peers;                    // bound flags (n = 0: none), my_rank from the call: the CTA that finishes last signals
     // slot-list sweep (rpk_status_diff_slots): records[i] is the state of global slot slots[i] (ascending), whose previous
     // hash is hash_prev[slots[i] - idx_base]; entries outside [idx_base, idx_base + col_n) are skipped.  N = list length.
     const uint32_t* slots;  // null: whole-table sweep
@@ -181,6 +236,17 @@ void launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cu
     RPK_CUDA(cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...));
 }
 
+// cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): set it once per (thread, device), so a
+// warmed-up launch path issues nothing but launches (stream capture).  attr_dev: the call site's thread_local record.
+template <typename K>
+void allow_smem(K kernel, int bytes, int* attr_dev) {
+    int dev = 0;
+    RPK_CUDA(cudaGetDevice(&dev));
+    if (*attr_dev == dev) return;
+    RPK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+    *attr_dev = dev;
+}
+
 struct OfferIngest {   // raw device columns in, views out
     uint32_t G;
     const int32_t* mem; const int32_t* vcpu; const int32_t* ram;  // vcpu/ram never null here (zero-filled)
@@ -190,14 +256,14 @@ struct OfferIngest {   // raw device columns in, views out
 struct DeviceState;
 int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st);
 struct PersistPlan;
-int launch_select(const SelectArgs& a, int rows_per_warp, const PersistPlan* pl, cudaStream_t st);
+int launch_select(const SelectArgs& a, int rows_per_warp, const PersistPlan* pl, int sm_count, cudaStream_t st);
 uint32_t select_tiles_max(uint32_t P, int rows_per_warp);
 int pick_rows_per_warp(uint32_t P, int sm_count);
-int launch_status_diff(const StatusArgs& a, cudaStream_t st);
-struct PeerFenceArgs { uint32_t* flags[RPK_MAX_GPUS]; int n; int my_rank; uint32_t epoch; };
-int launch_peer_fence(const PeerFenceArgs& a, cudaStream_t st);
-int launch_peer_signal(const PeerFenceArgs& a, uint32_t word0, cudaStream_t st);
-int launch_peer_wait(const PeerFenceArgs& a, uint32_t what, cudaStream_t st);
+int launch_status_diff(const StatusArgs& a, int sm_count, cudaStream_t st);
+// one warp behind the stream's earlier work: signal the group's select words (epoch 0: self-counting), with `wait` also
+// wait for every rank's signal; what: bit 0 = wait for the select epoch, bit 1 = the status epoch
+int launch_peer_signal(const PeerGroup& g, uint32_t epoch, bool wait, cudaStream_t st);
+int launch_peer_wait(const PeerGroup& g, uint32_t what, cudaStream_t st);
 // persistent bit-sliced select (select_persist.cu)
 struct PersistPlan { uint32_t S, per, qspan, grid, smem_bytes, slice, n_cursors; int sm_count; };
 PersistPlan persist_plan(const SelectArgs& a, int sm_count);  // a.pk.bm_words and a.nsub non-zero

@@ -13,7 +13,8 @@
 //                     applies price < maxPrice to the winner (the bound is a prefix of the sorted order) and stores
 //                     the offer index into every peer's assignment vector (the fused all-gather).
 //   k_select_top5*    optional: the whole <=5 gpuTypeIds list per row (runpod_client.go:502-509).
-//   k_peer_fence      one warp: signal / wait across GPUs after the fused gather.
+//   k_gather_push     several output vectors: copies the finished slice to the peers; k_peer_signal (select_persist.cu)
+//                     then signals a bound peer group.
 #include <math_constants.h>
 
 #include <cstdlib>
@@ -24,12 +25,6 @@
 
 namespace rpk {
 using namespace dev;
-
-__device__ __forceinline__ uint32_t lower_bound_i32(const int32_t* __restrict__ a, uint32_t n, int32_t x) {
-    uint32_t lo = 0, hi = n;
-    while (lo < hi) { uint32_t mid = (lo + hi) >> 1; if (__ldg(a + mid) < x) lo = mid + 1; else hi = mid; }
-    return lo;
-}
 
 // ---------------------------------------------------------------------------------------------------------
 // K0: per-row preparation
@@ -55,12 +50,8 @@ __global__ void __launch_bounds__(1024) k_pod_prep(SelectArgs a) {
             need = (tv != 0 ? 2u : 0u) | (tr != 0 ? 1u : 0u);
             a.rw[p] = (tm << a.pk.sh_mem) | (tv << a.pk.sh_vcpu) | (tr << a.pk.sh_ram);
         }
-        if (c <= 1) {
-            grp = c * 4u + need;
-        } else {  // neither SECURE nor COMMUNITY -> nothing feasible (runpod_client.go:469-475)
-            store_best(a, p, -1);
-            if (a.top5) for (int k = 0; k < RPK_TOPK; ++k) a.top5[(size_t)p * RPK_TOPK + k] = -1;
-        }
+        if (c <= 1) grp = c * 4u + need;
+        else finish_row_no_cloud(a, p);
     }
     // one atomic per (group, 1024-row block): the counters are shared by the whole grid
     __shared__ uint32_t s_cnt[kGroups][32], s_base[kGroups];
@@ -117,8 +108,7 @@ __device__ __forceinline__ uint32_t tile_row(const SelectArgs& a, const TileInfo
     return a.order[(size_t)t.group * a.P + t.row_base + slot];
 }
 
-// Merge the segment result, and let the last CTA of the tile finish the rows: price < maxPrice on the
-// winner (strict, runpod_client.go:478) and sorted position -> offer index.
+// Merge the segment result, and let the last CTA of the tile finish the rows (finish_row).
 __device__ __forceinline__ void finish_tile(const SelectArgs& a, const TileInfo& t, uint32_t tile, uint32_t S, int* s_last) {
     __syncthreads();
     if (threadIdx.x == 0) {
@@ -131,14 +121,7 @@ __device__ __forceinline__ void finish_tile(const SelectArgs& a, const TileInfo&
     __threadfence();
     for (uint32_t slot = threadIdx.x; slot < t.nrows; slot += blockDim.x) {
         const uint32_t row = tile_row(a, t, slot);
-        const uint32_t p = __ldcg(a.pos + row);
-        int32_t b = -1;
-        if (p != kNone) {
-            const double pr = a.view[t.cloud].price[p];
-            const double mx = a.max_price ? a.max_price[row] : RPK_DEFAULT_MAX_PRICE;
-            if (pr < mx) b = a.view[t.cloud].perm[p];
-        }
-        store_best(a, row, b);
+        finish_row(a, a.view[t.cloud], row, __ldcg(a.pos + row));
     }
     if (a.n_out > 1 && a.self_out < 0) __threadfence_system();  // direct peer stores are performed system-wide before this grid completes
     // The counters clean themselves (no memset launch per call): this CTA is the last one to touch the tile's
@@ -330,14 +313,7 @@ __global__ void __launch_bounds__(kCtaThreads) k_select_fused(SelectArgs a, uint
             __syncthreads();  // everyone is done with the segment before the next bulk copy overwrites it
         }
     }
-    if (!valid) return;
-    int32_t b = -1;
-    if (cls < 2 && gpos != kNone) {  // winner's price < maxPrice (strict, runpod_client.go:478); the bound is a prefix of the order
-        const double pr = a.view[cls].price[gpos];
-        const double mx = a.max_price ? a.max_price[p] : RPK_DEFAULT_MAX_PRICE;
-        if (pr < mx) b = a.view[cls].perm[gpos];
-    }
-    store_best(a, p, b);
+    if (valid) finish_row(a, a.view[cls], p, gpos);  // a row of neither cloud walked nothing: gpos = kNone
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -472,17 +448,11 @@ __global__ void __launch_bounds__(256) k_gather_push(PushArgs a) {
     pdl_trigger();  // the peer fence may be scheduled behind this grid
     const int32_t* src = a.src;  // read with ld.global.cg: written by the grid this kernel overlaps with (never the .nc path)
     int32_t* dst = a.dst[blockIdx.y];
-    // all vectors share the slice offset and 256-byte aligned bases, so one head/body/tail split fits source and peers
-    const uint32_t mis = (uint32_t)((reinterpret_cast<uintptr_t>(src) & 15u) >> 2);
-    const uint32_t head = min(a.count, (4u - mis) & 3u);
-    const uint32_t nvec = (a.count - head) >> 2;
-    const uint32_t tail0 = head + (nvec << 2);
-    if (blockIdx.x == 0) {
-        if (threadIdx.x < head) dst[threadIdx.x] = __ldcg(src + threadIdx.x);
-        if (threadIdx.x < a.count - tail0) dst[tail0 + threadIdx.x] = __ldcg(src + tail0 + threadIdx.x);
-    }
-    const uint4* s4 = reinterpret_cast<const uint4*>(src + head);
-    uint4* d4 = reinterpret_cast<uint4*>(dst + head);
+    const SliceSplit sp = slice_split(src, a.count);  // the host checked that every vector shares the slice's 16-byte phase
+    const uint32_t nvec = sp.nvec;
+    if (blockIdx.x == 0) copy_slice_edges(src, 0, a.count, sp, threadIdx.x, 1, -1, [&](int) { return dst; });
+    const uint4* s4 = reinterpret_cast<const uint4*>(src + sp.head);
+    uint4* d4 = reinterpret_cast<uint4*>(dst + sp.head);
     // four 16-byte loads in flight per thread before the first store: the copy is latency-bound, not bandwidth-bound
     constexpr int kU = 4;
     const uint32_t stride = gridDim.x * blockDim.x;
@@ -495,30 +465,6 @@ __global__ void __launch_bounds__(256) k_gather_push(PushArgs a) {
     }
     __threadfence_system();  // this thread's peer stores are performed system-wide before the grid completes
 }
-
-// ---------------------------------------------------------------------------------------------------------
-// cross-GPU fence after the fused gather: signal every peer, then wait for every peer (one warp)
-// ---------------------------------------------------------------------------------------------------------
-constexpr int kFenceCounterWord = 32;  // word of a rank's own flag array that counts its fences (epoch = 0 mode)
-
-__global__ void k_peer_fence(PeerFenceArgs a) {
-    const int r = (int)threadIdx.x;
-    pdl_wait();  // launched early behind the select grid (PDL): its peer stores are complete from here on
-    uint32_t epoch = a.epoch;
-    if (epoch == 0) {  // self-counting: the launch carries no per-call value, so it can be captured in a CUDA graph and replayed
-        uint32_t e = 0;
-        if (r == 0) { e = a.flags[a.my_rank][kFenceCounterWord] + 1u; a.flags[a.my_rank][kFenceCounterWord] = e; }
-        epoch = __shfl_sync(0xFFFFFFFFu, e, 0);
-    }
-    if (r < a.n) {
-        __threadfence_system();  // everything this stream did before (the epilogue's NVLink stores) is ordered before the flag
-        *reinterpret_cast<volatile uint32_t*>(a.flags[r] + a.my_rank) = epoch;
-        const volatile uint32_t* mine = a.flags[a.my_rank] + r;
-        while ((int32_t)(*mine - epoch) < 0) __nanosleep(64);
-        __threadfence_system();
-    }
-}
-
 
 // ---------------------------------------------------------------------------------------------------------
 // host side
@@ -564,24 +510,6 @@ int pick_rows_per_warp(uint32_t P, int sm_count) {
     return 1;
 }
 
-static int device_sm_count() {
-    int dev = 0, sms = 0;
-    RPK_CUDA(cudaGetDevice(&dev));
-    RPK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    return sms;
-}
-
-// cudaFuncAttributeMaxDynamicSharedMemorySize is per (function, device): set it once per (thread, device), so a
-// warmed-up launch path issues nothing but launches (stream capture)
-template <typename K>
-static void allow_smem(K kernel, int bytes, int* attr_dev) {
-    int dev = 0;
-    RPK_CUDA(cudaGetDevice(&dev));
-    if (*attr_dev == dev) return;
-    RPK_CUDA(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
-    *attr_dev = dev;
-}
-
 template <int R>
 static void launch_grid(const SelectArgs& a, cudaStream_t st) {
     static thread_local int dev_pos = -1, dev_packed = -1, dev_wide = -1;
@@ -612,30 +540,21 @@ template <int STRIDE>
 static void launch_fused(const SelectArgs& a, cudaStream_t st) {
     constexpr uint32_t kSegChunks = kBmSegBytes / (STRIDE * 4);
     static thread_local int attr_dev = -1;
-    int dev = 0;
-    RPK_CUDA(cudaGetDevice(&dev));
-    if (attr_dev != dev) {
-        RPK_CUDA(cudaFuncSetAttribute(k_select_fused<STRIDE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kBmSegBytes));
-        attr_dev = dev;
-    }
+    allow_smem(k_select_fused<STRIDE>, (int)kBmSegBytes, &attr_dev);
     // small tables need a small stage: size the dynamic shared memory to the table
     const uint32_t total_chunks = (a.G + 31) / 32;
     const uint32_t chunks = total_chunks < kSegChunks ? (total_chunks ? total_chunks : 1) : kSegChunks;
     k_select_fused<STRIDE><<<(a.P + kCtaThreads - 1) / kCtaThreads, kCtaThreads, (size_t)chunks * STRIDE * 4, st>>>(a, kSegChunks);
 }
 
-static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* pl, cudaStream_t st, bool* fused_push);
+static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* pl, int sm_count, cudaStream_t st, bool* fused_push);
 
-int launch_select(const SelectArgs& args, int R, const PersistPlan* pl, cudaStream_t st) {
+int launch_select(const SelectArgs& args, int R, const PersistPlan* pl, int sm_count, cudaStream_t st) {
     SelectArgs a = args;
-    PeerFenceArgs fa{};
-    for (int r = 0; r < a.n_flags; ++r) fa.flags[r] = a.flags[r];
-    fa.n = a.n_flags; fa.my_rank = a.my_rank; fa.epoch = a.inline_wait ? 1u : 0u;  // k_peer_signal: non-zero = wait here too
-    if (args.P == 0) return a.n_flags > 0 ? launch_peer_signal(fa, 0, st) : 0;  // an empty shard still tells its peers it is done
     a.tune_natural_order = read_tune().natural_order ? 1u : 0u;
     if (a.n_out == 1) a.self_out = 0;
     bool fused_push = false;  // the persistent kernel pushes (and signals) itself
-    int launches = launch_select_kernels(a, R, pl, st, &fused_push);
+    int launches = launch_select_kernels(a, R, pl, sm_count, st, &fused_push);
     if (fused_push) return launches;
     if (a.n_out > 1 && a.self_out >= 0) {  // forward the finished slice to the peers (the all-gather)
         PushArgs pa{};
@@ -645,16 +564,16 @@ int launch_select(const SelectArgs& args, int R, const PersistPlan* pl, cudaStre
         pa.count = a.P;
         const uint32_t nvec = a.P / 4;
         uint32_t per_peer = (nvec + 1023) / 1024;  // one pass of four 16-byte units per thread, up to two CTAs per SM
-        const uint32_t max_per_peer = 2u * (uint32_t)device_sm_count();
+        const uint32_t max_per_peer = 2u * (uint32_t)sm_count;
         per_peer = per_peer < 1 ? 1 : per_peer > max_per_peer ? max_per_peer : per_peer;
         launch_pdl(k_gather_push, dim3(per_peer, (unsigned)np), dim3(256), 0, st, read_tune().pdl, pa);
         ++launches;
     }
-    if (a.n_flags > 0) launches += launch_peer_signal(fa, 0, st);
+    if (a.peers.n > 0) launches += launch_peer_signal(a.peers, 0, a.peers.inline_wait != 0, st);
     return launches;
 }
 
-static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* pl, cudaStream_t st, bool* fused_push) {
+static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* pl, int sm_count, cudaStream_t st, bool* fused_push) {
     int launches = 0;
     if (a.pk.bm_words) {
         if (pl) {  // persistent kernel on the transposed view: sorts, selects, pushes, signals
@@ -683,17 +602,11 @@ static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* 
     }
     ++launches;
     if (a.top5) {
-        const uint32_t blocks = (uint32_t)min((uint64_t)(a.P + 7) / 8, (uint64_t)device_sm_count() * 32);
+        const uint32_t blocks = (uint32_t)min((uint64_t)(a.P + 7) / 8, (uint64_t)sm_count * 32);
         k_select_top5<<<blocks, 256, 0, st>>>(a); ++launches;
     }
     RPK_CUDA(cudaGetLastError());
     return launches;
-}
-
-int launch_peer_fence(const PeerFenceArgs& a, cudaStream_t st) {
-    launch_pdl(k_peer_fence, dim3(1), dim3(32), 0, st, read_tune().pdl, a);
-    RPK_CUDA(cudaGetLastError());
-    return 1;
 }
 
 }  // namespace rpk

@@ -90,6 +90,7 @@ __device__ __forceinline__ uint32_t slice_rw(const ClassDims& cd, const PackLayo
     return i1 | (i2 << 8) | (i1 << 16);
 }
 
+// lower_bound_i32 on a shared-memory array (that one loads through __ldg, which is for global memory only)
 __device__ __forceinline__ uint32_t lb_smem(const int32_t* a, uint32_t n, int32_t x) {
     uint32_t lo = 0, hi = n;
     while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (a[mid] < x) lo = mid + 1; else hi = mid; }
@@ -107,21 +108,10 @@ __device__ __forceinline__ void push_share(const SelectArgs& a) {
     const uint32_t wpc = blockDim.x >> 5, gw = blockIdx.x * wpc + (threadIdx.x >> 5), nw = gridDim.x * wpc;
     const int32_t* src = a.best_out[a.self_out];
     const uint32_t g_lo = a.row0, n = a.P;
-    // all vectors share the slice's 16-byte phase (checked on the host), so one head / body / tail split fits all
-    const uint32_t mis = (uint32_t)((reinterpret_cast<uintptr_t>(src + g_lo) & 15u) >> 2);
-    const uint32_t head = min(n, (4u - mis) & 3u);
-    const uint32_t nvec = (n - head) >> 2;
-    const uint32_t tail0 = head + (nvec << 2);
-    if (gw == 0) {  // the <= 3 + 3 elements off the 16-byte grid
-        int32_t hv = 0, tv = 0;
-        if (lane < head) hv = __ldcg(src + g_lo + lane);
-        if (lane < n - tail0) tv = __ldcg(src + g_lo + tail0 + lane);
-        for (int o = 0; o < a.n_out; ++o) {
-            if (o == a.self_out) continue;
-            if (lane < head) a.best_out[o][g_lo + lane] = hv;
-            if (lane < n - tail0) a.best_out[o][g_lo + tail0 + lane] = tv;
-        }
-    }
+    const SliceSplit sp = slice_split(src + g_lo, n);  // the host checked that every vector shares the slice's 16-byte phase
+    const uint32_t head = sp.head, nvec = sp.nvec;
+    if (gw == 0)
+        copy_slice_edges(src, g_lo, n, sp, lane, a.n_out, a.self_out, [&](int o) { return a.best_out[o]; });
     const uint32_t per = (nvec + nw - 1) / nw;
     const uint32_t v_lo = min(nvec, gw * per), v_hi = min(nvec, v_lo + per);
     const uint4* s4 = reinterpret_cast<const uint4*>(src + g_lo + head);
@@ -137,29 +127,6 @@ __device__ __forceinline__ void push_share(const SelectArgs& a) {
         }
     }
 }
-
-// first warp of the CTA that pushed last: every peer store of this grid is performed system-wide (each pusher fenced
-// before its CTA counted itself), so the flags may go out
-__device__ __forceinline__ void signal_peers(const SelectArgs& a, uint32_t word0, uint32_t counter_word) {
-    const uint32_t lane = threadIdx.x & 31;
-    uint32_t e = 0;
-    if (lane == 0) { e = a.flags[a.my_rank][counter_word] + 1u; a.flags[a.my_rank][counter_word] = e; }
-    e = __shfl_sync(0xFFFFFFFFu, e, 0);
-    __threadfence_system();
-    if ((int)lane < a.n_flags) {
-        *reinterpret_cast<volatile uint32_t*>(a.flags[lane] + word0 + a.my_rank) = e;
-        if (a.inline_wait) {  // the other half of the fence, without a kernel of its own: this warp is the grid's last worker anyway
-            const volatile uint32_t* mine = a.flags[a.my_rank] + word0 + lane;
-            while ((int32_t)(*mine - e) < 0) __nanosleep(32);
-            __threadfence_system();
-        }
-    }
-}
-
-constexpr uint32_t kFlagSelect = 0;       // words [0, 8): select epochs per source rank
-constexpr uint32_t kFlagStatus = 8;       // words [8, 16): status-sweep epochs per source rank
-constexpr uint32_t kFlagSelectCtr = 32;   // own select epoch counter
-constexpr uint32_t kFlagStatusCtr = 33;   // own status epoch counter
 
 // Fused all-gather, the way it works: natural-order push blocks only become complete near the END of the grid kernel
 // (the rows of any 1024-row block are spread over all classes, and the classes are processed one after the other), so
@@ -197,7 +164,9 @@ __device__ __forceinline__ void push_tail(const SelectArgs& a) {
         uint32_t last = 0;
         if (threadIdx.x == 0) last = atomicAdd(&a.hdr[kHdrPushed], 1u) + 1u == gridDim.x ? 1u : 0u;
         last = __shfl_sync(0xFFFFFFFFu, last, 0);
-        if (last && a.n_flags > 0) signal_peers(a, kFlagSelect, kFlagSelectCtr);
+        // every peer store of this grid is performed system-wide (each pusher fenced before its CTA counted itself); with
+        // inline_wait this warp, the grid's last worker anyway, also does the other half of the fence
+        if (last && a.peers.n > 0) signal_peers(a.peers, kFlagSelect, kFlagSelectCtr, 0, a.peers.inline_wait != 0);
     }
 }
 
@@ -321,10 +290,7 @@ __global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
             const uint32_t w = a.rw[p];
             a.ord_rw[dst] = make_uint2(p, cd.slice ? slice_rw(cd, a.pk, w) : w);  // the one scattered store of the sort
         }
-        if (neither) {
-            store_best(a, p, -1);
-            if (a.top5) for (int k = 0; k < RPK_TOPK; ++k) a.top5[(size_t)p * RPK_TOPK + k] = -1;
-        }
+        if (neither) finish_row_no_cloud(a, p);
         n_neither += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, neither));
     }
     if (n_neither) count_rows_done(a, n_neither);
@@ -518,16 +484,6 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
             const uint32_t local = (item / Qi) * RPI + (uint32_t)r * 32 + lane;
             w_cur[r] = item < n_items && local < n_c ? __ldcg(a.ord_rw + c_start + local).y : w_none;
         }
-        // the offer at sorted position p wins row `row` if it is under the row's price bound (strict, runpod_client.go:478)
-        auto finish = [&](uint32_t row, uint32_t p) {
-            int32_t b = -1;
-            if (p != kNone) {
-                const double pr = a.view[c].price[p];
-                const double mx = a.max_price ? a.max_price[row] : RPK_DEFAULT_MAX_PRICE;
-                if (pr < mx) b = a.view[c].perm[p];
-            }
-            store_best(a, row, b);
-        };
         uint32_t pend1_blk = kNone, pend2_blk = kNone, pend2_ticket = 0;  // merge pipeline (see below)
         // the row block whose ticket was taken one iteration ago: if that was its last ticket, every segment of its rows
         // has been merged -- price < maxPrice on the winner, position -> offer index
@@ -542,7 +498,7 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
                 const uint32_t local = rblk * RPI + (uint32_t)r * 32 + lane;
                 const bool ok = local < n_c;
                 n_final += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, ok));
-                if (ok) finish(a.ord_rw[c_start + local].x, __ldcg(a.pos + c_start + local));
+                if (ok) finish_row(a, a.view[c], a.ord_rw[c_start + local].x, __ldcg(a.pos + c_start + local));
             }
             count_rows_done(a, n_final);
             if (a.n_out > 1 && a.self_out < 0) __threadfence_system();  // direct peer stores: performed before the grid completes
@@ -612,7 +568,7 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
                 }
                 if (direct) {
                     n_final += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, valid[r]));
-                    if (valid[r]) finish(a.ord_rw[idx[r]].x, p);
+                    if (valid[r]) finish_row(a, a.view[c], a.ord_rw[idx[r]].x, p);
                 } else if (p != kNone) {
                     atomicMin(&a.pos[idx[r]], p);
                 }
@@ -645,31 +601,20 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// peer signal / wait (flags bound with rpk_peer_bind).  The persistent kernel signals from its last pusher; the
-// other select paths launch k_peer_signal behind their copy kernel; k_peer_wait is what remains of the fence.
+// peer signal / wait.  The persistent kernel signals from its last pusher; the other select paths and an empty shard
+// launch k_peer_signal behind their kernels, and so does rpk_peer_fence (signal and wait in one); k_peer_wait is the
+// wait half for a bound group.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void k_peer_signal(PeerFenceArgs a, uint32_t word0, uint32_t counter_word) {
+__global__ void k_peer_signal(PeerGroup g, uint32_t epoch, uint32_t wait) {
     pdl_wait();  // everything this stream did before (peer stores included) has completed
-    const uint32_t lane = threadIdx.x;
-    uint32_t e = 0;
-    if (lane == 0) { e = a.flags[a.my_rank][counter_word] + 1u; a.flags[a.my_rank][counter_word] = e; }
-    e = __shfl_sync(0xFFFFFFFFu, e, 0);
-    __threadfence_system();
-    if ((int)lane < a.n) {
-        *reinterpret_cast<volatile uint32_t*>(a.flags[lane] + word0 + a.my_rank) = e;
-        if (a.epoch) {  // epoch != 0 doubles as "wait here too" for this kernel (inline-wait mode)
-            const volatile uint32_t* mine = a.flags[a.my_rank] + word0 + lane;
-            while ((int32_t)(*mine - e) < 0) __nanosleep(32);
-            __threadfence_system();
-        }
-    }
+    signal_peers(g, kFlagSelect, kFlagSelectCtr, epoch, wait != 0);
 }
 
-__global__ void k_peer_wait(PeerFenceArgs a, uint32_t what) {
+__global__ void k_peer_wait(PeerGroup g, uint32_t what) {
     pdl_wait();  // the kernels that signalled for this rank have completed: the own epoch counters are final
     const uint32_t lane = threadIdx.x;
-    const volatile uint32_t* mine = a.flags[a.my_rank];
-    if ((int)lane < a.n) {
+    const volatile uint32_t* mine = g.flags[g.my_rank];
+    if ((int)lane < g.n) {
         if (what & 1u) { const uint32_t e = mine[kFlagSelectCtr]; while ((int32_t)(mine[kFlagSelect + lane] - e) < 0) __nanosleep(32); }
         if (what & 2u) { const uint32_t e = mine[kFlagStatusCtr]; while ((int32_t)(mine[kFlagStatus + lane] - e) < 0) __nanosleep(32); }
         __threadfence_system();
@@ -736,23 +681,21 @@ int launch_select_persist(const SelectArgs& args, const PersistPlan& pl, cudaStr
     const uint32_t blocks = chunks < k0ctas ? (chunks ? chunks : 1u) : k0ctas;
     k_pod_classify<<<blocks, kPThreads, 0, st>>>(a, pl.n_cursors);
     launch_pdl(k_pod_scatter, dim3(blocks), dim3(kPThreads), 0, st, t.pdl, a);
-    static thread_local int attr_dev = -1;  // the attribute is per device: set it once per (thread, device)
-    int dev = 0;
-    RPK_CUDA(cudaGetDevice(&dev));
-    if (attr_dev != dev) { RPK_CUDA(cudaFuncSetAttribute(k_select_persist, cudaFuncAttributeMaxDynamicSharedMemorySize, 224 * 1024)); attr_dev = dev; }
+    static thread_local int attr_dev = -1;
+    allow_smem(k_select_persist, 224 * 1024, &attr_dev);
     launch_pdl(k_select_persist, dim3(pl.grid), dim3(kPThreads), pl.smem_bytes, st, t.pdl, a, pa);
     RPK_CUDA(cudaGetLastError());
     return 3;
 }
 
-int launch_peer_signal(const PeerFenceArgs& a, uint32_t word0, cudaStream_t st) {
-    launch_pdl(k_peer_signal, dim3(1), dim3(32), 0, st, read_tune().pdl, a, word0, word0 == kFlagSelect ? kFlagSelectCtr : kFlagStatusCtr);
+int launch_peer_signal(const PeerGroup& g, uint32_t epoch, bool wait, cudaStream_t st) {
+    launch_pdl(k_peer_signal, dim3(1), dim3(32), 0, st, read_tune().pdl, g, epoch, wait ? 1u : 0u);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }
 
-int launch_peer_wait(const PeerFenceArgs& a, uint32_t what, cudaStream_t st) {
-    launch_pdl(k_peer_wait, dim3(1), dim3(32), 0, st, read_tune().pdl, a, what);
+int launch_peer_wait(const PeerGroup& g, uint32_t what, cudaStream_t st) {
+    launch_pdl(k_peer_wait, dim3(1), dim3(32), 0, st, read_tune().pdl, g, what);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

@@ -311,7 +311,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
             s_excl = excl; s_carry = 0;
             if (cid == n_ctas - 1) {  // the last CTA in slot order owns the count
                 *a.n_changed = excl + total;
-                for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_count[o][a.my_rank] = excl + total;
+                for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_count[o][a.peers.my_rank] = excl + total;
             }
         }
     }
@@ -357,20 +357,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
     // last CTA to finish: every look-back is over -- clean the state for the next call, then tell the peers
     for (uint32_t i = tid; i < n_ctas; i += kSThreads) a.tile_state[i] = 0ull;
     if (tid == 0) { a.tile_counter[0] = 0u; a.tile_counter[1] = 0u; }
-    if (!SLOTS && a.n_flags > 0 && warp == 0) {
-        uint32_t e = 0;
-        if (lane == 0) { e = a.flags[a.my_rank][33] + 1u; a.flags[a.my_rank][33] = e; }  // status epoch counter
-        e = __shfl_sync(0xFFFFFFFFu, e, 0);
-        __threadfence_system();
-        if ((int)lane < a.n_flags) {
-            *reinterpret_cast<volatile uint32_t*>(a.flags[lane] + 8 + a.my_rank) = e;
-            if (a.inline_wait) {  // the other half of the fence without a kernel of its own
-                const volatile uint32_t* mine = a.flags[a.my_rank] + 8 + lane;
-                while ((int32_t)(*mine - e) < 0) __nanosleep(32);
-                __threadfence_system();
-            }
-        }
-    }
+    if (!SLOTS && a.peers.n > 0 && warp == 0) signal_peers(a.peers, kFlagStatus, kFlagStatusCtr, 0, a.peers.inline_wait != 0);
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -494,19 +481,16 @@ uint32_t status_state_words(uint32_t N, uint32_t stride, int sm_count) {  // u64
 
 // SLOTS: a slot-list sweep, whose launch shape follows from the list length (a.N) exactly as a table's does from N
 template <bool SLOTS>
-static int launch_status(const StatusArgs& a, cudaStream_t st) {
+static int launch_status(const StatusArgs& a, int sm_count, cudaStream_t st) {
     if (a.N == 0) {
         if (a.n_changed) RPK_CUDA(cudaMemsetAsync(a.n_changed, 0, sizeof(uint32_t), st));
         // an empty shard of a sharded sweep still has to publish its (zero) count and signal: one tiny CTA does it
-        if (a.n_out == 0 && a.n_flags == 0) return 0;
+        if (a.n_out == 0 && a.peers.n == 0) return 0;
     }
     if (a.stride == 16 || a.stride == 32) {
-        int dev = 0, sms = 132;
-        RPK_CUDA(cudaGetDevice(&dev));
-        RPK_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
         const uint32_t n_units = (a.N + kUnit - 1) / kUnit;
         const bool big = a.N >= kBigTable;
-        const uint32_t warps = big ? 32u : 8u, max_grid = (uint32_t)sms;
+        const uint32_t warps = big ? 32u : 8u, max_grid = (uint32_t)sm_count;
         // one unit per warp until every SM has its CTA, then longer runs per warp
         uint32_t grid = (n_units + warps - 1) / warps;
         if (grid > max_grid) grid = max_grid;
@@ -526,34 +510,23 @@ static int launch_status(const StatusArgs& a, cudaStream_t st) {
         RPK_CUDA(cudaGetLastError());
         return 1;
     }
-    const int items = items_for_stride(a.stride);
+    const int items = items_for_stride(a.stride);  // 2 or 1: strides 16 / 32 took the streaming kernel above
     const uint32_t tiles = status_tiles(a.N, a.stride);
     const size_t smem = (size_t)kStThreads * items * (a.stride + 4);
-    static thread_local int attr_dev[3] = {-1, -1, -1};
-    int dev = 0;
-    RPK_CUDA(cudaGetDevice(&dev));
-    switch (items) {
-        case 4:  // strides 16 / 32 take the streaming kernel above
-            if constexpr (!SLOTS) {
-                if (attr_dev[0] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[0] = dev; }
-                k_status_diff<4><<<tiles, kStThreads, smem, st>>>(a);
-            }
-            break;
-        case 2:
-            if (attr_dev[1] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<2, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[1] = dev; }
-            k_status_diff<2, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
-            break;
-        default:
-            if (attr_dev[2] != dev) { RPK_CUDA(cudaFuncSetAttribute(k_status_diff<1, SLOTS>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024)); attr_dev[2] = dev; }
-            k_status_diff<1, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
-            break;
+    static thread_local int attr_dev[2] = {-1, -1};
+    if (items == 2) {
+        allow_smem(k_status_diff<2, SLOTS>, 160 * 1024, &attr_dev[0]);
+        k_status_diff<2, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
+    } else {
+        allow_smem(k_status_diff<1, SLOTS>, 160 * 1024, &attr_dev[1]);
+        k_status_diff<1, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
     }
     RPK_CUDA(cudaGetLastError());
     return 1;
 }
 
-int launch_status_diff(const StatusArgs& a, cudaStream_t st) {
-    return a.slots ? launch_status<true>(a, st) : launch_status<false>(a, st);
+int launch_status_diff(const StatusArgs& a, int sm_count, cudaStream_t st) {
+    return a.slots ? launch_status<true>(a, sm_count, st) : launch_status<false>(a, sm_count, st);
 }
 
 }  // namespace rpk
