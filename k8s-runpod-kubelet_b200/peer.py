@@ -19,27 +19,6 @@ def as_int32_tensor(ptr: int, n: int, device):
     return torch.as_tensor(_RawCudaBuffer(ptr, n, "<i4"), device=device)
 
 
-def exchange_peer_vectors(engine, n_elems: int, rank: int, world: int, device):
-    """-> (own vector as an int32 torch view, [device pointer of rank r's vector for r in range(world)])."""
-    import torch.distributed as dist
-
-    own_ptr, handle = engine.ipc_alloc(n_elems * 4)
-    handles = [None] * world
-    dist.all_gather_object(handles, handle)
-    ptrs = [own_ptr if r == rank else engine.ipc_open(handles[r]) for r in range(world)]
-    return as_int32_tensor(own_ptr, n_elems, device), ptrs
-
-
-def exchange_peer_flags(engine, rank: int, world: int):
-    """-> [device pointer of rank r's zero-initialised 64-word flag array for r in range(world)] (rpk_peer_fence)."""
-    import torch.distributed as dist
-
-    own_ptr, handle = engine.ipc_alloc(64 * 4)
-    handles = [None] * world
-    dist.all_gather_object(handles, handle)
-    return [own_ptr if r == rank else engine.ipc_open(handles[r]) for r in range(world)]
-
-
 def exchange_peer_buffer(engine, nbytes: int, rank: int, world: int):
     """-> (own device pointer, [device pointer of rank r's zero-initialised buffer for r in range(world)])."""
     import torch.distributed as dist
@@ -48,3 +27,14 @@ def exchange_peer_buffer(engine, nbytes: int, rank: int, world: int):
     handles = [None] * world
     dist.all_gather_object(handles, handle)
     return own_ptr, [own_ptr if r == rank else engine.ipc_open(handles[r]) for r in range(world)]
+
+
+def exchange_peer_vectors(engine, n_elems: int, rank: int, world: int, device):
+    """-> (own vector as an int32 torch view, [device pointer of rank r's vector for r in range(world)])."""
+    own_ptr, ptrs = exchange_peer_buffer(engine, n_elems * 4, rank, world)
+    return as_int32_tensor(own_ptr, n_elems, device), ptrs
+
+
+def exchange_peer_flags(engine, rank: int, world: int):
+    """-> [device pointer of rank r's zero-initialised 64-word flag array for r in range(world)] (rpk_peer_fence)."""
+    return exchange_peer_buffer(engine, 64 * 4, rank, world)[1]

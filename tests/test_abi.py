@@ -11,10 +11,50 @@ import rpk
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-def header_symbols():
+def header_source():
+    """include/rpk.h without comments and preprocessor lines, whitespace collapsed (multi-line declarations joined)"""
     src = open(os.path.join(ROOT, "include", "rpk.h")).read()
     src = re.sub(r"/\*.*?\*/", "", src, flags=re.S)
-    return sorted(set(re.findall(r"\b(rpk_[a-z0-9_]+)\s*\(", src)))
+    src = re.sub(r"^\s*#.*$", "", src, flags=re.M)
+    return " ".join(src.split())
+
+
+def header_symbols():
+    return sorted(set(re.findall(r"\b(rpk_[a-z0-9_]+)\s*\(", header_source())))
+
+
+def header_prototypes():
+    """-> {name: (return type, [parameter declarations])}"""
+    protos = {}
+    for ret, name, params in re.findall(r"(?:^|(?<=[;{}]))\s*([A-Za-z_][\w\s*]*?)\s*\b(rpk_\w+)\s*\(([^()]*)\)\s*;", header_source()):
+        params = [p.strip() for p in params.split(",")]
+        protos[name] = (ret.strip(), [] if params == ["void"] else params)
+    return protos
+
+
+# C scalar type -> (kind, bytes, signed)
+C_SCALARS = {"int": ("int", 4, True), "unsigned": ("int", 4, False), "int32_t": ("int", 4, True), "uint32_t": ("int", 4, False),
+             "uint64_t": ("int", 8, False), "size_t": ("int", C.sizeof(C.c_size_t), False), "float": ("float", 4, True)}
+
+
+def c_sig(decl: str, is_param: bool):
+    """C type of a parameter declaration (with its name) or of a return type -> "void", "pointer" or a C_SCALARS entry"""
+    if "*" in decl or "[" in decl:
+        return "pointer"
+    words = [w for w in decl.split() if w != "const"]
+    if is_param:
+        words = words[:-1]
+    return "void" if words == ["void"] else C_SCALARS[" ".join(words)]
+
+
+def ctypes_sig(t):
+    if t is None:
+        return "void"
+    if t in (C.c_void_p, C.c_char_p) or issubclass(t, C._Pointer):
+        return "pointer"
+    if t in (C.c_float, C.c_double):
+        return ("float", C.sizeof(t), True)
+    return ("int", C.sizeof(t), t(-1).value < 0)
 
 
 def test_library_exports_every_declared_symbol():
@@ -24,6 +64,27 @@ def test_library_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(lib, name), f"{name} declared in include/rpk.h but not exported by librpk.so"
     assert sorted(rpk._ffi.SYMBOLS) == declared, "python binding out of sync with include/rpk.h"
+
+
+def test_binding_types_match_the_header():
+    """Every ctypes declaration has the header's parameter count, and each parameter and return value its C type's kind
+    (pointer or scalar), width and signedness: a size_t declared 32-bit or a uint32_t declared signed would truncate or
+    sign-extend silently.  RpkStats has rpk_stats's fields, in order, with their types."""
+    protos = header_prototypes()
+    assert sorted(protos) == header_symbols()
+    for name, (restype, argtypes) in rpk._ffi.ABI.items():
+        ret, params = protos[name]
+        assert len(argtypes) == len(params), f"{name}: {len(argtypes)} argtypes for {len(params)} parameters"
+        for i, (t, p) in enumerate(zip(argtypes, params)):
+            assert ctypes_sig(t) == c_sig(p, True), f"{name} parameter {i} `{p}` declared as {t.__name__}"
+        assert ctypes_sig(restype) == c_sig(ret, False), f"{name}: returns `{ret}`, restype {restype}"
+
+    body = re.search(r"typedef struct rpk_stats \{(.*?)\} rpk_stats;", header_source()).group(1)
+    fields = []
+    for decl in filter(None, (d.strip() for d in body.split(";"))):
+        ctype, names = decl.split(None, 1)
+        fields += [(n.strip(), C_SCALARS[ctype]) for n in names.split(",")]
+    assert [(n, ctypes_sig(t)) for n, t in rpk._ffi.RpkStats._fields_] == fields
 
 
 def test_abi_version_and_null_handling():
