@@ -167,15 +167,15 @@ int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaSt
         ln.key.reserve(P); ln.ord_rw.reserve(P);
         const size_t hdr_words = persist_hdr_words(pl);
         const bool fresh = !ln.hist.p || hdr_words > ln.hdr.cap;
-        ln.hist.reserve(2 * kMaxClasses); ln.cursor.reserve(2 * kMaxClasses); ln.hdr.reserve(hdr_words);
+        ln.hist.reserve(2 * kMaxClasses); ln.hdr.reserve(hdr_words);
+        ln.k0_base.reserve((size_t)pl.k0_blocks * kMaxClasses);  // written by k_pod_classify before k_pod_scatter reads it: never zeroed
         if (fresh || ln.persist_dirty) {  // zero between calls by construction (k_pod_classify's last block, the pushers)
             RPK_CUDA(cudaMemset(ln.hist.p, 0, ln.hist.cap * sizeof(uint32_t)));
-            RPK_CUDA(cudaMemset(ln.cursor.p, 0, ln.cursor.cap * sizeof(uint32_t)));
             RPK_CUDA(cudaMemset(ln.hdr.p, 0, ln.hdr.cap * sizeof(uint32_t)));
             RPK_CUDA(cudaDeviceSynchronize());
             ln.persist_dirty = false;
         }
-        a.key = ln.key.p; a.ord_rw = ln.ord_rw.p; a.hist = ln.hist.p; a.cursor = ln.cursor.p; a.hdr = ln.hdr.p;
+        a.key = ln.key.p; a.ord_rw = ln.ord_rw.p; a.hist = ln.hist.p; a.k0_base = ln.k0_base.p; a.hdr = ln.hdr.p;
     }
     // the lane's counters are suspect until every launch of the call was accepted
     ln.ctrs_dirty = true; ln.persist_dirty = true;

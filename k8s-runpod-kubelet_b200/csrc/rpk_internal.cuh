@@ -138,8 +138,8 @@ struct SelectArgs {
     uint32_t nsub;       // 64-chunk sub-ranges of the transposed view
     uint16_t* key;       // [P] row class (0xFFFF: neither cloud)
     uint2* ord_rw;       // [P] {row id, threshold word} in class order (pos[] is indexed the same way): ONE scattered store per row
-    uint32_t* hist;      // [kMaxClasses] rows per class       } zero between calls (k_pod_classify's last block)
-    uint32_t* cursor;    // [kMaxClasses] class write cursors
+    uint32_t* hist;      // [kMaxClasses] rows per class: zero between calls (the grid kernel's block 0 clears it)
+    uint32_t* k0_base;   // [K0 CTAs][kMaxClasses] first position of each class-sort CTA inside each class it has rows of
     uint32_t* hdr;       // control words, kHdr*
     PeerGroup peers;     // bound with rpk_peer_bind: the gather signals every peer once its slice has landed
     uint32_t tune_natural_order;  // tuning hook (RPK_TUNE=order=natural): row tiles in group order instead of heaviest first
@@ -265,7 +265,7 @@ int launch_status_diff(const StatusArgs& a, int sm_count, cudaStream_t st);
 int launch_peer_signal(const PeerGroup& g, uint32_t epoch, bool wait, cudaStream_t st);
 int launch_peer_wait(const PeerGroup& g, uint32_t what, cudaStream_t st);
 // persistent bit-sliced select (select_persist.cu)
-struct PersistPlan { uint32_t S, per, qspan, grid, smem_bytes, slice, n_cursors; int sm_count; };
+struct PersistPlan { uint32_t S, per, qspan, grid, smem_bytes, slice, n_cursors, k0_blocks; int sm_count; };
 PersistPlan persist_plan(const SelectArgs& a, int sm_count);  // a.pk.bm_words and a.nsub non-zero
 uint32_t persist_hdr_words(const PersistPlan& pl);
 int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream_t st);
@@ -338,7 +338,7 @@ struct DeviceState {
         DevBuf<int32_t> p_req_mem, p_req_vcpu, p_req_ram; DevBuf<double> p_max_price; DevBuf<uint8_t> p_cloud;
         DevBuf<int32_t> top5;
         DevBuf<uint32_t> rw, order, pos, ctrs;
-        DevBuf<uint16_t> key; DevBuf<uint2> ord_rw; DevBuf<uint32_t> hist, cursor, hdr;  // persistent path
+        DevBuf<uint16_t> key; DevBuf<uint2> ord_rw; DevBuf<uint32_t> hist, k0_base, hdr;  // persistent path
         bool ctrs_dirty = false;  // a select on this lane failed between its launches: re-zero the counters before the next one
         bool persist_dirty = false;
     };

@@ -3,10 +3,12 @@
 // is how the mask words reach the lanes and who owns a stage of the offer table:
 //
 //   k_pod_classify   row -> rank thresholds -> class key (cloud, thresholds; see class_key for the order); one wave of
-//                    CTAs, each looping over 512-row chunks: shared-memory histogram -> global class counts; fills
-//                    pos[] = none; block 0 resets the queue state of the grid kernel.
-//   k_pod_scatter    counting-sort scatter, same CTA shape: every CTA scans the class counts itself, reserves its rows
-//                    per class with one atomic per non-empty class and writes ONE {row, thresholds} pair per row in
+//                    CTAs, each looping over 512-row chunks: shared-memory histogram -> global class counts, one
+//                    atomic per non-empty class whose return value is the CTA's first position inside the class
+//                    (k0_base); fills pos[] = none when the grid kernel merges through it; block 0 resets the queue
+//                    state of the grid kernel.
+//   k_pod_scatter    counting-sort scatter, same CTAs and rows: every CTA scans the class counts itself, adds its
+//                    class bases from classify and writes ONE {row, thresholds} pair per row in
 //                    class order (ord_rw[]); block 0 publishes per-group row / work totals (a group is a cloud, or a
 //                    (cloud, mem threshold) pair on the per-mem-threshold view).  Rows of neither cloud are final here
 //                    (-1, runpod_client.go:469-475).
@@ -45,6 +47,7 @@ constexpr int kPThreads = 512;
 constexpr int kPWarps = kPThreads / 32;
 constexpr int kCopyGroups = 8;
 constexpr int kRpl = 2;  // pod rows per lane
+constexpr int kK0Batch = 4;  // K0: rows per thread whose loads are in flight together (one per 512-row chunk of the CTA)
 constexpr uint32_t kSubWords = kSubStride;
 
 // ---------------------------------------------------------------------------------------------------------
@@ -173,8 +176,11 @@ __device__ __forceinline__ void push_tail(const SelectArgs& a) {
 // ---------------------------------------------------------------------------------------------------------
 // K0a: classify.  No block waits for another one: the class counts are only added to here (the grid kernel of the
 // previous call zeroed them once the scatter kernel was done with them); block 0 resets the grid kernel's queue cursors.
+// Both K0 kernels run four CTAs per SM in one wave (launch_select_persist), so they are held to 32 registers.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kPThreads) k_pod_classify(SelectArgs a, uint32_t n_cursors) {
+// fill_pos: the grid kernel merges row blocks through pos[] (more than one item per row block); a direct plan never
+// reads it, so its 4 bytes per row are not written.
+__global__ void __launch_bounds__(kPThreads, 4) k_pod_classify(SelectArgs a, uint32_t n_cursors, uint32_t fill_pos) {
     pdl_trigger();  // k_pod_scatter may be scheduled; it waits before it reads anything written here
     __shared__ int32_t s_dist[3][64];
     __shared__ uint32_t s_hist[kMaxClasses];
@@ -191,107 +197,135 @@ __global__ void __launch_bounds__(kPThreads) k_pod_classify(SelectArgs a, uint32
         if (tid == 0) { a.hdr[kHdrPushed] = 0u; a.hdr[kHdrRowsDone] = 0u; }
     }
     __syncthreads();
-    // a CTA takes 512-row chunks b, b + grid, ...: the 4096-bin histogram (zeroing, flush) is paid once per CTA, not per chunk
-    for (uint32_t p = blockIdx.x * kPThreads + tid; p < a.P; p += gridDim.x * kPThreads) {
-        const uint8_t c = a.cloud ? a.cloud[p] : (uint8_t)RPK_CLOUD_SECURE;
-        const uint32_t tm1 = lb_smem(s_dist[0], a.D[0], a.req_mem[p]);
-        const uint32_t tv = lb_smem(s_dist[1], a.D[1], a.req_vcpu ? a.req_vcpu[p] : 0);
-        const uint32_t tr = lb_smem(s_dist[2], a.D[2], a.req_ram ? a.req_ram[p] : 0);
-        a.rw[p] = tm1 | ((a.pk.bm_off_vcpu + tv) << 8) | ((a.pk.bm_off_ram + tr) << 16);  // bitmap words (the top-5 kernel reads these)
-        uint32_t key = 0xFFFFu;  // neither SECURE nor COMMUNITY: nothing is feasible (runpod_client.go:469-475)
-        if (c <= 1) { key = class_key(cd, c, tm1, tv, tr); atomicAdd(&s_hist[key], 1u); }
-        a.key[p] = (uint16_t)key;
-        a.pos[p] = kNone;  // "no feasible offer yet" for sorted position p (positions [0, valid rows) are used: a coalesced fill)
+    // a CTA takes 512-row chunks b, b + grid, ...: the 4096-bin histogram (zeroing, flush) is paid once per CTA, not per
+    // chunk.  A thread loads the columns of its next kK0Batch rows before it searches any of them, so their DRAM trips
+    // overlap instead of one per row.
+    const uint32_t stride = gridDim.x * kPThreads;
+    for (uint32_t p0 = blockIdx.x * kPThreads + tid; p0 < a.P; p0 += kK0Batch * stride) {
+        uint32_t c[kK0Batch];
+        int32_t m[kK0Batch], v[kK0Batch], r[kK0Batch];
+#pragma unroll
+        for (int u = 0; u < kK0Batch; ++u) {
+            const uint32_t p = p0 + (uint32_t)u * stride;
+            const bool ok = p < a.P;
+            c[u] = !ok ? 2u : a.cloud ? a.cloud[p] : (uint32_t)RPK_CLOUD_SECURE;
+            m[u] = ok ? a.req_mem[p] : 0;
+            v[u] = ok && a.req_vcpu ? a.req_vcpu[p] : 0;
+            r[u] = ok && a.req_ram ? a.req_ram[p] : 0;
+        }
+#pragma unroll
+        for (int u = 0; u < kK0Batch; ++u) {
+            const uint32_t p = p0 + (uint32_t)u * stride;
+            if (p >= a.P) break;
+            const uint32_t tm1 = lb_smem(s_dist[0], a.D[0], m[u]);
+            const uint32_t tv = lb_smem(s_dist[1], a.D[1], v[u]);
+            const uint32_t tr = lb_smem(s_dist[2], a.D[2], r[u]);
+            a.rw[p] = tm1 | ((a.pk.bm_off_vcpu + tv) << 8) | ((a.pk.bm_off_ram + tr) << 16);  // bitmap words (the top-5 kernel reads these)
+            uint32_t key = 0xFFFFu;  // neither SECURE nor COMMUNITY: nothing is feasible (runpod_client.go:469-475)
+            if (c[u] <= 1) { key = class_key(cd, c[u], tm1, tv, tr); atomicAdd(&s_hist[key], 1u); }
+            a.key[p] = (uint16_t)key;
+            if (fill_pos) a.pos[p] = kNone;  // "no feasible offer yet" for sorted position p (positions [0, valid rows) are used: a coalesced fill)
+        }
     }
     __syncthreads();
-    for (uint32_t i = tid; i < cd.C; i += kPThreads) { const uint32_t v = s_hist[i]; if (v) atomicAdd(&hist[i], v); }
+    // flush: one atomic per non-empty class.  What it returns -- the rows of the class that CTAs before this one flushed --
+    // is this CTA's first position inside the class, which the scatter kernel reads back instead of counting its rows
+    // and reserving them again.  Class i is flushed by thread i % 512, whose <= 8 atomics go out back to back.
+    uint32_t* base = a.k0_base + (size_t)blockIdx.x * kMaxClasses;
+    constexpr uint32_t kPer = kMaxClasses / kPThreads;
+    uint32_t n[kPer], got[kPer];
+#pragma unroll
+    for (uint32_t k = 0; k < kPer; ++k) { const uint32_t i = tid + k * kPThreads; n[k] = i < cd.C ? s_hist[i] : 0u; }
+#pragma unroll
+    for (uint32_t k = 0; k < kPer; ++k) got[k] = n[k] ? atomicAdd(&hist[tid + k * kPThreads], n[k]) : 0u;
+#pragma unroll
+    for (uint32_t k = 0; k < kPer; ++k) if (n[k]) base[tid + k * kPThreads] = got[k];
+}
+
+// Block 0 of the scatter: rows and mask-word work per row group, which the grid kernel shares its CTAs out by.  A group
+// is a run of classes, so warp w sums groups w, w + 16, ... over the class totals (L2): a lane per class, the work in
+// 64 bits per lane, then a warp reduction -- no shared-memory atomics.
+__device__ __forceinline__ void publish_group_totals(const SelectArgs& a, const ClassDims& cd) {
+    const uint32_t tid = threadIdx.x, lane = tid & 31;
+    const uint32_t n_groups = cd.slice ? 2u * cd.Dm1 : 2u, per_group = cd.C / n_groups;  // class_group
+    for (uint32_t g = tid >> 5; g < n_groups; g += kPWarps) {
+        uint32_t rows = 0;
+        unsigned long long work = 0ull;
+        for (uint32_t i = g * per_group + lane; i < (g + 1) * per_group; i += 32) {
+            const uint32_t n = __ldcg(a.hist + i);
+            rows += n; work += (unsigned long long)n * class_weight(cd, i);
+        }
+#pragma unroll
+        for (int d = 16; d; d >>= 1) { rows += __shfl_xor_sync(0xFFFFFFFFu, rows, d); work += __shfl_xor_sync(0xFFFFFFFFu, work, d); }
+        if (lane == 0) {
+            a.hdr[kHdrGroupRows + g] = rows;
+            a.hdr[kHdrGroupWork + g] = (uint32_t)min(work >> 2, 0xFFFFFFFFull);
+        }
+    }
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// K0b: scatter into class order.  A CTA takes 512-row chunks b, b + grid, ... (the same rows in both passes below).
-// Pass 1 counts its rows per class in shared memory while the class totals arrive from L2; every CTA scans the totals
-// itself (<= 4096 words: cheaper than a serial "last block" phase in the kernel before) and adds its counts to the
-// global class cursors with one atomic per non-empty class, which turns its shared table into "next free position per
-// class"; pass 2 re-reads the keys (L2 hits) and hands every row its position.  The per-CTA cost of the 4096-bin
-// tables is paid once per CTA, not once per 512 rows.  Block 0 also publishes the per-group row / work totals the grid
-// kernel shares its CTAs out by.
+// K0b: scatter into class order.  A CTA takes the same 512-row chunks b, b + grid, ... as in k_pod_classify.  Every
+// CTA scans the <= 4096 class totals itself (cheaper than a serial "last block" phase in the kernel before) and adds
+// its own first position inside each class, which its classify flush returned: that is the shared table "next free
+// position per class", with no counting pass and no reservation here.  Pass 2 re-reads the keys (L2 hits) and hands
+// every row its position.  The per-CTA cost of the 4096-bin table is paid once per CTA, not once per 512 rows.  Block
+// 0 also publishes the per-group row / work totals the grid kernel shares its CTAs out by.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kPThreads) k_pod_scatter(SelectArgs a) {
-    __shared__ uint32_t s_cnt[kMaxClasses], s_base[kMaxClasses];
+__global__ void __launch_bounds__(kPThreads, 4) k_pod_scatter(SelectArgs a) {
+    __shared__ uint32_t s_base[kMaxClasses];
     __shared__ uint32_t s_warp[kPWarps];
-    __shared__ unsigned long long s_work[kMaxGroups];
-    __shared__ uint32_t s_rows[kMaxGroups];
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const ClassDims cd = class_dims(a.D, a.slice);
-    const uint32_t n_groups = cd.slice ? 2u * cd.Dm1 : 2u;
-    for (uint32_t i = tid; i < cd.C; i += kPThreads) s_cnt[i] = 0u;
-    if (tid < kMaxGroups) { s_work[tid] = 0ull; s_rows[tid] = 0u; }
-    __syncthreads();
-    pdl_wait();     // k_pod_classify has completed: keys, rw, class counts
+    pdl_wait();     // k_pod_classify has completed: keys, rw, class counts, per-CTA class bases
     pdl_trigger();  // the grid kernel may be scheduled; it waits before it reads anything written here
-    const uint32_t* hist = a.hist;
-    uint32_t* cursor = a.cursor;
     const uint32_t stride = gridDim.x * kPThreads;
-    // the class totals first (independent of pass 1: the loads overlap it); thread t owns classes [8t, 8t + 8)
+    // thread t owns classes [8t, 8t + 8): their totals and this CTA's bases, two 16-byte loads each (both buffers hold
+    // kMaxClasses words per row; words at or above the class count are not used)
     constexpr uint32_t kPer = kMaxClasses / kPThreads;
-    uint32_t v[kPer], sum = 0;
+    static_assert(kPer == 8, "two uint4 per thread");
+    const uint4* h4 = reinterpret_cast<const uint4*>(a.hist + tid * kPer);
+    const uint4* b4 = reinterpret_cast<const uint4*>(a.k0_base + (size_t)blockIdx.x * kMaxClasses + tid * kPer);
+    const uint4 h0 = __ldcg(h4), h1 = __ldcg(h4 + 1), b0 = __ldcg(b4), b1 = __ldcg(b4 + 1);
+    const uint32_t v[kPer] = {h0.x, h0.y, h0.z, h0.w, h1.x, h1.y, h1.z, h1.w}, b[kPer] = {b0.x, b0.y, b0.z, b0.w, b1.x, b1.y, b1.z, b1.w};
+    uint32_t sum = 0;
 #pragma unroll
-    for (uint32_t k = 0; k < kPer; ++k) {
-        const uint32_t i = tid * kPer + k;
-        v[k] = i < cd.C ? __ldcg(hist + i) : 0u;
-    }
-    // pass 1: this CTA's rows per class
-    for (uint32_t p = blockIdx.x * kPThreads + tid; p < a.P; p += stride) {
-        const uint32_t key = (uint32_t)a.key[p];
-        if (key != 0xFFFFu) atomicAdd(&s_cnt[key], 1u);
-    }
-#pragma unroll
-    for (uint32_t k = 0; k < kPer; ++k) sum += v[k];
+    for (uint32_t k = 0; k < kPer; ++k) sum += tid * kPer + k < cd.C ? v[k] : 0u;
     uint32_t inc = sum;
 #pragma unroll
     for (int d = 1; d < 32; d <<= 1) { const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, inc, d); if ((int)lane >= d) inc += n; }
     if (lane == 31) s_warp[warp] = inc;
-    __syncthreads();  // s_warp, and every row of pass 1 is counted
+    __syncthreads();
     uint32_t run = inc - sum;
     for (uint32_t w = 0; w < warp; ++w) run += s_warp[w];
-    if (blockIdx.x == 0) {  // this thread's classes, one run per group
-        uint32_t g_run = 0, rows = 0;
-        unsigned long long work = 0ull;
 #pragma unroll
-        for (uint32_t k = 0; k < kPer; ++k) {
-            const uint32_t i = tid * kPer + k;
-            if (!v[k]) continue;
-            const uint32_t g = class_group(cd, i);
-            if (rows && g != g_run) { atomicAdd(&s_rows[g_run], rows); atomicAdd(&s_work[g_run], work); rows = 0; work = 0ull; }
-            g_run = g; rows += v[k]; work += (unsigned long long)v[k] * class_weight(cd, i);
-        }
-        if (rows) { atomicAdd(&s_rows[g_run], rows); atomicAdd(&s_work[g_run], work); }
-    }
-    // class start + this CTA's share of the class = the first position this CTA may use
-#pragma unroll
-    for (uint32_t k = 0; k < kPer; ++k) {
+    for (uint32_t k = 0; k < kPer; ++k) {  // class start + this CTA's first position inside the class
         const uint32_t i = tid * kPer + k;
-        if (i < cd.C) { const uint32_t c = s_cnt[i]; s_base[i] = run + (c ? atomicAdd(&cursor[i], c) : 0u); }
-        run += v[k];
+        if (i < cd.C) { s_base[i] = run + b[k]; run += v[k]; }
     }
     __syncthreads();
-    if (blockIdx.x == 0 && tid < n_groups) {
-        a.hdr[kHdrGroupRows + tid] = s_rows[tid];
-        a.hdr[kHdrGroupWork + tid] = (uint32_t)min(s_work[tid] >> 2, 0xFFFFFFFFull);
-    }
-    // pass 2: positions (the order inside a class is arbitrary -- results go back by row id)
+    if (blockIdx.x == 0) publish_group_totals(a, cd);
+    // pass 2: positions (the order inside a class is arbitrary -- results go back by row id).  kK0Batch chunks at a
+    // time: every key and threshold word is loaded, then every position taken, then every pair stored.
     uint32_t n_neither = 0;
-    for (uint32_t p0 = blockIdx.x * kPThreads; p0 < a.P; p0 += stride) {  // whole warps: the ballot below
-        const uint32_t p = p0 + tid;
-        const uint32_t key = p < a.P ? (uint32_t)a.key[p] : 0u;
-        const bool neither = p < a.P && key == 0xFFFFu;
-        if (p < a.P && !neither) {
-            const uint32_t dst = atomicAdd(&s_base[key], 1u);
-            const uint32_t w = a.rw[p];
-            a.ord_rw[dst] = make_uint2(p, cd.slice ? slice_rw(cd, a.pk, w) : w);  // the one scattered store of the sort
+    for (uint32_t c0 = blockIdx.x * kPThreads; c0 < a.P; c0 += kK0Batch * stride) {  // whole warps: the ballot below
+        uint32_t key[kK0Batch], w[kK0Batch], dst[kK0Batch];
+#pragma unroll
+        for (int u = 0; u < kK0Batch; ++u) {
+            const uint32_t p = c0 + (uint32_t)u * stride + tid;
+            key[u] = p < a.P ? (uint32_t)a.key[p] : kNone;
+            w[u] = p < a.P ? a.rw[p] : 0u;
         }
-        if (neither) finish_row_no_cloud(a, p);
-        n_neither += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, neither));
+#pragma unroll
+        for (int u = 0; u < kK0Batch; ++u) dst[u] = key[u] < 0xFFFFu ? atomicAdd(&s_base[key[u]], 1u) : 0u;
+#pragma unroll
+        for (int u = 0; u < kK0Batch; ++u) {
+            const uint32_t p = c0 + (uint32_t)u * stride + tid;
+            const bool neither = key[u] == 0xFFFFu;
+            if (key[u] < 0xFFFFu) a.ord_rw[dst[u]] = make_uint2(p, cd.slice ? slice_rw(cd, a.pk, w[u]) : w[u]);  // the one scattered store of the sort
+            if (neither) finish_row_no_cloud(a, p);
+            n_neither += (uint32_t)__popc(__ballot_sync(0xFFFFFFFFu, neither));
+        }
     }
     if (n_neither) count_rows_done(a, n_neither);
 }
@@ -403,9 +437,9 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
     }
     pdl_wait();     // k_pod_scatter (and k_pod_classify before it) has completed
     pdl_trigger();  // a dependent (the peer wait) may be scheduled; it waits for this grid to complete
-    // the scatter kernel is done with the class counts and cursors: zero them for the next call (all kMaxClasses words --
-    // the table, and with it the class count, may change between calls)
-    if (blockIdx.x == 0) for (uint32_t i = tid; i < kMaxClasses; i += kPThreads) { a.hist[i] = 0u; a.cursor[i] = 0u; }
+    // the scatter kernel is done with the class counts: zero them for the next call (all kMaxClasses words -- the table,
+    // and with it the class count, may change between calls)
+    if (blockIdx.x == 0) for (uint32_t i = tid; i < kMaxClasses; i += kPThreads) a.hist[i] = 0u;
     if (tid < 32) {
         uint32_t row_run = 0, blk_run = 0, n_ne = 0;
         for (uint32_t g0 = 0; g0 < pa.groups; g0 += 32) {
@@ -655,6 +689,13 @@ PersistPlan persist_plan(const SelectArgs& a, int sm_count) {
     if (Qi > per) Qi = per;
     pl.qspan = (uint32_t)((per + Qi - 1) / Qi);
     pl.n_cursors = (pl.slice ? 2u * (a.D[0] + 1u) : 2u) * pl.S;
+    // K0: one wave of CTAs (four per SM), each looping over 512-row chunks.  Four fill an SM's threads, so a status
+    // sweep enqueued beside the select waits for K0 and then runs beside K1.  Three per SM would let the sweep in
+    // beside K0, but the two then share HBM and K0 is on the select's critical path: with a 1M-slot sweep beside it, a
+    // 1M-row select took 383 us that way against 376 us with four (H100 SXM, 400 W, profiles/h100_step_sweep.json).
+    const uint32_t chunks = (a.P + kPThreads - 1) / kPThreads;
+    const uint32_t k0ctas = t.k0ctas > 0 ? (uint32_t)t.k0ctas : 4u * (uint32_t)sm_count;
+    pl.k0_blocks = chunks < k0ctas ? (chunks ? chunks : 1u) : k0ctas;
     return pl;
 }
 
@@ -672,14 +713,10 @@ int launch_select_persist(const SelectArgs& args, const PersistPlan& pl, cudaStr
         tickets += (nsubs + pl.qspan - 1) / pl.qspan;
     }
     pa.tickets_per_block = tickets;
-    // K0: one wave of CTAs (four per SM), each looping over 512-row chunks.  Four fill an SM's threads, so a status
-    // sweep enqueued beside the select waits for K0 and then runs beside K1.  Three per SM would let the sweep in
-    // beside K0, but the two then share HBM and K0 is on the select's critical path: with a 1M-slot sweep beside it, a
-    // 1M-row select took 383 us that way against 376 us with four (H100 SXM, 400 W, profiles/h100_step_sweep.json).
-    const uint32_t chunks = (a.P + kPThreads - 1) / kPThreads;
-    const uint32_t k0ctas = t.k0ctas > 0 ? (uint32_t)t.k0ctas : 4u * (uint32_t)pl.sm_count;
-    const uint32_t blocks = chunks < k0ctas ? (chunks ? chunks : 1u) : k0ctas;
-    k_pod_classify<<<blocks, kPThreads, 0, st>>>(a, pl.n_cursors);
+    // K0 over pl.k0_blocks CTAs: both kernels must use the same grid (a scatter CTA reads the class bases its classify
+    // twin wrote for the same rows)
+    const uint32_t blocks = pl.k0_blocks;
+    k_pod_classify<<<blocks, kPThreads, 0, st>>>(a, pl.n_cursors, pa.tickets_per_block != 1 ? 1u : 0u);
     launch_pdl(k_pod_scatter, dim3(blocks), dim3(kPThreads), 0, st, t.pdl, a);
     static thread_local int attr_dev = -1;
     allow_smem(k_select_persist, 224 * 1024, &attr_dev);
