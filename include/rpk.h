@@ -138,6 +138,26 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
                              const uint8_t* d_cloud, int n_out, int32_t* const* d_best_full, uint32_t row0,
                              int32_t* d_top5, void* stream);
 
+/* The same gather carrying the whole gpuTypeIds lists: one-process-per-GPU callers that deploy with the list (as
+ * GetGPUTypes + PrepareRunPodParameters do, runpod_client.go:497-509, :1339) get every pod's list without a second
+ * collective.
+ *   - Outputs: the shard's results land at [row0, row0+P) of every d_best_full[o], exactly as rpk_select_device_gather
+ *     puts them (same rules, direct-store fallback included); its lists land at elements [5*row0, 5*(row0+P)) of every
+ *     d_top5_full[o], in rpk_select's top5 order and -1 padding.  n_out counts both arrays.
+ *   - Placement: one of the d_top5_full vectors must live on GPU `shard` and all of them must share its 16-byte phase;
+ *     the top-5 kernel writes that one, and the 16-byte push kernel copies the finished lists to the others.
+ *   - One signal: with flags bound (rpk_peer_bind) and n_out > 1 the call signals the select epoch ONCE, behind the
+ *     lists' push -- after both slices have reached every vector -- so a peer past rpk_peer_wait(what = 1) or the inline
+ *     wait can read both.  The flag words move exactly as for rpk_select_device_gather (+1 on word my_rank of every
+ *     peer and on word 32).  P == 0 signals and writes nothing.
+ *   - RPK_EINVAL, before anything is enqueued and without signalling: no top-5 vector on GPU `shard`, top-5 vectors of
+ *     different 16-byte phase, a NULL vector pointer, n_out outside 1..8, or 5*P beyond uint32_t.
+ *   - After one call of a given size the function only enqueues launches (CUDA-graph capturable). */
+int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb,
+                                  const int32_t* d_req_vcpu, const int32_t* d_req_ram_gb, const double* d_max_price,
+                                  const uint8_t* d_cloud, int n_out, int32_t* const* d_best_full,
+                                  int32_t* const* d_top5_full, uint32_t row0, void* stream);
+
 /* Cross-process peer vectors for one-process-per-GPU callers (torchrun-style): allocate a plain cudaMalloc
  * buffer on GPU `shard` and export its 64-byte CUDA IPC handle; another process opens the handle and gets a
  * device pointer it can pass in d_best_full[] of rpk_select_device_gather (peer access over NVLink is

@@ -136,8 +136,9 @@ struct PodCols { const int32_t* req_mem; const int32_t* req_vcpu; const int32_t*
 
 // One select on ds in lane ln's scratch: `a` holds the pod columns, P and the outputs; this adds the offer views and the
 // scratch and launches on st.  A bit-sliced table takes the persistent kernel above the fused kernel's batch size and
-// the fused kernel otherwise (which also serves an empty table at any batch size).  Returns the kernels launched.
-int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaStream_t st) {
+// the fused kernel otherwise (which also serves an empty table at any batch size).  t5: the top-5 lists' gather, if
+// any.  Returns the kernels launched.
+int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaStream_t st, const Top5Gather* t5 = nullptr) {
     for (int c = 0; c < 2; ++c) {
         a.view[c].packed = ds.v_packed[c].p; a.view[c].bitmap = ds.v_bitmap[c].p; a.view[c].bitmapT = ds.v_bitmapT[c].p;
         a.view[c].bitmapM = ds.pk.slice_rows ? ds.v_bitmapM[c].p : nullptr; a.view[c].wide = ds.v_wide[c].p;
@@ -179,7 +180,7 @@ int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaSt
     }
     // the lane's counters are suspect until every launch of the call was accepted
     ln.ctrs_dirty = true; ln.persist_dirty = true;
-    const int n = launch_select(a, R, persist ? &pl : nullptr, ds.sm_count, st);
+    const int n = launch_select(a, R, persist ? &pl : nullptr, ds.sm_count, st, t5);
     ln.ctrs_dirty = false; ln.persist_dirty = false;
     return n;
 }
@@ -209,12 +210,16 @@ struct ScratchGuard {
     }
 };
 
-// Which of the output vectors lives on GPU `shard` (the others are peers' memory); -1 if none does.  Vectors this ctx
+// The push kernel moves 16-byte units: every vector must share the slice's alignment.
+bool same_phase(int n_out, int32_t* const* ptrs) {
+    for (int o = 1; o < n_out; ++o)
+        if (((uintptr_t)ptrs[o] & 15u) != ((uintptr_t)ptrs[0] & 15u)) return false;
+    return true;
+}
+
+// Which of the vectors lives on GPU `shard` (the others are peers' memory); -1 if none does.  Vectors this ctx
 // allocated (rpk_ipc_alloc) or mapped from a peer (rpk_ipc_open) are known exactly; anything else is asked of the driver.
-int find_local_vector(const rpk_ctx* ctx, int shard, int dev, int n_out, int32_t* const* ptrs) {
-    if (n_out == 1) return 0;
-    for (int o = 1; o < n_out; ++o)  // the push kernel moves 16-byte units: every vector must share the slice's alignment
-        if (((uintptr_t)ptrs[o] & 15u) != ((uintptr_t)ptrs[0] & 15u)) return -1;
+int local_vector(const rpk_ctx* ctx, int shard, int dev, int n_out, int32_t* const* ptrs) {
     for (int o = 0; o < n_out; ++o)
         for (const auto& m : ctx->ipc_owned) if (m.first == shard && m.second == (void*)ptrs[o]) return o;
     for (int o = 0; o < n_out; ++o) {
@@ -226,6 +231,13 @@ int find_local_vector(const rpk_ctx* ctx, int shard, int dev, int n_out, int32_t
         if (at.type == cudaMemoryTypeDevice && at.device == dev) return o;
     }
     return -1;
+}
+
+// The output vector of an assignment gather the select kernels write (-1: they store into every vector directly).  A
+// single vector is written whatever memory it is.
+int find_local_vector(const rpk_ctx* ctx, int shard, int dev, int n_out, int32_t* const* ptrs) {
+    if (n_out == 1) return 0;
+    return same_phase(n_out, ptrs) ? local_vector(ctx, shard, dev, n_out, ptrs) : -1;
 }
 
 // Row sub-batches of the host entry point.  The first one is small, so that the first kernel starts after ~3 MB of
@@ -356,6 +368,45 @@ void enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodCols& pods, 
         RPK_CUDA(cudaStreamWaitEvent(ds.stream, ln.done, 0));
     }
     RPK_CUDA(cudaEventRecord(ds.ev[3], ds.stream));
+}
+
+// rpk_select_device_gather, and rpk_select_device_gather_top5 with t5 (its own arguments checked, a.top5 then points
+// into the local top-5 vector).  The shard is in range.
+int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
+                         const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud, int n_out,
+                         int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, const Top5Gather* t5, void* stream) {
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    const PeerGroup& peers = ctx->bind[(size_t)shard];
+    cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+    if (P == 0) {  // nothing to select, but a bound gather still tells its peers that this (empty) shard is done
+        if (n_out <= 1 || peers.n == 0) return RPK_OK;
+        return guarded(ctx, [&]() -> int {
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);  // orders the epoch counter after the last gather's
+            ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
+            guard.done();
+            return RPK_OK;
+        });
+    }
+    if (!d_req_mem_gb || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
+    for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device: NULL output vector");
+    if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
+    return guarded(ctx, [&]() -> int {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        SelectArgs a{};
+        a.req_mem = d_req_mem_gb; a.req_vcpu = d_req_vcpu; a.req_ram = d_req_ram_gb; a.max_price = d_max_price; a.cloud = d_cloud;
+        a.P = P;
+        for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
+        a.n_out = n_out; a.row0 = row0;
+        a.top5 = t5 ? t5->out[t5->self_out] + (size_t)RPK_TOPK * row0 : d_top5;
+        a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
+        if (n_out > 1) a.peers = peers;
+        ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);
+        ctx->launches += (uint64_t)enqueue_select(ds, ds.lane[0], a, st, t5);
+        guard.done();
+        count_select(ctx, P, ds.G);
+        return RPK_OK;
+    });
 }
 
 }  // namespace
@@ -494,37 +545,35 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
                              int n_out, int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device: shard out of range");
+    return select_device_gather(ctx, shard, P, d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud, n_out, d_best_full,
+                                row0, d_top5, nullptr, stream);
+}
+
+int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
+                                  const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud, int n_out,
+                                  int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
+    if (!ctx) return RPK_EINVAL;
+    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: shard out of range");
+    if (!d_best_full || !d_top5_full || n_out < 1 || n_out > RPK_MAX_GPUS)
+        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 1..8 best and top-5 vectors are required");
+    for (int o = 0; o < n_out; ++o)
+        if (!d_best_full[o] || !d_top5_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: NULL output vector");
+    if ((uint64_t)P * RPK_TOPK > UINT32_MAX) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 5*P does not fit in uint32_t");
+    if (!same_phase(n_out, d_top5_full))
+        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: the top-5 vectors differ in 16-byte phase");
     DeviceState& ds = ctx->devs[(size_t)shard];
-    const PeerGroup& peers = ctx->bind[(size_t)shard];
-    cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
-    if (P == 0) {  // nothing to select, but a bound gather still tells its peers that this (empty) shard is done
-        if (n_out <= 1 || peers.n == 0) return RPK_OK;
-        return guarded(ctx, [&]() -> int {
-            RPK_CUDA(cudaSetDevice(ds.dev));
-            ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);  // orders the epoch counter after the last gather's
-            ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
-            guard.done();
-            return RPK_OK;
-        });
-    }
-    if (!d_req_mem_gb || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
-    for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device: NULL output vector");
-    if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
-    return guarded(ctx, [&]() -> int {
+    Top5Gather t5{};
+    const int rc = guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
-        SelectArgs a{};
-        a.req_mem = d_req_mem_gb; a.req_vcpu = d_req_vcpu; a.req_ram = d_req_ram_gb; a.max_price = d_max_price; a.cloud = d_cloud;
-        a.P = P;
-        for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
-        a.n_out = n_out; a.row0 = row0; a.top5 = d_top5;
-        a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
-        if (n_out > 1) a.peers = peers;
-        ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);
-        ctx->launches += (uint64_t)enqueue_select(ds, ds.lane[0], a, st);
-        guard.done();
-        count_select(ctx, P, ds.G);
+        t5.self_out = local_vector(ctx, shard, ds.dev, n_out, d_top5_full);
         return RPK_OK;
     });
+    if (rc != RPK_OK) return rc;
+    if (t5.self_out < 0) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: no top-5 vector lives on GPU `shard`");
+    for (int o = 0; o < n_out; ++o) t5.out[o] = d_top5_full[o];
+    t5.n_out = n_out;
+    return select_device_gather(ctx, shard, P, d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud, n_out, d_best_full,
+                                row0, nullptr, &t5, stream);
 }
 
 int rpk_select_device(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,

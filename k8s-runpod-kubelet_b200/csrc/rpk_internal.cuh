@@ -256,7 +256,11 @@ struct OfferIngest {   // raw device columns in, views out
 struct DeviceState;
 int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st);
 struct PersistPlan;
-int launch_select(const SelectArgs& a, int rows_per_warp, const PersistPlan* pl, int sm_count, cudaStream_t st);
+// The top-5 lists' all-gather (rpk_select_device_gather_top5): the top-5 kernel writes out[self_out] (SelectArgs::top5
+// points into it at 5 * row0), and the finished slice [5 * row0, 5 * (row0 + P)) is pushed into the other vectors.
+struct Top5Gather { int32_t* out[RPK_MAX_GPUS]; int n_out; int self_out; };
+int launch_select(const SelectArgs& a, int rows_per_warp, const PersistPlan* pl, int sm_count, cudaStream_t st,
+                  const Top5Gather* t5 = nullptr);
 uint32_t select_tiles_max(uint32_t P, int rows_per_warp);
 int pick_rows_per_warp(uint32_t P, int sm_count);
 int launch_status_diff(const StatusArgs& a, int sm_count, cudaStream_t st);

@@ -13,8 +13,9 @@
 //                     applies price < maxPrice to the winner (the bound is a prefix of the sorted order) and stores
 //                     the offer index into every peer's assignment vector (the fused all-gather).
 //   k_select_top5*    optional: the whole <=5 gpuTypeIds list per row (runpod_client.go:502-509).
-//   k_gather_push     several output vectors: copies the finished slice to the peers; k_peer_signal (select_persist.cu)
-//                     then signals a bound peer group.
+//   k_gather_push     several output vectors: copies the finished slice to the peers (a second launch copies the top-5
+//                     lists' slice for rpk_select_device_gather_top5); k_peer_signal (select_persist.cu) then signals a
+//                     bound peer group.
 #include <math_constants.h>
 
 #include <cstdlib>
@@ -549,27 +550,35 @@ static void launch_fused(const SelectArgs& a, cudaStream_t st) {
 
 static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* pl, int sm_count, cudaStream_t st, bool* fused_push);
 
-int launch_select(const SelectArgs& args, int R, const PersistPlan* pl, int sm_count, cudaStream_t st) {
+// Forward the finished slice [off, off + count) of outs[self] to every other vector of outs (the all-gather), with PDL
+// behind the kernel that finished it.
+static int launch_gather_push(int32_t* const* outs, int n_out, int self, size_t off, uint32_t count, int sm_count, cudaStream_t st) {
+    PushArgs pa{};
+    pa.src = outs[self] + off;
+    int np = 0;
+    for (int o = 0; o < n_out; ++o) if (o != self) pa.dst[np++] = outs[o] + off;
+    pa.count = count;
+    const uint32_t nvec = count / 4;
+    uint32_t per_peer = (nvec + 1023) / 1024;  // one pass of four 16-byte units per thread, up to two CTAs per SM
+    const uint32_t max_per_peer = 2u * (uint32_t)sm_count;
+    per_peer = per_peer < 1 ? 1 : per_peer > max_per_peer ? max_per_peer : per_peer;
+    launch_pdl(k_gather_push, dim3(per_peer, (unsigned)np), dim3(256), 0, st, read_tune().pdl, pa);
+    return 1;
+}
+
+int launch_select(const SelectArgs& args, int R, const PersistPlan* pl, int sm_count, cudaStream_t st, const Top5Gather* t5) {
     SelectArgs a = args;
     a.tune_natural_order = read_tune().natural_order ? 1u : 0u;
     if (a.n_out == 1) a.self_out = 0;
+    // The signal must follow the last peer store.  With a top-5 gather that is the lists' push behind the top-5 kernel,
+    // so the select kernels (the persistent one signals from its last pusher) get no peer group to signal.
+    const bool t5_push = t5 && t5->n_out > 1;
+    if (t5_push) a.peers.n = 0;
     bool fused_push = false;  // the persistent kernel pushes (and signals) itself
     int launches = launch_select_kernels(a, R, pl, sm_count, st, &fused_push);
-    if (fused_push) return launches;
-    if (a.n_out > 1 && a.self_out >= 0) {  // forward the finished slice to the peers (the all-gather)
-        PushArgs pa{};
-        pa.src = a.best_out[a.self_out] + a.row0;
-        int np = 0;
-        for (int o = 0; o < a.n_out; ++o) if (o != a.self_out) pa.dst[np++] = a.best_out[o] + a.row0;
-        pa.count = a.P;
-        const uint32_t nvec = a.P / 4;
-        uint32_t per_peer = (nvec + 1023) / 1024;  // one pass of four 16-byte units per thread, up to two CTAs per SM
-        const uint32_t max_per_peer = 2u * (uint32_t)sm_count;
-        per_peer = per_peer < 1 ? 1 : per_peer > max_per_peer ? max_per_peer : per_peer;
-        launch_pdl(k_gather_push, dim3(per_peer, (unsigned)np), dim3(256), 0, st, read_tune().pdl, pa);
-        ++launches;
-    }
-    if (a.peers.n > 0) launches += launch_peer_signal(a.peers, 0, a.peers.inline_wait != 0, st);
+    if (!fused_push && a.n_out > 1 && a.self_out >= 0) launches += launch_gather_push(a.best_out, a.n_out, a.self_out, a.row0, a.P, sm_count, st);
+    if (t5_push) launches += launch_gather_push(t5->out, t5->n_out, t5->self_out, (size_t)RPK_TOPK * a.row0, RPK_TOPK * a.P, sm_count, st);
+    if (args.peers.n > 0 && (!fused_push || t5_push)) launches += launch_peer_signal(args.peers, 0, args.peers.inline_wait != 0, st);
     return launches;
 }
 

@@ -635,9 +635,9 @@ __global__ void __maxnreg__(96) k_select_persist(SelectArgs a, PersistArgs pa) {
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// peer signal / wait.  The persistent kernel signals from its last pusher; the other select paths and an empty shard
-// launch k_peer_signal behind their kernels, and so does rpk_peer_fence (signal and wait in one); k_peer_wait is the
-// wait half for a bound group.
+// peer signal / wait.  The persistent kernel signals from its last pusher; the other select paths, a top-5 gather (behind
+// the lists' push) and an empty shard launch k_peer_signal behind their kernels, and so does rpk_peer_fence (signal and
+// wait in one); k_peer_wait is the wait half for a bound group.
 // ---------------------------------------------------------------------------------------------------------
 __global__ void k_peer_signal(PeerGroup g, uint32_t epoch, uint32_t wait) {
     pdl_wait();  // everything this stream did before (peer stores included) has completed

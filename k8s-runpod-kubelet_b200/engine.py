@@ -177,11 +177,22 @@ class Engine:
             self._ctx, shard, P, *cols, self._dev_ptr(d_best, "d_best", shard, P), self._dev_ptr(d_top5, "d_top5", shard, P * 5),
             self._stream(stream, shard)))
 
-    def select_device_gather(self, pods: dict, full_ptrs, row0: int, d_top5=None, shard: int = 0, stream=None):
+    def select_device_gather(self, pods: dict, full_ptrs, row0: int, d_top5=None, shard: int = 0, stream=None, top5_ptrs=None):
         """Shard + fused all-gather: results land at [row0, row0+P) of every vector in ``full_ptrs`` (raw
-        device pointers: own vector first or anywhere, peers' via IPC / peer access)."""
+        device pointers: own vector first or anywhere, peers' via IPC / peer access).  ``top5_ptrs`` (one per vector of
+        ``full_ptrs``, one of them on the shard's GPU) gathers the gpuTypeIds lists too: elements [5*row0, 5*(row0+P)) of
+        every one of them (rpk_select_device_gather_top5); ``d_top5`` keeps the lists local instead."""
         P, cols = self._dev_pods(pods, shard)
         n_out, outs = _ptr_array(full_ptrs)
+        if top5_ptrs is not None:
+            if d_top5 is not None:
+                raise ValueError("d_top5 and top5_ptrs: pass one (top5_ptrs gathers the lists into every vector)")
+            n_t5, t5 = _ptr_array(top5_ptrs)
+            if n_t5 != n_out:
+                raise ValueError(f"top5_ptrs: expected one vector per vector of full_ptrs ({n_out}), got {n_t5}")
+            self._check(self._lib.rpk_select_device_gather_top5(
+                self._ctx, shard, P, *cols, n_out, outs, t5, row0, self._stream(stream, shard)))
+            return
         self._check(self._lib.rpk_select_device_gather(
             self._ctx, shard, P, *cols, n_out, outs, row0, self._dev_ptr(d_top5, "d_top5", shard, P * 5), self._stream(stream, shard)))
 
