@@ -759,9 +759,9 @@ namespace {
 // Scratch of a sweep over N records (or list entries) on ds: the look-back state and tickets -- zero between calls by
 // construction, zeroed here when (re)allocated -- and the per-warp index stage, its code stage (`codes`) and the
 // per-unit counts.
-void reserve_sweep_scratch(DeviceState& ds, uint32_t N, uint32_t stride, bool codes) {
+void reserve_sweep_scratch(DeviceState& ds, uint32_t N, bool codes) {
     const uint32_t cap = N ? N : 1;
-    const size_t need = status_state_words(cap, stride, ds.sm_count);
+    const size_t need = status_state_words(ds.sm_count);
     if (need > ds.s_tile_state.cap || !ds.s_misc.p || ds.status_dirty) {
         ds.s_tile_state.reserve(need);
         ds.s_misc.reserve(64);
@@ -812,7 +812,7 @@ void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
     ds.s_records.reserve((size_t)cap * h.stride);
     if (h.slots) ds.s_seed_slots.reserve(cap);
     if (h.hashes_out) ds.s_hash_out.reserve(cap);
-    reserve_sweep_scratch(ds, Ns, h.stride, h.changed_code != nullptr);
+    reserve_sweep_scratch(ds, Ns, h.changed_code != nullptr);
     ds.h_changed.reserve(h.report ? (size_t)cap * (h.changed_code ? 6 : 4) + 64 : 64);
 }
 
@@ -1024,7 +1024,7 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
         const bool codes = d_changed_code || n_out > 0;
-        reserve_sweep_scratch(ds, N, stride, codes);
+        reserve_sweep_scratch(ds, N, codes);
         StatusArgs a{};
         a.records = d_records; a.stride = stride; a.N = N; a.hash_prev = d_hash_prev; a.hash_out = nullptr;
         a.changed_idx = d_changed_idx; a.changed_code = d_changed_code; a.n_changed = d_n_changed; a.idx_base = idx_base;

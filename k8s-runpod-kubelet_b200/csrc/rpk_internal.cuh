@@ -189,11 +189,11 @@ struct StatusArgs {
     uint16_t* changed_code; // nullable: translateRunPodStatus code per changed slot (rpk.h RPK_CODE_*)
     uint32_t* n_changed;    // nullable (seed)
     uint32_t idx_base;      // added to emitted indices (shard offset)
-    unsigned long long* tile_state;  // look-back state: one entry per CTA (strides 16/32) or per tile (other strides); zero between calls
+    unsigned long long* tile_state;  // look-back state: one entry per CTA; zero between calls
     uint32_t* tile_counter;          // [2] scheduling ticket, finished CTAs; zero between calls
-    uint32_t* stage_idx;             // [N] per-warp ordered index segments (strides 16/32)
+    uint32_t* stage_idx;             // [N] per-warp ordered index segments
     uint16_t* stage_code;            // [N] codes staged alongside
-    uint32_t* unit_cnt;              // [N / 64 + 1] changed slots per 64-slot unit (strides 16/32)
+    uint32_t* unit_cnt;              // [N / 64 + 1] changed slots per 64-slot unit
     // sharded sweep: the changed list also goes into region `peers.my_rank` of every rank's exchange buffer
     int n_out;
     uint32_t* out_idx[RPK_MAX_GPUS];    // start of this rank's index region in rank o's buffer
@@ -273,8 +273,7 @@ struct PersistPlan { uint32_t S, per, qspan, grid, smem_bytes, slice, n_cursors,
 PersistPlan persist_plan(const SelectArgs& a, int sm_count);  // a.pk.bm_words and a.nsub non-zero
 uint32_t persist_hdr_words(const PersistPlan& pl);
 int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream_t st);
-uint32_t status_tiles(uint32_t N, uint32_t stride);
-uint32_t status_state_words(uint32_t N, uint32_t stride, int sm_count);
+uint32_t status_state_words(int sm_count);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 

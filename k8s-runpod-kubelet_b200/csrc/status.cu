@@ -14,16 +14,17 @@
 //
 // Kernels:
 //   k_status_stream<STRIDE, THREADS>
-//                            strides 16 and 32: HBM-bound scan.  Persistent CTAs; every WARP owns a contiguous run of
+//                            every stride: HBM-bound scan.  Persistent CTAs; every WARP owns a contiguous run of
 //                            slots and streams it with 16-byte global loads, the next unit's loads in flight while
 //                            the current one is hashed; changed slots are staged in slot order in the warp's own
 //                            part of a staging array -- no CTA barrier in the loop.  At the end each CTA publishes
 //                            its count, finds its offset by decoupled look-back over the CTAs before it (ids are
 //                            handed out in scheduling order) and copies its staged indices / codes to their final,
 //                            ascending position (and, for the sharded sweep, into every peer's exchange buffer).
-//   k_status_diff<ITEMS>     the other strides (48..256): padded shared-memory tile + look-back per tile.
+//                            STRIDE 16 and 32 are compiled for their stride; STRIDE 0 is the wide form (48..256),
+//                            which takes the stride from the arguments.
 //   k_status_seed_slots      previous state of individual slots (CreatePod writes ONE InstanceInfo, kubelet.go:391-401).
-// The first two also sweep a list of slots (template flag SLOTS, rpk_status_diff_slots): the listed slots' packed
+// The first also sweeps a list of slots (template flag SLOTS, rpk_status_diff_slots): the listed slots' packed
 // records are a table of their own, streamed the same way; only the hash row (slots[i] - idx_base) and the id
 // reported (slots[i]) differ.  updateAllPodStatuses compares only the pods it fetched this cycle (kubelet.go:836-864).
 #include "rpk_device.cuh"
@@ -52,7 +53,11 @@ __device__ __noinline__ u64 xxh64_stripe32(u64 l0, u64 l1, u64 l2, u64 l3) {  //
     h = xmerge(h, v1); h = xmerge(h, v2); h = xmerge(h, v3); h = xmerge(h, v4);
     return avalanche(h + 32ull);
 }
-__device__ __forceinline__ u64 xxh64_lanes4(u64 l0, u64 l1, u64 l2, u64 l3, uint32_t nl) {
+__device__ __noinline__ u64 xxh64_words(const uint32_t* w, uint32_t nbytes, uint32_t w0);
+// WIDE (strides 48..256): a record of nl > 4 lanes goes on past the 32 bytes in l0..l3, so every record of 4 or more
+// lanes is hashed in one out-of-line call over `rec`, the record in global memory
+template <bool WIDE = false>
+__device__ __forceinline__ u64 xxh64_lanes4(u64 l0, u64 l1, u64 l2, u64 l3, uint32_t nl, const uint32_t* rec = nullptr) {
     u64 h = P5 + (u64)(nl * 8u);
     h = step8(h, l0);
     const u64 h2 = step8(h, l1);
@@ -61,7 +66,14 @@ __device__ __forceinline__ u64 xxh64_lanes4(u64 l0, u64 l1, u64 l2, u64 l3, uint
     // and kept out of line so that the hot path does not carry their registers
     if (__any_sync(0xFFFFFFFFu, nl >= 3)) {
         if (nl == 3) h = step8(h, l2);
-        if (__any_sync(0xFFFFFFFFu, nl >= 4)) { const u64 hs = xxh64_stripe32(l0, l1, l2, l3); if (nl >= 4) return hs; }
+        if (__any_sync(0xFFFFFFFFu, nl >= 4)) {
+            if constexpr (WIDE) {
+                if (nl >= 4) return xxh64_words(rec, nl * 8u, (uint32_t)l0);
+            } else {
+                const u64 hs = xxh64_stripe32(l0, l1, l2, l3);
+                if (nl >= 4) return hs;
+            }
+        }
     }
     return avalanche(h);
 }
@@ -72,8 +84,9 @@ __device__ __forceinline__ u64 xxh64_lanes2(u64 l0, u64 l1, uint32_t nl) {  // 1
     return avalanche(nl >= 2 ? h2 : h);
 }
 
-// General form over 32-bit words in memory, nbytes a multiple of 8 (generic strides, per-slot seed).
-__device__ u64 xxh64_words(const uint32_t* w, uint32_t nbytes, uint32_t w0) {  // w0: word 0 with the flag bit cleared
+// General form over 32-bit words in memory, nbytes a multiple of 8 (records of 4+ lanes at wide strides, per-slot seed).
+// Out of line, like the stripe: the wide sweep calls it for rare long records and must not carry its registers.
+__device__ __noinline__ u64 xxh64_words(const uint32_t* w, uint32_t nbytes, uint32_t w0) {  // w0: word 0 with the flag bit cleared
     uint32_t off = 0;  // in words
     u64 h;
     auto rd = [&](uint32_t q) { return mk64(q == 0 ? w0 : w[q], w[q + 1]); };
@@ -127,48 +140,13 @@ __device__ __forceinline__ uint32_t classify_status(u64 l0, u64 l1, uint32_t len
     return kind;
 }
 
-constexpr int kStThreads = 256;
 #define kFlagAgg (1ull << 32)
-#define kFlagPrefix (2ull << 32)
 #define kFlagMask (3ull << 32)
 
-static int items_for_stride(uint32_t stride) { return stride <= 32 ? 4 : stride <= 64 ? 2 : 1; }
-uint32_t status_tiles(uint32_t N, uint32_t stride) {
-    const uint32_t tile = (uint32_t)(kStThreads * items_for_stride(stride));
-    return (N + tile - 1) / tile;
-}
-
-// Decoupled look-back over the entries before `id` (one warp): returns the exclusive prefix.  Entries carry
-// kFlagAgg | count until their owner knows its own prefix, then kFlagPrefix | inclusive prefix.
-__device__ __forceinline__ uint32_t look_back(volatile u64* st, uint32_t id, uint32_t total, uint32_t lane) {
-    uint32_t excl = 0;
-    if (id == 0) {
-        if (lane == 0) st[0] = kFlagPrefix | total;
-        return 0;
-    }
-    if (lane == 0) st[id] = kFlagAgg | total;
-    int look = (int)id - 1;
-    while (true) {
-        const int idx = look - (int)lane;
-        u64 v;
-        do { v = kFlagPrefix; if (idx >= 0) v = st[idx]; } while (__any_sync(0xFFFFFFFFu, (v & kFlagMask) == 0));
-        const uint32_t pm = __ballot_sync(0xFFFFFFFFu, (v & kFlagMask) == kFlagPrefix);
-        const int first = pm ? __ffs(pm) - 1 : 31;
-        uint32_t val = (int)lane <= first ? (uint32_t)v : 0u;
-#pragma unroll
-        for (int d = 16; d >= 1; d >>= 1) val += __shfl_xor_sync(0xFFFFFFFFu, val, d);
-        excl += val;
-        if (pm) break;
-        look -= 32;
-    }
-    if (lane == 0) st[id] = kFlagPrefix | (u64)(excl + total);
-    return excl;
-}
-
-// The stream kernel's variant: at most one CTA per SM, and they all finish at about the same time, so walking back
-// window by window would cost one L2 round trip per 32 predecessors.  Every CTA publishes its count once
-// (kFlagAgg | count) and sums ALL entries before it in one pass of independent loads, retrying only the ones that
-// are not there yet.
+// Decoupled look-back over the CTAs before `id` (one warp): returns the exclusive prefix.  There is at most one CTA
+// per SM, and they all finish at about the same time, so walking back window by window would cost one L2 round trip
+// per 32 predecessors.  Every CTA publishes its count once (kFlagAgg | count; an entry without a flag bit is not there
+// yet) and sums ALL entries before it in one pass of independent loads, retrying only the ones that are not there yet.
 __device__ __forceinline__ uint32_t sum_before(volatile u64* st, uint32_t id, uint32_t total, uint32_t lane) {
     if (lane == 0) st[id] = kFlagAgg | total;
     uint32_t acc = 0;
@@ -190,7 +168,7 @@ __device__ __forceinline__ uint32_t sum_before(volatile u64* st, uint32_t id, ui
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// strides 16 / 32: streamed scan
+// streamed scan
 // ---------------------------------------------------------------------------------------------------------
 // One 1024-thread CTA per SM owns a contiguous range of units (64 slots each); its 32 warps take the units of the range
 // round-robin, so the CTA reads ONE sequential stream, 32 units (64 KB of 32-byte slots + 16 KB of hashes) per round --
@@ -213,6 +191,11 @@ constexpr uint32_t kBigTable = 4u << 20;
 // col (SLOTS only): the entry's row of hash_prev, kNone when the slot lies outside the column
 template <int STRIDE> struct SlotData { uint4 lo; uint4 hi; u64 prev; uint32_t col; };
 
+// Bytes per record: STRIDE, or the call's stride in the wide form (STRIDE 0, strides 48..256).  The wide form loads
+// the first 32 bytes of a slot as stride 32 does: the status code reads two lanes, and a hash over more than four
+// lanes goes back to the record (xxh64_lanes4<true>).
+template <int STRIDE> __device__ __forceinline__ uint32_t rec_stride(const StatusArgs& a) { return STRIDE ? (uint32_t)STRIDE : a.stride; }
+
 template <int STRIDE, bool SLOTS>
 __device__ __forceinline__ void load_unit(const StatusArgs& a, uint32_t base, uint32_t lane, SlotData<STRIDE> (&d)[kStreamItems]) {
 #pragma unroll
@@ -221,9 +204,9 @@ __device__ __forceinline__ void load_unit(const StatusArgs& a, uint32_t base, ui
         d[k].lo = make_uint4(0, 0, 0, 0); d[k].hi = d[k].lo; d[k].prev = 0;
         if constexpr (SLOTS) d[k].col = kNone;
         if (s < a.N) {
-            const uint4* p = reinterpret_cast<const uint4*>(a.records + (size_t)s * STRIDE);
+            const uint4* p = reinterpret_cast<const uint4*>(a.records + (size_t)s * rec_stride<STRIDE>(a));
             d[k].lo = __ldg(p);  // the two halves of a 32-byte slot share a sector: the second load hits L1
-            if (STRIDE == 32) d[k].hi = __ldg(p + 1);
+            if (STRIDE != 16) d[k].hi = __ldg(p + 1);
             if constexpr (SLOTS) {
                 const uint32_t c = __ldg(a.slots + s) - a.idx_base;  // below idx_base wraps around: outside
                 if (c < a.col_n) { d[k].col = c; d[k].prev = a.hash_prev[c]; }
@@ -255,12 +238,14 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
 #pragma unroll
         for (int k = 0; k < kStreamItems; ++k) {
             const uint32_t s = u * kUnit + (uint32_t)k * 32 + lane;
-            const uint32_t len = min(d[k].lo.x & 0x7Fu, (uint32_t)STRIDE - 1u);
+            const uint32_t len = min(d[k].lo.x & 0x7Fu, rec_stride<STRIDE>(a) - 1u);
             const uint32_t nl = (len + 8u) >> 3;  // lanes covering bytes [0, 1 + len)
             const u64 l0 = mk64(d[k].lo.x & ~0x80u, d[k].lo.y), l1 = mk64(d[k].lo.z, d[k].lo.w);
+            const u64 l2 = mk64(d[k].hi.x, d[k].hi.y), l3 = mk64(d[k].hi.z, d[k].hi.w);
             u64 h;
             if (STRIDE == 16) h = xxh64_lanes2(l0, l1, nl);
-            else h = xxh64_lanes4(l0, l1, mk64(d[k].hi.x, d[k].hi.y), mk64(d[k].hi.z, d[k].hi.w), nl);
+            else if (STRIDE == 32) h = xxh64_lanes4(l0, l1, l2, l3, nl);
+            else h = xxh64_lanes4<true>(l0, l1, l2, l3, nl, reinterpret_cast<const uint32_t*>(a.records + (size_t)s * a.stride));
             bool changed = false;
             if constexpr (SLOTS) {
                 if (s < a.N && d[k].col != kNone) {
@@ -335,9 +320,9 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
             if (a.changed_idx) a.changed_idx[off + i] = x;
             for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_idx[o][off + i] = x;
             if (want_codes) {  // translateRunPodStatus's decision, for the changed slots only: their records are read once more
-                const uint4 r = __ldg(reinterpret_cast<const uint4*>(a.records + (size_t)slot * STRIDE));
+                const uint4 r = __ldg(reinterpret_cast<const uint4*>(a.records + (size_t)slot * rec_stride<STRIDE>(a)));
                 bool ports;
-                const uint32_t len = min(r.x & 0x7Fu, (uint32_t)STRIDE - 1u);
+                const uint32_t len = min(r.x & 0x7Fu, rec_stride<STRIDE>(a) - 1u);
                 const uint32_t kind = classify_status(mk64(r.x & ~0x80u, r.y), mk64(r.z, r.w), len, &ports);
                 const uint16_t cc = (uint16_t)status_code(kind, ports, (r.x & 0x80u) != 0u);
                 if (a.changed_code) a.changed_code[off + i] = cc;
@@ -358,99 +343,6 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
     for (uint32_t i = tid; i < n_ctas; i += kSThreads) a.tile_state[i] = 0ull;
     if (tid == 0) { a.tile_counter[0] = 0u; a.tile_counter[1] = 0u; }
     if (!SLOTS && a.peers.n > 0 && warp == 0) signal_peers(a.peers, kFlagStatus, kFlagStatusCtr, 0, a.peers.inline_wait != 0);
-}
-
-// ---------------------------------------------------------------------------------------------------------
-// other strides: padded shared-memory tile, decoupled look-back per tile
-// ---------------------------------------------------------------------------------------------------------
-template <int ITEMS, bool SLOTS = false>  // SLOTS: as k_status_stream
-__global__ void __launch_bounds__(kStThreads) k_status_diff(StatusArgs a) {
-    extern __shared__ __align__(16) uint32_t s_rec[];  // tile_recs rows of (stride/4 + 1) words
-    __shared__ uint32_t s_tile, s_excl, s_last;
-    __shared__ uint32_t s_wcnt[ITEMS * (kStThreads / 32)];
-    const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    // reporting sweeps take tile ids from the ticket (scheduling order: the look-back cannot starve); a seed has no
-    // look-back and returns before the last-CTA cleanup below, so it must not touch the ticket (nobody would reset it)
-    if (tid == 0) s_tile = a.changed_idx != nullptr ? atomicAdd(a.tile_counter, 1u) : blockIdx.x;
-    __syncthreads();
-    const uint32_t tile = s_tile;
-    constexpr uint32_t kTileRecs = kStThreads * ITEMS;
-    const uint32_t rec0 = tile * kTileRecs;
-    const uint32_t nrec = min(kTileRecs, a.N - rec0);
-    const uint32_t wps = a.stride >> 2, row = wps + 1, u16 = a.stride >> 4;  // words / padded row / 16B units per slot
-
-    // coalesced copy of the tile into padded rows (bank-conflict-free per-thread row walks)
-    const uint4* __restrict__ src = reinterpret_cast<const uint4*>(a.records + (size_t)rec0 * a.stride);
-    const uint32_t units = nrec * u16;
-    for (uint32_t u = tid; u < units; u += kStThreads) {
-        const uint4 v = __ldcs(src + u);  // streamed once
-        const uint32_t r = u / u16, part = u - r * u16;
-        uint32_t* d = s_rec + r * row + part * 4;
-        d[0] = v.x; d[1] = v.y; d[2] = v.z; d[3] = v.w;
-    }
-    __syncthreads();
-
-    bool changed[ITEMS];
-    uint32_t bal[ITEMS], code[ITEMS];
-#pragma unroll
-    for (int k = 0; k < ITEMS; ++k) {
-        const uint32_t lr = (uint32_t)k * kStThreads + tid;
-        changed[k] = false; code[k] = 0;
-        // SLOTS: row slots[i] - idx_base of hash_prev, and nothing for a slot outside the column
-        const uint32_t col = SLOTS && lr < nrec ? a.slots[rec0 + lr] - a.idx_base : kNone;
-        if (lr < nrec && (!SLOTS || col < a.col_n)) {
-            const uint32_t* w = s_rec + lr * row;
-            const uint32_t b0 = w[0] & 0xFFu;
-            const uint32_t len = min(b0 & 0x7Fu, a.stride - 1);
-            const uint32_t nbytes = min(((len + 8u) >> 3) << 3, a.stride);
-            const u64 h = xxh64_words(w, nbytes, w[0] & ~0x80u);
-            const u64 prev = a.hash_prev[SLOTS ? col : rec0 + lr];
-            changed[k] = (prev == 0ull) || (h != prev);  // 0 = never seen (after reset)
-            if (changed[k]) a.hash_prev[SLOTS ? col : rec0 + lr] = h;  // kubelet.go:875-880: state replaced only on change
-            if (!SLOTS && a.hash_out) a.hash_out[rec0 + lr] = h;
-            if (changed[k] && a.changed_code) {
-                bool ports;
-                const uint32_t kind = classify_status(mk64(w[0] & ~0x80u, w[1]), mk64(w[2], w[3]), len, &ports);
-                code[k] = status_code(kind, ports, (b0 & 0x80u) != 0u);
-            }
-        }
-        bal[k] = __ballot_sync(0xFFFFFFFFu, changed[k]);
-        if (lane == 0) s_wcnt[k * (kStThreads / 32) + warp] = __popc(bal[k]);
-    }
-    if (a.changed_idx == nullptr) return;  // seed
-    __syncthreads();
-    if (warp == 0) {  // exclusive scan of the per-(item, warp) counts, then the tile's offset
-        constexpr uint32_t kCnt = ITEMS * (kStThreads / 32);  // <= 32
-        const uint32_t c = lane < kCnt ? s_wcnt[lane] : 0u;
-        uint32_t inc = c;
-#pragma unroll
-        for (int d = 1; d < 32; d <<= 1) { const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, inc, d); if ((int)lane >= d) inc += n; }
-        const uint32_t total = __shfl_sync(0xFFFFFFFFu, inc, 31);
-        if (lane < kCnt) s_wcnt[lane] = inc - c;
-        const uint32_t excl = look_back(a.tile_state, tile, total, lane);
-        if (lane == 0) {
-            s_excl = excl;
-            if (rec0 + nrec == a.N) *a.n_changed = excl + total;  // the last tile in record order owns the count
-        }
-    }
-    __syncthreads();
-    const uint32_t excl = s_excl;
-#pragma unroll
-    for (int k = 0; k < ITEMS; ++k) {
-        if (changed[k]) {
-            const uint32_t posn = excl + s_wcnt[k * (kStThreads / 32) + warp] + __popc(bal[k] & ((1u << lane) - 1));
-            if constexpr (SLOTS) a.changed_idx[posn] = a.slots[rec0 + (uint32_t)k * kStThreads + tid];
-            else a.changed_idx[posn] = a.idx_base + rec0 + (uint32_t)k * kStThreads + tid;
-            if (a.changed_code) a.changed_code[posn] = (uint16_t)code[k];
-        }
-    }
-    __threadfence();
-    __syncthreads();
-    if (tid == 0) s_last = atomicAdd(a.tile_counter + 1, 1u) == gridDim.x - 1 ? 1u : 0u;
-    __syncthreads();
-    if (!s_last) return;
-    for (uint32_t i = tid; i < gridDim.x; i += kStThreads) a.tile_state[i] = 0ull;  // self-cleaning
-    if (tid == 0) { a.tile_counter[0] = 0u; a.tile_counter[1] = 0u; }
 }
 
 // previous state of individual slots: hash_prev[slots[i] - idx_base] = hash(records[i]) for the slots of this shard
@@ -474,10 +366,8 @@ int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t*
     return 1;
 }
 
-uint32_t status_state_words(uint32_t N, uint32_t stride, int sm_count) {  // u64 entries of StatusArgs::tile_state
-    const uint32_t a = status_tiles(N ? N : 1, stride), b = (uint32_t)(4 * sm_count);
-    return (a > b ? a : b) + 8;
-}
+// u64 entries of StatusArgs::tile_state: one per CTA, and launch_status never launches more CTAs than SMs
+uint32_t status_state_words(int sm_count) { return (uint32_t)sm_count + 8; }
 
 // SLOTS: a slot-list sweep, whose launch shape follows from the list length (a.N) exactly as a table's does from N
 template <bool SLOTS>
@@ -487,39 +377,26 @@ static int launch_status(const StatusArgs& a, int sm_count, cudaStream_t st) {
         // an empty shard of a sharded sweep still has to publish its (zero) count and signal: one tiny CTA does it
         if (a.n_out == 0 && a.peers.n == 0) return 0;
     }
-    if (a.stride == 16 || a.stride == 32) {
-        const uint32_t n_units = (a.N + kUnit - 1) / kUnit;
-        const bool big = a.N >= kBigTable;
-        const uint32_t warps = big ? 32u : 8u, max_grid = (uint32_t)sm_count;
-        // one unit per warp until every SM has its CTA, then longer runs per warp
-        uint32_t grid = (n_units + warps - 1) / warps;
-        if (grid > max_grid) grid = max_grid;
-        if (grid == 0) grid = 1;
-        StatusArgs b = a;
-        if (a.changed_idx == nullptr && a.n_out == 0) { b.stage_idx = nullptr; b.stage_code = nullptr; }
-        // one loop, two launch shapes (see kBigTable).  Other loops -- three or four half-unit register sets, a per-warp
-        // shared-memory ring filled by bulk copies -- were within 4 % of it at 16.8M slots on an H100 SXM (700 W) and
-        // none was faster at both strides (DESIGN §4, profiles/h100_k2_tune.json)
-        if (big) {
-            if (a.stride == 16) k_status_stream<16, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
-            else k_status_stream<32, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
-        } else {
-            if (a.stride == 16) k_status_stream<16, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
-            else k_status_stream<32, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
-        }
-        RPK_CUDA(cudaGetLastError());
-        return 1;
-    }
-    const int items = items_for_stride(a.stride);  // 2 or 1: strides 16 / 32 took the streaming kernel above
-    const uint32_t tiles = status_tiles(a.N, a.stride);
-    const size_t smem = (size_t)kStThreads * items * (a.stride + 4);
-    static thread_local int attr_dev[2] = {-1, -1};
-    if (items == 2) {
-        allow_smem(k_status_diff<2, SLOTS>, 160 * 1024, &attr_dev[0]);
-        k_status_diff<2, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
+    const uint32_t n_units = (a.N + kUnit - 1) / kUnit;
+    const bool big = a.N >= kBigTable;
+    const uint32_t warps = big ? 32u : 8u, max_grid = (uint32_t)sm_count;
+    // one unit per warp until every SM has its CTA, then longer runs per warp
+    uint32_t grid = (n_units + warps - 1) / warps;
+    if (grid > max_grid) grid = max_grid;
+    if (grid == 0) grid = 1;
+    StatusArgs b = a;
+    if (a.changed_idx == nullptr && a.n_out == 0) { b.stage_idx = nullptr; b.stage_code = nullptr; }
+    // one loop, two launch shapes (see kBigTable).  Other loops -- three or four half-unit register sets, a per-warp
+    // shared-memory ring filled by bulk copies -- were within 4 % of it at 16.8M slots on an H100 SXM (700 W) and
+    // none was faster at both strides (DESIGN §4, profiles/h100_k2_tune.json)
+    if (big) {
+        if (a.stride == 16) k_status_stream<16, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
+        else if (a.stride == 32) k_status_stream<32, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
+        else k_status_stream<0, 1024, SLOTS><<<grid, 1024, 0, st>>>(b, n_units);
     } else {
-        allow_smem(k_status_diff<1, SLOTS>, 160 * 1024, &attr_dev[1]);
-        k_status_diff<1, SLOTS><<<tiles, kStThreads, smem, st>>>(a);
+        if (a.stride == 16) k_status_stream<16, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
+        else if (a.stride == 32) k_status_stream<32, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
+        else k_status_stream<0, 256, SLOTS><<<grid, 256, 0, st>>>(b, n_units);
     }
     RPK_CUDA(cudaGetLastError());
     return 1;

@@ -364,14 +364,14 @@ static void TestLongStatusStrings() {
     CHECK_EQ(notified.size(), 1u); CHECK_EQ(notified[0], "l2:Succeeded:");
 }
 
-// Statuses of 30 and 62 characters widen the table to 64 and 128 bytes: strides of the tiled kernel.  Each widening
+// Statuses of 30 and 62 characters widen the table to 64 and 128 bytes: the sweep's wide form.  Each widening
 // seeds the whole table at the new stride right before the sweep at that stride (WidenRecords), so that sweep must
 // start from a clean context, not from whatever the seed's launch left behind.  125 characters (len byte 127, the most
 // a record holds) still fit 128 bytes; one more is compared on the host and the table stays at 128.
 static void TestWideStatusStrings() {
     auto api = std::make_shared<FakeRunPod>();
     api->types = KatTable();
-    Provider prov(api, 1, 600);  // more than one tile (512 slots at 64 bytes, 256 above) at every tiled stride
+    Provider prov(api, 1, 600);  // 600 slots: nine 64-slot streaming units and a ragged tenth
     std::vector<std::string> notified;
     prov.NotifyPods([&](const PodPtr& p) { notified.push_back(p->name + ":" + p->status.phase + ":" + p->status.container_message); });
     for (int i = 0; i < 6; ++i) prov.CreatePod(MakePod("v" + std::to_string(i)));

@@ -187,9 +187,9 @@ def test_tick_matches_separate_calls():
 def test_code_corpus_every_stride(stride):
     """The adversarial corpus (each known status, each with one byte changed at every position, one byte short or
     long, lower-cased; unknown strings of a known status's length; empty and one-character statuses) x ports x
-    message flag: the code of every slot equals translateRunPodStatus of the decoded string.  Strides 16 / 32 run it
-    through both streaming shapes (the corpus as it is, and tiled past the 4M-slot big-table boundary), the other
-    strides through the tiled kernel."""
+    message flag: the code of every slot equals translateRunPodStatus of the decoded string.  Every stride runs the
+    corpus as it is (the 256-thread streaming shape); strides 16 / 32 also run it repeated past the 4M-slot big-table
+    boundary (the 1024-thread shape)."""
     recs, sts, ports, flags = sc.corpus_records(stride)
     want = sc.translated_codes(sts, ports, flags)
     shapes = [1] + ([-(-(4 << 20) // len(recs))] if stride <= 32 else [])

@@ -1,9 +1,11 @@
-"""GPU tests of the streaming status sweep (strides 16 and 32) on both sides of its two launch boundaries, each call
-checked against oracle.StatusTable.
+"""GPU tests of the streaming status sweep on both sides of its two launch boundaries, each call checked against
+oracle.StatusTable.
 
 Below the big-table threshold the sweep runs one 8-warp CTA per SM (so that it fits beside the persistent select), and
 every warp takes one 64-slot unit until SMs * 8 * 64 slots; past that point the warps take longer runs.  At 4M slots
-the sweep switches to 1024-thread CTAs.  Each size runs a host-entry sequence (seed, diff with codes and hashes, an
+the sweep switches to 1024-thread CTAs.  The boundaries are the same at every stride; they are crossed at strides 16
+and 32, and at the wide strides 48, 64 and 256, whose sweep takes the stride from its arguments (the 4M boundary at 48
+only, which keeps host memory modest).  Each size runs a host-entry sequence (seed, diff with codes and hashes, an
 unchanged diff, reset, diff), a device-entry diff of a caller-owned hash column, and an rpk_tick."""
 import numpy as np
 import pytest
@@ -30,8 +32,12 @@ def resolve(size: str) -> int:
     return n + int(off) if "+" in size else n - int(off or 0)
 
 
-@pytest.mark.parametrize("stride", [16, 32])
-@pytest.mark.parametrize("size", ["sat-1", "sat", "sat+1", "big-1", "big", "big+1"])
+SAT_SIZES, BIG_SIZES = ["sat-1", "sat", "sat+1"], ["big-1", "big", "big+1"]
+BOUNDARY_CASES = ([(size, stride) for size in SAT_SIZES + BIG_SIZES for stride in (16, 32)]
+                  + [(size, stride) for size in SAT_SIZES for stride in (48, 64, 256)])
+
+
+@pytest.mark.parametrize("size,stride", BOUNDARY_CASES)
 def test_sweep_at_launch_boundary(size, stride):
     import torch
 
@@ -80,7 +86,7 @@ def test_sweep_at_launch_boundary(size, stride):
         assert np.array_equal(codes, oracle.record_codes(nxt)[want]), f"N {N}: tick codes"
 
 
-@pytest.mark.parametrize("stride", [16, 32])
+@pytest.mark.parametrize("stride", [16, 32, 48])
 def test_big_table_boundary(stride):
     """One context over the big-table boundary (4M - 1 slots: the largest 256-thread table; 4M; 4M + 37: a ragged last
     unit), host entry point; then the device entry point on a caller-owned column, and a misaligned column refused."""

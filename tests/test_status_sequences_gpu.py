@@ -1,14 +1,13 @@
 """GPU tests of the status sweep (K2) over sequences of calls on one context, against the oracle's state model.
 
 Every status kernel of a context shares its scheduling ticket and look-back state, whichever entry point (host or
-device) and whichever kernel family (strides 16 / 32: streaming; 48..256: tiled) runs it, so a call can go wrong
+device) and whichever instantiation (strides 16 / 32, or the wide form for 48..256) runs it, so a call can go wrong
 because of what the call before it left behind.  Each program below is a seeded random sequence of resets, seeds,
 per-slot seeds, diffs (with and without codes and hashes), ticks and device-column diffs at every stride, with the
 stride changing the way Provider::WidenRecords changes it (whole-table seed at the new stride, then the sweep at it),
-checked against oracle.StatusTable after every step.  Sizes sit on every boundary of the launch code: the streaming
-unit (64 slots), the tile (512 slots at strides 48 / 64, 256 above), more than 33 and more than 1024 tiles (the
-look-back crosses several 32-entry windows), and the point where the small-table streaming grid saturates (four
-8-warp CTAs per SM, one 64-slot unit per warp)."""
+checked against oracle.StatusTable after every step.  Sizes sit on the streaming unit (64 slots), on blocks of 512
+slots (strides 48 / 64) and 256 (above) with more than 33 and more than 1024 of them, and past the point where the
+small-table streaming grid saturates (four 8-warp CTAs per SM, one 64-slot unit per warp)."""
 import numpy as np
 import pytest
 
@@ -168,7 +167,7 @@ def test_status_call_sequences(size):
 
 @pytest.mark.parametrize("stride", [s for s in sc.STRIDES if s > 32])
 def test_seed_at_wide_stride_then_diff(stride):
-    """A whole-table seed at a tiled-kernel stride, then sweeps at that stride and at both streaming strides, then
+    """A whole-table seed at a wide stride, then sweeps at that stride and at strides 16 and 32, then
     device-column sweeps on the same context: nothing is reported until something changes, and then exactly that."""
     N = 3 * 512 + 5
     p = Program(N, stride)

@@ -2,9 +2,10 @@
 state model (status_slots_model.diff_slots over oracle.StatusTable) and oracle.record_codes.
 
 List lengths sit on every boundary of the launch code, which picks its shape from the list length exactly as it does
-from N for a whole table: the streaming unit (64 entries), the tile (512 entries at strides 48 / 64, 256 above), more
-than 33 and more than 1024 tiles, the point where the small-shape streaming grid saturates (one 8-warp CTA per SM,
-one 64-entry unit per warp) and the 1024-thread shape from 4M entries up."""
+from N for a whole table: the streaming unit (64 entries), the point where the small-shape streaming grid saturates
+(one 8-warp CTA per SM, one 64-entry unit per warp) and the 1024-thread shape from 4M entries up (up to stride 64).
+Wide strides also take lengths ragged against blocks of 512 entries (strides 48 / 64) or 256 (above): one block
+± 1, and 34 and 1025 blocks + 1."""
 import ctypes as C
 
 import numpy as np
@@ -27,12 +28,14 @@ def sm_count() -> int:
 
 
 def list_lengths(stride: int) -> list:
-    base = [0, 1, 63, 64, 65]
-    if stride in (16, 32):
-        sat = sm_count() * 8 * 64
-        return base + [sat - 1, sat, sat + 1, BIG + 37]
-    tile = 512 if stride <= 64 else 256
-    return base + [tile - 1, tile, tile + 1, 34 * tile + 1, 1025 * tile + 1]
+    sat = sm_count() * 8 * 64
+    lengths = [0, 1, 63, 64, 65, sat - 1, sat, sat + 1]
+    if stride <= 64:  # a 4M-entry table of the widest records would take gigabytes of host memory
+        lengths.append(BIG + 37)
+    if stride > 32:
+        block = 512 if stride <= 64 else 256
+        lengths += [block - 1, block, block + 1, 34 * block + 1, 1025 * block + 1]
+    return lengths
 
 
 def check_codes(codes, recs, changed):
