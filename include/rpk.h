@@ -295,11 +295,29 @@ int rpk_status_diff_device_codes(rpk_ctx* ctx, int shard, uint32_t N, const uint
  *   [0, 8) count per source rank | [8 + r*cap, ...) ids of rank r | then uint16 codes: region r at
  *   ((uint16*)(words + 8 + n_ranks*cap)) + r*cap.
  * With flags bound (rpk_peer_bind) the CTA that finishes last signals the status epoch; rpk_peer_wait(what = 2) on
- * every rank makes all regions readable.  Strides 16 and 32. */
+ * every rank makes all regions readable.  Every stride of rpk_status_diff (16..256), so a table that
+ * Provider::WidenRecords has widened for a long status string keeps the exchange.  A rank with N = 0 still publishes
+ * its zero count and signals.  Graph-capturable after one call of the size. */
 size_t rpk_xchg_bytes(int n_ranks, uint32_t cap);
 int rpk_status_diff_device_gather(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                                   uint64_t* d_hash_prev, uint32_t idx_base, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,
                                   int my_rank, uint32_t* d_n_changed, void* stream);
+/* The slot-list sweep (rpk_status_diff_slots_device) with the same exchange: the sweep one process per GPU runs when it
+ * compares only the pods it fetched.  d_slots[0..n_slots) lists global slot ids, d_records holds their n_slots packed
+ * records, and rank `my_rank`'s column d_hash_prev holds global slots [idx_base, idx_base + N) (entries outside it are
+ * skipped: never read, written or reported).  Region `my_rank` of every buffer d_xchg[0..n_ranks) receives the count,
+ * the global slot ids of the listed entries that changed in list order, and their codes, in the rpk_xchg_bytes layout
+ * above; *d_n_changed gets the count.  Buffers, bound signal (an empty list publishes 0 and signals too), inline wait
+ * and graph capture as for rpk_status_diff_device_gather.  List order is a precondition, not checked, so n_slots is
+ * what must fit: n_slots > cap, d_slots NULL with n_slots > 0, n_ranks outside 1..8, my_rank outside [0, n_ranks), a
+ * NULL buffer, d_records or d_hash_prev not 16-byte aligned, or a bad stride: RPK_EINVAL before anything is enqueued.
+ * When rank r's column precedes rank r+1's and every list is ascending, the regions concatenated in rank order are the
+ * ascending global changed list.  Hand each rank only its own part of the global list (one searchsorted of the column
+ * boundaries on the host): a rank handed the whole list is still correct, but reads every listed record. */
+int rpk_status_diff_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t N, uint32_t idx_base, uint32_t n_slots,
+                                        const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride,
+                                        uint64_t* d_hash_prev, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,
+                                        int my_rank, uint32_t* d_n_changed, void* stream);
 
 int rpk_stats_get(const rpk_ctx* ctx, rpk_stats* out);
 

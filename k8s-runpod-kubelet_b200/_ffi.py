@@ -62,6 +62,7 @@ ABI = {
     "rpk_status_diff_device_codes": (_int, [_p, _int, _u32, _p, _u32, _p, _p, _p, _p, _p]),
     "rpk_xchg_bytes": (_size, [_int, _u32]),
     "rpk_status_diff_device_gather": (_int, [_p, _int, _u32, _p, _u32, _p, _u32, _int, _pp, _u32, _int, _p, _p]),
+    "rpk_status_diff_slots_device_gather": (_int, [_p, _int, _u32, _u32, _u32, _p, _p, _u32, _p, _int, _pp, _u32, _int, _p, _p]),
     "rpk_stats_get": (_int, [_p, C.POINTER(RpkStats)]),
     "rpk_launch_count": (C.c_uint64, [_p]),
 }

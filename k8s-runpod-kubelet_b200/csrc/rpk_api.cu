@@ -1017,7 +1017,7 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
     if (((uintptr_t)d_records | (uintptr_t)d_hash_prev) & 15) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: d_records and d_hash_prev must be 16-byte aligned");
     if (n_out < 0 || n_out > RPK_MAX_GPUS || (n_out > 0 && (!d_xchg || my_rank < 0 || my_rank >= n_out || N > cap)))
         return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: bad exchange arguments (N must fit the per-rank capacity)");
-    if (n_out > 0 && stride != 16 && stride != 32) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: strides 16 and 32 only");
+    for (int o = 0; o < n_out; ++o) if (!d_xchg[o]) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: NULL exchange buffer");
     if (d_slots == nullptr && col_n != 0) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: d_slots is NULL");
     if ((uint64_t)idx_base + col_n > (1ull << 32)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: idx_base + N exceeds the slot range");
     DeviceState& ds = ctx->devs[(size_t)shard];
@@ -1075,6 +1075,17 @@ int rpk_status_diff_device_gather(rpk_ctx* ctx, int shard, uint32_t N, const uin
                                   uint64_t* d_hash_prev, uint32_t idx_base, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,
                                   int my_rank, uint32_t* d_n_changed, void* stream) {
     return status_device(ctx, shard, N, d_records, stride, d_hash_prev, idx_base, nullptr, nullptr, d_n_changed, n_ranks, d_xchg, cap, my_rank, stream);
+}
+
+// n_slots bounds what a region receives (list order is not checked on the device), so it is what must fit the capacity
+int rpk_status_diff_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t N, uint32_t idx_base, uint32_t n_slots,
+                                        const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride,
+                                        uint64_t* d_hash_prev, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,
+                                        int my_rank, uint32_t* d_n_changed, void* stream) {
+    if (ctx && n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device_gather: d_slots is NULL");
+    if (ctx && n_ranks < 1) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device_gather: n_ranks must be 1..8");
+    return status_device(ctx, shard, n_slots, d_records, stride, d_hash_prev, idx_base, nullptr, nullptr, d_n_changed, n_ranks,
+                         d_xchg, cap, my_rank, stream, n_slots > 0 ? d_slots : nullptr, n_slots > 0 ? N : 0);
 }
 
 int rpk_stats_get(const rpk_ctx* ctx, rpk_stats* out) {

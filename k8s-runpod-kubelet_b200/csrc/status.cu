@@ -27,6 +27,8 @@
 // The first also sweeps a list of slots (template flag SLOTS, rpk_status_diff_slots): the listed slots' packed
 // records are a table of their own, streamed the same way; only the hash row (slots[i] - idx_base) and the id
 // reported (slots[i]) differ.  updateAllPodStatuses compares only the pods it fetched this cycle (kubelet.go:836-864).
+// A sharded list sweep exchanges its changed list with its peers exactly as a whole-table one does
+// (rpk_status_diff_slots_device_gather).
 #include "rpk_device.cuh"
 #include "rpk_internal.cuh"
 
@@ -217,7 +219,8 @@ __device__ __forceinline__ void load_unit(const StatusArgs& a, uint32_t base, ui
     }
 }
 
-// SLOTS: the table is a packed slot list (StatusArgs::slots); the exchange outputs (n_out, flags) are not used
+// SLOTS: the table is a packed slot list (StatusArgs::slots).  The exchange (n_out, flags) is the same for both forms:
+// what it publishes is the list of global slot ids the final copy computes
 template <int STRIDE, int THREADS, bool SLOTS = false>
 __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(StatusArgs a, uint32_t n_units) {
     constexpr int kSThreads = THREADS, kSWarps = THREADS / 32;
@@ -296,12 +299,12 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
             s_excl = excl; s_carry = 0;
             if (cid == n_ctas - 1) {  // the last CTA in slot order owns the count
                 *a.n_changed = excl + total;
-                for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_count[o][a.peers.my_rank] = excl + total;
+                for (int o = 0; o < a.n_out; ++o) a.out_count[o][a.peers.my_rank] = excl + total;
             }
         }
     }
     __syncthreads();
-    const bool want_codes = a.changed_code != nullptr || (!SLOTS && a.n_out > 0 && a.out_code[0] != nullptr);
+    const bool want_codes = a.changed_code != nullptr || (a.n_out > 0 && a.out_code[0] != nullptr);
     // exclusive scan of the unit counts in unit order, 1024 units per round; thread t copies unit t's staged entries
     for (uint32_t r0 = c_lo; r0 < c_hi; r0 += kSThreads) {
         const uint32_t v = r0 + tid;
@@ -318,7 +321,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
             const uint32_t slot = a.stage_idx[v * kUnit + i];
             const uint32_t x = SLOTS ? __ldg(a.slots + slot) : a.idx_base + slot;  // SLOTS: slot is the list position
             if (a.changed_idx) a.changed_idx[off + i] = x;
-            for (int o = 0; !SLOTS && o < a.n_out; ++o) a.out_idx[o][off + i] = x;
+            for (int o = 0; o < a.n_out; ++o) a.out_idx[o][off + i] = x;
             if (want_codes) {  // translateRunPodStatus's decision, for the changed slots only: their records are read once more
                 const uint4 r = __ldg(reinterpret_cast<const uint4*>(a.records + (size_t)slot * rec_stride<STRIDE>(a)));
                 bool ports;
@@ -326,14 +329,14 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
                 const uint32_t kind = classify_status(mk64(r.x & ~0x80u, r.y), mk64(r.z, r.w), len, &ports);
                 const uint16_t cc = (uint16_t)status_code(kind, ports, (r.x & 0x80u) != 0u);
                 if (a.changed_code) a.changed_code[off + i] = cc;
-                for (int o = 0; !SLOTS && o < a.n_out; ++o) if (a.out_code[o]) a.out_code[o][off + i] = cc;
+                for (int o = 0; o < a.n_out; ++o) if (a.out_code[o]) a.out_code[o][off + i] = cc;
             }
         }
         __syncthreads();
         if (tid == kSThreads - 1) s_carry += wbase + inc;  // this round's total
         __syncthreads();
     }
-    if (!SLOTS && a.n_out > 0) __threadfence_system();  // peer stores are performed system-wide before this CTA counts as finished
+    if (a.n_out > 0) __threadfence_system();  // peer stores are performed system-wide before this CTA counts as finished
     else __threadfence();
     __syncthreads();
     if (tid == 0) s_last = atomicAdd(a.tile_counter + 1, 1u) == n_ctas - 1 ? 1u : 0u;
@@ -342,7 +345,7 @@ __global__ void __launch_bounds__(THREADS, 1024 / THREADS) k_status_stream(Statu
     // last CTA to finish: every look-back is over -- clean the state for the next call, then tell the peers
     for (uint32_t i = tid; i < n_ctas; i += kSThreads) a.tile_state[i] = 0ull;
     if (tid == 0) { a.tile_counter[0] = 0u; a.tile_counter[1] = 0u; }
-    if (!SLOTS && a.peers.n > 0 && warp == 0) signal_peers(a.peers, kFlagStatus, kFlagStatusCtr, 0, a.peers.inline_wait != 0);
+    if (a.peers.n > 0 && warp == 0) signal_peers(a.peers, kFlagStatus, kFlagStatusCtr, 0, a.peers.inline_wait != 0);
 }
 
 // previous state of individual slots: hash_prev[slots[i] - idx_base] = hash(records[i]) for the slots of this shard

@@ -316,3 +316,15 @@ class Engine:
             self._ctx, shard, N, self._dev_ptr(d_records, "d_records", shard, N * stride), stride,
             self._dev_ptr(d_hash_prev, "d_hash_prev", shard), idx_base, n_ranks, xchg, cap, my_rank,
             self._dev_ptr(d_n_changed, "d_n_changed", shard, at_least=1), self._stream(stream, shard)))
+
+    def status_diff_slots_device_gather(self, d_slots, d_records, stride: int, d_hash_prev, idx_base: int, xchg_ptrs, cap: int,
+                                        my_rank: int, d_n_changed, shard: int = 0, stream=None):
+        """Sharded slot-list sweep: the listed slots that lie in this rank's column (global slots [idx_base, idx_base + N),
+        N = d_hash_prev.numel()) are compared, and the changed ones (count, global ids in list order, codes) land in
+        region ``my_rank`` of every rank's exchange buffer (rpk_status_diff_slots_device_gather)."""
+        N, n = int(d_hash_prev.numel()), int(d_slots.numel())
+        n_ranks, xchg = _ptr_array(xchg_ptrs)
+        self._check(self._lib.rpk_status_diff_slots_device_gather(
+            self._ctx, shard, N, idx_base, n, self._dev_ptr(d_slots, "d_slots", shard),
+            self._dev_ptr(d_records, "d_records", shard, n * stride), stride, self._dev_ptr(d_hash_prev, "d_hash_prev", shard),
+            n_ranks, xchg, cap, my_rank, self._dev_ptr(d_n_changed, "d_n_changed", shard, at_least=1), self._stream(stream, shard)))
