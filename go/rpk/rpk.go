@@ -154,6 +154,58 @@ func (e *Engine) Select(p *Pods, wantTop5 bool) (best []int32, top5 []int32, err
 	return best, top5, nil
 }
 
+// PodsReset sizes the device pod table to n slots (the slot ids the status table uses) and sets every row to the
+// columns of a pod with no annotations: 16 GB, vcpu 0, ram 0, max price 0.5, SECURE (rpk_pods_reset).
+func (e *Engine) PodsReset(n int) error {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if rc := C.rpk_pods_reset(e.ctx, C.uint32_t(n)); rc != C.RPK_OK {
+		return lastError(e.ctx, rc)
+	}
+	return nil
+}
+
+// PodsSeedSlots writes row slots[i] of the pod table from row i of p (slots strictly ascending; nil optional columns
+// take Select's defaults).  processPendingPods (kubelet.go:747-814) seeds only the rows whose columns changed.
+func (e *Engine) PodsSeedSlots(slots []uint32, p *Pods) error {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if len(slots) == 0 {
+		return nil
+	}
+	if len(p.ReqMemGb) != len(slots) {
+		return fmt.Errorf("rpk: %d slots for %d pod rows", len(slots), len(p.ReqMemGb))
+	}
+	rc := C.rpk_pods_seed_slots(e.ctx, C.uint32_t(len(slots)), (*C.uint32_t)(unsafe.Pointer(&slots[0])), i32p(p.ReqMemGb),
+		i32p(p.ReqVCPU), i32p(p.ReqRAMGb), f64p(p.MaxPrice), u8p(p.Cloud))
+	if rc != C.RPK_OK {
+		return lastError(e.ctx, rc)
+	}
+	return nil
+}
+
+// SelectSlots is Select over rows of the pod table: best[i] / top5[5i:5i+5] are what Select returns for the row held at
+// slots[i] (any order, repeats allowed).  4 bytes go up per pod instead of its 21 bytes of columns.
+func (e *Engine) SelectSlots(slots []uint32, wantTop5 bool) (best []int32, top5 []int32, err error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	n := len(slots)
+	best = make([]int32, n)
+	if n == 0 {
+		return best, nil, nil
+	}
+	var t5 *C.int32_t
+	if wantTop5 {
+		top5 = make([]int32, n*TopK)
+		t5 = i32p(top5)
+	}
+	rc := C.rpk_select_slots(e.ctx, C.uint32_t(n), (*C.uint32_t)(unsafe.Pointer(&slots[0])), i32p(best), t5)
+	if rc != C.RPK_OK {
+		return nil, nil, lastError(e.ctx, rc)
+	}
+	return best, top5, nil
+}
+
 // StatusDiff is the batched predicate of updateAllPodStatuses (kubelet.go:870-873): records holds one
 // fixed slot per tracked pod (see EncodeStatusRecord); the indices of the slots whose (status, ports)
 // pair differs from the previous sweep come back ascending.

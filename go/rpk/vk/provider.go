@@ -2,7 +2,8 @@
 // PodLifecycleHandler / PodNotifier signatures of pkg/virtual_kubelet (kubelet.go:384,421,621,654,670,699,713),
 // whose two data-parallel loop bodies go through the rpk engine instead of per-pod Go loops:
 //
-//	processPendingPods  (kubelet.go:747-814)  one Engine.Select over ALL pending pods per tick
+//	processPendingPods  (kubelet.go:747-814)  one Engine.SelectSlots over ALL pending pods per tick, after
+//	                                          Engine.PodsSeedSlots of the rows whose columns changed
 //	updateAllPodStatuses (kubelet.go:816-974) one Engine.StatusDiffSlots over the slots fetched this tick
 //
 // NOT BUILT IN THIS REPOSITORY: the image has no Go toolchain and the reference's dependencies (client-go,
@@ -76,6 +77,10 @@ type Provider struct {
 	slotKey   []string // slot -> pod key
 	freeSlots []uint32
 
+	seedMutex sync.Mutex // the device pod table and its mirror: one deployBatch seeds and selects at a time
+	seededMem []int32    // maxPods: the columns the device pod table holds per slot
+	seededCld []uint8
+
 	notifyMutex sync.RWMutex
 	notifyFunc  func(*v1.Pod)
 	sweepMutex  sync.Mutex // one sweep at a time (two tickers reach it: kubelet.go:292-303, 718-729)
@@ -97,6 +102,13 @@ func NewProvider(api RunPodAPI, nGPUs, maxPods int) (*Provider, error) {
 	}
 	if err := e.StatusSeed(p.records, stride); err != nil { // empty slots hold the all-zero record: they never report
 		return nil, err
+	}
+	if err := e.PodsReset(maxPods); err != nil { // every slot: the columns of a pod with no annotations
+		return nil, err
+	}
+	p.seededMem, p.seededCld = make([]int32, maxPods), make([]uint8, maxPods)
+	for s := range p.seededMem {
+		p.seededMem[s], p.seededCld[s] = 16, rpk.CloudSecure
 	}
 	go p.tick(30*time.Second, p.updateAllPodStatuses) // startPeriodicStatusUpdates, kubelet.go:292-303
 	go p.tick(30*time.Second, p.processPendingPods)   // startPendingPodProcessor, kubelet.go:734-745
@@ -236,16 +248,49 @@ func (p *Provider) processPendingPods() {
 	}
 }
 
+// seedAndSelect seeds the pod-table rows whose columns differ from what the slot holds on the device (a changed pod or
+// owner Job, or a slot reused by another pod), in ascending slot order, then selects the batch by slot.  seedMutex held.
+func (p *Provider) seedAndSelect(slots []uint32, cols *rpk.Pods) ([]int32, error) {
+	idx := make([]int, 0, len(slots))
+	for i, s := range slots {
+		if cols.ReqMemGb[i] != p.seededMem[s] || cols.Cloud[i] != p.seededCld[s] {
+			idx = append(idx, i)
+		}
+	}
+	if len(idx) > 0 {
+		sort.Slice(idx, func(a, b int) bool { return slots[idx[a]] < slots[idx[b]] })
+		seed, seedSlots := &rpk.Pods{}, make([]uint32, 0, len(idx))
+		for _, i := range idx {
+			seedSlots = append(seedSlots, slots[i])
+			seed.ReqMemGb = append(seed.ReqMemGb, cols.ReqMemGb[i])
+			seed.Cloud = append(seed.Cloud, cols.Cloud[i])
+		}
+		if err := p.engine.PodsSeedSlots(seedSlots, seed); err != nil {
+			return nil, err
+		}
+		for k, s := range seedSlots {
+			p.seededMem[s], p.seededCld[s] = seed.ReqMemGb[k], seed.Cloud[k]
+		}
+	}
+	_, top5, err := p.engine.SelectSlots(slots, true)
+	return top5, err
+}
+
 func (p *Provider) deployBatch(keys []string) {
 	cols := &rpk.Pods{}
 	var pods []*v1.Pod
+	var slots []uint32
 	p.podsMutex.RLock()
 	for _, k := range keys {
-		if pod, ok := p.pods[k]; ok {
+		pod, ok := p.pods[k]
+		info, tracked := p.podStatus[k]
+		if ok && tracked {
+			// derived on every retry, owner Job included, as the reference does (runpod_client.go:1250-1281)
 			job := p.api.OwnerJobAnnotations(pod)
 			cols.ReqMemGb = append(cols.ReqMemGb, rpk.ReqMemColumn(rpk.AnnotationWithFallback(pod.Annotations, job, GpuMemoryAnnotation, "")))
 			cols.Cloud = append(cols.Cloud, rpk.CloudColumn(rpk.AnnotationWithFallback(pod.Annotations, job, CloudTypeAnnotation, "")))
 			pods = append(pods, pod)
+			slots = append(slots, info.slot)
 		}
 	}
 	p.podsMutex.RUnlock()
@@ -253,13 +298,16 @@ func (p *Provider) deployBatch(keys []string) {
 	if err != nil {
 		return
 	}
+	p.seedMutex.Lock()
 	if p.offers == nil || !sameTable(p.offers, offers) {
 		if err := p.engine.UploadOffers(offers); err != nil {
+			p.seedMutex.Unlock()
 			return
 		}
 		p.offers = offers
 	}
-	_, top5, err := p.engine.Select(cols, true)
+	top5, err := p.seedAndSelect(slots, cols)
+	p.seedMutex.Unlock()
 	if err != nil {
 		return
 	}

@@ -62,7 +62,7 @@ extern "C" {
 typedef struct rpk_ctx rpk_ctx;
 
 typedef struct rpk_stats {
-    uint64_t select_calls;        /* rpk_select + rpk_select_device */
+    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_device */
     uint64_t offer_scores;        /* sum of P*G over those calls */
     uint64_t status_calls;
     uint64_t status_records;      /* sum of N */
@@ -115,6 +115,30 @@ int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int
 int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t* req_vcpu,
                const int32_t* req_ram_gb, const double* max_price, const uint8_t* cloud, int32_t* best,
                int32_t* top5);
+
+/* ---- pod-requirement table: the selection over a list of pending slots ---------------------------------- */
+
+/* processPendingPods (kubelet.go:747-814) retries every tracked pod that is still Pending without a RunPod id, every
+ * 30 s, and its columns are usually the same as on the last tick.  The pod table keeps the five columns of every
+ * tracked slot on the device (the slot ids the caller gives the status table), so a tick seeds the rows that changed
+ * and selects by slot id: 4 bytes up per pending pod instead of 21.
+ *
+ * (Re)size the pod table to N slots on every GPU of the ctx and set every row to the columns of a pod with no
+ * annotations: req_mem_gb 16 (extractGPUMemory(""), runpod_client.go:1182), vcpu 0, ram 0, max_price 0.5, SECURE.
+ * Independent of rpk_status_reset.  The table is replicated: 21 bytes x N on each GPU. */
+int rpk_pods_reset(rpk_ctx* ctx, uint32_t N);
+/* Row slots[i] := element i of each column.  Columns may be NULL exactly where rpk_select's may, with the same defaults
+ * (req_mem_gb is required).  slots must be strictly ascending and < N of the pod table (else RPK_EINVAL, nothing
+ * written; no pod table: RPK_ESTATE).  Rows not listed are not touched.  Every GPU of the ctx gets the rows.
+ * n_slots == 0 is a no-op. */
+int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const int32_t* req_mem_gb,
+                        const int32_t* req_vcpu, const int32_t* req_ram_gb, const double* max_price, const uint8_t* cloud);
+/* rpk_select over rows of the pod table: best[i] / top5[5i, 5i+5) (top5 nullable) are what rpk_select returns for the
+ * row held at slot slots[i], bit for bit.  The list may be in any order and may repeat a slot.  An entry >= N of the
+ * pod table: RPK_EINVAL, best and top5 unspecified, no table or offer state changed (each sub-batch's part of the list
+ * is checked just before its upload).  No pod table or no offer table: RPK_ESTATE.  Counts as one select in rpk_stats
+ * (select_calls, offer_scores += n_slots * G).  n_slots == 0 is a no-op. */
+int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int32_t* best, int32_t* top5);
 
 /* Same on device-resident columns of GPU `shard` (index into the ctx's device list), enqueued on `stream`
  * (a cudaStream_t; NULL = the ctx's own stream for that shard; pass cudaStreamLegacy (0x1) for the legacy
@@ -200,7 +224,7 @@ int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream);
  * allocates synchronises its device, which would wait for a kernel that waits for a peer not launched yet. */
 int rpk_peer_inline_wait(rpk_ctx* ctx, int shard, int on);
 
-/* Device pointer of GPU `shard`'s copy of the full assignment vector written by the last rpk_select
+/* Device pointer of GPU `shard`'s copy of the full assignment vector written by the last rpk_select or rpk_select_slots
  * (ctx-owned; every GPU of the ctx holds the whole vector after the call). */
 const int32_t* rpk_best_device_ptr(const rpk_ctx* ctx, int shard);
 

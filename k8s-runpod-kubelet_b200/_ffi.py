@@ -38,6 +38,9 @@ ABI = {
     "rpk_host_free": (None, [_p]),
     "rpk_offers_upload": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
     "rpk_select": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p, _p]),
+    "rpk_pods_reset": (_int, [_p, _u32]),
+    "rpk_pods_seed_slots": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
+    "rpk_select_slots": (_int, [_p, _u32, _p, _p, _p]),
     "rpk_select_device": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_select_device_gather": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _int, _pp, _u32, _p, _p]),
     "rpk_select_device_gather_top5": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _int, _pp, _pp, _u32, _p]),

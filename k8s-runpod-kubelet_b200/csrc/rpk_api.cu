@@ -131,8 +131,34 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
     *hi = (uint32_t)((uint64_t)total * (uint64_t)(s + 1) / (uint64_t)n);
 }
 
-// The pod columns of a host select (rpk_select, rpk_tick); the optional ones are null when not passed.
-struct PodCols { const int32_t* req_mem; const int32_t* req_vcpu; const int32_t* req_ram; const double* max_price; const uint8_t* cloud; };
+// Where the rows of a host select come from: the caller's host columns (rpk_select, rpk_tick), or rows of the pod table
+// (rpk_select_slots), for which each sub-batch uploads its slot ids and gathers the five columns on the device.
+struct PodSource {
+    PodCols cols;
+    const uint32_t* slots;  // non-null: row i of the call is pod-table row slots[i]; cols is unused
+};
+
+// every entry of slots[0, n) is a row of a pod table of N rows.  The pipelined select runs this per sub-batch on the
+// thread that enqueues the next sub-batch, so its cost lands on the call in full: the CPU reads the list, measured at
+// 0.3-0.65 ns per id on an H100 host (0.35-0.56 ms per 1M ids, DESIGN section 4 "Pod table").
+// RPK_MEASURE_UNCHECKED_SLOTS: only for the copy of the library tools/select_slots_probe.py builds to time the check; it
+// accepts every list (k_pod_gather still skips entries outside the table, so no kernel reads outside it).
+bool slots_below(const uint32_t* slots, uint32_t n, uint32_t N) {
+#ifdef RPK_MEASURE_UNCHECKED_SLOTS
+    return true;
+#endif
+    uint32_t bad = 0;
+    for (uint32_t i = 0; i < n; ++i) bad |= (uint32_t)(slots[i] >= N);
+    return bad == 0;
+}
+
+// The gather of n pod-table rows whose slot ids are at d_slots (device) into lane ln's pod columns, on st; a's pod columns
+// then point at them.  Returns the kernels launched.
+int gather_pod_rows(DeviceState& ds, DeviceState::Lane& ln, uint32_t n, const uint32_t* d_slots, SelectArgs& a, cudaStream_t st) {
+    const PodRows out{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
+    a.req_mem = out.mem; a.req_vcpu = out.vcpu; a.req_ram = out.ram; a.max_price = out.max_price; a.cloud = out.cloud;
+    return launch_pod_gather(ds.pods_table(), ds.podsN, n, d_slots, out, st);
+}
 
 // One select on ds in lane ln's scratch: `a` holds the pod columns, P and the outputs; this adds the offer views and the
 // scratch and launches on st.  A bit-sliced table takes the persistent kernel above the fused kernel's batch size and
@@ -256,33 +282,43 @@ inline uint32_t sub_batch_cap(uint32_t Ps) {  // largest sub-batch a shard of Ps
     return cap ? cap : 1;
 }
 
-// Latency path of the host entry point (micro-batches, one GPU): the five pod columns are packed into one
-// pinned block -> ONE H2D; best and top5 come back in ONE D2H; one stream synchronise.  Same kernels.  Returns the
-// kernels launched.
-int select_small(DeviceState& ds, uint32_t P, const PodCols& pods, int32_t* best, int32_t* top5) {
+// Latency path of the host entry point (micro-batches, one GPU): the five pod columns -- or, from the pod table, the
+// slot ids -- are packed into one pinned block -> ONE H2D (then the gather, for slots); best and top5 come back in ONE
+// D2H; one stream synchronise.  Same kernels.  Slot ids are in range here.  Returns the kernels launched.
+int select_small(DeviceState& ds, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5) {
     RPK_CUDA(cudaSetDevice(ds.dev));
     const size_t in_cap = (size_t)kSmallBatch * 24, out_cap = (size_t)kSmallBatch * 6 * 4;
     ds.h_small.reserve(in_cap + out_cap);
     ds.d_small_in.reserve(in_cap); ds.d_small_out.reserve((size_t)kSmallBatch * 6);
-    const size_t o_mem = 0, o_vcpu = (size_t)P * 4, o_ram = (size_t)P * 8, o_price = ((size_t)P * 12 + 7) & ~(size_t)7,
-                 o_cloud = o_price + (size_t)P * 8, total = o_cloud + P;
     unsigned char* h = ds.h_small.h;
-    memcpy(h + o_mem, pods.req_mem, (size_t)P * 4);
-    if (pods.req_vcpu) memcpy(h + o_vcpu, pods.req_vcpu, (size_t)P * 4);
-    if (pods.req_ram) memcpy(h + o_ram, pods.req_ram, (size_t)P * 4);
-    if (pods.max_price) memcpy(h + o_price, pods.max_price, (size_t)P * 8);
-    if (pods.cloud) memcpy(h + o_cloud, pods.cloud, P);
     DeviceState::Lane& ln = ds.lane[0];
     cudaStream_t st = ln.stream;
     unsigned char* d = ds.d_small_in.p;
-    RPK_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, st));
     SelectArgs a{};
-    a.req_mem = (const int32_t*)(d + o_mem); a.req_vcpu = pods.req_vcpu ? (const int32_t*)(d + o_vcpu) : nullptr;
-    a.req_ram = pods.req_ram ? (const int32_t*)(d + o_ram) : nullptr; a.max_price = pods.max_price ? (const double*)(d + o_price) : nullptr;
-    a.cloud = pods.cloud ? (const uint8_t*)(d + o_cloud) : nullptr;
+    int launches = 0;
+    if (src.slots) {
+        ln.p_req_mem.reserve(kSmallBatch); ln.p_req_vcpu.reserve(kSmallBatch); ln.p_req_ram.reserve(kSmallBatch);
+        ln.p_max_price.reserve(kSmallBatch); ln.p_cloud.reserve(kSmallBatch);
+        memcpy(h, src.slots, (size_t)P * 4);
+        RPK_CUDA(cudaMemcpyAsync(d, h, (size_t)P * 4, cudaMemcpyHostToDevice, st));
+        launches += gather_pod_rows(ds, ln, P, (const uint32_t*)d, a, st);
+    } else {
+        const PodCols& pods = src.cols;
+        const size_t o_mem = 0, o_vcpu = (size_t)P * 4, o_ram = (size_t)P * 8, o_price = ((size_t)P * 12 + 7) & ~(size_t)7,
+                     o_cloud = o_price + (size_t)P * 8, total = o_cloud + P;
+        memcpy(h + o_mem, pods.req_mem, (size_t)P * 4);
+        if (pods.req_vcpu) memcpy(h + o_vcpu, pods.req_vcpu, (size_t)P * 4);
+        if (pods.req_ram) memcpy(h + o_ram, pods.req_ram, (size_t)P * 4);
+        if (pods.max_price) memcpy(h + o_price, pods.max_price, (size_t)P * 8);
+        if (pods.cloud) memcpy(h + o_cloud, pods.cloud, P);
+        RPK_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, st));
+        a.req_mem = (const int32_t*)(d + o_mem); a.req_vcpu = pods.req_vcpu ? (const int32_t*)(d + o_vcpu) : nullptr;
+        a.req_ram = pods.req_ram ? (const int32_t*)(d + o_ram) : nullptr; a.max_price = pods.max_price ? (const double*)(d + o_price) : nullptr;
+        a.cloud = pods.cloud ? (const uint8_t*)(d + o_cloud) : nullptr;
+    }
     a.P = P;
     a.best_out[0] = ds.d_small_out.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = top5 ? ds.d_small_out.p + P : nullptr;
-    const int launches = enqueue_select(ds, ln, a, st);
+    launches += enqueue_select(ds, ln, a, st);
     int32_t* hout = (int32_t*)(h + in_cap);
     RPK_CUDA(cudaMemcpyAsync(hout, ds.d_small_out.p, (size_t)P * 4 * (top5 ? 6 : 1), cudaMemcpyDeviceToHost, st));
     RPK_CUDA(cudaStreamSynchronize(st));
@@ -301,8 +337,11 @@ bool has_int32_max(const int32_t* col, uint32_t n) {
 // Buffers of the pipelined host select, sized from the calling thread (peers write into each other's best_full, so
 // every GPU's vector must exist before any shard is enqueued).  After the first call of a size this only compares
 // capacities.
-void reserve_select(rpk_ctx* ctx, uint32_t P, const PodCols& pods, bool top5) {
+void reserve_select(rpk_ctx* ctx, uint32_t P, const PodSource& src, bool top5) {
     const int n = (int)ctx->devs.size();
+    const PodCols& pods = src.cols;
+    const bool all = src.slots != nullptr;  // the gather writes all five columns
+    const bool vcpu = all || pods.req_vcpu, ram = all || pods.req_ram, price = all || pods.max_price, cloud = all || pods.cloud;
     for (int s = 0; s < n; ++s) {
         DeviceState& ds = ctx->devs[(size_t)s];
         uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
@@ -310,8 +349,8 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, const PodCols& pods, bool top5) {
         const uint32_t cap = sub_batch_cap(Ps);
         bool grow = P > ds.best_full.cap;
         for (auto& ln : ds.lane) {
-            grow = grow || cap > ln.p_req_mem.cap || (pods.req_vcpu && cap > ln.p_req_vcpu.cap) || (pods.req_ram && cap > ln.p_req_ram.cap) ||
-                   (pods.max_price && cap > ln.p_max_price.cap) || (pods.cloud && cap > ln.p_cloud.cap) ||
+            grow = grow || cap > ln.p_req_mem.cap || (vcpu && cap > ln.p_req_vcpu.cap) || (ram && cap > ln.p_req_ram.cap) ||
+                   (price && cap > ln.p_max_price.cap) || (cloud && cap > ln.p_cloud.cap) || (all && cap > ln.p_slots.cap) ||
                    (top5 && (size_t)cap * RPK_TOPK > ln.top5.cap);
             if (cap == Ps) break;  // a single sub-batch uses lane 0 only
         }
@@ -320,10 +359,11 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, const PodCols& pods, bool top5) {
         ds.best_full.reserve(P);
         for (auto& ln : ds.lane) {
             ln.p_req_mem.reserve(cap);
-            if (pods.req_vcpu) ln.p_req_vcpu.reserve(cap);
-            if (pods.req_ram) ln.p_req_ram.reserve(cap);
-            if (pods.max_price) ln.p_max_price.reserve(cap);
-            if (pods.cloud) ln.p_cloud.reserve(cap);
+            if (vcpu) ln.p_req_vcpu.reserve(cap);
+            if (ram) ln.p_req_ram.reserve(cap);
+            if (price) ln.p_max_price.reserve(cap);
+            if (cloud) ln.p_cloud.reserve(cap);
+            if (all) ln.p_slots.reserve(cap);
             if (top5) ln.top5.reserve((size_t)cap * RPK_TOPK);
             if (cap == Ps) break;
         }
@@ -332,29 +372,38 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, const PodCols& pods, bool top5) {
 
 // One shard's half of the host select: row sub-batches rotate over the lanes; within a lane everything is stream
 // ordered (H2D -> kernels -> D2H), across lanes copies and kernels overlap.  ds.ev[0] / ds.ev[3] bracket it on ds.stream;
-// the caller synchronises ds.stream.
-void enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodCols& pods, int32_t* best, int32_t* top5, uint64_t* launches) {
+// the caller synchronises ds.stream.  Slot ids are checked per sub-batch just before their upload: false = an entry
+// outside the pod table, and nothing from that sub-batch on was enqueued (the lanes still drain into ds.stream).
+bool enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5, uint64_t* launches) {
     const int n = (int)ctx->devs.size();
     DeviceState& ds = ctx->devs[(size_t)s];
     uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
     RPK_CUDA(cudaSetDevice(ds.dev));
     RPK_CUDA(cudaEventRecord(ds.ev[0], ds.stream));
     for (auto& ln : ds.lane) RPK_CUDA(cudaStreamWaitEvent(ln.stream, ds.ev[0], 0));
+    bool ok = true;
     int j = 0;
     for (uint32_t b0 = lo, nb = 0; b0 < hi; b0 += nb, ++j) {
         nb = sub_batch_rows(j, hi - b0);
         DeviceState::Lane& ln = ds.lane[j % DeviceState::kLanes];
         cudaStream_t st = ln.stream;
-        // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
-        auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
-            if (!col) return nullptr;
-            RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
-            return buf.p;
-        };
         SelectArgs a{};
-        a.req_mem = upload(ln.p_req_mem, pods.req_mem); a.req_vcpu = upload(ln.p_req_vcpu, pods.req_vcpu);
-        a.req_ram = upload(ln.p_req_ram, pods.req_ram); a.max_price = upload(ln.p_max_price, pods.max_price);
-        a.cloud = upload(ln.p_cloud, pods.cloud);
+        if (src.slots) {
+            if (!slots_below(src.slots + b0, nb, ds.podsN)) { ok = false; break; }
+            RPK_CUDA(cudaMemcpyAsync(ln.p_slots.p, src.slots + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
+            *launches += (uint64_t)gather_pod_rows(ds, ln, nb, ln.p_slots.p, a, st);
+        } else {
+            const PodCols& pods = src.cols;
+            // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
+            auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
+                if (!col) return nullptr;
+                RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
+                return buf.p;
+            };
+            a.req_mem = upload(ln.p_req_mem, pods.req_mem); a.req_vcpu = upload(ln.p_req_vcpu, pods.req_vcpu);
+            a.req_ram = upload(ln.p_req_ram, pods.req_ram); a.max_price = upload(ln.p_max_price, pods.max_price);
+            a.cloud = upload(ln.p_cloud, pods.cloud);
+        }
         a.P = nb;
         for (int o = 0; o < n; ++o) a.best_out[o] = ctx->devs[(size_t)o].best_full.p;
         a.n_out = n; a.row0 = b0; a.top5 = top5 ? ln.top5.p : nullptr;
@@ -368,6 +417,42 @@ void enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodCols& pods, 
         RPK_CUDA(cudaStreamWaitEvent(ds.stream, ln.done, 0));
     }
     RPK_CUDA(cudaEventRecord(ds.ev[3], ds.stream));
+    return ok;
+}
+
+// rpk_select and rpk_select_slots once their arguments are checked: one GPU and up to kSmallBatch rows take the latency
+// path, everything else the sub-batch pipeline on every GPU.  A slot id outside the pod table: RPK_EINVAL (best and
+// top5 unspecified, stats untouched).
+int select_host(rpk_ctx* ctx, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5, const char* who) {
+    return guarded(ctx, [&]() -> int {
+        const int n = (int)ctx->devs.size();
+        float tmax = 0.f;
+        bool ok = true;
+        if (n == 1 && P <= kSmallBatch) {
+            ok = !src.slots || slots_below(src.slots, P, ctx->devs[0].podsN);
+            if (ok) ctx->launches += (uint64_t)select_small(ctx->devs[0], P, src, best, top5);
+        } else {
+            std::vector<uint64_t> launches((size_t)n, 0);
+            std::vector<float> ms((size_t)n, 0.f);
+            std::vector<char> shard_ok((size_t)n, 1);
+            reserve_select(ctx, P, src, top5 != nullptr);
+            ctx->workers.run(n, [&](int s) {
+                shard_ok[(size_t)s] = enqueue_select_shard(ctx, s, P, src, best, top5, &launches[(size_t)s]);
+                DeviceState& ds = ctx->devs[(size_t)s];
+                RPK_CUDA(cudaStreamSynchronize(ds.stream));
+                RPK_CUDA(cudaEventElapsedTime(&ms[(size_t)s], ds.ev[0], ds.ev[3]));
+            });
+            for (int s = 0; s < n; ++s) {
+                ctx->launches += launches[(size_t)s]; tmax = ms[(size_t)s] > tmax ? ms[(size_t)s] : tmax;
+                ok = ok && shard_ok[(size_t)s];
+            }
+        }
+        if (!ok) return fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
+        ctx->stats.last_select_kernel_ms = 0.f;  // copies and kernels overlap in the pipelined host path: only the total is meaningful
+        ctx->stats.last_select_total_ms = tmax;  // 0 on the single-copy path
+        count_select(ctx, P, ctx->devs[0].G);
+        return RPK_OK;
+    });
 }
 
 // rpk_select_device_gather, and rpk_select_device_gather_top5 with t5 (its own arguments checked, a.top5 then points
@@ -589,29 +674,70 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
     if (P == 0) return RPK_OK;
     if (!req_mem_gb || !best) return fail(ctx, RPK_EINVAL, "rpk_select: req_mem_gb and best are required");
     for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
+    return select_host(ctx, P, PodSource{PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr}, best, top5, "rpk_select");
+}
+
+// ---- pod-requirement table -------------------------------------------------------------------------------
+
+int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
+    if (!ctx) return RPK_EINVAL;
+    for (auto& ds : ctx->devs) ds.pods_sized = false;  // a failure below leaves no table rather than a mix of sizes
     return guarded(ctx, [&]() -> int {
-        const PodCols pods{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud};
-        const int n = (int)ctx->devs.size();
-        float tmax = 0.f;
-        if (n == 1 && P <= kSmallBatch) {
-            ctx->launches += (uint64_t)select_small(ctx->devs[0], P, pods, best, top5);
-        } else {
-            std::vector<uint64_t> launches((size_t)n, 0);
-            std::vector<float> ms((size_t)n, 0.f);
-            reserve_select(ctx, P, pods, top5 != nullptr);
-            ctx->workers.run(n, [&](int s) {
-                enqueue_select_shard(ctx, s, P, pods, best, top5, &launches[(size_t)s]);
-                DeviceState& ds = ctx->devs[(size_t)s];
-                RPK_CUDA(cudaStreamSynchronize(ds.stream));
-                RPK_CUDA(cudaEventElapsedTime(&ms[(size_t)s], ds.ev[0], ds.ev[3]));
-            });
-            for (int s = 0; s < n; ++s) { ctx->launches += launches[(size_t)s]; tmax = ms[(size_t)s] > tmax ? ms[(size_t)s] : tmax; }
+        for (auto& ds : ctx->devs) {
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            const size_t cap = N ? N : 1;
+            ds.pt_mem.reserve(cap); ds.pt_vcpu.reserve(cap); ds.pt_ram.reserve(cap); ds.pt_max_price.reserve(cap); ds.pt_cloud.reserve(cap);
+            ctx->launches += (uint64_t)launch_pod_fill(ds.pods_table(), N, ds.sm_count, ds.stream);
+            RPK_CUDA(cudaStreamSynchronize(ds.stream));
+            ds.podsN = N;
         }
-        ctx->stats.last_select_kernel_ms = 0.f;  // copies and kernels overlap in the pipelined host path: only the total is meaningful
-        ctx->stats.last_select_total_ms = tmax;  // 0 on the single-copy path
-        count_select(ctx, P, ctx->devs[0].G);
+        for (auto& ds : ctx->devs) ds.pods_sized = true;
         return RPK_OK;
     });
+}
+
+int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const int32_t* req_mem_gb, const int32_t* req_vcpu,
+                        const int32_t* req_ram_gb, const double* max_price, const uint8_t* cloud) {
+    if (!ctx) return RPK_EINVAL;
+    if (n_slots == 0) return RPK_OK;
+    if (!slots || !req_mem_gb) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slots and req_mem_gb are required");
+    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_seed_slots: no pod table (call rpk_pods_reset first)");
+    const uint32_t N = ctx->devs[0].podsN;
+    for (uint32_t i = 0; i < n_slots; ++i) {
+        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slot index outside the pod table");
+        if (i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slots must be strictly ascending");
+    }
+    return guarded(ctx, [&]() -> int {
+        // staging block: [slots : 4n][mem : 4n][vcpu : 4n][ram : 4n][max_price : 8n, 8-byte aligned][cloud : n]
+        const size_t n = n_slots, o_mem = 4 * n, o_vcpu = 8 * n, o_ram = 12 * n, o_price = (16 * n + 7) & ~(size_t)7,
+                     o_cloud = o_price + 8 * n;
+        for (auto& ds : ctx->devs) {  // the table is replicated: every GPU gets every row
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ds.pt_seed.reserve(o_cloud + n);
+            unsigned char* d = ds.pt_seed.p;
+            auto up = [&](size_t off, const void* col, size_t bytes) -> const unsigned char* {
+                if (!col) return nullptr;
+                RPK_CUDA(cudaMemcpyAsync(d + off, col, bytes, cudaMemcpyHostToDevice, ds.stream));
+                return d + off;
+            };
+            const uint32_t* d_slots = (const uint32_t*)up(0, slots, 4 * n);
+            const PodCols in{(const int32_t*)up(o_mem, req_mem_gb, 4 * n), (const int32_t*)up(o_vcpu, req_vcpu, 4 * n),
+                             (const int32_t*)up(o_ram, req_ram_gb, 4 * n), (const double*)up(o_price, max_price, 8 * n),
+                             (const uint8_t*)up(o_cloud, cloud, n)};
+            ctx->launches += (uint64_t)launch_pod_seed(ds.pods_table(), ds.podsN, n_slots, d_slots, in, ds.stream);
+            RPK_CUDA(cudaStreamSynchronize(ds.stream));
+        }
+        return RPK_OK;
+    });
+}
+
+int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int32_t* best, int32_t* top5) {
+    if (!ctx) return RPK_EINVAL;
+    if (n_slots == 0) return RPK_OK;
+    if (!slots || !best) return fail(ctx, RPK_EINVAL, "rpk_select_slots: slots and best are required");
+    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_slots: no pod table (call rpk_pods_reset first)");
+    for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select_slots: no offer table uploaded (call rpk_offers_upload first)");
+    return select_host(ctx, n_slots, PodSource{PodCols{}, slots}, best, top5, "rpk_select_slots");
 }
 
 // ---- cross-process peer vectors (CUDA IPC) ---------------------------------------------------------------
@@ -979,7 +1105,7 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
     const StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
     if (int rc = check_sweep(ctx, h, "rpk_tick")) return rc;
     return guarded(ctx, [&]() -> int {
-        const PodCols pods{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud};
+        const PodSource pods{PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr};
         const int n = (int)ctx->devs.size();
         if (P > 0) reserve_select(ctx, P, pods, top5 != nullptr);
         for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, h);

@@ -274,6 +274,15 @@ PersistPlan persist_plan(const SelectArgs& a, int sm_count);  // a.pk.bm_words a
 uint32_t persist_hdr_words(const PersistPlan& pl);
 int launch_select_persist(const SelectArgs& a, const PersistPlan& pl, cudaStream_t st);
 uint32_t status_state_words(int sm_count);
+// The five pod columns of a select: the caller's host columns (rpk_select, rpk_tick; the optional ones null when not
+// passed), or staged device columns of a pod-table seed (same nullability).
+struct PodCols { const int32_t* req_mem; const int32_t* req_vcpu; const int32_t* req_ram; const double* max_price; const uint8_t* cloud; };
+// Five device columns, none null: the pod-requirement table (rows = slots) or a lane's compact pod columns
+struct PodRows { int32_t* mem; int32_t* vcpu; int32_t* ram; double* max_price; uint8_t* cloud; };
+// pod-requirement table (pods.cu): N = the table's rows; entries of d_slots outside [0, N) are skipped
+int launch_pod_fill(const PodRows& t, uint32_t N, int sm_count, cudaStream_t st);
+int launch_pod_seed(const PodRows& t, uint32_t N, uint32_t n, const uint32_t* d_slots, const PodCols& in, cudaStream_t st);
+int launch_pod_gather(const PodRows& t, uint32_t N, uint32_t n, const uint32_t* d_slots, const PodRows& out, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
@@ -339,6 +348,7 @@ struct DeviceState {
         cudaStream_t stream = nullptr;
         cudaEvent_t done = nullptr;
         DevBuf<int32_t> p_req_mem, p_req_vcpu, p_req_ram; DevBuf<double> p_max_price; DevBuf<uint8_t> p_cloud;
+        DevBuf<uint32_t> p_slots;  // rpk_select_slots: the sub-batch's slot ids, gathered into the five p_* columns
         DevBuf<int32_t> top5;
         DevBuf<uint32_t> rw, order, pos, ctrs;
         DevBuf<uint16_t> key; DevBuf<uint2> ord_rw; DevBuf<uint32_t> hist, k0_base, hdr;  // persistent path
@@ -361,6 +371,11 @@ struct DeviceState {
     cudaEvent_t ev_sel = nullptr, ev_st = nullptr;
     bool status_dirty = false;             // a status launch failed midway: re-zero the look-back state before the next one
     uint32_t statusN = 0; bool status_sized = false;
+    // pod-requirement table (rpk_pods_reset): the five columns of podsN slots, the whole table on every GPU of the ctx
+    DevBuf<int32_t> pt_mem, pt_vcpu, pt_ram; DevBuf<double> pt_max_price; DevBuf<uint8_t> pt_cloud;
+    DevBuf<unsigned char> pt_seed;         // rpk_pods_seed_slots: the slot ids and the columns of one seed
+    uint32_t podsN = 0; bool pods_sized = false;
+    PodRows pods_table() { return PodRows{pt_mem.p, pt_vcpu.p, pt_ram.p, pt_max_price.p, pt_cloud.p}; }
     ~DeviceState();
 };
 

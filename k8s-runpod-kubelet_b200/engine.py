@@ -170,6 +170,32 @@ class Engine:
             _np_ptr(top5, np.int32, P * 5, "top5") if top5 is not None else None))
         return best, top5
 
+    # -- pod-requirement table: selection over slot lists -----------------------------------------------
+    def pods_reset(self, N: int):
+        """(Re)size the pod table to N slots, every row the columns of a pod with no annotations (rpk_pods_reset)."""
+        self._check(self._lib.rpk_pods_reset(self._ctx, N))
+
+    def pods_seed_slots(self, slots: np.ndarray, pods: dict):
+        """Row slots[i] := row i of the host columns ``pods`` (as ``select`` takes them; slots strictly ascending)."""
+        n = int(pods["req_mem_gb"].shape[0])
+        slots = np.ascontiguousarray(slots, np.uint32)  # keep the converted array alive across the call
+        self._check(self._lib.rpk_pods_seed_slots(
+            self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(pods["req_mem_gb"], np.int32, n, "req_mem_gb"),
+            _np_ptr(pods.get("req_vcpu"), np.int32, n, "req_vcpu"), _np_ptr(pods.get("req_ram_gb"), np.int32, n, "req_ram_gb"),
+            _np_ptr(pods.get("max_price"), np.float64, n, "max_price"), _np_ptr(pods.get("cloud"), np.uint8, n, "cloud")))
+
+    def select_slots(self, slots: np.ndarray, want_top5: bool = False, out_best=None, out_top5=None):
+        """``select`` over rows of the pod table: ``(best[n], top5[n,5] | None)`` for the rows held at ``slots`` (any
+        order, repeats allowed)."""
+        slots = np.ascontiguousarray(slots, np.uint32)  # keep the converted array alive across the call
+        n = int(slots.size)
+        best = out_best if out_best is not None else np.empty(n, np.int32)
+        top5 = (out_top5 if out_top5 is not None else np.empty((n, 5), np.int32)) if want_top5 else None
+        self._check(self._lib.rpk_select_slots(
+            self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(best, np.int32, n, "best"),
+            _np_ptr(top5, np.int32, n * 5, "top5") if top5 is not None else None))
+        return best, top5
+
     def select_device(self, pods: dict, d_best, d_top5=None, shard: int = 0, stream=None):
         """torch CUDA columns in, result enqueued on ``stream`` (default: torch's current stream on the shard's GPU)."""
         P, cols = self._dev_pods(pods, shard)

@@ -326,6 +326,10 @@ Provider::Provider(std::shared_ptr<RunPodAPI> api, int n_gpus, uint32_t max_pods
     if (rpk_status_reset(ctx_, max_pods_) != RPK_OK) throw std::runtime_error(rpk_last_error(ctx_));
     // empty slots hold the all-zero record from now on: seed it so they never report
     if (rpk_status_seed(ctx_, max_pods_, records_.data(), stride_) != RPK_OK) throw std::runtime_error(rpk_last_error(ctx_));
+    // the pod table starts as the columns of a pod with no annotations in every slot; the mirror says the same
+    if (rpk_pods_reset(ctx_, max_pods_) != RPK_OK) throw std::runtime_error(rpk_last_error(ctx_));
+    seeded_.req_mem_gb.assign(max_pods_, 16); seeded_.req_vcpu.assign(max_pods_, 0); seeded_.req_ram_gb.assign(max_pods_, 0);
+    seeded_.max_price.assign(max_pods_, DefaultMaxPrice); seeded_.cloud.assign(max_pods_, RPK_CLOUD_SECURE);
     if (opt_.self_tick) {  // go provider.startPeriodicStatusUpdates(); go provider.startPendingPodProcessor() -- kubelet.go:374-376
         StartTicker(opt_.periodic_interval_s, [this] { UpdateAllPodStatuses(); });
         StartTicker(opt_.pending_interval_s, [this] { ProcessPendingPods(); });
@@ -527,30 +531,63 @@ bool Provider::RefreshOffersLocked(std::string* err) {
 }
 
 // DeployPodToRunPod for a batch (kubelet.go:435-503 + runpod_client.go:1250-1343): columns from
-// annotations -> ONE rpk_select over the whole batch -> gpuTypeIds per pod -> DeployPod -> annotations.
+// annotations -> the rows that changed since the last tick into the device pod table -> ONE rpk_select_slots over the
+// whole batch -> gpuTypeIds per pod -> DeployPod -> annotations.
 bool Provider::DeployBatch(const std::vector<std::string>& keys) {
     std::vector<PodPtr> pods;
     std::vector<std::string> live;
+    std::vector<uint32_t> slots;
     {
         std::lock_guard<std::mutex> g(pods_mutex_);
         for (const auto& k : keys) {
             auto it = pods_.find(k);
-            if (it != pods_.end() && it->second.pod) { pods.push_back(it->second.pod); live.push_back(k); }
+            if (it != pods_.end() && it->second.pod) { pods.push_back(it->second.pod); live.push_back(k); slots.push_back(it->second.slot); }
         }
     }
     if (pods.empty()) return true;
     std::string err;
     const uint32_t P = (uint32_t)pods.size();
     PodColumnsSoA cols;
-    PrepareColumnsBatch(pods, &cols);  // the whole batch's annotations -> columns, over the host threads
+    // the whole batch's annotations -> columns, over the host threads, on every retry as the reference derives them
+    // (runpod_client.go:1250-1281): a changed pod or owner-Job annotation is picked up by the compare below
+    PrepareColumnsBatch(pods, &cols);
     std::vector<int32_t> best(P), top5((size_t)P * RPK_TOPK);
     std::vector<std::vector<std::string>> gpu_type_ids(P);  // params["gpuTypeIds"], runpod_client.go:1339
     {   // table refresh, selection and index -> id lookup under ONE lock: another thread's refresh cannot swap the table
         // between the select and the lookup (indices would resolve against a different, possibly shorter, table)
         std::lock_guard<std::mutex> g(engine_mutex_);
         if (!RefreshOffersLocked(&err)) return false;  // "failed to get GPU types": every pod of the batch retries later
-        if (rpk_select(ctx_, P, cols.req_mem_gb.data(), cols.req_vcpu.data(), cols.req_ram_gb.data(), cols.max_price.data(),
-                       cols.cloud.data(), best.data(), top5.data()) != RPK_OK) return false;
+        // rows whose columns differ from what the slot holds on the device (a changed pod, or a slot reused by another
+        // pod), in ascending slot order; prices compare bit for bit, so a NaN bound is not re-seeded every tick
+        std::vector<std::pair<uint32_t, uint32_t>> changed;  // (slot, batch row)
+        for (uint32_t i = 0; i < P; ++i) {
+            const uint32_t s = slots[i];
+            if (cols.req_mem_gb[i] != seeded_.req_mem_gb[s] || cols.req_vcpu[i] != seeded_.req_vcpu[s] ||
+                cols.req_ram_gb[i] != seeded_.req_ram_gb[s] || cols.cloud[i] != seeded_.cloud[s] ||
+                std::memcmp(&cols.max_price[i], &seeded_.max_price[s], sizeof(double)) != 0)
+                changed.emplace_back(s, i);
+        }
+        if (!changed.empty()) {
+            std::sort(changed.begin(), changed.end());
+            PodColumnsSoA seed;
+            seed.resize(changed.size());
+            std::vector<uint32_t> seed_slots(changed.size());
+            for (size_t k = 0; k < changed.size(); ++k) {
+                const uint32_t i = changed[k].second;
+                seed_slots[k] = changed[k].first;
+                seed.req_mem_gb[k] = cols.req_mem_gb[i]; seed.req_vcpu[k] = cols.req_vcpu[i]; seed.req_ram_gb[k] = cols.req_ram_gb[i];
+                seed.max_price[k] = cols.max_price[i]; seed.cloud[k] = cols.cloud[i];
+            }
+            if (rpk_pods_seed_slots(ctx_, (uint32_t)changed.size(), seed_slots.data(), seed.req_mem_gb.data(), seed.req_vcpu.data(),
+                                    seed.req_ram_gb.data(), seed.max_price.data(), seed.cloud.data()) != RPK_OK) return false;
+            for (size_t k = 0; k < changed.size(); ++k) {
+                const uint32_t s = seed_slots[k];
+                seeded_.req_mem_gb[s] = seed.req_mem_gb[k]; seeded_.req_vcpu[s] = seed.req_vcpu[k]; seeded_.req_ram_gb[s] = seed.req_ram_gb[k];
+                seeded_.max_price[s] = seed.max_price[k]; seeded_.cloud[s] = seed.cloud[k];
+            }
+            pod_seeds_ += changed.size();
+        }
+        if (rpk_select_slots(ctx_, P, slots.data(), best.data(), top5.data()) != RPK_OK) return false;
         ++select_calls_;
         for (uint32_t i = 0; i < P; ++i)
             for (int k = 0; k < RPK_TOPK; ++k) {

@@ -5,8 +5,9 @@
 // meaning and error behaviour follow pkg/virtual_kubelet:
 //
 //   Provider::CreatePod/UpdatePod/DeletePod/GetPod/GetPodStatus/GetPods/NotifyPods   kubelet.go:384-731
-//   Provider::ProcessPendingPods     kubelet.go:747-814   (now ONE rpk_select per tick instead of one
-//                                                           GraphQL fetch + filter + sort per pod)
+//   Provider::ProcessPendingPods     kubelet.go:747-814   (now ONE rpk_select_slots per tick instead of one
+//                                                           GraphQL fetch + filter + sort per pod; only rows whose
+//                                                           columns changed are seeded into the device pod table)
 //   Provider::UpdateAllPodStatuses   kubelet.go:816-974   (now ONE rpk_status_diff per tick)
 //   PrepareColumns / column producers runpod_client.go:1102-1134, 1181-1191, 1261-1281
 //   CheckPortsExposed                kubelet.go:566-605
@@ -185,6 +186,7 @@ public:
     // observability for tests / the benchmark harness
     const InstanceInfo* Info(const std::string& ns, const std::string& name);
     uint64_t SelectCalls() const { return select_calls_; }
+    uint64_t PodSeeds() const { return pod_seeds_; }  // pod-table rows re-seeded because a pending pod's columns changed
     uint64_t StatusCalls() const { return status_calls_; }
     uint64_t OfferUploads() const { return offer_uploads_; }
     uint64_t HostCompares() const { return host_compares_; }  // sweeps' pods compared on the host (status longer than any slot)
@@ -224,9 +226,10 @@ private:
     std::vector<uint32_t> free_slots_;
     std::vector<std::string> slot_key_;
     uint32_t max_pods_;
+    PodColumnsSoA seeded_;              // max_pods rows: what the device pod table holds per slot (engine_mutex_)
     ProviderOptions opt_;
     double now_ = 0;
-    uint64_t select_calls_ = 0, status_calls_ = 0, offer_uploads_ = 0;
+    uint64_t select_calls_ = 0, status_calls_ = 0, offer_uploads_ = 0, pod_seeds_ = 0;
 };
 
 }  // namespace rpkhost

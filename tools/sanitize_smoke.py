@@ -25,6 +25,18 @@ for force in () if ONLY_MULTI else (None, "bitmap_grouped", "packed_pos", "packe
         ob, ot = oracle.select(offers, pods, n_threads=8)
         assert np.array_equal(best, ob) and np.array_equal(t5, ot), (force, P)
 os.environ.pop("RPK_FORCE_KERNEL", None)
+# the pod table: one seed, then a select by slot on the latency path and on the pipelined path (the gather indexes the
+# table with caller input)
+if not ONLY_MULTI:
+    eng.upload_offers(offers)
+    pods = rpk.synth.make_pods(200_000, seed=11)
+    eng.pods_reset(200_000)
+    eng.pods_seed_slots(np.arange(200_000, dtype=np.uint32), pods)
+    for n in (37, 140_000):
+        sl = np.random.default_rng(n).integers(0, 200_000, n).astype(np.uint32)
+        best, t5 = eng.select_slots(sl, want_top5=True)
+        ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, n_threads=8)
+        assert np.array_equal(best, ob) and np.array_equal(t5, ot), n
 for stride in () if ONLY_MULTI else (16, 32, 64):
     tab = oracle.StatusTable(30_000, stride)
     e2 = rpk.Engine(1)
