@@ -62,7 +62,7 @@ extern "C" {
 typedef struct rpk_ctx rpk_ctx;
 
 typedef struct rpk_stats {
-    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_device */
+    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_device + rpk_select_slots_device */
     uint64_t offer_scores;        /* sum of P*G over those calls */
     uint64_t status_calls;
     uint64_t status_records;      /* sum of N */
@@ -181,6 +181,33 @@ int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int
                                   const int32_t* d_req_vcpu, const int32_t* d_req_ram_gb, const double* d_max_price,
                                   const uint8_t* d_cloud, int n_out, int32_t* const* d_best_full,
                                   int32_t* const* d_top5_full, uint32_t row0, void* stream);
+
+/* The three calls above over rows of the pod table, for one-process-per-GPU callers: the pending pods are a device list
+ * of slot ids instead of five device columns (4 bytes per pod instead of 21; the table is seeded from the host with
+ * rpk_pods_seed_slots as the rows change).
+ *   - Rows: output row i is what rpk_select_slots returns for list entry i, bit for bit.  The row is read from GPU
+ *     `shard`'s copy of the ctx's pod table; the table is replicated, so every shard of a multi-GPU ctx has it.
+ *   - List: d_slots[0, n_slots) is device memory on GPU `shard`, in any order, and may repeat a slot.
+ *   - Entries outside the table: nothing checks the list on the host.  An entry >= N of the pod table gives -1 and a
+ *     list of five -1, the result of a pod with nothing feasible.  No kernel reads outside the table.
+ *   - Outputs, placement, alignment, direct-store fallback, signal, inline wait and refusals: exactly as the column call
+ *     of the same name, with n_slots in place of P.  n_slots == 0 behaves like P == 0 there: a bound gather signals, and
+ *     nothing else happens.
+ *   - No pod table or no offer table on GPU `shard`: RPK_ESTATE.  d_slots NULL with n_slots > 0: RPK_EINVAL.  Both
+ *     before anything is enqueued.
+ *   - Counts as one select in rpk_stats (offer_scores += n_slots * G).  One gather kernel runs ahead of the select.
+ *   - rpk_pods_seed_slots and rpk_pods_reset wait for a device select still running before they touch the table.
+ *   - After one call of a given size the call only enqueues launches, so it can be captured in a CUDA graph.  A replay
+ *     reads the table as it is at replay time, so seeds between replays are picked up (the caller orders a seed after
+ *     a replay still in flight; the library does not see replays).  rpk_pods_reset invalidates a captured graph: the
+ *     graph keeps the old N and possibly buffers the reset freed. */
+int rpk_select_slots_device(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int32_t* d_best,
+                            int32_t* d_top5, void* stream);
+int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
+                                   int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream);
+int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
+                                        int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0,
+                                        void* stream);
 
 /* Cross-process peer vectors for one-process-per-GPU callers (torchrun-style): allocate a plain cudaMalloc
  * buffer on GPU `shard` and export its 64-byte CUDA IPC handle; another process opens the handle and gets a

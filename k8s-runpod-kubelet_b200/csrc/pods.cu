@@ -5,10 +5,13 @@
 // Kernels:
 //   k_pod_fill      every row := the columns of a pod with no annotations (rpk_pods_reset)
 //   k_pod_seed      row slots[i] := element i of each staged column; a NULL column writes its default (rpk_pods_seed_slots)
-//   k_pod_gather    compact columns of one sub-batch of rpk_select_slots: element i := row slots[i] of the table, written
-//                   into the lane's pod-column buffers, which the select kernels then read as rpk_select's uploaded ones
-// Every slot read here was checked against the table's N on the host before its upload; the kernels skip an entry
-// outside [0, N) all the same, so no caller input can make them touch memory outside the table.
+//   k_pod_gather    compact columns of one rpk_select_slots sub-batch, or of one rpk_select_slots_device* call: element
+//                   i := row slots[i] of the table, written into the lane's pod-column buffers, which the select kernels
+//                   then read as rpk_select's uploaded ones
+// The host entry points check every slot against the table's N before its upload.  The device entry points cannot, so
+// an entry outside [0, N) is defined here: the seed skips it, and the gather writes a row with cloud byte kCloudNone,
+// which every select path finishes as "neither cloud" (runpod_client.go:469-475): -1 and five -1.  No caller input
+// can make these kernels touch memory outside the table.
 #include <algorithm>
 
 #include "rpk_internal.cuh"
@@ -17,6 +20,7 @@ namespace rpk {
 
 constexpr int kPodThreads = 256;
 constexpr int32_t kDefaultMemGb = 16;  // extractGPUMemory("") (runpod_client.go:1182)
+constexpr uint8_t kCloudNone = 2;      // neither RPK_CLOUD_SECURE nor RPK_CLOUD_COMMUNITY: no offer is feasible
 
 __global__ void k_pod_fill(PodRows t, uint32_t N) {
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < N; i += gridDim.x * blockDim.x) {
@@ -40,7 +44,10 @@ __global__ void k_pod_gather(PodRows t, uint32_t N, uint32_t n, const uint32_t* 
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const uint32_t s = slots[i];
-    if (s >= N) return;
+    if (s >= N) {  // a row nothing matches; the other columns hold a pod with no annotations
+        out.mem[i] = kDefaultMemGb; out.vcpu[i] = 0; out.ram[i] = 0; out.max_price[i] = RPK_DEFAULT_MAX_PRICE; out.cloud[i] = kCloudNone;
+        return;
+    }
     out.mem[i] = __ldg(t.mem + s); out.vcpu[i] = __ldg(t.vcpu + s); out.ram[i] = __ldg(t.ram + s);
     out.max_price[i] = __ldg(t.max_price + s); out.cloud[i] = __ldg(t.cloud + s);
 }

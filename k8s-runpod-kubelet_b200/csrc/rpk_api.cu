@@ -131,8 +131,9 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
     *hi = (uint32_t)((uint64_t)total * (uint64_t)(s + 1) / (uint64_t)n);
 }
 
-// Where the rows of a host select come from: the caller's host columns (rpk_select, rpk_tick), or rows of the pod table
-// (rpk_select_slots), for which each sub-batch uploads its slot ids and gathers the five columns on the device.
+// Where the rows of a select come from: the caller's columns (rpk_select, rpk_tick: host memory; rpk_select_device*:
+// device memory), or rows of the pod table (rpk_select_slots: a host list, each sub-batch uploads its slot ids and
+// gathers the five columns on the device; rpk_select_slots_device*: a device list, gathered in one pass).
 struct PodSource {
     PodCols cols;
     const uint32_t* slots;  // non-null: row i of the call is pod-table row slots[i]; cols is unused
@@ -142,7 +143,7 @@ struct PodSource {
 // thread that enqueues the next sub-batch, so its cost lands on the call in full: the CPU reads the list, measured at
 // 0.3-0.65 ns per id on an H100 host (0.35-0.56 ms per 1M ids, DESIGN section 4 "Pod table").
 // RPK_MEASURE_UNCHECKED_SLOTS: only for the copy of the library tools/select_slots_probe.py builds to time the check; it
-// accepts every list (k_pod_gather still skips entries outside the table, so no kernel reads outside it).
+// accepts every list (k_pod_gather gathers an entry outside the table as a row nothing matches and reads nothing there).
 bool slots_below(const uint32_t* slots, uint32_t n, uint32_t N) {
 #ifdef RPK_MEASURE_UNCHECKED_SLOTS
     return true;
@@ -456,10 +457,10 @@ int select_host(rpk_ctx* ctx, uint32_t P, const PodSource& src, int32_t* best, i
 }
 
 // rpk_select_device_gather, and rpk_select_device_gather_top5 with t5 (its own arguments checked, a.top5 then points
-// into the local top-5 vector).  The shard is in range.
-int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
-                         const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud, int n_out,
-                         int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, const Top5Gather* t5, void* stream) {
+// into the local top-5 vector); with src.slots, the rpk_select_slots_device* calls of the same name (a NULL list with
+// P > 0 already refused).  The shard is in range.
+int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& src, int n_out, int32_t* const* d_best_full,
+                         uint32_t row0, int32_t* d_top5, const Top5Gather* t5, void* stream) {
     DeviceState& ds = ctx->devs[(size_t)shard];
     const PeerGroup& peers = ctx->bind[(size_t)shard];
     cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
@@ -473,25 +474,60 @@ int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_r
             return RPK_OK;
         });
     }
-    if (!d_req_mem_gb || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
+    if ((!src.slots && !src.cols.req_mem) || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
     for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device: NULL output vector");
+    if (src.slots && !ds.pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_slots_device: no pod table on this shard (call rpk_pods_reset first)");
     if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
+        DeviceState::Lane& ln = ds.lane[0];
+        if (src.slots) {  // the gather's compact columns: allocated on the first call of a size only
+            ln.p_req_mem.reserve(P); ln.p_req_vcpu.reserve(P); ln.p_req_ram.reserve(P); ln.p_max_price.reserve(P); ln.p_cloud.reserve(P);
+        }
         SelectArgs a{};
-        a.req_mem = d_req_mem_gb; a.req_vcpu = d_req_vcpu; a.req_ram = d_req_ram_gb; a.max_price = d_max_price; a.cloud = d_cloud;
+        ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);  // the gather writes lane 0's columns: after the last select
+        if (src.slots) {
+            ctx->launches += (uint64_t)gather_pod_rows(ds, ln, P, src.slots, a, st);
+        } else {
+            const PodCols& c = src.cols;
+            a.req_mem = c.req_mem; a.req_vcpu = c.req_vcpu; a.req_ram = c.req_ram; a.max_price = c.max_price; a.cloud = c.cloud;
+        }
         a.P = P;
         for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
         a.n_out = n_out; a.row0 = row0;
         a.top5 = t5 ? t5->out[t5->self_out] + (size_t)RPK_TOPK * row0 : d_top5;
         a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
         if (n_out > 1) a.peers = peers;
-        ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);
-        ctx->launches += (uint64_t)enqueue_select(ds, ds.lane[0], a, st, t5);
+        ctx->launches += (uint64_t)enqueue_select(ds, ln, a, st, t5);
         guard.done();
         count_select(ctx, P, ds.G);
         return RPK_OK;
     });
+}
+
+// rpk_select_device_gather_top5 and rpk_select_slots_device_gather_top5: the top-5 vectors' checks, then the gather.
+// The shard is in range.
+int select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& src, int n_out, int32_t* const* d_best_full,
+                              int32_t* const* d_top5_full, uint32_t row0, void* stream) {
+    if (!d_best_full || !d_top5_full || n_out < 1 || n_out > RPK_MAX_GPUS)
+        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 1..8 best and top-5 vectors are required");
+    for (int o = 0; o < n_out; ++o)
+        if (!d_best_full[o] || !d_top5_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: NULL output vector");
+    if ((uint64_t)P * RPK_TOPK > UINT32_MAX) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 5*P does not fit in uint32_t");
+    if (!same_phase(n_out, d_top5_full))
+        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: the top-5 vectors differ in 16-byte phase");
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    Top5Gather t5{};
+    const int rc = guarded(ctx, [&]() -> int {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        t5.self_out = local_vector(ctx, shard, ds.dev, n_out, d_top5_full);
+        return RPK_OK;
+    });
+    if (rc != RPK_OK) return rc;
+    if (t5.self_out < 0) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: no top-5 vector lives on GPU `shard`");
+    for (int o = 0; o < n_out; ++o) t5.out[o] = d_top5_full[o];
+    t5.n_out = n_out;
+    return select_device_gather(ctx, shard, P, src, n_out, d_best_full, row0, nullptr, &t5, stream);
 }
 
 }  // namespace
@@ -630,8 +666,8 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
                              int n_out, int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device: shard out of range");
-    return select_device_gather(ctx, shard, P, d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud, n_out, d_best_full,
-                                row0, d_top5, nullptr, stream);
+    const PodSource src{PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
+    return select_device_gather(ctx, shard, P, src, n_out, d_best_full, row0, d_top5, nullptr, stream);
 }
 
 int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
@@ -639,26 +675,8 @@ int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int
                                   int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
     if (!ctx) return RPK_EINVAL;
     if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: shard out of range");
-    if (!d_best_full || !d_top5_full || n_out < 1 || n_out > RPK_MAX_GPUS)
-        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 1..8 best and top-5 vectors are required");
-    for (int o = 0; o < n_out; ++o)
-        if (!d_best_full[o] || !d_top5_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: NULL output vector");
-    if ((uint64_t)P * RPK_TOPK > UINT32_MAX) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 5*P does not fit in uint32_t");
-    if (!same_phase(n_out, d_top5_full))
-        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: the top-5 vectors differ in 16-byte phase");
-    DeviceState& ds = ctx->devs[(size_t)shard];
-    Top5Gather t5{};
-    const int rc = guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        t5.self_out = local_vector(ctx, shard, ds.dev, n_out, d_top5_full);
-        return RPK_OK;
-    });
-    if (rc != RPK_OK) return rc;
-    if (t5.self_out < 0) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: no top-5 vector lives on GPU `shard`");
-    for (int o = 0; o < n_out; ++o) t5.out[o] = d_top5_full[o];
-    t5.n_out = n_out;
-    return select_device_gather(ctx, shard, P, d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud, n_out, d_best_full,
-                                row0, nullptr, &t5, stream);
+    const PodSource src{PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
+    return select_device_gather_top5(ctx, shard, P, src, n_out, d_best_full, d_top5_full, row0, stream);
 }
 
 int rpk_select_device(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
@@ -685,6 +703,7 @@ int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
     return guarded(ctx, [&]() -> int {
         for (auto& ds : ctx->devs) {
             RPK_CUDA(cudaSetDevice(ds.dev));
+            if (ds.sel_last_stream) RPK_CUDA(cudaEventSynchronize(ds.ev_sel));  // a device select may still gather from the table
             const size_t cap = N ? N : 1;
             ds.pt_mem.reserve(cap); ds.pt_vcpu.reserve(cap); ds.pt_ram.reserve(cap); ds.pt_max_price.reserve(cap); ds.pt_cloud.reserve(cap);
             ctx->launches += (uint64_t)launch_pod_fill(ds.pods_table(), N, ds.sm_count, ds.stream);
@@ -713,6 +732,7 @@ int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, c
                      o_cloud = o_price + 8 * n;
         for (auto& ds : ctx->devs) {  // the table is replicated: every GPU gets every row
             RPK_CUDA(cudaSetDevice(ds.dev));
+            if (ds.sel_last_stream) RPK_CUDA(cudaStreamWaitEvent(ds.stream, ds.ev_sel, 0));  // after a device select's gather
             ds.pt_seed.reserve(o_cloud + n);
             unsigned char* d = ds.pt_seed.p;
             auto up = [&](size_t off, const void* col, size_t bytes) -> const unsigned char* {
@@ -738,6 +758,28 @@ int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int3
     if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_slots: no pod table (call rpk_pods_reset first)");
     for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select_slots: no offer table uploaded (call rpk_offers_upload first)");
     return select_host(ctx, n_slots, PodSource{PodCols{}, slots}, best, top5, "rpk_select_slots");
+}
+
+int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
+                                   int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
+    if (!ctx) return RPK_EINVAL;
+    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: shard out of range");
+    if (n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: d_slots is required");
+    return select_device_gather(ctx, shard, n_slots, PodSource{PodCols{}, d_slots}, n_out, d_best_full, row0, d_top5, nullptr, stream);
+}
+
+int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
+                                        int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
+    if (!ctx) return RPK_EINVAL;
+    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: shard out of range");
+    if (n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: d_slots is required");
+    return select_device_gather_top5(ctx, shard, n_slots, PodSource{PodCols{}, d_slots}, n_out, d_best_full, d_top5_full, row0, stream);
+}
+
+int rpk_select_slots_device(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int32_t* d_best, int32_t* d_top5,
+                            void* stream) {
+    int32_t* outs[1] = {d_best};
+    return rpk_select_slots_device_gather(ctx, shard, n_slots, d_slots, 1, outs, 0, d_top5, stream);
 }
 
 // ---- cross-process peer vectors (CUDA IPC) ---------------------------------------------------------------

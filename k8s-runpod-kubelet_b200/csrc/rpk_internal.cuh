@@ -279,7 +279,8 @@ uint32_t status_state_words(int sm_count);
 struct PodCols { const int32_t* req_mem; const int32_t* req_vcpu; const int32_t* req_ram; const double* max_price; const uint8_t* cloud; };
 // Five device columns, none null: the pod-requirement table (rows = slots) or a lane's compact pod columns
 struct PodRows { int32_t* mem; int32_t* vcpu; int32_t* ram; double* max_price; uint8_t* cloud; };
-// pod-requirement table (pods.cu): N = the table's rows; entries of d_slots outside [0, N) are skipped
+// pod-requirement table (pods.cu): N = the table's rows; an entry of d_slots outside [0, N) is skipped by the seed and
+// gathered as a row nothing matches (cloud byte 2)
 int launch_pod_fill(const PodRows& t, uint32_t N, int sm_count, cudaStream_t st);
 int launch_pod_seed(const PodRows& t, uint32_t N, uint32_t n, const uint32_t* d_slots, const PodCols& in, cudaStream_t st);
 int launch_pod_gather(const PodRows& t, uint32_t N, uint32_t n, const uint32_t* d_slots, const PodRows& out, cudaStream_t st);

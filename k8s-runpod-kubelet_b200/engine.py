@@ -222,6 +222,35 @@ class Engine:
         self._check(self._lib.rpk_select_device_gather(
             self._ctx, shard, P, *cols, n_out, outs, row0, self._dev_ptr(d_top5, "d_top5", shard, P * 5), self._stream(stream, shard)))
 
+    def select_slots_device(self, d_slots, d_best, d_top5=None, shard: int = 0, stream=None):
+        """``select_device`` over rows of the pod table: ``d_best[i]`` (and ``d_top5[5i, 5i+5)``) for the row held at slot
+        ``d_slots[i]`` (a torch CUDA tensor on the shard's GPU; any order, repeats allowed; an entry outside the table
+        gives -1 and five -1), enqueued on ``stream``."""
+        n = int(d_slots.numel())
+        self._check(self._lib.rpk_select_slots_device(
+            self._ctx, shard, n, self._dev_ptr(d_slots, "d_slots", shard), self._dev_ptr(d_best, "d_best", shard, at_least=n),
+            self._dev_ptr(d_top5, "d_top5", shard, at_least=5 * n), self._stream(stream, shard)))
+
+    def select_slots_device_gather(self, d_slots, full_ptrs, row0: int, d_top5=None, shard: int = 0, stream=None, top5_ptrs=None):
+        """``select_device_gather`` over rows of the pod table listed in ``d_slots``: the results land at [row0, row0+n)
+        of every vector in ``full_ptrs`` and, with ``top5_ptrs``, the lists at [5*row0, 5*(row0+n)) of every one of
+        those (rpk_select_slots_device_gather, rpk_select_slots_device_gather_top5)."""
+        n = int(d_slots.numel())
+        slots = self._dev_ptr(d_slots, "d_slots", shard)
+        n_out, outs = _ptr_array(full_ptrs)
+        if top5_ptrs is not None:
+            if d_top5 is not None:
+                raise ValueError("d_top5 and top5_ptrs: pass one (top5_ptrs gathers the lists into every vector)")
+            n_t5, t5 = _ptr_array(top5_ptrs)
+            if n_t5 != n_out:
+                raise ValueError(f"top5_ptrs: expected one vector per vector of full_ptrs ({n_out}), got {n_t5}")
+            self._check(self._lib.rpk_select_slots_device_gather_top5(
+                self._ctx, shard, n, slots, n_out, outs, t5, row0, self._stream(stream, shard)))
+            return
+        self._check(self._lib.rpk_select_slots_device_gather(
+            self._ctx, shard, n, slots, n_out, outs, row0, self._dev_ptr(d_top5, "d_top5", shard, at_least=5 * n),
+            self._stream(stream, shard)))
+
     # -- cross-process peer vectors (CUDA IPC) ------------------------------------------------------------
     def ipc_alloc(self, nbytes: int, shard: int = 0):
         """-> (device pointer, 64-byte handle) of a fresh cudaMalloc buffer other processes can map."""

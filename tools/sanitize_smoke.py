@@ -29,7 +29,7 @@ os.environ.pop("RPK_FORCE_KERNEL", None)
 # table with caller input)
 if not ONLY_MULTI:
     eng.upload_offers(offers)
-    pods = rpk.synth.make_pods(200_000, seed=11)
+    pods = pods_t = rpk.synth.make_pods(200_000, seed=11)
     eng.pods_reset(200_000)
     eng.pods_seed_slots(np.arange(200_000, dtype=np.uint32), pods)
     for n in (37, 140_000):
@@ -89,6 +89,20 @@ for P in (20_001, 70_003):
         torch.cuda.synchronize()
         assert np.array_equal(va[3:].cpu().numpy(), ob) and np.array_equal(vb[3:].cpu().numpy(), ob), P
         assert int((va[:3] != -9).sum()) == 0 and int((vb[:3] != -9).sum()) == 0
+# the device select over a slot list, whose entries nothing checks on the host: entries outside the table (a defined
+# result, -1 and five -1) show that the gather stays inside it
+if not ONLY_MULTI:  # the pod table was seeded above
+    sl = np.random.default_rng(5).integers(0, 200_000, 30_001).astype(np.uint32)
+    sl[[7, 30_000]] = [200_000, 0xFFFFFFFF]
+    va, vb = torch.full((len(sl) + 3,), -9, dtype=torch.int32, device=dev), torch.full((len(sl) + 3,), -9, dtype=torch.int32, device=dev)
+    t5 = torch.full((5 * len(sl),), -9, dtype=torch.int32, device=dev)
+    eng.select_slots_device_gather(torch.from_numpy(sl.view(np.int32)).to(dev), [va.data_ptr(), vb.data_ptr()], 3, d_top5=t5)
+    torch.cuda.synchronize()
+    ok = sl < 200_000
+    ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl[ok]]) for k, v in pods_t.items()}, n_threads=8)
+    got, gt = va[3:].cpu().numpy(), t5.cpu().numpy().reshape(-1, 5)
+    assert np.array_equal(got[ok], ob) and np.array_equal(gt[ok], ot) and (got[~ok] == -1).all() and (gt[~ok] == -1).all()
+    assert np.array_equal(vb.cpu().numpy(), va.cpu().numpy())
 eng.close()
 
 # two GPUs: the fused push + signal + wait, and the sharded sweep's exchange (racecheck / memcheck see peer stores)
