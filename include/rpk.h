@@ -26,6 +26,17 @@
  *   - "host" entry points take host pointers (pageable or pinned; pinned from rpk_host_alloc is faster);
  *     "_device" entry points take device pointers on the shard's GPU and enqueue on the given stream
  *     without synchronising it.
+ *   - Ordering.  The calls on one shard share ctx-owned buffers in two scopes: the select scope (the offer table, the
+ *     pod table and the select scratch) and the status scope (the sweep scratch).  A _device call issued on another
+ *     stream than the last _device call of its scope first waits for that call, so any streams may be used.  A host
+ *     call waits for the last _device call of its scopes before it touches anything, and returns after its own work is
+ *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_pods_reset,
+ *     rpk_pods_seed_slots, rpk_select, rpk_select_slots, and rpk_tick with P > 0.  Status scope: rpk_status_diff,
+ *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset and
+ *     rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
+ *     capture neither waits nor is waited for (keep each captured entry point on one stream), and the library does
+ *     not see replays of a captured graph: a caller that replays a captured device step orders its host calls after
+ *     the replay itself.
  */
 #ifndef RPK_H_
 #define RPK_H_
@@ -196,7 +207,6 @@ int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int
  *   - No pod table or no offer table on GPU `shard`: RPK_ESTATE.  d_slots NULL with n_slots > 0: RPK_EINVAL.  Both
  *     before anything is enqueued.
  *   - Counts as one select in rpk_stats (offer_scores += n_slots * G).  One gather kernel runs ahead of the select.
- *   - rpk_pods_seed_slots and rpk_pods_reset wait for a device select still running before they touch the table.
  *   - After one call of a given size the call only enqueues launches, so it can be captured in a CUDA graph.  A replay
  *     reads the table as it is at replay time, so seeds between replays are picked up (the caller orders a seed after
  *     a replay still in flight; the library does not see replays).  rpk_pods_reset invalidates a captured graph: the
@@ -331,8 +341,7 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
 /* Device-resident variant on GPU `shard`: d_records N*stride bytes, d_hash_prev N uint64 updated in place
  * (caller-owned column; 0 = never seen; both 16-byte aligned, else RPK_EINVAL), d_changed_idx capacity N, d_n_changed
  * one uint32.  Enqueued on
- * `stream`, no synchronisation.  The _device entry points of one shard share ctx-owned scratch: issue them from one
- * stream per shard (select) / one stream per shard (status) at a time. */
+ * `stream`, no synchronisation.  Ordering against the shard's other calls: see "Ordering" at the top. */
 int rpk_status_diff_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                            uint64_t* d_hash_prev, uint32_t* d_changed_idx, uint32_t* d_n_changed, void* stream);
 int rpk_status_diff_device_codes(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,

@@ -94,8 +94,8 @@ rpk::DeviceState::~DeviceState() {
         if (ln.stream) cudaStreamDestroy(ln.stream);
     }
     for (cudaEvent_t e : ev) if (e) cudaEventDestroy(e);
-    if (ev_sel) cudaEventDestroy(ev_sel);
-    if (ev_st) cudaEventDestroy(ev_st);
+    if (sel_scope.ev) cudaEventDestroy(sel_scope.ev);
+    if (status_scope.ev) cudaEventDestroy(status_scope.ev);
     if (status_stream) cudaStreamDestroy(status_stream);
     if (stream) cudaStreamDestroy(stream);
     cudaGetLastError();
@@ -217,26 +217,6 @@ void count_select(rpk_ctx* ctx, uint32_t P, uint32_t G) {
     ctx->stats.offer_scores += (uint64_t)P * G;
 }
 
-// The device entry points of a shard share ctx-owned scratch (tickets, queue cursors, look-back state).  Calls on ONE
-// stream are ordered by the stream; a call on a different stream than the previous one first waits for that one's
-// completion event, so two streams can never run on the same scratch at once.  Inside a stream capture the guard is
-// skipped (events recorded outside a capture cannot be waited on inside it): a captured step must keep each entry
-// point on one stream, as bench.py does.
-struct ScratchGuard {
-    cudaStream_t* last; cudaEvent_t ev; cudaStream_t st; bool capturing = false;
-    ScratchGuard(cudaStream_t* last_stream, cudaEvent_t event, cudaStream_t stream) : last(last_stream), ev(event), st(stream) {
-        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
-        if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) { cudaGetLastError(); cs = cudaStreamCaptureStatusNone; }
-        capturing = cs != cudaStreamCaptureStatusNone;
-        if (!capturing && *last != nullptr && *last != st) RPK_CUDA(cudaStreamWaitEvent(st, ev, 0));
-    }
-    void done() {
-        if (capturing) return;
-        RPK_CUDA(cudaEventRecord(ev, st));
-        *last = st;
-    }
-};
-
 // The push kernel moves 16-byte units: every vector must share the slice's alignment.
 bool same_phase(int n_out, int32_t* const* ptrs) {
     for (int o = 1; o < n_out; ++o)
@@ -288,6 +268,7 @@ inline uint32_t sub_batch_cap(uint32_t Ps) {  // largest sub-batch a shard of Ps
 // D2H; one stream synchronise.  Same kernels.  Slot ids are in range here.  Returns the kernels launched.
 int select_small(DeviceState& ds, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5) {
     RPK_CUDA(cudaSetDevice(ds.dev));
+    ds.sel_scope.host_wait();
     const size_t in_cap = (size_t)kSmallBatch * 24, out_cap = (size_t)kSmallBatch * 6 * 4;
     ds.h_small.reserve(in_cap + out_cap);
     ds.d_small_in.reserve(in_cap); ds.d_small_out.reserve((size_t)kSmallBatch * 6);
@@ -421,38 +402,183 @@ bool enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodSource& src,
     return ok;
 }
 
+// Scratch of a sweep over N records (or list entries) on ds: the look-back state and tickets -- zero between calls by
+// construction, zeroed here when (re)allocated -- and the per-warp index stage, its code stage (`codes`) and the
+// per-unit counts.
+void reserve_sweep_scratch(DeviceState& ds, uint32_t N, bool codes) {
+    const uint32_t cap = N ? N : 1;
+    const size_t need = status_state_words(ds.sm_count);
+    if (need > ds.s_tile_state.cap || !ds.s_misc.p || ds.status_dirty) {
+        ds.s_tile_state.reserve(need);
+        ds.s_misc.reserve(64);
+        RPK_CUDA(cudaMemset(ds.s_tile_state.p, 0, ds.s_tile_state.cap * sizeof(unsigned long long)));
+        RPK_CUDA(cudaMemset(ds.s_misc.p, 0, ds.s_misc.cap * sizeof(uint32_t)));
+        RPK_CUDA(cudaDeviceSynchronize());
+        ds.status_dirty = false;
+    }
+    ds.s_stage_idx.reserve(cap + 64); ds.s_unit_cnt.reserve(cap / 32 + 2);
+    if (codes) ds.s_stage_code.reserve(cap + 64);
+}
+
+// the StatusArgs fields of the scratch reserve_sweep_scratch sized
+void sweep_scratch_args(const DeviceState& ds, bool codes, StatusArgs& a) {
+    a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
+    a.stage_idx = ds.s_stage_idx.p; a.stage_code = codes ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
+}
+
+struct StatusHostArgs {
+    uint32_t N; const uint8_t* records; uint32_t stride;
+    uint32_t* changed_idx; uint16_t* changed_code; uint32_t* n_changed; uint64_t* hashes_out; bool report;
+    const uint32_t* slots; uint32_t n_slots;  // rpk_status_diff_slots: records holds the n_slots listed slots (ascending)
+};
+
+// Shard s of a host sweep: its hash column holds global slots [lo, hi); its records are [p0, p1) of the caller's table
+// (the same range) or, for a slot list, the entries whose slot lies in [lo, hi) -- two binary searches, since the list
+// is ascending.
+struct ShardPart { uint32_t lo, hi, p0, p1; };
+ShardPart shard_part(const rpk_ctx* ctx, int s, const StatusHostArgs& h) {
+    ShardPart p;
+    shard_range(h.N, (int)ctx->devs.size(), s, &p.lo, &p.hi);
+    p.p0 = p.lo; p.p1 = p.hi;
+    if (h.slots) {
+        p.p0 = (uint32_t)(std::lower_bound(h.slots, h.slots + h.n_slots, p.lo) - h.slots);
+        p.p1 = (uint32_t)(std::lower_bound(h.slots, h.slots + h.n_slots, p.hi) - h.slots);
+    }
+    return p;
+}
+
+// Sizes one shard's buffers (calling thread).  The changed list comes back through mapped pinned memory -- the kernel's
+// final copy writes indices, codes and the count straight into it, so the host needs ONE stream synchronise and no
+// device-to-host copy whose size it would first have to learn.
+void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
+    DeviceState& ds = ctx->devs[(size_t)s];
+    const ShardPart sp = shard_part(ctx, s, h);
+    const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
+    RPK_CUDA(cudaSetDevice(ds.dev));
+    ds.s_records.reserve((size_t)cap * h.stride);
+    if (h.slots) ds.s_seed_slots.reserve(cap);
+    if (h.hashes_out) ds.s_hash_out.reserve(cap);
+    reserve_sweep_scratch(ds, Ns, h.changed_code != nullptr);
+    ds.h_changed.reserve(h.report ? (size_t)cap * (h.changed_code ? 6 : 4) + 64 : 64);
+}
+
+// One shard's half of a host sweep, enqueued on st (ds.ev[0..2] bracket copy and kernel, ds.ev[3] follows the hash
+// copy); the caller synchronises.
+void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, cudaStream_t st, uint64_t* launches) {
+    DeviceState& ds = ctx->devs[(size_t)s];
+    const ShardPart sp = shard_part(ctx, s, h);
+    const uint32_t lo = sp.lo, Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
+    RPK_CUDA(cudaSetDevice(ds.dev));
+    RPK_CUDA(cudaEventRecord(ds.ev[0], st));
+    if (Ns) RPK_CUDA(cudaMemcpyAsync(ds.s_records.p, h.records + (size_t)sp.p0 * h.stride, (size_t)Ns * h.stride, cudaMemcpyHostToDevice, st));
+    if (Ns && h.slots) RPK_CUDA(cudaMemcpyAsync(ds.s_seed_slots.p, h.slots + sp.p0, (size_t)Ns * 4, cudaMemcpyHostToDevice, st));
+    RPK_CUDA(cudaEventRecord(ds.ev[1], st));
+    // mapped block: [count : 64 bytes][indices : cap u32][codes : cap u16]
+    uint32_t* m_count = reinterpret_cast<uint32_t*>(ds.h_changed.d);
+    uint32_t* m_idx = reinterpret_cast<uint32_t*>(ds.h_changed.d + 64);
+    uint16_t* m_code = reinterpret_cast<uint16_t*>(ds.h_changed.d + 64 + (size_t)cap * 4);
+    *reinterpret_cast<volatile uint32_t*>(ds.h_changed.h) = 0u;
+    StatusArgs a{};
+    a.records = ds.s_records.p; a.stride = h.stride; a.N = Ns; a.hash_prev = ds.s_hash_prev.p;
+    a.hash_out = h.hashes_out ? ds.s_hash_out.p : nullptr;
+    a.changed_idx = h.report ? m_idx : nullptr; a.n_changed = h.report ? m_count : nullptr;
+    a.changed_code = h.report && h.changed_code ? m_code : nullptr;
+    a.idx_base = lo;
+    sweep_scratch_args(ds, h.changed_code != nullptr, a);
+    if (h.slots) { a.slots = ds.s_seed_slots.p; a.col_n = sp.hi - sp.lo; }
+    ds.status_dirty = true;
+    if (Ns) *launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
+    ds.status_dirty = false;
+    RPK_CUDA(cudaEventRecord(ds.ev[2], st));
+    if (h.hashes_out && Ns) RPK_CUDA(cudaMemcpyAsync(h.hashes_out + lo, ds.s_hash_out.p, (size_t)Ns * 8, cudaMemcpyDeviceToHost, st));
+    RPK_CUDA(cudaEventRecord(ds.ev[3], st));
+}
+
+// after the shard's stream has been synchronised: this shard's part of the caller's arrays (ascending over shards)
+uint32_t collect_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint32_t out_at) {
+    DeviceState& ds = ctx->devs[(size_t)s];
+    const ShardPart sp = shard_part(ctx, s, h);
+    const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
+    if (!h.report || !Ns) return 0;
+    const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(ds.h_changed.h);
+    memcpy(h.changed_idx + out_at, ds.h_changed.h + 64, (size_t)cnt * 4);
+    if (h.changed_code) memcpy(h.changed_code + out_at, ds.h_changed.h + 64 + (size_t)cap * 4, (size_t)cnt * 2);
+    return cnt;
+}
+
+// The pipelined host select of a run_host call: P rows from src into the caller's best and top5 (nullable)
+struct HostSelect { uint32_t P; PodSource src; int32_t* best; int32_t* top5; };
+
+// The host calls' shard loop, once their arguments are checked: the pipelined host select (sel), a host sweep (h), or
+// both in a tick (tick: the sweep runs on status_stream beside the select, and no timing is reported, since both halves
+// record ds.ev).  Every shard first waits for the last device call in the scopes it uses; then the calling thread sizes
+// the buffers, every shard enqueues and synchronises on its worker, and the outputs, launches and stats are collected.
+// false: a slot id outside the pod table (best and top5 unspecified, stats untouched).
+bool run_host(rpk_ctx* ctx, const HostSelect* sel, const StatusHostArgs* h, bool tick) {
+    const int n = (int)ctx->devs.size();
+    for (auto& ds : ctx->devs) {
+        if (sel) ds.sel_scope.host_wait();
+        if (h) ds.status_scope.host_wait();
+    }
+    if (sel) reserve_select(ctx, sel->P, sel->src, sel->top5 != nullptr);
+    if (h) for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, *h);
+    std::vector<uint64_t> launches((size_t)n, 0);
+    std::vector<float> km((size_t)n, 0.f), tm((size_t)n, 0.f);
+    std::vector<char> shard_ok((size_t)n, 1);
+    ctx->workers.run(n, [&](int s) {
+        DeviceState& ds = ctx->devs[(size_t)s];
+        const cudaStream_t sweep = tick ? ds.status_stream : ds.stream;
+        // the selection goes first: its kernels are the long pole and start after the first 128k-row sub-batch has
+        // landed; in a tick the sweep's records follow on the status stream, concurrent with the lanes, and its kernel
+        // runs under the selection's tail
+        if (sel) shard_ok[(size_t)s] = enqueue_select_shard(ctx, s, sel->P, sel->src, sel->best, sel->top5, &launches[(size_t)s]);
+        if (h) enqueue_status_shard(ctx, s, *h, sweep, &launches[(size_t)s]);
+        if (h) RPK_CUDA(cudaStreamSynchronize(sweep));
+        if (sel) RPK_CUDA(cudaStreamSynchronize(ds.stream));
+        if (tick) return;
+        if (h) RPK_CUDA(cudaEventElapsedTime(&km[(size_t)s], ds.ev[1], ds.ev[2]));
+        RPK_CUDA(cudaEventElapsedTime(&tm[(size_t)s], ds.ev[0], ds.ev[3]));
+    });
+    uint32_t total = 0;
+    float kmax = 0.f, tmax = 0.f;
+    bool ok = true;
+    for (int s = 0; s < n; ++s) {
+        if (h) total += collect_status_shard(ctx, s, *h, total);
+        ctx->launches += launches[(size_t)s];
+        kmax = km[(size_t)s] > kmax ? km[(size_t)s] : kmax; tmax = tm[(size_t)s] > tmax ? tm[(size_t)s] : tmax;
+        ok = ok && shard_ok[(size_t)s];
+    }
+    if (!ok) return false;
+    if (sel && !tick) {  // copies and kernels overlap in the pipelined host path: only the total is meaningful
+        ctx->stats.last_select_kernel_ms = 0.f; ctx->stats.last_select_total_ms = tmax;
+    }
+    if (sel) count_select(ctx, sel->P, ctx->devs[0].G);
+    if (h) {
+        if (h->report) *h->n_changed = total;
+        if (!tick) { ctx->stats.last_status_kernel_ms = kmax; ctx->stats.last_status_total_ms = tmax; }
+        ctx->stats.status_calls += 1; ctx->stats.status_records += h->slots ? h->n_slots : h->N;
+    }
+    return true;
+}
+
 // rpk_select and rpk_select_slots once their arguments are checked: one GPU and up to kSmallBatch rows take the latency
 // path, everything else the sub-batch pipeline on every GPU.  A slot id outside the pod table: RPK_EINVAL (best and
 // top5 unspecified, stats untouched).
 int select_host(rpk_ctx* ctx, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5, const char* who) {
     return guarded(ctx, [&]() -> int {
-        const int n = (int)ctx->devs.size();
-        float tmax = 0.f;
-        bool ok = true;
-        if (n == 1 && P <= kSmallBatch) {
+        bool ok;
+        if (ctx->devs.size() == 1 && P <= kSmallBatch) {
             ok = !src.slots || slots_below(src.slots, P, ctx->devs[0].podsN);
-            if (ok) ctx->launches += (uint64_t)select_small(ctx->devs[0], P, src, best, top5);
-        } else {
-            std::vector<uint64_t> launches((size_t)n, 0);
-            std::vector<float> ms((size_t)n, 0.f);
-            std::vector<char> shard_ok((size_t)n, 1);
-            reserve_select(ctx, P, src, top5 != nullptr);
-            ctx->workers.run(n, [&](int s) {
-                shard_ok[(size_t)s] = enqueue_select_shard(ctx, s, P, src, best, top5, &launches[(size_t)s]);
-                DeviceState& ds = ctx->devs[(size_t)s];
-                RPK_CUDA(cudaStreamSynchronize(ds.stream));
-                RPK_CUDA(cudaEventElapsedTime(&ms[(size_t)s], ds.ev[0], ds.ev[3]));
-            });
-            for (int s = 0; s < n; ++s) {
-                ctx->launches += launches[(size_t)s]; tmax = ms[(size_t)s] > tmax ? ms[(size_t)s] : tmax;
-                ok = ok && shard_ok[(size_t)s];
+            if (ok) {
+                ctx->launches += (uint64_t)select_small(ctx->devs[0], P, src, best, top5);
+                ctx->stats.last_select_kernel_ms = 0.f; ctx->stats.last_select_total_ms = 0.f;  // single copy: not timed
+                count_select(ctx, P, ctx->devs[0].G);
             }
+        } else {
+            const HostSelect sel{P, src, best, top5};
+            ok = run_host(ctx, &sel, nullptr, false);
         }
-        if (!ok) return fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
-        ctx->stats.last_select_kernel_ms = 0.f;  // copies and kernels overlap in the pipelined host path: only the total is meaningful
-        ctx->stats.last_select_total_ms = tmax;  // 0 on the single-copy path
-        count_select(ctx, P, ctx->devs[0].G);
-        return RPK_OK;
+        return ok ? RPK_OK : fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
     });
 }
 
@@ -468,9 +594,9 @@ int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& s
         if (n_out <= 1 || peers.n == 0) return RPK_OK;
         return guarded(ctx, [&]() -> int {
             RPK_CUDA(cudaSetDevice(ds.dev));
-            ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);  // orders the epoch counter after the last gather's
+            const bool tracked = ds.sel_scope.device_begin(st);  // orders the epoch counter after the last gather's
             ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
-            guard.done();
+            ds.sel_scope.device_end(st, tracked);
             return RPK_OK;
         });
     }
@@ -485,7 +611,7 @@ int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& s
             ln.p_req_mem.reserve(P); ln.p_req_vcpu.reserve(P); ln.p_req_ram.reserve(P); ln.p_max_price.reserve(P); ln.p_cloud.reserve(P);
         }
         SelectArgs a{};
-        ScratchGuard guard(&ds.sel_last_stream, ds.ev_sel, st);  // the gather writes lane 0's columns: after the last select
+        const bool tracked = ds.sel_scope.device_begin(st);  // the gather writes lane 0's columns: after the last select
         if (src.slots) {
             ctx->launches += (uint64_t)gather_pod_rows(ds, ln, P, src.slots, a, st);
         } else {
@@ -499,7 +625,7 @@ int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& s
         a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
         if (n_out > 1) a.peers = peers;
         ctx->launches += (uint64_t)enqueue_select(ds, ln, a, st, t5);
-        guard.done();
+        ds.sel_scope.device_end(st, tracked);
         count_select(ctx, P, ds.G);
         return RPK_OK;
     });
@@ -580,8 +706,8 @@ int rpk_create(int n_gpus, const int* device_ids, rpk_ctx** out) {
             RPK_CUDA(cudaStreamCreateWithPriority(&ds.stream, cudaStreamNonBlocking, prio_hi));
             RPK_CUDA(cudaStreamCreateWithPriority(&ds.status_stream, cudaStreamNonBlocking, prio_lo));
             for (auto& ev : ds.ev) RPK_CUDA(cudaEventCreate(&ev));
-            RPK_CUDA(cudaEventCreateWithFlags(&ds.ev_sel, cudaEventDisableTiming));
-            RPK_CUDA(cudaEventCreateWithFlags(&ds.ev_st, cudaEventDisableTiming));
+            RPK_CUDA(cudaEventCreateWithFlags(&ds.sel_scope.ev, cudaEventDisableTiming));
+            RPK_CUDA(cudaEventCreateWithFlags(&ds.status_scope.ev, cudaEventDisableTiming));
             for (auto& ln : ds.lane) {
                 RPK_CUDA(cudaStreamCreateWithPriority(&ln.stream, cudaStreamNonBlocking, prio_hi));
                 RPK_CUDA(cudaEventCreateWithFlags(&ln.done, cudaEventDisableTiming));
@@ -628,6 +754,7 @@ int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int
     return guarded(ctx, [&]() -> int {
         for (auto& ds : ctx->devs) {
             RPK_CUDA(cudaSetDevice(ds.dev));
+            ds.sel_scope.host_wait();  // a device select may still read the views rewritten below
             ds.offers_ready = false;
             ds.force_kind = 0;
             // test hook (exercise every kernel on any table): consulted once per table upload, never on the select path
@@ -703,7 +830,7 @@ int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
     return guarded(ctx, [&]() -> int {
         for (auto& ds : ctx->devs) {
             RPK_CUDA(cudaSetDevice(ds.dev));
-            if (ds.sel_last_stream) RPK_CUDA(cudaEventSynchronize(ds.ev_sel));  // a device select may still gather from the table
+            ds.sel_scope.host_wait();  // a device select may still gather from the table
             const size_t cap = N ? N : 1;
             ds.pt_mem.reserve(cap); ds.pt_vcpu.reserve(cap); ds.pt_ram.reserve(cap); ds.pt_max_price.reserve(cap); ds.pt_cloud.reserve(cap);
             ctx->launches += (uint64_t)launch_pod_fill(ds.pods_table(), N, ds.sm_count, ds.stream);
@@ -732,7 +859,7 @@ int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, c
                      o_cloud = o_price + 8 * n;
         for (auto& ds : ctx->devs) {  // the table is replicated: every GPU gets every row
             RPK_CUDA(cudaSetDevice(ds.dev));
-            if (ds.sel_last_stream) RPK_CUDA(cudaStreamWaitEvent(ds.stream, ds.ev_sel, 0));  // after a device select's gather
+            ds.sel_scope.host_wait();  // after a device select's gather
             ds.pt_seed.reserve(o_cloud + n);
             unsigned char* d = ds.pt_seed.p;
             auto up = [&](size_t off, const void* col, size_t bytes) -> const unsigned char* {
@@ -924,108 +1051,6 @@ int rpk_status_reset(rpk_ctx* ctx, uint32_t N) {
 
 namespace {
 
-// Scratch of a sweep over N records (or list entries) on ds: the look-back state and tickets -- zero between calls by
-// construction, zeroed here when (re)allocated -- and the per-warp index stage, its code stage (`codes`) and the
-// per-unit counts.
-void reserve_sweep_scratch(DeviceState& ds, uint32_t N, bool codes) {
-    const uint32_t cap = N ? N : 1;
-    const size_t need = status_state_words(ds.sm_count);
-    if (need > ds.s_tile_state.cap || !ds.s_misc.p || ds.status_dirty) {
-        ds.s_tile_state.reserve(need);
-        ds.s_misc.reserve(64);
-        RPK_CUDA(cudaMemset(ds.s_tile_state.p, 0, ds.s_tile_state.cap * sizeof(unsigned long long)));
-        RPK_CUDA(cudaMemset(ds.s_misc.p, 0, ds.s_misc.cap * sizeof(uint32_t)));
-        RPK_CUDA(cudaDeviceSynchronize());
-        ds.status_dirty = false;
-    }
-    ds.s_stage_idx.reserve(cap + 64); ds.s_unit_cnt.reserve(cap / 32 + 2);
-    if (codes) ds.s_stage_code.reserve(cap + 64);
-}
-
-// the StatusArgs fields of the scratch reserve_sweep_scratch sized
-void sweep_scratch_args(const DeviceState& ds, bool codes, StatusArgs& a) {
-    a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
-    a.stage_idx = ds.s_stage_idx.p; a.stage_code = codes ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
-}
-
-struct StatusHostArgs {
-    uint32_t N; const uint8_t* records; uint32_t stride;
-    uint32_t* changed_idx; uint16_t* changed_code; uint32_t* n_changed; uint64_t* hashes_out; bool report;
-    const uint32_t* slots; uint32_t n_slots;  // rpk_status_diff_slots: records holds the n_slots listed slots (ascending)
-};
-
-// Shard s of a host sweep: its hash column holds global slots [lo, hi); its records are [p0, p1) of the caller's table
-// (the same range) or, for a slot list, the entries whose slot lies in [lo, hi) -- two binary searches, since the list
-// is ascending.
-struct ShardPart { uint32_t lo, hi, p0, p1; };
-ShardPart shard_part(const rpk_ctx* ctx, int s, const StatusHostArgs& h) {
-    ShardPart p;
-    shard_range(h.N, (int)ctx->devs.size(), s, &p.lo, &p.hi);
-    p.p0 = p.lo; p.p1 = p.hi;
-    if (h.slots) {
-        p.p0 = (uint32_t)(std::lower_bound(h.slots, h.slots + h.n_slots, p.lo) - h.slots);
-        p.p1 = (uint32_t)(std::lower_bound(h.slots, h.slots + h.n_slots, p.hi) - h.slots);
-    }
-    return p;
-}
-
-// Sizes one shard's buffers (calling thread).  The changed list comes back through mapped pinned memory -- the kernel's
-// final copy writes indices, codes and the count straight into it, so the host needs ONE stream synchronise and no
-// device-to-host copy whose size it would first have to learn.
-void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
-    DeviceState& ds = ctx->devs[(size_t)s];
-    const ShardPart sp = shard_part(ctx, s, h);
-    const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
-    RPK_CUDA(cudaSetDevice(ds.dev));
-    ds.s_records.reserve((size_t)cap * h.stride);
-    if (h.slots) ds.s_seed_slots.reserve(cap);
-    if (h.hashes_out) ds.s_hash_out.reserve(cap);
-    reserve_sweep_scratch(ds, Ns, h.changed_code != nullptr);
-    ds.h_changed.reserve(h.report ? (size_t)cap * (h.changed_code ? 6 : 4) + 64 : 64);
-}
-
-// One shard's half of a host sweep, enqueued on st (ds.ev[0..2] bracket copy and kernel); the caller synchronises.
-void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, cudaStream_t st, uint64_t* launches) {
-    DeviceState& ds = ctx->devs[(size_t)s];
-    const ShardPart sp = shard_part(ctx, s, h);
-    const uint32_t lo = sp.lo, Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
-    RPK_CUDA(cudaSetDevice(ds.dev));
-    RPK_CUDA(cudaEventRecord(ds.ev[0], st));
-    if (Ns) RPK_CUDA(cudaMemcpyAsync(ds.s_records.p, h.records + (size_t)sp.p0 * h.stride, (size_t)Ns * h.stride, cudaMemcpyHostToDevice, st));
-    if (Ns && h.slots) RPK_CUDA(cudaMemcpyAsync(ds.s_seed_slots.p, h.slots + sp.p0, (size_t)Ns * 4, cudaMemcpyHostToDevice, st));
-    RPK_CUDA(cudaEventRecord(ds.ev[1], st));
-    // mapped block: [count : 64 bytes][indices : cap u32][codes : cap u16]
-    uint32_t* m_count = reinterpret_cast<uint32_t*>(ds.h_changed.d);
-    uint32_t* m_idx = reinterpret_cast<uint32_t*>(ds.h_changed.d + 64);
-    uint16_t* m_code = reinterpret_cast<uint16_t*>(ds.h_changed.d + 64 + (size_t)cap * 4);
-    *reinterpret_cast<volatile uint32_t*>(ds.h_changed.h) = 0u;
-    StatusArgs a{};
-    a.records = ds.s_records.p; a.stride = h.stride; a.N = Ns; a.hash_prev = ds.s_hash_prev.p;
-    a.hash_out = h.hashes_out ? ds.s_hash_out.p : nullptr;
-    a.changed_idx = h.report ? m_idx : nullptr; a.n_changed = h.report ? m_count : nullptr;
-    a.changed_code = h.report && h.changed_code ? m_code : nullptr;
-    a.idx_base = lo;
-    sweep_scratch_args(ds, h.changed_code != nullptr, a);
-    if (h.slots) { a.slots = ds.s_seed_slots.p; a.col_n = sp.hi - sp.lo; }
-    ds.status_dirty = true;
-    if (Ns) *launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
-    ds.status_dirty = false;
-    RPK_CUDA(cudaEventRecord(ds.ev[2], st));
-    if (h.hashes_out && Ns) RPK_CUDA(cudaMemcpyAsync(h.hashes_out + lo, ds.s_hash_out.p, (size_t)Ns * 8, cudaMemcpyDeviceToHost, st));
-}
-
-// after the shard's stream has been synchronised: this shard's part of the caller's arrays (ascending over shards)
-uint32_t collect_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint32_t out_at) {
-    DeviceState& ds = ctx->devs[(size_t)s];
-    const ShardPart sp = shard_part(ctx, s, h);
-    const uint32_t Ns = sp.p1 - sp.p0, cap = Ns ? Ns : 1;
-    if (!h.report || !Ns) return 0;
-    const uint32_t cnt = *reinterpret_cast<volatile uint32_t*>(ds.h_changed.h);
-    memcpy(h.changed_idx + out_at, ds.h_changed.h + 64, (size_t)cnt * 4);
-    if (h.changed_code) memcpy(h.changed_code + out_at, ds.h_changed.h + 64 + (size_t)cap * 4, (size_t)cnt * 2);
-    return cnt;
-}
-
 // The argument checks of a whole-table host sweep (rpk_status_diff*, rpk_status_seed, rpk_tick; `who` names the entry
 // point in the messages).  The first sweep of a ctx sizes the tracked table to its N.
 int check_sweep(rpk_ctx* ctx, const StatusHostArgs& h, const char* who) {
@@ -1038,39 +1063,10 @@ int check_sweep(rpk_ctx* ctx, const StatusHostArgs& h, const char* who) {
     return RPK_OK;
 }
 
-// a host sweep whose arguments have been checked: every shard uploads its part, sweeps it and synchronises once
-int run_status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
-    return guarded(ctx, [&]() -> int {
-        const int n = (int)ctx->devs.size();
-        for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, h);
-        std::vector<uint64_t> launches((size_t)n, 0);
-        std::vector<float> km((size_t)n, 0.f), tm((size_t)n, 0.f);
-        ctx->workers.run(n, [&](int s) {
-            DeviceState& ds = ctx->devs[(size_t)s];
-            enqueue_status_shard(ctx, s, h, ds.stream, &launches[(size_t)s]);
-            RPK_CUDA(cudaEventRecord(ds.ev[3], ds.stream));
-            RPK_CUDA(cudaStreamSynchronize(ds.stream));
-            RPK_CUDA(cudaEventElapsedTime(&km[(size_t)s], ds.ev[1], ds.ev[2]));
-            RPK_CUDA(cudaEventElapsedTime(&tm[(size_t)s], ds.ev[0], ds.ev[3]));
-        });
-        uint32_t total = 0;
-        float kmax = 0.f, tmax = 0.f;
-        for (int s = 0; s < n; ++s) {
-            total += collect_status_shard(ctx, s, h, total);
-            ctx->launches += launches[(size_t)s];
-            kmax = km[(size_t)s] > kmax ? km[(size_t)s] : kmax; tmax = tm[(size_t)s] > tmax ? tm[(size_t)s] : tmax;
-        }
-        if (h.report) *h.n_changed = total;
-        ctx->stats.last_status_kernel_ms = kmax; ctx->stats.last_status_total_ms = tmax;
-        ctx->stats.status_calls += 1; ctx->stats.status_records += h.slots ? h.n_slots : h.N;
-        return RPK_OK;
-    });
-}
-
 int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
     if (!ctx) return RPK_EINVAL;
     if (int rc = check_sweep(ctx, h, "rpk_status_diff")) return rc;
-    return run_status_host(ctx, h);
+    return guarded(ctx, [&]() -> int { run_host(ctx, nullptr, &h, false); return RPK_OK; });
 }
 
 }  // namespace
@@ -1131,7 +1127,7 @@ int rpk_status_diff_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
     }
     StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
     h.slots = slots; h.n_slots = n_slots;
-    return run_status_host(ctx, h);
+    return guarded(ctx, [&]() -> int { run_host(ctx, nullptr, &h, false); return RPK_OK; });
 }
 
 // One tick of the kubelet: the pending-pod selection (processPendingPods, kubelet.go:747-814) and the status sweep
@@ -1146,29 +1142,8 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
     if (P > 0) for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_tick: no offer table uploaded (call rpk_offers_upload first)");
     const StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
     if (int rc = check_sweep(ctx, h, "rpk_tick")) return rc;
-    return guarded(ctx, [&]() -> int {
-        const PodSource pods{PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr};
-        const int n = (int)ctx->devs.size();
-        if (P > 0) reserve_select(ctx, P, pods, top5 != nullptr);
-        for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, h);
-        std::vector<uint64_t> launches((size_t)n, 0);
-        ctx->workers.run(n, [&](int s) {
-            DeviceState& ds = ctx->devs[(size_t)s];
-            // the selection goes first: its kernels are the long pole and start after the first 128k-row sub-batch has
-            // landed; the sweep's records follow on the status stream, concurrent with the lanes, and its kernel runs
-            // under the selection's tail
-            if (P > 0) enqueue_select_shard(ctx, s, P, pods, best, top5, &launches[(size_t)s]);
-            enqueue_status_shard(ctx, s, h, ds.status_stream, &launches[(size_t)s]);
-            RPK_CUDA(cudaStreamSynchronize(ds.status_stream));
-            if (P > 0) RPK_CUDA(cudaStreamSynchronize(ds.stream));
-        });
-        uint32_t total = 0;
-        for (int s = 0; s < n; ++s) { total += collect_status_shard(ctx, s, h, total); ctx->launches += launches[(size_t)s]; }
-        *n_changed = total;
-        ctx->stats.status_calls += 1; ctx->stats.status_records += N;
-        if (P > 0) count_select(ctx, P, ctx->devs[0].G);
-        return RPK_OK;
-    });
+    const HostSelect sel{P, PodSource{PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr}, best, top5};
+    return guarded(ctx, [&]() -> int { run_host(ctx, P > 0 ? &sel : nullptr, &h, true); return RPK_OK; });
 }
 
 namespace {
@@ -1208,11 +1183,11 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
         if (n_out > 0) a.peers = ctx->bind[(size_t)shard];
         a.peers.my_rank = my_rank;  // the sweep fills and signals under the rank its call names
         cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
-        ScratchGuard guard(&ds.st_last_stream, ds.ev_st, st);
+        const bool tracked = ds.status_scope.device_begin(st);
         ds.status_dirty = true;
         ctx->launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
         ds.status_dirty = false;
-        guard.done();
+        ds.status_scope.device_end(st, tracked);
         ctx->stats.status_calls += 1; ctx->stats.status_records += N;
         return RPK_OK;
     });

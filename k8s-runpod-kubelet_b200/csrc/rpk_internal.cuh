@@ -324,6 +324,28 @@ struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches i
     }
 };
 
+// Buffers that a shard's host and device entry points share, and the last device call that used them: the ordering rule
+// of rpk.h.  Inside a stream capture a device call neither waits nor records (an event recorded outside a capture cannot
+// be waited on inside it), so a captured step keeps each entry point on one stream, as bench.py does.
+struct ScratchScope {
+    cudaStream_t last = nullptr;  // the stream of the last device call outside a capture
+    cudaEvent_t ev = nullptr;     // recorded behind it
+    // a device entry point, before its launches on st: false inside a capture, and then device_end records nothing
+    bool device_begin(cudaStream_t st) {
+        cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+        if (cudaStreamIsCapturing(st, &cs) != cudaSuccess) { cudaGetLastError(); cs = cudaStreamCaptureStatusNone; }
+        if (cs != cudaStreamCaptureStatusNone) return false;
+        if (last != nullptr && last != st) RPK_CUDA(cudaStreamWaitEvent(st, ev, 0));
+        return true;
+    }
+    void device_end(cudaStream_t st, bool tracked) {
+        if (!tracked) return;
+        RPK_CUDA(cudaEventRecord(ev, st));
+        last = st;
+    }
+    void host_wait() { if (last) RPK_CUDA(cudaEventSynchronize(ev)); }
+};
+
 // One GPU of a ctx.  Built once at its final place (never copied or moved); the destructor synchronises the streams
 // and destroys them and the events, then the members free the buffers with this device still current.
 struct DeviceState {
@@ -367,9 +389,7 @@ struct DeviceState {
     DevBuf<uint32_t> s_seed_slots; DevBuf<uint8_t> s_seed_recs;  // slot lists of rpk_status_seed_slots and rpk_status_diff_slots
     PinnedBuf h_changed;                   // the host sweep's changed list: count, indices, codes
     cudaStream_t status_stream = nullptr;  // rpk_tick: the sweep next to the selection
-    // device entry points: the stream that last used the select / status scratch, and its completion event
-    cudaStream_t sel_last_stream = nullptr, st_last_stream = nullptr;
-    cudaEvent_t ev_sel = nullptr, ev_st = nullptr;
+    ScratchScope sel_scope, status_scope;  // the offer views, the pod table and lane 0; the sweep scratch
     bool status_dirty = false;             // a status launch failed midway: re-zero the look-back state before the next one
     uint32_t statusN = 0; bool status_sized = false;
     // pod-requirement table (rpk_pods_reset): the five columns of podsN slots, the whole table on every GPU of the ctx

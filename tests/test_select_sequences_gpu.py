@@ -74,7 +74,7 @@ class Program:
                 got = sc.run_host(self.eng, pods, top5)
             elif op == "dev_a":
                 got = sc.run_device(self.eng, pods, top5)
-            elif op == "dev_b":  # the scratch guard moves to the other stream
+            elif op == "dev_b":  # the select scope moves to the other stream
                 got = sc.run_device(self.eng, pods, top5, stream=self.stream_b)
             elif op == "gather":
                 got = sc.run_gather(self.eng, pods, top5, row0)

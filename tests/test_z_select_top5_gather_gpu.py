@@ -248,7 +248,7 @@ def test_replay_from_a_cuda_graph(group, P):
 
 def test_sequences_on_one_context(group):
     """the lists' gather interleaved with the plain gather, the host select with top5 and the lists' gather on a second
-    stream, at changing sizes on one ctx: every step is checked (the scratch guard orders the two streams)"""
+    stream, at changing sizes on one ctx: every step is checked (the select scope orders the two streams)"""
     import torch
 
     eng, offers, flags, words = group
