@@ -206,6 +206,62 @@ func (e *Engine) SelectSlots(slots []uint32, wantTop5 bool) (best []int32, top5 
 	return best, top5, nil
 }
 
+// PodsMarkPending sets the pending flag of slot slots[i] to pending[i] != 0 (slots strictly ascending): the predicate of
+// processPendingPods (Phase == Pending and no runpod.io/pod-id, kubelet.go:752, :768), kept per slot on the device.
+func (e *Engine) PodsMarkPending(slots []uint32, pending []uint8) error {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if len(slots) == 0 {
+		return nil
+	}
+	if len(pending) != len(slots) {
+		return fmt.Errorf("rpk: %d slots for %d flags", len(slots), len(pending))
+	}
+	rc := C.rpk_pods_mark_pending(e.ctx, C.uint32_t(len(slots)), (*C.uint32_t)(unsafe.Pointer(&slots[0])), u8p(pending))
+	if rc != C.RPK_OK {
+		return lastError(e.ctx, rc)
+	}
+	return nil
+}
+
+// SelectPending is SelectSlots over every pending slot of the pod table, ascending, with no list from the caller: the
+// device builds it from the flags.  capacity bounds the outputs; with more slots pending the call fails and n says how
+// many there are.  slots[i] is the slot of row i.
+func (e *Engine) SelectPending(capacity int, wantTop5 bool) (slots []uint32, best []int32, top5 []int32, n int, err error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	slots = make([]uint32, capacity+1)
+	best = make([]int32, capacity+1)
+	var t5 *C.int32_t
+	if wantTop5 {
+		top5 = make([]int32, (capacity+1)*TopK)
+		t5 = i32p(top5)
+	}
+	var cnt C.uint32_t
+	rc := C.rpk_select_pending(e.ctx, C.uint32_t(capacity), (*C.uint32_t)(unsafe.Pointer(&slots[0])), &cnt, i32p(best), t5)
+	n = int(cnt)
+	if rc != C.RPK_OK {
+		return nil, nil, nil, n, lastError(e.ctx, rc)
+	}
+	if wantTop5 {
+		top5 = top5[:n*TopK]
+	}
+	return slots[:n], best[:n], top5, n, nil
+}
+
+// PodsPendingListDevice enqueues the pending list alone on GPU shard: dSlotsOut (device memory, one entry per slot of
+// the pod table) receives the pending slot ids ascending, dN their number.  The caller passes the list and the count
+// it read to the rpk_select_slots_device calls.
+func (e *Engine) PodsPendingListDevice(shard int, dSlotsOut, dN, stream unsafe.Pointer) error {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	rc := C.rpk_pods_pending_list_device(e.ctx, C.int(shard), (*C.uint32_t)(dSlotsOut), (*C.uint32_t)(dN), stream)
+	if rc != C.RPK_OK {
+		return lastError(e.ctx, rc)
+	}
+	return nil
+}
+
 // StatusDiff is the batched predicate of updateAllPodStatuses (kubelet.go:870-873): records holds one
 // fixed slot per tracked pod (see EncodeStatusRecord); the indices of the slots whose (status, ports)
 // pair differs from the previous sweep come back ascending.

@@ -31,7 +31,8 @@
  *     stream than the last _device call of its scope first waits for that call, so any streams may be used.  A host
  *     call waits for the last _device call of its scopes before it touches anything, and returns after its own work is
  *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_pods_reset,
- *     rpk_pods_seed_slots, rpk_select, rpk_select_slots, and rpk_tick with P > 0.  Status scope: rpk_status_diff,
+ *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending, the _device call
+ *     rpk_pods_pending_list_device, and rpk_tick with P > 0.  Status scope: rpk_status_diff,
  *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset and
  *     rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
  *     capture neither waits nor is waited for (keep each captured entry point on one stream), and the library does
@@ -73,7 +74,7 @@ extern "C" {
 typedef struct rpk_ctx rpk_ctx;
 
 typedef struct rpk_stats {
-    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_device + rpk_select_slots_device */
+    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_pending + rpk_select_device + rpk_select_slots_device */
     uint64_t offer_scores;        /* sum of P*G over those calls */
     uint64_t status_calls;
     uint64_t status_records;      /* sum of N */
@@ -136,7 +137,8 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
  *
  * (Re)size the pod table to N slots on every GPU of the ctx and set every row to the columns of a pod with no
  * annotations: req_mem_gb 16 (extractGPUMemory(""), runpod_client.go:1182), vcpu 0, ram 0, max_price 0.5, SECURE.
- * Independent of rpk_status_reset.  The table is replicated: 21 bytes x N on each GPU. */
+ * No slot is pending afterwards (rpk_pods_mark_pending).  Independent of rpk_status_reset.  The table is replicated:
+ * 22 bytes x N on each GPU (the five columns and the pending flag). */
 int rpk_pods_reset(rpk_ctx* ctx, uint32_t N);
 /* Row slots[i] := element i of each column.  Columns may be NULL exactly where rpk_select's may, with the same defaults
  * (req_mem_gb is required).  slots must be strictly ascending and < N of the pod table (else RPK_EINVAL, nothing
@@ -150,6 +152,27 @@ int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, c
  * is checked just before its upload).  No pod table or no offer table: RPK_ESTATE.  Counts as one select in rpk_stats
  * (select_calls, offer_scores += n_slots * G).  n_slots == 0 is a no-op. */
 int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int32_t* best, int32_t* top5);
+
+/* The pending set: which slots processPendingPods would retry, kept in the table next to the columns, so that a tick
+ * sends no list at all.  The set changes as slowly as the columns do: a pod enters it in CreatePod and leaves it when a
+ * deploy succeeds, the pod is deleted, or it is failed after 15 minutes.
+ *
+ * pending[i] != 0 marks slot slots[i] pending, 0 clears it: processPendingPods' predicate (Phase == Pending and no
+ * runpod.io/pod-id, kubelet.go:752, :768), kept per slot.  slots strictly ascending and < N of the pod table (else
+ * RPK_EINVAL, nothing written; no pod table: RPK_ESTATE), as rpk_pods_seed_slots.  Every GPU of the ctx gets the
+ * flags.  Slots not listed are not touched.  rpk_pods_seed_slots changes no flag and this call no column.
+ * n_slots == 0 is a no-op.  Select scope, host call. */
+int rpk_pods_mark_pending(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* pending);
+/* rpk_select_slots over every pending slot of the pod table, ascending, with no list from the caller: the device builds
+ * the list from the flags (in range by construction: nothing to check, nothing to upload).
+ *   *n_pending   the number of pending slots (always written on RPK_OK and on the cap refusal below)
+ *   slots_out    nullable, capacity cap: the pending slot ids, ascending (a caller that mirrors the flags knows them)
+ *   best, top5   capacity cap and 5*cap (top5 nullable): row i is what rpk_select_slots returns for slot slots_out[i],
+ *                bit for bit
+ * More than cap slots pending: RPK_EINVAL, *n_pending set, no other output written, nothing counted.  No pod table or
+ * no offer table: RPK_ESTATE.  Zero pending: RPK_OK, *n_pending = 0, and what rpk_select_slots does for n_slots == 0.
+ * Counts as one select in rpk_stats (offer_scores += n_pending * G).  Select scope, host call. */
+int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t* n_pending, int32_t* best, int32_t* top5);
 
 /* Same on device-resident columns of GPU `shard` (index into the ctx's device list), enqueued on `stream`
  * (a cudaStream_t; NULL = the ctx's own stream for that shard; pass cudaStreamLegacy (0x1) for the legacy
@@ -218,6 +241,16 @@ int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, co
 int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
                                         int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0,
                                         void* stream);
+
+/* The pending list only, for one-process-per-GPU callers: d_slots_out (capacity N of the pod table, on GPU `shard`)
+ * receives the pending slot ids ascending, *d_n (device memory on GPU `shard`) their number; entries of d_slots_out
+ * beyond *d_n are not written.  It is the launch rpk_select_pending makes, exposed: one kernel, no memset before it.
+ * Enqueued on `stream`, no synchronisation; select scope, device call (ordered like rpk_select_slots_device).  The
+ * select kernels take no device-side row count: the caller reads *d_n (or knows it from its own mirror of the flags)
+ * and passes it as n_slots, with the list, to rpk_select_slots_device[_gather[_top5]].  No pod table: RPK_ESTATE; NULL
+ * output: RPK_EINVAL; both before anything is enqueued.  Graph-capturable after one call; a replay reads the flags as
+ * they are at replay time. */
+int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out, uint32_t* d_n, void* stream);
 
 /* Cross-process peer vectors for one-process-per-GPU callers (torchrun-style): allocate a plain cudaMalloc
  * buffer on GPU `shard` and export its 64-byte CUDA IPC handle; another process opens the handle and gets a

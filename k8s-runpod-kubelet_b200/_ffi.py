@@ -41,12 +41,15 @@ ABI = {
     "rpk_pods_reset": (_int, [_p, _u32]),
     "rpk_pods_seed_slots": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
     "rpk_select_slots": (_int, [_p, _u32, _p, _p, _p]),
+    "rpk_pods_mark_pending": (_int, [_p, _u32, _p, _p]),
+    "rpk_select_pending": (_int, [_p, _u32, _p, _p, _p, _p]),
     "rpk_select_device": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_select_device_gather": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _int, _pp, _u32, _p, _p]),
     "rpk_select_device_gather_top5": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _int, _pp, _pp, _u32, _p]),
     "rpk_select_slots_device": (_int, [_p, _int, _u32, _p, _p, _p, _p]),
     "rpk_select_slots_device_gather": (_int, [_p, _int, _u32, _p, _int, _pp, _u32, _p, _p]),
     "rpk_select_slots_device_gather_top5": (_int, [_p, _int, _u32, _p, _int, _pp, _pp, _u32, _p]),
+    "rpk_pods_pending_list_device": (_int, [_p, _int, _p, _p, _p]),
     "rpk_ipc_alloc": (_int, [_p, _int, _size, _pp, C.c_char_p]),
     "rpk_ipc_open": (_int, [_p, _int, C.c_char_p, _pp]),
     "rpk_ipc_close": (_int, [_p, _int, _p]),

@@ -88,6 +88,7 @@ rpk::DeviceState::~DeviceState() {
     if (dev < 0 || cudaSetDevice(dev) != cudaSuccess) { cudaGetLastError(); return; }  // creation failed before this GPU
     if (stream) cudaStreamSynchronize(stream);
     if (status_stream) cudaStreamSynchronize(status_stream);
+    if (pending_stream) cudaStreamSynchronize(pending_stream);
     for (auto& ln : lane) if (ln.stream) cudaStreamSynchronize(ln.stream);
     for (auto& ln : lane) {
         if (ln.done) cudaEventDestroy(ln.done);
@@ -97,6 +98,7 @@ rpk::DeviceState::~DeviceState() {
     if (sel_scope.ev) cudaEventDestroy(sel_scope.ev);
     if (status_scope.ev) cudaEventDestroy(status_scope.ev);
     if (status_stream) cudaStreamDestroy(status_stream);
+    if (pending_stream) cudaStreamDestroy(pending_stream);
     if (stream) cudaStreamDestroy(stream);
     cudaGetLastError();
 }
@@ -133,10 +135,13 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
 
 // Where the rows of a select come from: the caller's columns (rpk_select, rpk_tick: host memory; rpk_select_device*:
 // device memory), or rows of the pod table (rpk_select_slots: a host list, each sub-batch uploads its slot ids and
-// gathers the five columns on the device; rpk_select_slots_device*: a device list, gathered in one pass).
+// gathers the five columns on the device; rpk_select_slots_device*: a device list, gathered in one pass;
+// rpk_select_pending: the list k_pod_pending left on every GPU, in range by construction, so a sub-batch has nothing to
+// check or upload and gathers from its part of the list in place).
 struct PodSource {
     PodCols cols;
     const uint32_t* slots;  // non-null: row i of the call is pod-table row slots[i]; cols is unused
+    bool pending = false;   // row i of the call is pod-table row pt_list[i] of the GPU that selects it; the rest is unused
 };
 
 // every entry of slots[0, n) is a row of a pod table of N rows.  The pipelined select runs this per sub-batch on the
@@ -257,9 +262,23 @@ inline uint32_t sub_batch_rows(int j, uint32_t remaining) {
     const uint32_t want = kSubBatchRows * (uint32_t)((j + 1) < (int)kSubBatchMaxMul ? (j + 1) : (int)kSubBatchMaxMul);
     return remaining < want + kSubBatchRows / 2 ? remaining : want;  // do not leave a sliver behind
 }
-inline uint32_t sub_batch_cap(uint32_t Ps) {  // largest sub-batch a shard of Ps rows produces
+// ... of a call whose rows come from src.  The pending list needs no upload for the sub-batches to hide, but they still
+// overlap the copies of best and top5 back to the host: measured at 1M rows on an H100 (700 W), the sub-batches take
+// 0.97 ms against 1.02 ms for one select over the whole list with top-5, which the Provider's tick asks for, and 0.55
+// against 0.52 ms without, each inside the other's spread (DESIGN section 4, "Pending set"): the list keeps the
+// pipeline's shape.
+// RPK_MEASURE_PENDING_ONE_SELECT: only for the copy of the library tools/select_pending_probe.py builds to time the other
+// shape.
+inline uint32_t sub_batch_rows(const PodSource& src, int j, uint32_t remaining) {
+#ifdef RPK_MEASURE_PENDING_ONE_SELECT
+    if (src.pending) return remaining;
+#endif
+    (void)src;
+    return sub_batch_rows(j, remaining);
+}
+inline uint32_t sub_batch_cap(const PodSource& src, uint32_t Ps) {  // largest sub-batch a shard of Ps rows produces
     uint32_t cap = 0, left = Ps;
-    for (int j = 0; left; ++j) { const uint32_t nb = sub_batch_rows(j, left); cap = nb > cap ? nb : cap; left -= nb; }
+    for (int j = 0; left; ++j) { const uint32_t nb = sub_batch_rows(src, j, left); cap = nb > cap ? nb : cap; left -= nb; }
     return cap ? cap : 1;
 }
 
@@ -278,12 +297,14 @@ int select_small(DeviceState& ds, uint32_t P, const PodSource& src, int32_t* bes
     unsigned char* d = ds.d_small_in.p;
     SelectArgs a{};
     int launches = 0;
-    if (src.slots) {
+    if (src.slots || src.pending) {
         ln.p_req_mem.reserve(kSmallBatch); ln.p_req_vcpu.reserve(kSmallBatch); ln.p_req_ram.reserve(kSmallBatch);
         ln.p_max_price.reserve(kSmallBatch); ln.p_cloud.reserve(kSmallBatch);
-        memcpy(h, src.slots, (size_t)P * 4);
-        RPK_CUDA(cudaMemcpyAsync(d, h, (size_t)P * 4, cudaMemcpyHostToDevice, st));
-        launches += gather_pod_rows(ds, ln, P, (const uint32_t*)d, a, st);
+        if (src.slots) {
+            memcpy(h, src.slots, (size_t)P * 4);
+            RPK_CUDA(cudaMemcpyAsync(d, h, (size_t)P * 4, cudaMemcpyHostToDevice, st));
+        }
+        launches += gather_pod_rows(ds, ln, P, src.slots ? (const uint32_t*)d : ds.pt_list.p, a, st);
     } else {
         const PodCols& pods = src.cols;
         const size_t o_mem = 0, o_vcpu = (size_t)P * 4, o_ram = (size_t)P * 8, o_price = ((size_t)P * 12 + 7) & ~(size_t)7,
@@ -322,17 +343,17 @@ bool has_int32_max(const int32_t* col, uint32_t n) {
 void reserve_select(rpk_ctx* ctx, uint32_t P, const PodSource& src, bool top5) {
     const int n = (int)ctx->devs.size();
     const PodCols& pods = src.cols;
-    const bool all = src.slots != nullptr;  // the gather writes all five columns
+    const bool all = src.slots || src.pending;  // the gather writes all five columns
     const bool vcpu = all || pods.req_vcpu, ram = all || pods.req_ram, price = all || pods.max_price, cloud = all || pods.cloud;
     for (int s = 0; s < n; ++s) {
         DeviceState& ds = ctx->devs[(size_t)s];
         uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
         const uint32_t Ps = hi - lo;
-        const uint32_t cap = sub_batch_cap(Ps);
+        const uint32_t cap = sub_batch_cap(src, Ps);
         bool grow = P > ds.best_full.cap;
         for (auto& ln : ds.lane) {
             grow = grow || cap > ln.p_req_mem.cap || (vcpu && cap > ln.p_req_vcpu.cap) || (ram && cap > ln.p_req_ram.cap) ||
-                   (price && cap > ln.p_max_price.cap) || (cloud && cap > ln.p_cloud.cap) || (all && cap > ln.p_slots.cap) ||
+                   (price && cap > ln.p_max_price.cap) || (cloud && cap > ln.p_cloud.cap) || (src.slots && cap > ln.p_slots.cap) ||
                    (top5 && (size_t)cap * RPK_TOPK > ln.top5.cap);
             if (cap == Ps) break;  // a single sub-batch uses lane 0 only
         }
@@ -345,7 +366,7 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, const PodSource& src, bool top5) {
             if (ram) ln.p_req_ram.reserve(cap);
             if (price) ln.p_max_price.reserve(cap);
             if (cloud) ln.p_cloud.reserve(cap);
-            if (all) ln.p_slots.reserve(cap);
+            if (src.slots) ln.p_slots.reserve(cap);
             if (top5) ln.top5.reserve((size_t)cap * RPK_TOPK);
             if (cap == Ps) break;
         }
@@ -366,11 +387,13 @@ bool enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodSource& src,
     bool ok = true;
     int j = 0;
     for (uint32_t b0 = lo, nb = 0; b0 < hi; b0 += nb, ++j) {
-        nb = sub_batch_rows(j, hi - b0);
+        nb = sub_batch_rows(src, j, hi - b0);
         DeviceState::Lane& ln = ds.lane[j % DeviceState::kLanes];
         cudaStream_t st = ln.stream;
         SelectArgs a{};
-        if (src.slots) {
+        if (src.pending) {
+            *launches += (uint64_t)gather_pod_rows(ds, ln, nb, ds.pt_list.p + b0, a, st);
+        } else if (src.slots) {
             if (!slots_below(src.slots + b0, nb, ds.podsN)) { ok = false; break; }
             RPK_CUDA(cudaMemcpyAsync(ln.p_slots.p, src.slots + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
             *launches += (uint64_t)gather_pod_rows(ds, ln, nb, ln.p_slots.p, a, st);
@@ -705,6 +728,7 @@ int rpk_create(int n_gpus, const int* device_ids, rpk_ctx** out) {
             RPK_CUDA(cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi));
             RPK_CUDA(cudaStreamCreateWithPriority(&ds.stream, cudaStreamNonBlocking, prio_hi));
             RPK_CUDA(cudaStreamCreateWithPriority(&ds.status_stream, cudaStreamNonBlocking, prio_lo));
+            RPK_CUDA(cudaStreamCreateWithPriority(&ds.pending_stream, cudaStreamNonBlocking, prio_lo));
             for (auto& ev : ds.ev) RPK_CUDA(cudaEventCreate(&ev));
             RPK_CUDA(cudaEventCreateWithFlags(&ds.sel_scope.ev, cudaEventDisableTiming));
             RPK_CUDA(cudaEventCreateWithFlags(&ds.status_scope.ev, cudaEventDisableTiming));
@@ -833,7 +857,8 @@ int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
             ds.sel_scope.host_wait();  // a device select may still gather from the table
             const size_t cap = N ? N : 1;
             ds.pt_mem.reserve(cap); ds.pt_vcpu.reserve(cap); ds.pt_ram.reserve(cap); ds.pt_max_price.reserve(cap); ds.pt_cloud.reserve(cap);
-            ctx->launches += (uint64_t)launch_pod_fill(ds.pods_table(), N, ds.sm_count, ds.stream);
+            ds.pt_pending.reserve(cap);
+            ctx->launches += (uint64_t)launch_pod_fill(ds.pods_table(), ds.pt_pending.p, N, ds.sm_count, ds.stream);
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
             ds.podsN = N;
         }
@@ -842,17 +867,23 @@ int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
     });
 }
 
+// slots[0, n) strictly ascending and inside the pod table (which exists): what the calls that write the table require
+static int check_pod_slots(rpk_ctx* ctx, uint32_t n, const uint32_t* slots, const char* who) {
+    const uint32_t N = ctx->devs[0].podsN;
+    for (uint32_t i = 0; i < n; ++i) {
+        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
+        if (i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, std::string(who) + ": slots must be strictly ascending");
+    }
+    return RPK_OK;
+}
+
 int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const int32_t* req_mem_gb, const int32_t* req_vcpu,
                         const int32_t* req_ram_gb, const double* max_price, const uint8_t* cloud) {
     if (!ctx) return RPK_EINVAL;
     if (n_slots == 0) return RPK_OK;
     if (!slots || !req_mem_gb) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slots and req_mem_gb are required");
     if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_seed_slots: no pod table (call rpk_pods_reset first)");
-    const uint32_t N = ctx->devs[0].podsN;
-    for (uint32_t i = 0; i < n_slots; ++i) {
-        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slot index outside the pod table");
-        if (i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slots must be strictly ascending");
-    }
+    if (int rc = check_pod_slots(ctx, n_slots, slots, "rpk_pods_seed_slots")) return rc;
     return guarded(ctx, [&]() -> int {
         // staging block: [slots : 4n][mem : 4n][vcpu : 4n][ram : 4n][max_price : 8n, 8-byte aligned][cloud : n]
         const size_t n = n_slots, o_mem = 4 * n, o_vcpu = 8 * n, o_ram = 12 * n, o_price = (16 * n + 7) & ~(size_t)7,
@@ -907,6 +938,111 @@ int rpk_select_slots_device(rpk_ctx* ctx, int shard, uint32_t n_slots, const uin
                             void* stream) {
     int32_t* outs[1] = {d_best};
     return rpk_select_slots_device_gather(ctx, shard, n_slots, d_slots, 1, outs, 0, d_top5, stream);
+}
+
+// ---- pending set of the pod table ---------------------------------------------------------------------------
+
+int rpk_pods_mark_pending(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* pending) {
+    if (!ctx) return RPK_EINVAL;
+    if (n_slots == 0) return RPK_OK;
+    if (!slots || !pending) return fail(ctx, RPK_EINVAL, "rpk_pods_mark_pending: slots and pending are required");
+    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_mark_pending: no pod table (call rpk_pods_reset first)");
+    if (int rc = check_pod_slots(ctx, n_slots, slots, "rpk_pods_mark_pending")) return rc;
+    return guarded(ctx, [&]() -> int {
+        const size_t n = n_slots;  // staging block: [slots : 4n][pending : n]
+        for (auto& ds : ctx->devs) {  // the table is replicated: every GPU gets every flag
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ds.sel_scope.host_wait();  // after a device call's pending list
+            ds.pt_seed.reserve(5 * n);
+            RPK_CUDA(cudaMemcpyAsync(ds.pt_seed.p, slots, 4 * n, cudaMemcpyHostToDevice, ds.stream));
+            RPK_CUDA(cudaMemcpyAsync(ds.pt_seed.p + 4 * n, pending, n, cudaMemcpyHostToDevice, ds.stream));
+            ctx->launches += (uint64_t)launch_pod_mark(ds.pt_pending.p, ds.podsN, n_slots, (const uint32_t*)ds.pt_seed.p, ds.pt_seed.p + 4 * n, ds.stream);
+            RPK_CUDA(cudaStreamSynchronize(ds.stream));
+        }
+        return RPK_OK;
+    });
+}
+
+namespace {
+// k_pod_pending on ds over its replica of the flags: the list into d_out (capacity podsN), its length into d_n
+int enqueue_pending_list(DeviceState& ds, uint32_t* d_out, uint32_t* d_n, cudaStream_t st) {
+    const size_t need = pending_state_words(ds.sm_count);
+    if (need > ds.pt_state.cap || !ds.pt_ticket.p) {  // zero between calls by construction (the kernel's last CTA)
+        ds.pt_state.reserve(need); ds.pt_ticket.reserve(2);
+        RPK_CUDA(cudaMemset(ds.pt_state.p, 0, ds.pt_state.cap * sizeof(unsigned long long)));
+        RPK_CUDA(cudaMemset(ds.pt_ticket.p, 0, ds.pt_ticket.cap * sizeof(uint32_t)));
+        RPK_CUDA(cudaDeviceSynchronize());
+    }
+    const PendingArgs a{ds.pt_pending.p, ds.podsN, d_out, d_n, ds.pt_state.p, ds.pt_ticket.p};
+    return launch_pod_pending(a, ds.sm_count, st);
+}
+}  // namespace
+
+int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out, uint32_t* d_n, void* stream) {
+    if (!ctx) return RPK_EINVAL;
+    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_pods_pending_list_device: shard out of range");
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    if (!ds.pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_pending_list_device: no pod table on this shard (call rpk_pods_reset first)");
+    if (!d_n || (ds.podsN > 0 && !d_slots_out)) return fail(ctx, RPK_EINVAL, "rpk_pods_pending_list_device: d_slots_out and d_n are required");
+    return guarded(ctx, [&]() -> int {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+        const bool tracked = ds.sel_scope.device_begin(st);  // the look-back state is the shard's: after the last list
+        ctx->launches += (uint64_t)enqueue_pending_list(ds, d_slots_out, d_n, st);
+        ds.sel_scope.device_end(st, tracked);
+        return RPK_OK;
+    });
+}
+
+int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t* n_pending, int32_t* best, int32_t* top5) {
+    if (!ctx) return RPK_EINVAL;
+    if (!n_pending || (cap > 0 && !best)) return fail(ctx, RPK_EINVAL, "rpk_select_pending: n_pending and best are required");
+    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_pending: no pod table (call rpk_pods_reset first)");
+    for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select_pending: no offer table uploaded (call rpk_offers_upload first)");
+    // every GPU compacts its own replica of the flags: the table is replicated and the order ascending, so the lists are
+    // identical, and each GPU then gathers its shard of the rows from its own copy.  The count lands in mapped pinned
+    // memory, so the one synchronise that the list's length costs needs no copy behind it.
+    uint32_t n = 0;
+    int rc = guarded(ctx, [&]() -> int {
+        for (auto& ds : ctx->devs) {
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ds.sel_scope.host_wait();
+            ds.pt_list.reserve(ds.podsN ? ds.podsN : 1);
+            ds.h_pending.reserve(64);
+            ctx->launches += (uint64_t)enqueue_pending_list(ds, ds.pt_list.p, reinterpret_cast<uint32_t*>(ds.h_pending.d), ds.stream);
+        }
+        for (auto& ds : ctx->devs) {
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            RPK_CUDA(cudaStreamSynchronize(ds.stream));
+        }
+        n = *reinterpret_cast<volatile uint32_t*>(ctx->devs[0].h_pending.h);
+        return RPK_OK;
+    });
+    if (rc != RPK_OK) return rc;
+    *n_pending = n;
+    if (n > cap) return fail(ctx, RPK_EINVAL, "rpk_select_pending: more slots pending than cap");
+    if (n == 0) return RPK_OK;
+    DeviceState& d0 = ctx->devs[0];
+    if (slots_out) {  // the list goes back on a stream of its own while the select runs
+        rc = guarded(ctx, [&]() -> int {
+            RPK_CUDA(cudaSetDevice(d0.dev));
+            RPK_CUDA(cudaMemcpyAsync(slots_out, d0.pt_list.p, (size_t)n * 4, cudaMemcpyDeviceToHost, d0.pending_stream));
+            return RPK_OK;
+        });
+        if (rc != RPK_OK) return rc;
+    }
+    PodSource src{};
+    src.pending = true;
+    rc = select_host(ctx, n, src, best, top5, "rpk_select_pending");
+    if (slots_out) {
+        const int rc2 = guarded(ctx, [&]() -> int {
+            RPK_CUDA(cudaSetDevice(d0.dev));
+            RPK_CUDA(cudaStreamSynchronize(d0.pending_stream));
+            return RPK_OK;
+        });
+        if (rc == RPK_OK) rc = rc2;
+    }
+    return rc;
 }
 
 // ---- cross-process peer vectors (CUDA IPC) ---------------------------------------------------------------

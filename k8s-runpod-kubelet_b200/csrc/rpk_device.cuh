@@ -1,5 +1,5 @@
 // rpk_device.cuh -- device-side primitives shared by the kernels: programmatic dependent launch, mbarrier +
-// bulk async copy (TMA, SASS UBLKCP), the 16-byte split of a result slice.
+// bulk async copy (TMA, SASS UBLKCP), the 16-byte split of a result slice, the look-back over CTA counts.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -66,6 +66,34 @@ __device__ __forceinline__ void copy_slice_edges(const int32_t* src, uint32_t of
         if (t < s.head) dst(o)[off + t] = hv;
         if (t < n - s.tail0) dst(o)[off + s.tail0 + t] = tv;
     }
+}
+
+#define kFlagAgg (1ull << 32)
+#define kFlagMask (3ull << 32)
+
+// Decoupled look-back over the CTAs before `id` (one warp): returns the exclusive prefix.  There is at most one CTA
+// per SM, and they all finish at about the same time, so walking back window by window would cost one L2 round trip
+// per 32 predecessors.  Every CTA publishes its count once (kFlagAgg | count; an entry without a flag bit is not there
+// yet) and sums ALL entries before it in one pass of independent loads, retrying only the ones that are not there yet.
+// Ids come from a scheduling ticket, so every CTA waited for has started.  Used by the status sweep and the pending list.
+__device__ __forceinline__ uint32_t sum_before(volatile unsigned long long* st, uint32_t id, uint32_t total, uint32_t lane) {
+    if (lane == 0) st[id] = kFlagAgg | total;
+    uint32_t acc = 0;
+    for (uint32_t base = 0; base < id; base += 128) {  // four independent loads per lane and pass
+        unsigned long long v[4];
+        bool need[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { const uint32_t i = base + (uint32_t)k * 32 + lane; need[k] = i < id; v[k] = need[k] ? st[i] : kFlagAgg; }
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+            const uint32_t i = base + (uint32_t)k * 32 + lane;
+            while (need[k] && (v[k] & kFlagMask) == 0) v[k] = st[i];
+            acc += (uint32_t)v[k];
+        }
+    }
+#pragma unroll
+    for (int d = 16; d >= 1; d >>= 1) acc += __shfl_xor_sync(0xFFFFFFFFu, acc, d);
+    return acc;
 }
 
 }  // namespace dev

@@ -281,9 +281,22 @@ struct PodCols { const int32_t* req_mem; const int32_t* req_vcpu; const int32_t*
 struct PodRows { int32_t* mem; int32_t* vcpu; int32_t* ram; double* max_price; uint8_t* cloud; };
 // pod-requirement table (pods.cu): N = the table's rows; an entry of d_slots outside [0, N) is skipped by the seed and
 // gathered as a row nothing matches (cloud byte 2)
-int launch_pod_fill(const PodRows& t, uint32_t N, int sm_count, cudaStream_t st);
+// pending is the table's flag column (one byte per slot), cleared with the rows
+int launch_pod_fill(const PodRows& t, uint8_t* pending, uint32_t N, int sm_count, cudaStream_t st);
 int launch_pod_seed(const PodRows& t, uint32_t N, uint32_t n, const uint32_t* d_slots, const PodCols& in, cudaStream_t st);
 int launch_pod_gather(const PodRows& t, uint32_t N, uint32_t n, const uint32_t* d_slots, const PodRows& out, cudaStream_t st);
+// pending set of the pod table (pods.cu): flags[s] != 0 marks slot s pending
+int launch_pod_mark(uint8_t* flags, uint32_t N, uint32_t n, const uint32_t* d_slots, const uint8_t* d_pending, cudaStream_t st);
+struct PendingArgs {
+    const uint8_t* flags;            // [N], 16-byte aligned
+    uint32_t N;
+    uint32_t* out;                   // [N] the pending slot ids, ascending
+    uint32_t* n_out;                 // their number (device or mapped host memory)
+    unsigned long long* tile_state;  // look-back state: pending_state_words entries; zero between calls
+    uint32_t* ticket;                // [2] scheduling ticket, finished CTAs; zero between calls
+};
+uint32_t pending_state_words(int sm_count);
+int launch_pod_pending(const PendingArgs& a, int sm_count, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
@@ -395,6 +408,11 @@ struct DeviceState {
     // pod-requirement table (rpk_pods_reset): the five columns of podsN slots, the whole table on every GPU of the ctx
     DevBuf<int32_t> pt_mem, pt_vcpu, pt_ram; DevBuf<double> pt_max_price; DevBuf<uint8_t> pt_cloud;
     DevBuf<unsigned char> pt_seed;         // rpk_pods_seed_slots: the slot ids and the columns of one seed
+    // pending set: one flag byte per slot, the list k_pod_pending makes of it, and that kernel's look-back state and
+    // tickets (zero between calls by construction, zeroed when allocated)
+    DevBuf<uint8_t> pt_pending; DevBuf<uint32_t> pt_list; DevBuf<unsigned long long> pt_state; DevBuf<uint32_t> pt_ticket;
+    PinnedBuf h_pending;                   // rpk_select_pending: the list's length, written by the kernel
+    cudaStream_t pending_stream = nullptr; // rpk_select_pending: the list's copy to the caller, beside the select
     uint32_t podsN = 0; bool pods_sized = false;
     PodRows pods_table() { return PodRows{pt_mem.p, pt_vcpu.p, pt_ram.p, pt_max_price.p, pt_cloud.p}; }
     ~DeviceState();

@@ -142,33 +142,6 @@ __device__ __forceinline__ uint32_t classify_status(u64 l0, u64 l1, uint32_t len
     return kind;
 }
 
-#define kFlagAgg (1ull << 32)
-#define kFlagMask (3ull << 32)
-
-// Decoupled look-back over the CTAs before `id` (one warp): returns the exclusive prefix.  There is at most one CTA
-// per SM, and they all finish at about the same time, so walking back window by window would cost one L2 round trip
-// per 32 predecessors.  Every CTA publishes its count once (kFlagAgg | count; an entry without a flag bit is not there
-// yet) and sums ALL entries before it in one pass of independent loads, retrying only the ones that are not there yet.
-__device__ __forceinline__ uint32_t sum_before(volatile u64* st, uint32_t id, uint32_t total, uint32_t lane) {
-    if (lane == 0) st[id] = kFlagAgg | total;
-    uint32_t acc = 0;
-    for (uint32_t base = 0; base < id; base += 128) {  // four independent loads per lane and pass
-        u64 v[4];
-        bool need[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) { const uint32_t i = base + (uint32_t)k * 32 + lane; need[k] = i < id; v[k] = need[k] ? st[i] : kFlagAgg; }
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t i = base + (uint32_t)k * 32 + lane;
-            while (need[k] && (v[k] & kFlagMask) == 0) v[k] = st[i];
-            acc += (uint32_t)v[k];
-        }
-    }
-#pragma unroll
-    for (int d = 16; d >= 1; d >>= 1) acc += __shfl_xor_sync(0xFFFFFFFFu, acc, d);
-    return acc;
-}
-
 // ---------------------------------------------------------------------------------------------------------
 // streamed scan
 // ---------------------------------------------------------------------------------------------------------

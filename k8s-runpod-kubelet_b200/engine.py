@@ -20,7 +20,8 @@ _DEV_DTYPES = {
     "req_mem_gb": ("int32",), "req_vcpu": ("int32",), "req_ram_gb": ("int32",), "max_price": ("float64",),
     "cloud": ("uint8",), "d_best": ("int32",), "d_top5": ("int32",), "d_records": ("uint8",),
     "d_hash_prev": ("int64", "uint64"), "d_changed_idx": ("int32", "uint32"), "d_changed_code": ("int16", "uint16"),
-    "d_n_changed": ("int32", "uint32"), "d_slots": ("int32", "uint32"),
+    "d_n_changed": ("int32", "uint32"), "d_slots": ("int32", "uint32"), "d_slots_out": ("int32", "uint32"),
+    "d_n": ("int32", "uint32"),
 }
 
 
@@ -75,6 +76,7 @@ class Engine:
         self.n_gpus = n_gpus
         self.device_ids = list(device_ids) if device_ids is not None else list(range(n_gpus))  # as rpk_create reads NULL
         self.G = 0
+        self._pods_n = 0
 
     # -- plumbing ------------------------------------------------------------------------------------
     def _check(self, rc: int):
@@ -174,6 +176,7 @@ class Engine:
     def pods_reset(self, N: int):
         """(Re)size the pod table to N slots, every row the columns of a pod with no annotations (rpk_pods_reset)."""
         self._check(self._lib.rpk_pods_reset(self._ctx, N))
+        self._pods_n = N  # the capacity pods_pending_list_device requires of its output
 
     def pods_seed_slots(self, slots: np.ndarray, pods: dict):
         """Row slots[i] := row i of the host columns ``pods`` (as ``select`` takes them; slots strictly ascending)."""
@@ -195,6 +198,39 @@ class Engine:
             self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(best, np.int32, n, "best"),
             _np_ptr(top5, np.int32, n * 5, "top5") if top5 is not None else None))
         return best, top5
+
+    def pods_mark_pending(self, slots: np.ndarray, pending: np.ndarray):
+        """Pending flag of slot slots[i] := pending[i] != 0 (slots strictly ascending; rpk_pods_mark_pending)."""
+        slots = np.ascontiguousarray(slots, np.uint32)  # keep the converted arrays alive across the call
+        pending = np.ascontiguousarray(pending, np.uint8)
+        n = int(slots.size)
+        self._check(self._lib.rpk_pods_mark_pending(
+            self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(pending, np.uint8, n, "pending")))
+
+    def select_pending(self, cap: int, want_top5: bool = False, want_slots: bool = True, out_best=None, out_top5=None, out_slots=None):
+        """``select_slots`` over every pending slot of the pod table, ascending, the list built on the device:
+        ``(slots[n] | None, best[n], top5[n,5] | None)``.  ``cap`` is the capacity of the outputs; more slots pending
+        than that raises RPK_EINVAL (rpk_select_pending), and ``n_pending`` of the exception says how many."""
+        best = out_best if out_best is not None else np.empty(cap, np.int32)
+        top5 = (out_top5 if out_top5 is not None else np.empty((cap, 5), np.int32)) if want_top5 else None
+        slots = (out_slots if out_slots is not None else np.empty(cap, np.uint32)) if want_slots else None
+        n = C.c_uint32(0)
+        rc = self._lib.rpk_select_pending(
+            self._ctx, cap, _np_ptr(slots, np.uint32, cap, "slots_out"), C.cast(C.byref(n), C.c_void_p),
+            _np_ptr(best, np.int32, cap, "best"), _np_ptr(top5, np.int32, cap * 5, "top5") if top5 is not None else None)
+        if rc != 0:
+            err = _ffi.RpkError(rc, (self._lib.rpk_last_error(self._ctx) or b"").decode())
+            err.n_pending = n.value
+            raise err
+        k = n.value
+        return (slots[:k] if want_slots else None), best[:k], (top5[:k] if want_top5 else None)
+
+    def pods_pending_list_device(self, d_slots_out, d_n, shard: int = 0, stream=None):
+        """The pending slot ids, ascending, into ``d_slots_out`` (a torch CUDA tensor with one element per slot of the
+        pod table) and their number into ``d_n``, enqueued on ``stream`` (rpk_pods_pending_list_device)."""
+        self._check(self._lib.rpk_pods_pending_list_device(
+            self._ctx, shard, self._dev_ptr(d_slots_out, "d_slots_out", shard, at_least=self._pods_n),
+            self._dev_ptr(d_n, "d_n", shard, at_least=1), self._stream(stream, shard)))
 
     def select_device(self, pods: dict, d_best, d_top5=None, shard: int = 0, stream=None):
         """torch CUDA columns in, result enqueued on ``stream`` (default: torch's current stream on the shard's GPU)."""

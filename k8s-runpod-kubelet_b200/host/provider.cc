@@ -330,6 +330,7 @@ Provider::Provider(std::shared_ptr<RunPodAPI> api, int n_gpus, uint32_t max_pods
     if (rpk_pods_reset(ctx_, max_pods_) != RPK_OK) throw std::runtime_error(rpk_last_error(ctx_));
     seeded_.req_mem_gb.assign(max_pods_, 16); seeded_.req_vcpu.assign(max_pods_, 0); seeded_.req_ram_gb.assign(max_pods_, 0);
     seeded_.max_price.assign(max_pods_, DefaultMaxPrice); seeded_.cloud.assign(max_pods_, RPK_CLOUD_SECURE);
+    want_pending_.assign(max_pods_, 0); marked_.assign(max_pods_, 0);  // rpk_pods_reset left no slot pending
     if (opt_.self_tick) {  // go provider.startPeriodicStatusUpdates(); go provider.startPendingPodProcessor() -- kubelet.go:374-376
         StartTicker(opt_.periodic_interval_s, [this] { UpdateAllPodStatuses(); });
         StartTicker(opt_.pending_interval_s, [this] { ProcessPendingPods(); });
@@ -367,6 +368,18 @@ uint32_t Provider::AllocSlot() {
     return s;
 }
 
+bool Provider::IsPending(const Pod& pod) {
+    if (pod.status.phase != "Pending") return false;                                // :753
+    auto a = pod.annotations.find(PodIDAnnotation);
+    return a == pod.annotations.end() || a->second.empty();                         // :769-775
+}
+
+void Provider::TrackPending(uint32_t slot, bool pending) {
+    if (want_pending_[slot] == (uint8_t)pending) return;
+    want_pending_[slot] = (uint8_t)pending;
+    pending_dirty_.push_back(slot);
+}
+
 void Provider::Notify(const PodPtr& pod) {
     std::function<void(const PodPtr&)> cb;
     { std::lock_guard<std::mutex> g(notify_mutex_); cb = notify_; }
@@ -401,6 +414,7 @@ std::string Provider::CreatePod(const PodPtr& pod) {
         slot_key_[t.slot] = key;
         EncodeStatusRecord(&records_[(size_t)t.slot * stride_], stride_, t.info.Status, t.info.PortsExposed);
         slot = t.slot;
+        TrackPending(slot, IsPending(*t.pod));
         pods_[key] = std::move(t);
     }
     SeedSlot(slot);  // previous state for the sweep = what InstanceInfo says now, for this slot only
@@ -417,9 +431,11 @@ std::string Provider::UpdatePod(const PodPtr& pod) {
         t.slot = AllocSlot();
         t.pod = std::make_shared<Pod>(*pod);
         slot_key_[t.slot] = Key(pod->ns, pod->name);
+        TrackPending(t.slot, IsPending(*t.pod));
         pods_[Key(pod->ns, pod->name)] = std::move(t);
     } else {
         it->second.pod = std::make_shared<Pod>(*pod);
+        TrackPending(it->second.slot, IsPending(*pod));  // a changed phase or RunPod id
     }
     return "";
 }
@@ -438,6 +454,7 @@ std::string Provider::DeletePod(const PodPtr& pod) {
         const uint32_t s = pt->second.slot;
         std::memset(&records_[(size_t)s * stride_], 0, stride_);
         slot_key_[s].clear();
+        TrackPending(s, false);
         free_slots_.push_back(s);
         pods_.erase(pt);
     }
@@ -532,8 +549,11 @@ bool Provider::RefreshOffersLocked(std::string* err) {
 
 // DeployPodToRunPod for a batch (kubelet.go:435-503 + runpod_client.go:1250-1343): columns from
 // annotations -> the rows that changed since the last tick into the device pod table -> ONE rpk_select_slots over the
-// whole batch -> gpuTypeIds per pod -> DeployPod -> annotations.
-bool Provider::DeployBatch(const std::vector<std::string>& keys) {
+// whole batch -> gpuTypeIds per pod -> DeployPod -> annotations.  The pending tick (marks) sends no list: the pending
+// flags that changed go up ahead of the seed, rpk_select_pending selects over the flagged slots and says which they
+// are, and a row is deployed only if its slot still holds the batch's pod and that pod is still pending -- a pod that
+// CreatePod deployed on its own meanwhile is not deployed twice.
+bool Provider::DeployBatch(const std::vector<std::string>& keys, const PendingMarkList* marks) {
     std::vector<PodPtr> pods;
     std::vector<std::string> live;
     std::vector<uint32_t> slots;
@@ -544,7 +564,7 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys) {
             if (it != pods_.end() && it->second.pod) { pods.push_back(it->second.pod); live.push_back(k); slots.push_back(it->second.slot); }
         }
     }
-    if (pods.empty()) return true;
+    if (pods.empty() && !marks) return true;
     std::string err;
     const uint32_t P = (uint32_t)pods.size();
     PodColumnsSoA cols;
@@ -553,9 +573,21 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys) {
     PrepareColumnsBatch(pods, &cols);
     std::vector<int32_t> best(P), top5((size_t)P * RPK_TOPK);
     std::vector<std::vector<std::string>> gpu_type_ids(P);  // params["gpuTypeIds"], runpod_client.go:1339
+    std::vector<char> selected(P, marks ? 0 : 1);           // the pending tick: the batch rows rpk_select_pending returned
     {   // table refresh, selection and index -> id lookup under ONE lock: another thread's refresh cannot swap the table
         // between the select and the lookup (indices would resolve against a different, possibly shorter, table)
         std::lock_guard<std::mutex> g(engine_mutex_);
+        if (marks) {  // first, and whatever happens below: the flags taken from the queue must reach the device
+            std::vector<uint32_t> ms;
+            std::vector<uint8_t> mv;
+            for (const auto& m : *marks) if (marked_[m.first] != m.second) { ms.push_back(m.first); mv.push_back(m.second); }
+            if (!ms.empty()) {
+                if (rpk_pods_mark_pending(ctx_, (uint32_t)ms.size(), ms.data(), mv.data()) != RPK_OK) return false;
+                for (size_t k = 0; k < ms.size(); ++k) marked_[ms[k]] = mv[k];
+                pending_marks_ += ms.size();
+            }
+        }
+        if (pods.empty()) return true;
         if (!RefreshOffersLocked(&err)) return false;  // "failed to get GPU types": every pod of the batch retries later
         // rows whose columns differ from what the slot holds on the device (a changed pod, or a slot reused by another
         // pod), in ascending slot order; prices compare bit for bit, so a NaN bound is not re-seeded every tick
@@ -587,17 +619,45 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys) {
             }
             pod_seeds_ += changed.size();
         }
-        if (rpk_select_slots(ctx_, P, slots.data(), best.data(), top5.data()) != RPK_OK) return false;
-        ++select_calls_;
+        std::vector<uint32_t> row_of(P);  // batch row -> its row of the select's outputs
+        if (marks) {
+            // the flagged slots are the batch's unless a flag upload failed earlier: room for the batch, and once more
+            // with the number the call reports
+            std::vector<uint32_t> sel(P);
+            uint32_t n = 0;
+            int rc = rpk_select_pending(ctx_, P, sel.data(), &n, best.data(), top5.data());
+            if (rc == RPK_EINVAL && n > P) {
+                sel.resize(n); best.resize(n); top5.resize((size_t)n * RPK_TOPK);
+                rc = rpk_select_pending(ctx_, n, sel.data(), &n, best.data(), top5.data());
+            }
+            if (rc != RPK_OK) return false;
+            if (n > 0) ++select_calls_;
+            std::vector<uint32_t> by_slot(P);  // both sides ascending by slot: one merge
+            for (uint32_t i = 0; i < P; ++i) by_slot[i] = i;
+            std::sort(by_slot.begin(), by_slot.end(), [&](uint32_t a, uint32_t b) { return slots[a] < slots[b]; });
+            for (uint32_t r = 0, k = 0; r < n && k < P; ++r) {
+                while (k < P && slots[by_slot[k]] < sel[r]) ++k;
+                for (; k < P && slots[by_slot[k]] == sel[r]; ++k) { row_of[by_slot[k]] = r; selected[by_slot[k]] = 1; }
+            }
+        } else {
+            if (rpk_select_slots(ctx_, P, slots.data(), best.data(), top5.data()) != RPK_OK) return false;
+            ++select_calls_;
+            for (uint32_t i = 0; i < P; ++i) row_of[i] = i;
+        }
         for (uint32_t i = 0; i < P; ++i)
-            for (int k = 0; k < RPK_TOPK; ++k) {
-                const int32_t g = top5[(size_t)i * RPK_TOPK + k];
+            for (int k = 0; k < RPK_TOPK && selected[i]; ++k) {
+                const int32_t g = top5[(size_t)row_of[i] * RPK_TOPK + k];
                 if (g >= 0 && (size_t)g < offers_.size()) gpu_type_ids[i].push_back(offers_[(size_t)g].ID);
             }
     }
     bool all_ok = true;
     for (uint32_t i = 0; i < P; ++i) {
         const std::vector<std::string>& ids = gpu_type_ids[i];
+        if (marks) {  // the slot was flagged when the tick began; deploy only what is still that pod, still pending
+            std::lock_guard<std::mutex> g(pods_mutex_);
+            auto it = pods_.find(live[i]);
+            if (!selected[i] || it == pods_.end() || it->second.slot != slots[i] || slot_key_[slots[i]] != live[i] || !IsPending(*it->second.pod)) continue;
+        }
         std::string id; double cost = 0;
         if (!api_->DeployPod(*pods[i], ids, cols.req_mem_gb[i], cols.cloud[i] == RPK_CLOUD_COMMUNITY ? "COMMUNITY" : "SECURE", &id, &cost, &err)) { all_ok = false; continue; }
         // updatePodWithRunPodInfo -- kubelet.go:505-562
@@ -609,6 +669,7 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys) {
         char buf[64]; snprintf(buf, sizeof(buf), "%f", cost);
         np->annotations[CostAnnotation] = buf;
         it->second.pod = np;
+        TrackPending(it->second.slot, false);  // deployed: it has a RunPod id now
         it->second.info.ID = id; it->second.info.CostPerHr = cost;
     }
     return all_ok;
@@ -617,19 +678,29 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys) {
 // processPendingPods -- kubelet.go:747-814: every tracked pod that is Pending and has no RunPod id is
 // (re)deployed; after 15 minutes of failures it is marked Failed and pushed through notifyFunc.
 void Provider::ProcessPendingPods() {
+    std::lock_guard<std::mutex> tick_guard(pending_tick_mutex_);
     std::vector<std::string> keys;
+    PendingMarkList marks;  // the slots whose flag changed since the last tick, with the flag they should have now
     {
         std::lock_guard<std::mutex> g(pods_mutex_);
-        for (auto& kv : pods_) {
-            const Pod& p = *kv.second.pod;
-            if (p.status.phase != "Pending") continue;                                  // :753
-            auto a = p.annotations.find(PodIDAnnotation);
-            if (a != p.annotations.end() && !a->second.empty()) continue;              // :769-775
-            keys.push_back(kv.first);
-        }
+        for (auto& kv : pods_)
+            if (IsPending(*kv.second.pod)) keys.push_back(kv.first);
+        std::sort(pending_dirty_.begin(), pending_dirty_.end());
+        pending_dirty_.erase(std::unique(pending_dirty_.begin(), pending_dirty_.end()), pending_dirty_.end());
+        for (uint32_t s : pending_dirty_) marks.emplace_back(s, want_pending_[s]);
+        pending_dirty_.clear();
     }
-    if (keys.empty()) return;
-    DeployBatch(keys);
+    if (keys.empty() && marks.empty()) return;
+    bool marked;
+    DeployBatch(keys, &marks);
+    {   // flags that did not reach the device (the upload failed) stay queued
+        std::lock_guard<std::mutex> g(engine_mutex_);
+        marked = std::all_of(marks.begin(), marks.end(), [&](const std::pair<uint32_t, uint8_t>& m) { return marked_[m.first] == m.second; });
+    }
+    if (!marked) {
+        std::lock_guard<std::mutex> g(pods_mutex_);
+        for (const auto& m : marks) pending_dirty_.push_back(m.first);
+    }
     for (const auto& k : keys) {  // give up after 15 minutes (:786-810)
         PodPtr failed;
         {
@@ -643,6 +714,7 @@ void Provider::ProcessPendingPods() {
             np->status.phase = "Failed"; np->status.reason = "RunPodDeploymentFailed";
             np->status.message = "Failed to deploy pod to RunPod after multiple attempts";
             it->second.pod = np;
+            TrackPending(it->second.slot, false);  // Failed: it leaves the set
             failed = np;
         }
         Notify(failed);
@@ -714,6 +786,7 @@ void Provider::UpdateAllPodStatuses() {
                 np->annotations.erase(PodIDAnnotation); np->annotations.erase(CostAnnotation);
                 np->status = TranslateRunPodStatus(PodNotFound, "RunPod instance was deleted", true);
                 it->second.pod = np;
+                TrackPending(slot, IsPending(*np));
                 it->second.info.ID.clear(); it->second.info.Status = PodExited; it->second.info.StatusMessage = "RunPod instance not found";
                 EncodeStatusRecord(&records_[(size_t)slot * stride_], stride_, it->second.info.Status, it->second.info.PortsExposed);
             }
@@ -762,6 +835,7 @@ void Provider::UpdateAllPodStatuses() {
         auto np = std::make_shared<Pod>(*it->second.pod);
         np->status = view;
         it->second.pod = np;
+        TrackPending(f.slot, IsPending(*np));
         return np;
     };
     std::vector<uint32_t> reseed;

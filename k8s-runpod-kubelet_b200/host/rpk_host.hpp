@@ -5,9 +5,10 @@
 // meaning and error behaviour follow pkg/virtual_kubelet:
 //
 //   Provider::CreatePod/UpdatePod/DeletePod/GetPod/GetPodStatus/GetPods/NotifyPods   kubelet.go:384-731
-//   Provider::ProcessPendingPods     kubelet.go:747-814   (now ONE rpk_select_slots per tick instead of one
+//   Provider::ProcessPendingPods     kubelet.go:747-814   (now ONE rpk_select_pending per tick instead of one
 //                                                           GraphQL fetch + filter + sort per pod; only rows whose
-//                                                           columns changed are seeded into the device pod table)
+//                                                           columns changed are seeded into the device pod table, only
+//                                                           pending flags that changed are marked, and no list goes up)
 //   Provider::UpdateAllPodStatuses   kubelet.go:816-974   (now ONE rpk_status_diff per tick)
 //   PrepareColumns / column producers runpod_client.go:1102-1134, 1181-1191, 1261-1281
 //   CheckPortsExposed                kubelet.go:566-605
@@ -187,6 +188,7 @@ public:
     const InstanceInfo* Info(const std::string& ns, const std::string& name);
     uint64_t SelectCalls() const { return select_calls_; }
     uint64_t PodSeeds() const { return pod_seeds_; }  // pod-table rows re-seeded because a pending pod's columns changed
+    uint64_t PendingMarks() const { return pending_marks_; }  // pending flags uploaded because a slot entered or left the set
     uint64_t StatusCalls() const { return status_calls_; }
     uint64_t OfferUploads() const { return offer_uploads_; }
     uint64_t HostCompares() const { return host_compares_; }  // sweeps' pods compared on the host (status longer than any slot)
@@ -202,7 +204,11 @@ private:
     };
     static std::string Key(const std::string& ns, const std::string& name) { return ns + "-" + name; }  // kubelet.go:386
     bool RefreshOffersLocked(std::string* err);  // engine_mutex_ held
-    bool DeployBatch(const std::vector<std::string>& keys);
+    // marks (the pending tick): flag changes to upload first; the batch is then selected with rpk_select_pending
+    using PendingMarkList = std::vector<std::pair<uint32_t, uint8_t>>;  // (slot, flag), slots strictly ascending
+    bool DeployBatch(const std::vector<std::string>& keys, const PendingMarkList* marks = nullptr);
+    static bool IsPending(const Pod& pod);       // processPendingPods' predicate (kubelet.go:752, :768)
+    void TrackPending(uint32_t slot, bool pending);  // pods_mutex_ held: the slot's wanted flag, queued for the next tick
     void Notify(const PodPtr& pod);
     uint32_t AllocSlot();
     void SeedSlot(uint32_t slot);                // device previous state of ONE slot := records_[slot]
@@ -227,9 +233,13 @@ private:
     std::vector<std::string> slot_key_;
     uint32_t max_pods_;
     PodColumnsSoA seeded_;              // max_pods rows: what the device pod table holds per slot (engine_mutex_)
+    std::vector<uint8_t> want_pending_; // max_pods flags: the slot's pod is Pending without a RunPod id (pods_mutex_)
+    std::vector<uint32_t> pending_dirty_;  // slots whose wanted flag changed since the last tick took them (pods_mutex_)
+    std::vector<uint8_t> marked_;       // max_pods flags: what the device pod table holds per slot (engine_mutex_)
+    std::mutex pending_tick_mutex_;     // one pending tick at a time (held around the others, like sweep_mutex_)
     ProviderOptions opt_;
     double now_ = 0;
-    uint64_t select_calls_ = 0, status_calls_ = 0, offer_uploads_ = 0, pod_seeds_ = 0;
+    uint64_t select_calls_ = 0, status_calls_ = 0, offer_uploads_ = 0, pod_seeds_ = 0, pending_marks_ = 0;
 };
 
 }  // namespace rpkhost

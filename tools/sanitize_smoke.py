@@ -37,6 +37,16 @@ if not ONLY_MULTI:
         best, t5 = eng.select_slots(sl, want_top5=True)
         ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, n_threads=8)
         assert np.array_equal(best, ob) and np.array_equal(t5, ot), n
+    # the pending set: mark, then the select over the list the device builds (k_pod_mark, k_pod_pending: latency path
+    # and pipelined path)
+    for n in (37, 140_000):
+        flags = np.zeros(200_000, np.uint8)
+        flags[np.random.default_rng(n + 1).choice(200_000, n, replace=False)] = 1
+        eng.pods_mark_pending(np.arange(200_000, dtype=np.uint32), flags)
+        sl, best, t5 = eng.select_pending(n, want_top5=True)
+        assert np.array_equal(sl, np.flatnonzero(flags)), n
+        ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, n_threads=8)
+        assert np.array_equal(best, ob) and np.array_equal(t5, ot), n
 for stride in () if ONLY_MULTI else (16, 32, 64):
     tab = oracle.StatusTable(30_000, stride)
     e2 = rpk.Engine(1)
