@@ -249,6 +249,26 @@ func (e *Engine) SelectPending(capacity int, wantTop5 bool) (slots []uint32, bes
 	return slots[:n], best[:n], top5, n, nil
 }
 
+// SelectPendingChanged reselects only the pending slots whose row or offer table changed since the call last reported
+// them, and returns only the rows whose gpuTypeIds list changed (ascending by slot; best is top5[5i]).  The caller keeps
+// a per-slot mirror and applies every row to it.  capacity bounds the outputs; with more slots to reselect the call
+// fails and nReselected says how many there are.
+func (e *Engine) SelectPendingChanged(capacity int) (slots []uint32, best []int32, top5 []int32, nPending, nReselected int, err error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	slots = make([]uint32, capacity+1)
+	best = make([]int32, capacity+1)
+	top5 = make([]int32, (capacity+1)*TopK)
+	var np, nr, nc C.uint32_t
+	rc := C.rpk_select_pending_changed(e.ctx, C.uint32_t(capacity), &np, &nr, (*C.uint32_t)(unsafe.Pointer(&slots[0])), i32p(best), i32p(top5), &nc)
+	nPending, nReselected = int(np), int(nr)
+	if rc != C.RPK_OK {
+		return nil, nil, nil, nPending, nReselected, lastError(e.ctx, rc)
+	}
+	n := int(nc)
+	return slots[:n], best[:n], top5[:n*TopK], nPending, nReselected, nil
+}
+
 // PodsPendingListDevice enqueues the pending list alone on GPU shard: dSlotsOut (device memory, one entry per slot of
 // the pod table) receives the pending slot ids ascending, dN their number.  The caller passes the list and the count
 // it read to the rpk_select_slots_device calls.

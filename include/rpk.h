@@ -31,7 +31,8 @@
  *     stream than the last _device call of its scope first waits for that call, so any streams may be used.  A host
  *     call waits for the last _device call of its scopes before it touches anything, and returns after its own work is
  *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_pods_reset,
- *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending, the _device call
+ *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
+ *     rpk_select_pending_changed, the _device call
  *     rpk_pods_pending_list_device, and rpk_tick with P > 0.  Status scope: rpk_status_diff,
  *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset and
  *     rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
@@ -74,7 +75,7 @@ extern "C" {
 typedef struct rpk_ctx rpk_ctx;
 
 typedef struct rpk_stats {
-    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_pending + rpk_select_device + rpk_select_slots_device */
+    uint64_t select_calls;        /* rpk_select + rpk_select_slots + rpk_select_pending + rpk_select_pending_changed + rpk_select_device + rpk_select_slots_device */
     uint64_t offer_scores;        /* sum of P*G over those calls */
     uint64_t status_calls;
     uint64_t status_records;      /* sum of N */
@@ -137,8 +138,11 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
  *
  * (Re)size the pod table to N slots on every GPU of the ctx and set every row to the columns of a pod with no
  * annotations: req_mem_gb 16 (extractGPUMemory(""), runpod_client.go:1182), vcpu 0, ram 0, max_price 0.5, SECURE.
- * No slot is pending afterwards (rpk_pods_mark_pending).  Independent of rpk_status_reset.  The table is replicated:
- * 22 bytes x N on each GPU (the five columns and the pending flag). */
+ * No slot is pending afterwards (rpk_pods_mark_pending), and every result rpk_select_pending_changed stored is cleared.
+ * Independent of rpk_status_reset.  The table is replicated: 22 bytes x N on each GPU (the five columns and the pending
+ * flag).  rpk_select_pending_changed adds, per slot a GPU owns, 45 bytes of stored results (the columns a result came
+ * from, an offer-table generation and the five list entries), about 36 bytes of device scratch and 28 bytes of pinned
+ * host memory for the rows it returns, all allocated by its first call, so callers that never use it pay nothing. */
 int rpk_pods_reset(rpk_ctx* ctx, uint32_t N);
 /* Row slots[i] := element i of each column.  Columns may be NULL exactly where rpk_select's may, with the same defaults
  * (req_mem_gb is required).  slots must be strictly ascending and < N of the pod table (else RPK_EINVAL, nothing
@@ -173,6 +177,32 @@ int rpk_pods_mark_pending(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
  * no offer table: RPK_ESTATE.  Zero pending: RPK_OK, *n_pending = 0, and what rpk_select_slots does for n_slots == 0.
  * Counts as one select in rpk_stats (offer_scores += n_pending * G).  Select scope, host call. */
 int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t* n_pending, int32_t* best, int32_t* top5);
+/* The pending tick without the rows that did not change.  A row's result depends only on its five columns and the offer
+ * table, and both change rarely, so the library keeps, per slot, the last result this call REPORTED for it, and
+ * reselects and reports only what may have changed.
+ *   - Result of a slot s: R(s) is what rpk_select_slots returns for s now, bit for bit, with its top-5 list (the deploy
+ *     sends the whole list); best is top5[0].
+ *   - Reselected: a pending slot with no reported result, whose five columns differ bit for bit from the ones its
+ *     reported result came from, or whose result predates the last rpk_offers_upload (an upload of an identical table
+ *     included).  No other pending slot is recomputed.  *n_reselected counts them.
+ *   - Reported, ascending by slot: every reselected slot whose R(s) differs from its reported result, or that has none.
+ *     Row i is slots_out[i], best[i], top5[5i, 5i+5); *n_changed <= *n_reselected rows.  Each reported R(s) becomes the
+ *     slot's reported result.  A caller that applies every report to a mirror kept per SLOT holds R(s) for every pending
+ *     slot afterwards.
+ *   - Stored results outlive the pending flag: a slot that leaves the set and comes back with the same columns and offer
+ *     table is not reported again, and a slot reused by another pod needs nothing special (the result depends on the
+ *     columns only).  rpk_pods_reset clears them all; no other call reads or writes them.
+ *   - *n_pending, *n_reselected and *n_changed are always required; with cap > 0 so are slots_out, best and top5
+ *     (capacities cap, cap and 5*cap); else RPK_EINVAL.  No pod table or no offer table: RPK_ESTATE.  Both before
+ *     anything is enqueued.
+ *   - More than cap slots to reselect: RPK_EINVAL with *n_pending and *n_reselected written, nothing else written, no
+ *     stored result changed, nothing counted; retry with cap = *n_reselected.
+ *   - Counts as one select in rpk_stats (offer_scores += n_reselected * G) when it reselects anything; a call that
+ *     reselects nothing counts no select.  Select scope, host call.
+ *   - Multi-GPU ctx: the stored results are sharded by slot range (GPU k owns a contiguous range, its boundaries on
+ *     16-slot units); each GPU reselects and diffs its own slots, and the rows come back in GPU order, ascending. */
+int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, uint32_t* n_reselected, uint32_t* slots_out,
+                               int32_t* best, int32_t* top5, uint32_t* n_changed);
 
 /* Same on device-resident columns of GPU `shard` (index into the ctx's device list), enqueued on `stream`
  * (a cudaStream_t; NULL = the ctx's own stream for that shard; pass cudaStreamLegacy (0x1) for the legacy

@@ -43,6 +43,7 @@ ABI = {
     "rpk_select_slots": (_int, [_p, _u32, _p, _p, _p]),
     "rpk_pods_mark_pending": (_int, [_p, _u32, _p, _p]),
     "rpk_select_pending": (_int, [_p, _u32, _p, _p, _p, _p]),
+    "rpk_select_pending_changed": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
     "rpk_select_device": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_select_device_gather": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _int, _pp, _u32, _p, _p]),
     "rpk_select_device_gather_top5": (_int, [_p, _int, _u32, _p, _p, _p, _p, _p, _int, _pp, _pp, _u32, _p]),

@@ -12,6 +12,10 @@
 //   k_pod_pending   the ascending list of the slots whose flag is set, and their number: what rpk_select_pending selects
 //                   over and rpk_pods_pending_list_device returns.  The list is in range by construction, so no host
 //                   check and no upload stand before the gather.
+//   k_pod_stale     of one GPU's owned slots: the ascending list of the pending slots whose stored result is stale, their
+//                   number and the number of pending slots (rpk_select_pending_changed, before its select)
+//   k_pod_result_diff  over the rows that select returned: store each row's result and write the rows whose list changed,
+//                   ascending, to the host (rpk_select_pending_changed, after its select)
 // The host entry points check every slot against the table's N before its upload.  The device entry points cannot, so
 // an entry outside [0, N) is defined here: the seed skips it, and the gather writes a row with cloud byte kCloudNone,
 // which every select path finishes as "neither cloud" (runpod_client.go:469-475): -1 and five -1.  No caller input
@@ -96,40 +100,56 @@ __device__ __forceinline__ uint32_t count_flags(const uint4& v) {
     return (uint32_t)(__popc(__vcmpne4(v.x, 0u)) + __popc(__vcmpne4(v.y, 0u)) + __popc(__vcmpne4(v.z, 0u)) + __popc(__vcmpne4(v.w, 0u))) >> 3;
 }
 
-__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_pending(PendingArgs a, uint32_t n_units) {
+// The compaction itself, shared by the three kernels that turn 16-item units into an ascending list: k_pod_pending (units
+// of the flag column), k_pod_stale (units of a GPU's owned slots) and k_pod_result_diff (units of the reselected rows).
+// The policy Pol says what a unit holds:
+//   V none()                        a unit past the CTA's share
+//   V load(u)                       pass 1's view of unit u
+//   V reload(u)                     pass 2's view of unit u (the thread that loaded u in pass 1: u - c_lo is the same
+//                                   modulo kPendThreads in both passes, so a policy may hand pass 2 what pass 1 wrote)
+//   Count count1(V)                 pass 1: the unit's kept items in the low 32 bits (anything else above them)
+//   uint32_t count(V), bool keep(V, k), uint32_t id(u, k), emit(i, id)   pass 2: list entry i := id of kept item k of u
+//   set_count(n)                    the list's length (the last CTA in unit order)
+//   cta_total(Count)                the CTA's pass-1 total, once per CTA
+//   last()                          thread 0 of the CTA that finishes last, after every other CTA is done
+template <class Pol>
+__device__ __forceinline__ void compact_units(Pol& p, uint32_t n_units, unsigned long long* tile_state, uint32_t* ticket) {
+    using V = typename Pol::V;
+    using Count = typename Pol::Count;
     constexpr uint32_t kWarps = kPendThreads / 32;
     __shared__ uint32_t s_ids[kPendTile];
-    __shared__ uint32_t s_warp[kWarps];
+    __shared__ Count s_warp[kWarps];
     __shared__ uint32_t s_id, s_excl, s_last;
     const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-    if (tid == 0) s_id = atomicAdd(a.ticket, 1u);
+    if (tid == 0) s_id = atomicAdd(ticket, 1u);
     __syncthreads();
     const uint32_t cid = s_id, n_ctas = gridDim.x;
     const uint32_t c_lo = (uint32_t)((unsigned long long)n_units * cid / n_ctas), c_hi = (uint32_t)((unsigned long long)n_units * (cid + 1) / n_ctas);
     // ---- pass 1: the CTA's count -> its offset among the CTAs ----
-    uint32_t mine = 0;
+    Count mine = 0;
     for (uint32_t u0 = c_lo + tid; u0 < c_hi; u0 += 4 * kPendThreads) {
-        uint4 v[4];
+        V v[4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) {
             const uint32_t u = u0 + (uint32_t)k * kPendThreads;
-            v[k] = u < c_hi ? load_flags(a.flags, u, a.N) : make_uint4(0u, 0u, 0u, 0u);
+            v[k] = u < c_hi ? p.load(u) : p.none();
         }
 #pragma unroll
-        for (int k = 0; k < 4; ++k) mine += count_flags(v[k]);
+        for (int k = 0; k < 4; ++k) mine += p.count1(v[k]);
     }
 #pragma unroll
     for (int d = 16; d >= 1; d >>= 1) mine += __shfl_xor_sync(0xFFFFFFFFu, mine, d);
     if (lane == 0) s_warp[warp] = mine;
     __syncthreads();
     if (warp == 0) {
-        uint32_t total = lane < kWarps ? s_warp[lane] : 0u;
+        Count total = lane < kWarps ? s_warp[lane] : (Count)0;
 #pragma unroll
         for (int d = 16; d >= 1; d >>= 1) total += __shfl_xor_sync(0xFFFFFFFFu, total, d);
-        const uint32_t excl = sum_before(a.tile_state, cid, total, lane);
+        const uint32_t excl = sum_before(tile_state, cid, (uint32_t)total, lane);
         if (lane == 0) {
             s_excl = excl;
-            if (cid == n_ctas - 1) *a.n_out = excl + total;  // the last CTA in slot order owns the count
+            if (cid == n_ctas - 1) p.set_count(excl + (uint32_t)total);  // the last CTA in unit order owns the count
+            p.cta_total(total);
         }
     }
     __syncthreads();
@@ -137,8 +157,8 @@ __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_pendi
     uint32_t at = s_excl;
     for (uint32_t r0 = c_lo; r0 < c_hi; r0 += kPendThreads) {
         const uint32_t u = r0 + tid;
-        const uint4 v = u < c_hi ? load_flags(a.flags, u, a.N) : make_uint4(0u, 0u, 0u, 0u);
-        const uint32_t c = count_flags(v);
+        const V v = u < c_hi ? p.reload(u) : p.none();
+        const uint32_t c = p.count(v);
         uint32_t inc = c;
 #pragma unroll
         for (int d = 1; d < 32; d <<= 1) { const uint32_t n = __shfl_up_sync(0xFFFFFFFFu, inc, d); if ((int)lane >= d) inc += n; }
@@ -146,25 +166,174 @@ __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_pendi
         __syncthreads();
         uint32_t wbase = 0, round = 0;
 #pragma unroll
-        for (uint32_t w = 0; w < kWarps; ++w) { const uint32_t x = s_warp[w]; if (w < warp) wbase += x; round += x; }
+        for (uint32_t w = 0; w < kWarps; ++w) { const uint32_t x = (uint32_t)s_warp[w]; if (w < warp) wbase += x; round += x; }
         uint32_t off = wbase + inc - c;
-        const uint32_t word[4] = {v.x, v.y, v.z, v.w};
 #pragma unroll
         for (uint32_t k = 0; k < kPendUnit; ++k)
-            if ((word[k >> 2] >> ((k & 3u) * 8u)) & 0xFFu) s_ids[off++] = u * kPendUnit + k;
+            if (p.keep(v, k)) s_ids[off++] = p.id(u, k);
         __syncthreads();
-        for (uint32_t i = tid; i < round; i += kPendThreads) a.out[at + i] = s_ids[i];
+        for (uint32_t i = tid; i < round; i += kPendThreads) p.emit(at + i, s_ids[i]);
         at += round;
         __syncthreads();  // the tile and the warp sums are rewritten by the next round
     }
     __threadfence();
     __syncthreads();
-    if (tid == 0) s_last = atomicAdd(a.ticket + 1, 1u) == n_ctas - 1 ? 1u : 0u;
+    if (tid == 0) s_last = atomicAdd(ticket + 1, 1u) == n_ctas - 1 ? 1u : 0u;
     __syncthreads();
     if (!s_last) return;
     // last CTA to finish: every look-back is over -- clean the state for the next call
-    for (uint32_t i = tid; i < n_ctas; i += kPendThreads) a.tile_state[i] = 0ull;
-    if (tid == 0) { a.ticket[0] = 0u; a.ticket[1] = 0u; }
+    for (uint32_t i = tid; i < n_ctas; i += kPendThreads) tile_state[i] = 0ull;
+    if (tid == 0) { ticket[0] = 0u; ticket[1] = 0u; p.last(); }
+}
+
+// k_pod_pending's units: 16 flag bytes, slot 16 u + k in byte k
+struct FlagUnits {
+    using V = uint4;
+    using Count = uint32_t;
+    const PendingArgs& a;
+    __device__ __forceinline__ V none() const { return make_uint4(0u, 0u, 0u, 0u); }
+    __device__ __forceinline__ V load(uint32_t u) const { return load_flags(a.flags, u, a.N); }
+    __device__ __forceinline__ V reload(uint32_t u) const { return load_flags(a.flags, u, a.N); }
+    __device__ __forceinline__ Count count1(const V& v) const { return count_flags(v); }
+    __device__ __forceinline__ uint32_t count(const V& v) const { return count_flags(v); }
+    __device__ __forceinline__ bool keep(const V& v, uint32_t k) const {
+        const uint32_t w = k < 4 ? v.x : k < 8 ? v.y : k < 12 ? v.z : v.w;
+        return (w >> ((k & 3u) * 8u)) & 0xFFu;
+    }
+    __device__ __forceinline__ uint32_t id(uint32_t u, uint32_t k) const { return u * kPendUnit + k; }
+    __device__ __forceinline__ void emit(uint32_t i, uint32_t id) const { a.out[i] = id; }
+    __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
+    __device__ __forceinline__ void cta_total(Count) const {}
+    __device__ __forceinline__ void last() const {}
+};
+
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_pending(PendingArgs a, uint32_t n_units) {
+    FlagUnits p{a};
+    compact_units(p, n_units, a.tile_state, a.ticket);
+}
+
+// ---- pending results (rpk_select_pending_changed) --------------------------------------------------------------
+// bit k of the result: byte k of the 16 bytes of v is non-zero
+__device__ __forceinline__ uint32_t nonzero_bytes16(const uint4& v) {
+    const uint32_t w[4] = {__vcmpne4(v.x, 0u), __vcmpne4(v.y, 0u), __vcmpne4(v.z, 0u), __vcmpne4(v.w, 0u)};
+    uint32_t m = 0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) m |= ((w[q] & 1u) | ((w[q] >> 7) & 2u) | ((w[q] >> 14) & 4u) | ((w[q] >> 21) & 8u)) << (4 * q);
+    return m;
+}
+// bit k: a[k] != b[k], bit for bit, over 16 elements of 4 or 8 bytes (16-byte aligned)
+__device__ __forceinline__ uint32_t differ16(const int32_t* a, const int32_t* b) {
+    uint32_t m = 0;
+#pragma unroll
+    for (int q = 0; q < 4; ++q) {
+        const int4 x = reinterpret_cast<const int4*>(a)[q], y = reinterpret_cast<const int4*>(b)[q];
+        m |= ((uint32_t)(x.x != y.x) | (uint32_t)(x.y != y.y) << 1 | (uint32_t)(x.z != y.z) << 2 | (uint32_t)(x.w != y.w) << 3) << (4 * q);
+    }
+    return m;
+}
+__device__ __forceinline__ uint32_t differ16(const double* a, const double* b) {
+    uint32_t m = 0;
+#pragma unroll
+    for (int q = 0; q < 8; ++q) {
+        const longlong2 x = reinterpret_cast<const longlong2*>(a)[q], y = reinterpret_cast<const longlong2*>(b)[q];
+        m |= ((uint32_t)(x.x != y.x) | (uint32_t)(x.y != y.y) << 1) << (2 * q);
+    }
+    return m;
+}
+__device__ __forceinline__ uint32_t differ16(const uint8_t* a, const uint8_t* b) {
+    const uint4 x = *reinterpret_cast<const uint4*>(a), y = *reinterpret_cast<const uint4*>(b);
+    return nonzero_bytes16(make_uint4(x.x ^ y.x, x.y ^ y.y, x.z ^ y.z, x.w ^ y.w));
+}
+
+// k_pod_stale's units: 16 owned slots.  A slot is kept when it is pending and its stored result is stale: a generation
+// other than the offer table's (0: never reported) or columns that differ from the table row.  Pass 1 leaves the kept
+// bits in mask[u] for pass 2 and counts the pending slots above the kept ones.
+struct StaleUnits {
+    struct V { uint32_t keep, pend; };
+    using Count = unsigned long long;
+    const StaleArgs& a;
+    __device__ __forceinline__ V none() const { return V{0u, 0u}; }
+    __device__ __forceinline__ V load(uint32_t u) const {
+        const uint32_t g = a.u_lo + u, j = u * kPendUnit;  // global unit, first owned index
+        const uint32_t pm = nonzero_bytes16(load_flags(a.flags, g, a.N));
+        uint32_t keep = 0;
+        if (pm) {
+            const uint32_t s = g * kPendUnit;
+            uint32_t gen = 0;
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const uint4 x = reinterpret_cast<const uint4*>(a.r.gen + j)[q];
+                gen |= ((uint32_t)(x.x != a.gen) | (uint32_t)(x.y != a.gen) << 1 | (uint32_t)(x.z != a.gen) << 2 | (uint32_t)(x.w != a.gen) << 3) << (4 * q);
+            }
+            const uint32_t cols = differ16(a.t.mem + s, a.r.mem + j) | differ16(a.t.vcpu + s, a.r.vcpu + j) |
+                                  differ16(a.t.ram + s, a.r.ram + j) | differ16(a.t.max_price + s, a.r.max_price + j) |
+                                  differ16(a.t.cloud + s, a.r.cloud + j);
+            keep = pm & (gen | cols);
+        }
+        a.mask[u] = (uint16_t)keep;
+        return V{keep, (uint32_t)__popc(pm)};
+    }
+    __device__ __forceinline__ V reload(uint32_t u) const { return V{a.mask[u], 0u}; }
+    __device__ __forceinline__ Count count1(const V& v) const { return (Count)v.pend << 32 | (uint32_t)__popc(v.keep); }
+    __device__ __forceinline__ uint32_t count(const V& v) const { return (uint32_t)__popc(v.keep); }
+    __device__ __forceinline__ bool keep(const V& v, uint32_t k) const { return (v.keep >> k) & 1u; }
+    __device__ __forceinline__ uint32_t id(uint32_t u, uint32_t k) const { return (a.u_lo + u) * kPendUnit + k; }
+    __device__ __forceinline__ void emit(uint32_t i, uint32_t id) const { a.out[i] = id; }
+    __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
+    __device__ __forceinline__ void cta_total(Count total) const { atomicAdd(a.ticket + 2, (uint32_t)(total >> 32)); }
+    __device__ __forceinline__ void last() const { *a.n_pending = atomicExch(a.ticket + 2, 0u); }
+};
+
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_stale(StaleArgs a, uint32_t n_units) {
+    StaleUnits p{a};
+    compact_units(p, n_units, a.tile_state, a.ticket);
+}
+
+// k_pod_result_diff's units: 16 reselected rows.  Pass 1 compares each row's new list with the stored one (a slot never
+// reported has none, and differs), stores the row's result -- its list, the columns the gather took it from and the
+// offer-table generation -- and leaves the changed bits in mask[u]; pass 2 writes the changed rows out.
+struct DiffUnits {
+    struct V { uint32_t keep; };
+    using Count = uint32_t;
+    const ResultDiffArgs& a;
+    __device__ __forceinline__ V none() const { return V{0u}; }
+    __device__ __forceinline__ V load(uint32_t u) const {
+        uint32_t keep = 0;
+        for (uint32_t k = 0; k < kPendUnit; ++k) {
+            const uint32_t i = u * kPendUnit + k;
+            if (i >= a.n) break;
+            const uint32_t j = a.list[i] - a.r_lo;
+            const int32_t* nt = a.top5 + (size_t)i * RPK_TOPK;
+            int32_t* ot = a.r.top5 + (size_t)j * RPK_TOPK;
+            bool ch = a.r.gen[j] == 0u;
+#pragma unroll
+            for (int q = 0; q < RPK_TOPK; ++q) { const int32_t x = nt[q]; ch |= ot[q] != x; ot[q] = x; }
+            a.r.mem[j] = a.cols.mem[i]; a.r.vcpu[j] = a.cols.vcpu[i]; a.r.ram[j] = a.cols.ram[i];
+            a.r.max_price[j] = a.cols.max_price[i]; a.r.cloud[j] = a.cols.cloud[i]; a.r.gen[j] = a.gen;
+            keep |= (uint32_t)ch << k;
+        }
+        a.mask[u] = (uint16_t)keep;
+        return V{keep};
+    }
+    __device__ __forceinline__ V reload(uint32_t u) const { return V{a.mask[u]}; }
+    __device__ __forceinline__ Count count1(const V& v) const { return (uint32_t)__popc(v.keep); }
+    __device__ __forceinline__ uint32_t count(const V& v) const { return (uint32_t)__popc(v.keep); }
+    __device__ __forceinline__ bool keep(const V& v, uint32_t k) const { return (v.keep >> k) & 1u; }
+    __device__ __forceinline__ uint32_t id(uint32_t u, uint32_t k) const { return u * kPendUnit + k; }
+    __device__ __forceinline__ void emit(uint32_t i, uint32_t row) const {  // best is the list's first entry
+        const int32_t* t = a.top5 + (size_t)row * RPK_TOPK;
+        a.out_slot[i] = a.list[row]; a.out_best[i] = t[0];
+#pragma unroll
+        for (int q = 0; q < RPK_TOPK; ++q) a.out_top5[(size_t)i * RPK_TOPK + q] = t[q];
+    }
+    __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
+    __device__ __forceinline__ void cta_total(Count) const {}
+    __device__ __forceinline__ void last() const {}
+};
+
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff(ResultDiffArgs a, uint32_t n_units) {
+    DiffUnits p{a};
+    compact_units(p, n_units, a.tile_state, a.ticket);
 }
 
 int launch_pod_fill(const PodRows& t, uint8_t* pending, uint32_t N, int sm_count, cudaStream_t st) {
@@ -199,16 +368,34 @@ int launch_pod_mark(uint8_t* flags, uint32_t N, uint32_t n, const uint32_t* d_sl
 // u64 entries of PendingArgs::tile_state: one per CTA, and launch_pod_pending never launches more CTAs than SMs
 uint32_t pending_state_words(int sm_count) { return (uint32_t)sm_count + 8; }
 
+// one tile per CTA until every SM has its CTA (at most one per SM: the launch fits beside a running select), then
+// longer shares
+static uint32_t compact_grid(uint32_t n_units, int sm_count) {
+    return std::min<uint32_t>((n_units + kPendThreads - 1) / kPendThreads, (uint32_t)sm_count);
+}
+
 int launch_pod_pending(const PendingArgs& a, int sm_count, cudaStream_t st) {
     if (a.N == 0) {
         RPK_CUDA(cudaMemsetAsync(a.n_out, 0, sizeof(uint32_t), st));
         return 0;
     }
     const uint32_t n_units = (a.N + kPendUnit - 1) / kPendUnit;
-    // one tile per CTA until every SM has its CTA (at most one per SM: the launch fits beside a running select), then
-    // longer shares
-    const uint32_t grid = std::min<uint32_t>((n_units + kPendThreads - 1) / kPendThreads, (uint32_t)sm_count);
-    k_pod_pending<<<grid, kPendThreads, 0, st>>>(a, n_units);
+    k_pod_pending<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st) {
+    if (n_units == 0) return 0;
+    k_pod_stale<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st) {
+    if (a.n == 0) return 0;
+    const uint32_t n_units = (a.n + kPendUnit - 1) / kPendUnit;
+    k_pod_result_diff<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

@@ -297,6 +297,31 @@ struct PendingArgs {
 };
 uint32_t pending_state_words(int sm_count);
 int launch_pod_pending(const PendingArgs& a, int sm_count, cudaStream_t st);
+// pending results (rpk_select_pending_changed): per owned slot j (global slot r_lo + j), the last reported result -- its
+// top-5 list, the five columns it was selected from and the offer-table generation it was selected against (0: none)
+struct StoredResults { int32_t* mem; int32_t* vcpu; int32_t* ram; double* max_price; uint8_t* cloud; uint32_t* gen; int32_t* top5; };
+struct StaleArgs {
+    const uint8_t* flags; PodRows t; uint32_t N;  // the pending flags and the pod table (N slots)
+    uint32_t u_lo;                   // first owned 16-slot unit; the owned slots start at 16 u_lo
+    StoredResults r; uint32_t gen;   // stored results of the owned slots, the ctx's offer-table generation
+    uint16_t* mask;                  // [units] scratch: the kept slots of each unit, from pass 1 to pass 2
+    uint32_t* out;                   // the stale slot ids, ascending
+    uint32_t* n_out;                 // their number (mapped host memory)
+    uint32_t* n_pending;             // the owned pending slots (mapped host memory)
+    unsigned long long* tile_state;  // look-back state: pending_state_words entries; zero between calls
+    uint32_t* ticket;                // [3] scheduling ticket, finished CTAs, pending count; zero between calls
+};
+struct ResultDiffArgs {
+    const uint32_t* list; uint32_t n;  // the reselected slots, ascending
+    PodRows cols; const int32_t* top5; // row i: the columns the gather took and the select's top-5 list
+    StoredResults r; uint32_t r_lo, gen;
+    uint16_t* mask;                    // [units] scratch, as StaleArgs::mask
+    uint32_t* out_slot; int32_t* out_best; int32_t* out_top5;  // the changed rows, ascending
+    uint32_t* n_out;                   // their number (mapped host memory)
+    unsigned long long* tile_state; uint32_t* ticket;  // as StaleArgs
+};
+int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
+int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
@@ -414,6 +439,16 @@ struct DeviceState {
     PinnedBuf h_pending;                   // rpk_select_pending: the list's length, written by the kernel
     cudaStream_t pending_stream = nullptr; // rpk_select_pending: the list's copy to the caller, beside the select
     uint32_t podsN = 0; bool pods_sized = false;
+    // pending results (rpk_select_pending_changed), allocated on its first call: the stored results of the owned slots,
+    // the stale list, its rows' best (the select needs a vector), the per-unit masks, the changed rows (r_out:
+    // [slots : cap][best : cap][top5 : 5 cap]) and their host copy behind the counts the kernels write
+    // (h_res: [counts : 64 bytes][the r_out layout]).  res_ready: allocated for this table and not cleared since
+    // (rpk_pods_reset, a failed call)
+    DevBuf<int32_t> r_mem, r_vcpu, r_ram, r_top5, r_best, r_out; DevBuf<double> r_max_price; DevBuf<uint8_t> r_cloud;
+    DevBuf<uint32_t> r_gen, r_list; DevBuf<uint16_t> r_mask;
+    PinnedBuf h_res;
+    bool res_ready = false;
+    StoredResults results() { return StoredResults{r_mem.p, r_vcpu.p, r_ram.p, r_max_price.p, r_cloud.p, r_gen.p, r_top5.p}; }
     PodRows pods_table() { return PodRows{pt_mem.p, pt_vcpu.p, pt_ram.p, pt_max_price.p, pt_cloud.p}; }
     ~DeviceState();
 };

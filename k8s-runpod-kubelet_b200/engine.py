@@ -225,6 +225,26 @@ class Engine:
         k = n.value
         return (slots[:k] if want_slots else None), best[:k], (top5[:k] if want_top5 else None)
 
+    def select_pending_changed(self, cap: int, out_slots=None, out_best=None, out_top5=None):
+        """The pending slots whose result changed since this call last reported them (rpk_select_pending_changed):
+        ``(n_pending, n_reselected, slots[n], best[n], top5[n,5])``, n = the rows reported, ascending by slot.  ``cap``
+        is the capacity of the outputs; more slots to reselect than that raises RPK_EINVAL, and ``n_pending`` and
+        ``n_reselected`` of the exception say how many."""
+        slots = out_slots if out_slots is not None else np.empty(cap, np.uint32)
+        best = out_best if out_best is not None else np.empty(cap, np.int32)
+        top5 = out_top5 if out_top5 is not None else np.empty((cap, 5), np.int32)
+        n_p, n_r, n_c = C.c_uint32(0), C.c_uint32(0), C.c_uint32(0)
+        rc = self._lib.rpk_select_pending_changed(
+            self._ctx, cap, C.cast(C.byref(n_p), C.c_void_p), C.cast(C.byref(n_r), C.c_void_p),
+            _np_ptr(slots, np.uint32, cap, "slots_out"), _np_ptr(best, np.int32, cap, "best"),
+            _np_ptr(top5, np.int32, cap * 5, "top5"), C.cast(C.byref(n_c), C.c_void_p))
+        if rc != 0:
+            err = _ffi.RpkError(rc, (self._lib.rpk_last_error(self._ctx) or b"").decode())
+            err.n_pending, err.n_reselected = n_p.value, n_r.value
+            raise err
+        k = n_c.value
+        return n_p.value, n_r.value, slots[:k], best[:k], top5[:k]
+
     def pods_pending_list_device(self, d_slots_out, d_n, shard: int = 0, stream=None):
         """The pending slot ids, ascending, into ``d_slots_out`` (a torch CUDA tensor with one element per slot of the
         pod table) and their number into ``d_n``, enqueued on ``stream`` (rpk_pods_pending_list_device)."""

@@ -330,6 +330,7 @@ Provider::Provider(std::shared_ptr<RunPodAPI> api, int n_gpus, uint32_t max_pods
     if (rpk_pods_reset(ctx_, max_pods_) != RPK_OK) throw std::runtime_error(rpk_last_error(ctx_));
     seeded_.req_mem_gb.assign(max_pods_, 16); seeded_.req_vcpu.assign(max_pods_, 0); seeded_.req_ram_gb.assign(max_pods_, 0);
     seeded_.max_price.assign(max_pods_, DefaultMaxPrice); seeded_.cloud.assign(max_pods_, RPK_CLOUD_SECURE);
+    lists_.assign((size_t)max_pods_ * RPK_TOPK, -1);
     want_pending_.assign(max_pods_, 0); marked_.assign(max_pods_, 0);  // rpk_pods_reset left no slot pending
     if (opt_.self_tick) {  // go provider.startPeriodicStatusUpdates(); go provider.startPendingPodProcessor() -- kubelet.go:374-376
         StartTicker(opt_.periodic_interval_s, [this] { UpdateAllPodStatuses(); });
@@ -549,10 +550,12 @@ bool Provider::RefreshOffersLocked(std::string* err) {
 
 // DeployPodToRunPod for a batch (kubelet.go:435-503 + runpod_client.go:1250-1343): columns from
 // annotations -> the rows that changed since the last tick into the device pod table -> ONE rpk_select_slots over the
-// whole batch -> gpuTypeIds per pod -> DeployPod -> annotations.  The pending tick (marks) sends no list: the pending
-// flags that changed go up ahead of the seed, rpk_select_pending selects over the flagged slots and says which they
-// are, and a row is deployed only if its slot still holds the batch's pod and that pod is still pending -- a pod that
-// CreatePod deployed on its own meanwhile is not deployed twice.
+// whole batch -> gpuTypeIds per pod -> DeployPod -> annotations.  The pending tick (marks) sends no list and gets back
+// only the lists that changed: the pending flags that changed go up ahead of the seed, rpk_select_pending_changed
+// reselects the flagged slots whose row or offer table changed and reports the lists that differ, which go into the
+// per-slot mirror (lists_); every flagged slot deploys from the mirror.  A row is deployed only if its slot still holds
+// the batch's pod and that pod is still pending -- a pod that CreatePod deployed on its own meanwhile is not deployed
+// twice.
 bool Provider::DeployBatch(const std::vector<std::string>& keys, const PendingMarkList* marks) {
     std::vector<PodPtr> pods;
     std::vector<std::string> live;
@@ -573,7 +576,7 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys, const PendingMa
     PrepareColumnsBatch(pods, &cols);
     std::vector<int32_t> best(P), top5((size_t)P * RPK_TOPK);
     std::vector<std::vector<std::string>> gpu_type_ids(P);  // params["gpuTypeIds"], runpod_client.go:1339
-    std::vector<char> selected(P, marks ? 0 : 1);           // the pending tick: the batch rows rpk_select_pending returned
+    std::vector<char> selected(P, marks ? 0 : 1);           // the pending tick: the batch rows whose slot is flagged
     {   // table refresh, selection and index -> id lookup under ONE lock: another thread's refresh cannot swap the table
         // between the select and the lookup (indices would resolve against a different, possibly shorter, table)
         std::lock_guard<std::mutex> g(engine_mutex_);
@@ -621,23 +624,26 @@ bool Provider::DeployBatch(const std::vector<std::string>& keys, const PendingMa
         }
         std::vector<uint32_t> row_of(P);  // batch row -> its row of the select's outputs
         if (marks) {
-            // the flagged slots are the batch's unless a flag upload failed earlier: room for the batch, and once more
-            // with the number the call reports
-            std::vector<uint32_t> sel(P);
-            uint32_t n = 0;
-            int rc = rpk_select_pending(ctx_, P, sel.data(), &n, best.data(), top5.data());
-            if (rc == RPK_EINVAL && n > P) {
-                sel.resize(n); best.resize(n); top5.resize((size_t)n * RPK_TOPK);
-                rc = rpk_select_pending(ctx_, n, sel.data(), &n, best.data(), top5.data());
+            // the slots to reselect are at most the batch's unless a flag upload failed earlier: room for the batch, and
+            // once more with the number the call reports
+            std::vector<uint32_t> ch(P);
+            uint32_t n_pending = 0, n_reselected = 0, n_changed = 0;
+            int rc = rpk_select_pending_changed(ctx_, P, &n_pending, &n_reselected, ch.data(), best.data(), top5.data(), &n_changed);
+            if (rc == RPK_EINVAL && n_reselected > P) {
+                ch.resize(n_reselected); best.resize(n_reselected); top5.resize((size_t)n_reselected * RPK_TOPK);
+                rc = rpk_select_pending_changed(ctx_, n_reselected, &n_pending, &n_reselected, ch.data(), best.data(), top5.data(), &n_changed);
             }
             if (rc != RPK_OK) return false;
-            if (n > 0) ++select_calls_;
-            std::vector<uint32_t> by_slot(P);  // both sides ascending by slot: one merge
-            for (uint32_t i = 0; i < P; ++i) by_slot[i] = i;
-            std::sort(by_slot.begin(), by_slot.end(), [&](uint32_t a, uint32_t b) { return slots[a] < slots[b]; });
-            for (uint32_t r = 0, k = 0; r < n && k < P; ++r) {
-                while (k < P && slots[by_slot[k]] < sel[r]) ++k;
-                for (; k < P && slots[by_slot[k]] == sel[r]; ++k) { row_of[by_slot[k]] = r; selected[by_slot[k]] = 1; }
+            if (n_pending > 0) ++select_calls_;  // one pending tick, however little of it was recomputed
+            reselected_rows_ += n_reselected; changed_lists_ += n_changed;
+            for (uint32_t k = 0; k < n_changed; ++k)
+                std::copy(&top5[(size_t)k * RPK_TOPK], &top5[(size_t)(k + 1) * RPK_TOPK], &lists_[(size_t)ch[k] * RPK_TOPK]);
+            // every flagged slot holds its current list in the mirror now: the batch rows read it there
+            top5.resize((size_t)P * RPK_TOPK);
+            for (uint32_t i = 0; i < P; ++i) {
+                selected[i] = marked_[slots[i]] != 0;
+                std::copy(&lists_[(size_t)slots[i] * RPK_TOPK], &lists_[(size_t)(slots[i] + 1) * RPK_TOPK], &top5[(size_t)i * RPK_TOPK]);
+                row_of[i] = i;
             }
         } else {
             if (rpk_select_slots(ctx_, P, slots.data(), best.data(), top5.data()) != RPK_OK) return false;

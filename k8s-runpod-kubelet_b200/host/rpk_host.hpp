@@ -5,7 +5,7 @@
 // meaning and error behaviour follow pkg/virtual_kubelet:
 //
 //   Provider::CreatePod/UpdatePod/DeletePod/GetPod/GetPodStatus/GetPods/NotifyPods   kubelet.go:384-731
-//   Provider::ProcessPendingPods     kubelet.go:747-814   (now ONE rpk_select_pending per tick instead of one
+//   Provider::ProcessPendingPods     kubelet.go:747-814   (now ONE rpk_select_pending_changed per tick instead of one
 //                                                           GraphQL fetch + filter + sort per pod; only rows whose
 //                                                           columns changed are seeded into the device pod table, only
 //                                                           pending flags that changed are marked, and no list goes up)
@@ -189,6 +189,8 @@ public:
     uint64_t SelectCalls() const { return select_calls_; }
     uint64_t PodSeeds() const { return pod_seeds_; }  // pod-table rows re-seeded because a pending pod's columns changed
     uint64_t PendingMarks() const { return pending_marks_; }  // pending flags uploaded because a slot entered or left the set
+    uint64_t ReselectedRows() const { return reselected_rows_; }  // pending rows the ticks recomputed (row or offers changed)
+    uint64_t ChangedLists() const { return changed_lists_; }      // gpuTypeIds lists the ticks got back because they changed
     uint64_t StatusCalls() const { return status_calls_; }
     uint64_t OfferUploads() const { return offer_uploads_; }
     uint64_t HostCompares() const { return host_compares_; }  // sweeps' pods compared on the host (status longer than any slot)
@@ -204,7 +206,8 @@ private:
     };
     static std::string Key(const std::string& ns, const std::string& name) { return ns + "-" + name; }  // kubelet.go:386
     bool RefreshOffersLocked(std::string* err);  // engine_mutex_ held
-    // marks (the pending tick): flag changes to upload first; the batch is then selected with rpk_select_pending
+    // marks (the pending tick): flag changes to upload first; the batch then deploys from the mirror of top-5 lists that
+    // rpk_select_pending_changed keeps current
     using PendingMarkList = std::vector<std::pair<uint32_t, uint8_t>>;  // (slot, flag), slots strictly ascending
     bool DeployBatch(const std::vector<std::string>& keys, const PendingMarkList* marks = nullptr);
     static bool IsPending(const Pod& pod);       // processPendingPods' predicate (kubelet.go:752, :768)
@@ -236,10 +239,13 @@ private:
     std::vector<uint8_t> want_pending_; // max_pods flags: the slot's pod is Pending without a RunPod id (pods_mutex_)
     std::vector<uint32_t> pending_dirty_;  // slots whose wanted flag changed since the last tick took them (pods_mutex_)
     std::vector<uint8_t> marked_;       // max_pods flags: what the device pod table holds per slot (engine_mutex_)
+    std::vector<int32_t> lists_;        // max_pods x 5 offer indices: the last list rpk_select_pending_changed reported per
+                                        // slot (engine_mutex_); resolved to ids against offers_ at deploy time
     std::mutex pending_tick_mutex_;     // one pending tick at a time (held around the others, like sweep_mutex_)
     ProviderOptions opt_;
     double now_ = 0;
     uint64_t select_calls_ = 0, status_calls_ = 0, offer_uploads_ = 0, pod_seeds_ = 0, pending_marks_ = 0;
+    uint64_t reselected_rows_ = 0, changed_lists_ = 0;
 };
 
 }  // namespace rpkhost

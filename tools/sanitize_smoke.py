@@ -47,6 +47,15 @@ if not ONLY_MULTI:
         assert np.array_equal(sl, np.flatnonzero(flags)), n
         ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, n_threads=8)
         assert np.array_equal(best, ob) and np.array_equal(t5, ot), n
+    # the pending results (k_pod_stale, k_pod_result_diff): a first call reports every pending slot, a steady call
+    # nothing, a call after an offer upload reselects every pending slot
+    pend = np.flatnonzero(flags)
+    n_p, n_r, sl, best, t5 = eng.select_pending_changed(len(pend))
+    assert n_r == len(pend) and np.array_equal(sl, pend)
+    assert eng.select_pending_changed(len(pend))[1] == 0
+    eng.upload_offers(offers)
+    n_p, n_r, sl, _, _ = eng.select_pending_changed(len(pend))
+    assert n_r == len(pend) and len(sl) == 0
 for stride in () if ONLY_MULTI else (16, 32, 64):
     tab = oracle.StatusTable(30_000, stride)
     e2 = rpk.Engine(1)
