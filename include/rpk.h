@@ -95,7 +95,10 @@ typedef struct rpk_stats {
 /* n_gpus in [1, RPK_MAX_GPUS]; device_ids == NULL means 0..n_gpus-1.  With n_gpus > 1 (one host process
  * driving a whole box, the shape a Go kubelet has) pod rows / status slots are split into contiguous
  * shards, one per GPU, and every GPU writes its shard of the assignment vector straight into all peers'
- * copies over NVLink (peer access is enabled here). */
+ * copies over NVLink (peer access is enabled here).  A device id may appear once.
+ * Test only: with RPK_TEST_SHARED_DEVICE=1 in the environment (read here, once per ctx, and nowhere else) a repeated
+ * device id is accepted and shards on the same GPU are not enabled as each other's peers, so a one-GPU machine can run
+ * an n-shard ctx.  Do not queue rpk_peer_fence, or a bound gather that waits, between shards that share a GPU. */
 int rpk_create(int n_gpus, const int* device_ids, rpk_ctx** out);
 void rpk_destroy(rpk_ctx* ctx);
 /* ctx-owned string, valid until the next call on that ctx; ctx == NULL returns the last rpk_create error

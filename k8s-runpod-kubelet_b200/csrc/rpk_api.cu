@@ -708,11 +708,16 @@ int rpk_create(int n_gpus, const int* device_ids, rpk_ctx** out) {
     rpk_ctx* ctx = nullptr;
     try { ctx = new rpk_ctx(n_gpus); } catch (const std::bad_alloc&) { return fail(nullptr, RPK_ENOMEM, "rpk_create: host allocation failed"); }
     memset(&ctx->stats, 0, sizeof(ctx->stats));
+    // test hook (several shards of one ctx on one GPU, so that a one-GPU machine runs the sharded host paths): consulted
+    // once per ctx, here, and never on a select or sweep path.  Shards that share a device already address each other's
+    // memory, so they are neither refused as duplicates nor enabled as peers.
+    const char* shared_env = getenv("RPK_TEST_SHARED_DEVICE");
+    const bool shared_device = shared_env && !strcmp(shared_env, "1");
     int rc = guarded(nullptr, [&]() -> int {
         for (int i = 0; i < n_gpus; ++i) {
             const int dev = device_ids ? device_ids[i] : i;
             if (dev < 0 || dev >= count) return fail(nullptr, RPK_EINVAL, "rpk_create: device id out of range");
-            for (int j = 0; j < i; ++j) if (ctx->devs[(size_t)j].dev == dev) return fail(nullptr, RPK_EINVAL, "rpk_create: duplicate device id");
+            for (int j = 0; j < i && !shared_device; ++j) if (ctx->devs[(size_t)j].dev == dev) return fail(nullptr, RPK_EINVAL, "rpk_create: duplicate device id");
             cudaDeviceProp prop;
             RPK_CUDA(cudaGetDeviceProperties(&prop, dev));
             if (prop.major != 9 || prop.minor != 0) {
@@ -741,7 +746,7 @@ int rpk_create(int n_gpus, const int* device_ids, rpk_ctx** out) {
         for (int i = 0; i < n_gpus && n_gpus > 1; ++i) {
             RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)i].dev));
             for (int j = 0; j < n_gpus; ++j) {
-                if (i == j) continue;
+                if (ctx->devs[(size_t)i].dev == ctx->devs[(size_t)j].dev) continue;  // itself, or a shard on the same GPU
                 int can = 0;
                 RPK_CUDA(cudaDeviceCanAccessPeer(&can, ctx->devs[(size_t)i].dev, ctx->devs[(size_t)j].dev));
                 if (!can) return fail(nullptr, RPK_ENODEV, "rpk_create: GPUs of the ctx cannot access each other (NVLink/P2P required for n_gpus > 1)");
