@@ -134,15 +134,16 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
     *hi = (uint32_t)((uint64_t)total * (uint64_t)(s + 1) / (uint64_t)n);
 }
 
-// Where the rows of a select come from: the caller's columns (rpk_select, rpk_tick: host memory; rpk_select_device*:
-// device memory), or rows of the pod table (rpk_select_slots: a host list, each sub-batch uploads its slot ids and
-// gathers the five columns on the device; rpk_select_slots_device*: a device list, gathered in one pass;
-// rpk_select_pending: the list k_pod_pending left on every GPU, in range by construction, so a sub-batch has nothing to
-// check or upload and gathers from its part of the list in place).
-struct PodSource {
-    PodCols cols;
-    const uint32_t* slots;  // non-null: row i of the call is pod-table row slots[i]; cols is unused
-    bool pending = false;   // row i of the call is pod-table row pt_list[i] of the GPU that selects it; the rest is unused
+bool bad_shard(const rpk_ctx* ctx, int shard) { return shard < 0 || (size_t)shard >= ctx->devs.size(); }
+
+// Where the rows of a select come from.  Host sources (rpk_select, rpk_tick: columns; rpk_select_slots: a list) become
+// device sources by their upload.  Device sources are on the selecting GPU (rpk_select_device*: columns;
+// rpk_select_slots_device*: a list; rpk_select_pending*: the list k_pod_pending or k_pod_stale left there).
+struct RowSource {
+    enum Kind { HostCols, HostList, DevCols, DevList };
+    Kind kind;
+    PodCols cols;           // HostCols, DevCols: row i of the call is row i of the columns (the optional ones nullable)
+    const uint32_t* slots;  // HostList, DevList: row i of the call is pod-table row slots[i]
 };
 
 // every entry of slots[0, n) is a row of a pod table of N rows.  The pipelined select runs this per sub-batch on the
@@ -159,12 +160,33 @@ bool slots_below(const uint32_t* slots, uint32_t n, uint32_t N) {
     return bad == 0;
 }
 
-// The gather of n pod-table rows whose slot ids are at d_slots (device) into lane ln's pod columns, on st; a's pod columns
-// then point at them.  Returns the kernels launched.
-int gather_pod_rows(DeviceState& ds, DeviceState::Lane& ln, uint32_t n, const uint32_t* d_slots, SelectArgs& a, cudaStream_t st) {
+// The buffers of lane ln that a select of `rows` rows from src writes: the pod columns it uploads or gathers, a host list's
+// slot ids, the top-5 lists.  Allocates only when one grows, so a device call stays capturable after a call of its size.
+void reserve_lane(DeviceState::Lane& ln, size_t rows, const RowSource& src, bool top5) {
+    if (src.kind != RowSource::DevCols) {
+        const bool all = src.kind != RowSource::HostCols;  // a list's gather writes all five
+        ln.p_req_mem.reserve(rows);
+        if (all || src.cols.req_vcpu) ln.p_req_vcpu.reserve(rows);
+        if (all || src.cols.req_ram) ln.p_req_ram.reserve(rows);
+        if (all || src.cols.max_price) ln.p_max_price.reserve(rows);
+        if (all || src.cols.cloud) ln.p_cloud.reserve(rows);
+    }
+    if (src.kind == RowSource::HostList) ln.p_slots.reserve(rows);
+    if (top5) ln.top5.reserve(rows * RPK_TOPK);
+}
+
+// a's pod columns: rows [b0, b0 + n) of the device source src.  Columns go in as pointers; a list is gathered from the
+// pod table into lane ln's columns on st.  Returns the kernels launched.
+int pod_columns(DeviceState& ds, DeviceState::Lane& ln, const RowSource& src, uint32_t b0, uint32_t n, SelectArgs& a, cudaStream_t st) {
+    if (src.kind == RowSource::DevCols) {
+        const PodCols& c = src.cols;
+        auto at = [b0](auto* col) { return col ? col + b0 : nullptr; };  // null stays null
+        a.req_mem = at(c.req_mem); a.req_vcpu = at(c.req_vcpu); a.req_ram = at(c.req_ram); a.max_price = at(c.max_price); a.cloud = at(c.cloud);
+        return 0;
+    }
     const PodRows out{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
     a.req_mem = out.mem; a.req_vcpu = out.vcpu; a.req_ram = out.ram; a.max_price = out.max_price; a.cloud = out.cloud;
-    return launch_pod_gather(ds.pods_table(), ds.podsN, n, d_slots, out, st);
+    return launch_pod_gather(ds.pods_table(), ds.podsN, n, src.slots + b0, out, st);
 }
 
 // One select on ds in lane ln's scratch: `a` holds the pod columns, P and the outputs; this adds the offer views and the
@@ -259,34 +281,30 @@ int find_local_vector(const rpk_ctx* ctx, int shard, int dev, int n_out, int32_t
 // is about as long as the upload of the next, larger sub-batch.
 constexpr uint32_t kSubBatchRows = 131072;
 constexpr uint32_t kSubBatchMaxMul = 4;
-inline uint32_t sub_batch_rows(int j, uint32_t remaining) {
+// The pending list (a device list in a host call) needs no upload for the sub-batches to hide, but they still overlap
+// the copies of best and top5 back to the host: measured at 1M rows on an H100 (700 W), the sub-batches take 0.97 ms
+// against 1.02 ms for one select over the whole list with top-5, which the Provider's tick asks for, and 0.55 against
+// 0.52 ms without, each inside the other's spread (DESIGN section 4, "Pending set"): the list keeps the pipeline's shape.
+// RPK_MEASURE_PENDING_ONE_SELECT: only for the copy of the library tools/select_pending_probe.py builds to time the other
+// shape.
+inline uint32_t sub_batch_rows(RowSource::Kind kind, int j, uint32_t remaining) {
+#ifdef RPK_MEASURE_PENDING_ONE_SELECT
+    if (kind == RowSource::DevList) return remaining;
+#endif
+    (void)kind;
     const uint32_t want = kSubBatchRows * (uint32_t)((j + 1) < (int)kSubBatchMaxMul ? (j + 1) : (int)kSubBatchMaxMul);
     return remaining < want + kSubBatchRows / 2 ? remaining : want;  // do not leave a sliver behind
 }
-// ... of a call whose rows come from src.  The pending list needs no upload for the sub-batches to hide, but they still
-// overlap the copies of best and top5 back to the host: measured at 1M rows on an H100 (700 W), the sub-batches take
-// 0.97 ms against 1.02 ms for one select over the whole list with top-5, which the Provider's tick asks for, and 0.55
-// against 0.52 ms without, each inside the other's spread (DESIGN section 4, "Pending set"): the list keeps the
-// pipeline's shape.
-// RPK_MEASURE_PENDING_ONE_SELECT: only for the copy of the library tools/select_pending_probe.py builds to time the other
-// shape.
-inline uint32_t sub_batch_rows(const PodSource& src, int j, uint32_t remaining) {
-#ifdef RPK_MEASURE_PENDING_ONE_SELECT
-    if (src.pending) return remaining;
-#endif
-    (void)src;
-    return sub_batch_rows(j, remaining);
-}
-inline uint32_t sub_batch_cap(const PodSource& src, uint32_t Ps) {  // largest sub-batch a shard of Ps rows produces
+inline uint32_t sub_batch_cap(RowSource::Kind kind, uint32_t Ps) {  // largest sub-batch a shard of Ps rows produces
     uint32_t cap = 0, left = Ps;
-    for (int j = 0; left; ++j) { const uint32_t nb = sub_batch_rows(src, j, left); cap = nb > cap ? nb : cap; left -= nb; }
+    for (int j = 0; left; ++j) { const uint32_t nb = sub_batch_rows(kind, j, left); cap = nb > cap ? nb : cap; left -= nb; }
     return cap ? cap : 1;
 }
 
 // Latency path of the host entry point (micro-batches, one GPU): the five pod columns -- or, from the pod table, the
 // slot ids -- are packed into one pinned block -> ONE H2D (then the gather, for slots); best and top5 come back in ONE
 // D2H; one stream synchronise.  Same kernels.  Slot ids are in range here.  Returns the kernels launched.
-int select_small(DeviceState& ds, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5) {
+int select_small(DeviceState& ds, uint32_t P, const RowSource& src, int32_t* best, int32_t* top5) {
     RPK_CUDA(cudaSetDevice(ds.dev));
     ds.sel_scope.host_wait();
     const size_t in_cap = (size_t)kSmallBatch * 24, out_cap = (size_t)kSmallBatch * 6 * 4;
@@ -296,30 +314,30 @@ int select_small(DeviceState& ds, uint32_t P, const PodSource& src, int32_t* bes
     DeviceState::Lane& ln = ds.lane[0];
     cudaStream_t st = ln.stream;
     unsigned char* d = ds.d_small_in.p;
-    SelectArgs a{};
-    int launches = 0;
-    if (src.slots || src.pending) {
-        ln.p_req_mem.reserve(kSmallBatch); ln.p_req_vcpu.reserve(kSmallBatch); ln.p_req_ram.reserve(kSmallBatch);
-        ln.p_max_price.reserve(kSmallBatch); ln.p_cloud.reserve(kSmallBatch);
-        if (src.slots) {
-            memcpy(h, src.slots, (size_t)P * 4);
-            RPK_CUDA(cudaMemcpyAsync(d, h, (size_t)P * 4, cudaMemcpyHostToDevice, st));
-        }
-        launches += gather_pod_rows(ds, ln, P, src.slots ? (const uint32_t*)d : ds.pt_list.p, a, st);
-    } else {
+    RowSource dev = src;  // the rows' device source: the block's columns or slot ids in d_small_in, or the pending list
+    size_t bytes = 0;
+    if (src.kind == RowSource::HostList) {
+        bytes = (size_t)P * 4;
+        memcpy(h, src.slots, bytes);
+        dev = RowSource{RowSource::DevList, PodCols{}, (const uint32_t*)d};
+    } else if (src.kind == RowSource::HostCols) {
         const PodCols& pods = src.cols;
         const size_t o_mem = 0, o_vcpu = (size_t)P * 4, o_ram = (size_t)P * 8, o_price = ((size_t)P * 12 + 7) & ~(size_t)7,
-                     o_cloud = o_price + (size_t)P * 8, total = o_cloud + P;
-        memcpy(h + o_mem, pods.req_mem, (size_t)P * 4);
-        if (pods.req_vcpu) memcpy(h + o_vcpu, pods.req_vcpu, (size_t)P * 4);
-        if (pods.req_ram) memcpy(h + o_ram, pods.req_ram, (size_t)P * 4);
-        if (pods.max_price) memcpy(h + o_price, pods.max_price, (size_t)P * 8);
-        if (pods.cloud) memcpy(h + o_cloud, pods.cloud, P);
-        RPK_CUDA(cudaMemcpyAsync(d, h, total, cudaMemcpyHostToDevice, st));
-        a.req_mem = (const int32_t*)(d + o_mem); a.req_vcpu = pods.req_vcpu ? (const int32_t*)(d + o_vcpu) : nullptr;
-        a.req_ram = pods.req_ram ? (const int32_t*)(d + o_ram) : nullptr; a.max_price = pods.max_price ? (const double*)(d + o_price) : nullptr;
-        a.cloud = pods.cloud ? (const uint8_t*)(d + o_cloud) : nullptr;
+                     o_cloud = o_price + (size_t)P * 8;
+        bytes = o_cloud + P;
+        // a column into the block at offset o; null stays null
+        auto pack = [&](const auto* col, size_t o) -> decltype(col) {
+            if (!col) return nullptr;
+            memcpy(h + o, col, (size_t)P * sizeof(*col));
+            return (decltype(col))(d + o);
+        };
+        dev = RowSource{RowSource::DevCols, PodCols{pack(pods.req_mem, o_mem), pack(pods.req_vcpu, o_vcpu), pack(pods.req_ram, o_ram),
+                                                    pack(pods.max_price, o_price), pack(pods.cloud, o_cloud)}, nullptr};
     }
+    reserve_lane(ln, kSmallBatch, dev, false);
+    if (bytes) RPK_CUDA(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
+    SelectArgs a{};
+    int launches = pod_columns(ds, ln, dev, 0, P, a, st);
     a.P = P;
     a.best_out[0] = ds.d_small_out.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = top5 ? ds.d_small_out.p + P : nullptr;
     launches += enqueue_select(ds, ln, a, st);
@@ -338,38 +356,23 @@ bool has_int32_max(const int32_t* col, uint32_t n) {
 }
 
 
+// The pipelined host select of a run_host call: P rows from src[s] on GPU s into the caller's best and top5 (nullable)
+struct HostSelect { uint32_t P; std::vector<RowSource> src; int32_t* best; int32_t* top5; };
+
 // Buffers of the pipelined host select, sized from the calling thread (peers write into each other's best_full, so
-// every GPU's vector must exist before any shard is enqueued).  After the first call of a size this only compares
-// capacities.
-void reserve_select(rpk_ctx* ctx, uint32_t P, const PodSource& src, bool top5) {
+// every GPU's vector must exist before any shard is enqueued).  After the first call of a size this allocates nothing.
+void reserve_select(rpk_ctx* ctx, const HostSelect& sel) {
     const int n = (int)ctx->devs.size();
-    const PodCols& pods = src.cols;
-    const bool all = src.slots || src.pending;  // the gather writes all five columns
-    const bool vcpu = all || pods.req_vcpu, ram = all || pods.req_ram, price = all || pods.max_price, cloud = all || pods.cloud;
     for (int s = 0; s < n; ++s) {
         DeviceState& ds = ctx->devs[(size_t)s];
-        uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
+        uint32_t lo, hi; shard_range(sel.P, n, s, &lo, &hi);
         const uint32_t Ps = hi - lo;
-        const uint32_t cap = sub_batch_cap(src, Ps);
-        bool grow = P > ds.best_full.cap;
-        for (auto& ln : ds.lane) {
-            grow = grow || cap > ln.p_req_mem.cap || (vcpu && cap > ln.p_req_vcpu.cap) || (ram && cap > ln.p_req_ram.cap) ||
-                   (price && cap > ln.p_max_price.cap) || (cloud && cap > ln.p_cloud.cap) || (src.slots && cap > ln.p_slots.cap) ||
-                   (top5 && (size_t)cap * RPK_TOPK > ln.top5.cap);
-            if (cap == Ps) break;  // a single sub-batch uses lane 0 only
-        }
-        if (!grow) continue;
+        const uint32_t cap = sub_batch_cap(sel.src[(size_t)s].kind, Ps);
         RPK_CUDA(cudaSetDevice(ds.dev));
-        ds.best_full.reserve(P);
+        ds.best_full.reserve(sel.P);
         for (auto& ln : ds.lane) {
-            ln.p_req_mem.reserve(cap);
-            if (vcpu) ln.p_req_vcpu.reserve(cap);
-            if (ram) ln.p_req_ram.reserve(cap);
-            if (price) ln.p_max_price.reserve(cap);
-            if (cloud) ln.p_cloud.reserve(cap);
-            if (src.slots) ln.p_slots.reserve(cap);
-            if (top5) ln.top5.reserve((size_t)cap * RPK_TOPK);
-            if (cap == Ps) break;
+            reserve_lane(ln, cap, sel.src[(size_t)s], sel.top5 != nullptr);
+            if (cap == Ps) break;  // a single sub-batch uses lane 0 only
         }
     }
 }
@@ -378,27 +381,26 @@ void reserve_select(rpk_ctx* ctx, uint32_t P, const PodSource& src, bool top5) {
 // ordered (H2D -> kernels -> D2H), across lanes copies and kernels overlap.  ds.ev[0] / ds.ev[3] bracket it on ds.stream;
 // the caller synchronises ds.stream.  Slot ids are checked per sub-batch just before their upload: false = an entry
 // outside the pod table, and nothing from that sub-batch on was enqueued (the lanes still drain into ds.stream).
-bool enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5, uint64_t* launches) {
+bool enqueue_select_shard(rpk_ctx* ctx, int s, const HostSelect& sel, uint64_t* launches) {
     const int n = (int)ctx->devs.size();
     DeviceState& ds = ctx->devs[(size_t)s];
-    uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
+    const RowSource& src = sel.src[(size_t)s];
+    uint32_t lo, hi; shard_range(sel.P, n, s, &lo, &hi);
     RPK_CUDA(cudaSetDevice(ds.dev));
     RPK_CUDA(cudaEventRecord(ds.ev[0], ds.stream));
     for (auto& ln : ds.lane) RPK_CUDA(cudaStreamWaitEvent(ln.stream, ds.ev[0], 0));
     bool ok = true;
     int j = 0;
     for (uint32_t b0 = lo, nb = 0; b0 < hi; b0 += nb, ++j) {
-        nb = sub_batch_rows(src, j, hi - b0);
+        nb = sub_batch_rows(src.kind, j, hi - b0);
         DeviceState::Lane& ln = ds.lane[j % DeviceState::kLanes];
         cudaStream_t st = ln.stream;
-        SelectArgs a{};
-        if (src.pending) {
-            *launches += (uint64_t)gather_pod_rows(ds, ln, nb, ds.pt_list.p + b0, a, st);
-        } else if (src.slots) {
+        RowSource dev = src; uint32_t at = b0;  // the sub-batch's device source and first row: a host source lands in the lane
+        if (src.kind == RowSource::HostList) {
             if (!slots_below(src.slots + b0, nb, ds.podsN)) { ok = false; break; }
             RPK_CUDA(cudaMemcpyAsync(ln.p_slots.p, src.slots + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
-            *launches += (uint64_t)gather_pod_rows(ds, ln, nb, ln.p_slots.p, a, st);
-        } else {
+            dev = RowSource{RowSource::DevList, PodCols{}, ln.p_slots.p}; at = 0;
+        } else if (src.kind == RowSource::HostCols) {
             const PodCols& pods = src.cols;
             // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
             auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
@@ -406,17 +408,19 @@ bool enqueue_select_shard(rpk_ctx* ctx, int s, uint32_t P, const PodSource& src,
                 RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
                 return buf.p;
             };
-            a.req_mem = upload(ln.p_req_mem, pods.req_mem); a.req_vcpu = upload(ln.p_req_vcpu, pods.req_vcpu);
-            a.req_ram = upload(ln.p_req_ram, pods.req_ram); a.max_price = upload(ln.p_max_price, pods.max_price);
-            a.cloud = upload(ln.p_cloud, pods.cloud);
+            dev = RowSource{RowSource::DevCols,
+                            PodCols{upload(ln.p_req_mem, pods.req_mem), upload(ln.p_req_vcpu, pods.req_vcpu), upload(ln.p_req_ram, pods.req_ram),
+                                    upload(ln.p_max_price, pods.max_price), upload(ln.p_cloud, pods.cloud)}, nullptr}; at = 0;
         }
+        SelectArgs a{};
+        *launches += (uint64_t)pod_columns(ds, ln, dev, at, nb, a, st);
         a.P = nb;
         for (int o = 0; o < n; ++o) a.best_out[o] = ctx->devs[(size_t)o].best_full.p;
-        a.n_out = n; a.row0 = b0; a.top5 = top5 ? ln.top5.p : nullptr;
+        a.n_out = n; a.row0 = b0; a.top5 = sel.top5 ? ln.top5.p : nullptr;
         a.self_out = s;  // own vector; finished push blocks / sub-batches are forwarded to the peers
         *launches += (uint64_t)enqueue_select(ds, ln, a, st);
-        RPK_CUDA(cudaMemcpyAsync(best + b0, ds.best_full.p + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, st));
-        if (top5) RPK_CUDA(cudaMemcpyAsync(top5 + (size_t)b0 * RPK_TOPK, ln.top5.p, (size_t)nb * RPK_TOPK * 4, cudaMemcpyDeviceToHost, st));
+        RPK_CUDA(cudaMemcpyAsync(sel.best + b0, ds.best_full.p + b0, (size_t)nb * 4, cudaMemcpyDeviceToHost, st));
+        if (sel.top5) RPK_CUDA(cudaMemcpyAsync(sel.top5 + (size_t)b0 * RPK_TOPK, ln.top5.p, (size_t)nb * RPK_TOPK * 4, cudaMemcpyDeviceToHost, st));
     }
     for (auto& ln : ds.lane) {
         RPK_CUDA(cudaEventRecord(ln.done, ln.stream));
@@ -530,9 +534,6 @@ uint32_t collect_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, uint
     return cnt;
 }
 
-// The pipelined host select of a run_host call: P rows from src into the caller's best and top5 (nullable)
-struct HostSelect { uint32_t P; PodSource src; int32_t* best; int32_t* top5; };
-
 // The host calls' shard loop, once their arguments are checked: the pipelined host select (sel), a host sweep (h), or
 // both in a tick (tick: the sweep runs on status_stream beside the select, and no timing is reported, since both halves
 // record ds.ev).  Every shard first waits for the last device call in the scopes it uses; then the calling thread sizes
@@ -544,7 +545,7 @@ bool run_host(rpk_ctx* ctx, const HostSelect* sel, const StatusHostArgs* h, bool
         if (sel) ds.sel_scope.host_wait();
         if (h) ds.status_scope.host_wait();
     }
-    if (sel) reserve_select(ctx, sel->P, sel->src, sel->top5 != nullptr);
+    if (sel) reserve_select(ctx, *sel);
     if (h) for (int s = 0; s < n; ++s) reserve_status_shard(ctx, s, *h);
     std::vector<uint64_t> launches((size_t)n, 0);
     std::vector<float> km((size_t)n, 0.f), tm((size_t)n, 0.f);
@@ -555,7 +556,7 @@ bool run_host(rpk_ctx* ctx, const HostSelect* sel, const StatusHostArgs* h, bool
         // the selection goes first: its kernels are the long pole and start after the first 128k-row sub-batch has
         // landed; in a tick the sweep's records follow on the status stream, concurrent with the lanes, and its kernel
         // runs under the selection's tail
-        if (sel) shard_ok[(size_t)s] = enqueue_select_shard(ctx, s, sel->P, sel->src, sel->best, sel->top5, &launches[(size_t)s]);
+        if (sel) shard_ok[(size_t)s] = enqueue_select_shard(ctx, s, *sel, &launches[(size_t)s]);
         if (h) enqueue_status_shard(ctx, s, *h, sweep, &launches[(size_t)s]);
         if (h) RPK_CUDA(cudaStreamSynchronize(sweep));
         if (sel) RPK_CUDA(cudaStreamSynchronize(ds.stream));
@@ -588,28 +589,38 @@ bool run_host(rpk_ctx* ctx, const HostSelect* sel, const StatusHostArgs* h, bool
 // rpk_select and rpk_select_slots once their arguments are checked: one GPU and up to kSmallBatch rows take the latency
 // path, everything else the sub-batch pipeline on every GPU.  A slot id outside the pod table: RPK_EINVAL (best and
 // top5 unspecified, stats untouched).
-int select_host(rpk_ctx* ctx, uint32_t P, const PodSource& src, int32_t* best, int32_t* top5, const char* who) {
+int select_host(rpk_ctx* ctx, const HostSelect& sel, const char* who) {
     return guarded(ctx, [&]() -> int {
         bool ok;
-        if (ctx->devs.size() == 1 && P <= kSmallBatch) {
-            ok = !src.slots || slots_below(src.slots, P, ctx->devs[0].podsN);
+        if (ctx->devs.size() == 1 && sel.P <= kSmallBatch) {
+            ok = sel.src[0].kind != RowSource::HostList || slots_below(sel.src[0].slots, sel.P, ctx->devs[0].podsN);
             if (ok) {
-                ctx->launches += (uint64_t)select_small(ctx->devs[0], P, src, best, top5);
+                ctx->launches += (uint64_t)select_small(ctx->devs[0], sel.P, sel.src[0], sel.best, sel.top5);
                 ctx->stats.last_select_kernel_ms = 0.f; ctx->stats.last_select_total_ms = 0.f;  // single copy: not timed
-                count_select(ctx, P, ctx->devs[0].G);
+                count_select(ctx, sel.P, ctx->devs[0].G);
             }
         } else {
-            const HostSelect sel{P, src, best, top5};
             ok = run_host(ctx, &sel, nullptr, false);
         }
         return ok ? RPK_OK : fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
     });
 }
 
+// RPK_ESTATE unless the tables a select reads exist: the pod table, for rows taken from it, and (needs_offers) the offer
+// table, on GPU `shard` or, with -1, on every GPU of the ctx.  The calls that write the pod table check it alone.
+int check_select_ready(rpk_ctx* ctx, const char* who, bool needs_pod_table, int shard = -1, bool needs_offers = true) {
+    for (size_t s = shard < 0 ? 0 : (size_t)shard, end = shard < 0 ? ctx->devs.size() : s + 1; s < end; ++s) {
+        if (needs_pod_table && !ctx->devs[s].pods_sized)
+            return fail(ctx, RPK_ESTATE, std::string(who) + (shard < 0 ? ": no pod table" : ": no pod table on this shard") + " (call rpk_pods_reset first)");
+        if (needs_offers && !ctx->devs[s].offers_ready) return fail(ctx, RPK_ESTATE, std::string(who) + ": no offer table uploaded (call rpk_offers_upload first)");
+    }
+    return RPK_OK;
+}
+
 // rpk_select_device_gather, and rpk_select_device_gather_top5 with t5 (its own arguments checked, a.top5 then points
-// into the local top-5 vector); with src.slots, the rpk_select_slots_device* calls of the same name (a NULL list with
-// P > 0 already refused).  The shard is in range.
-int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& src, int n_out, int32_t* const* d_best_full,
+// into the local top-5 vector); with a device list, the rpk_select_slots_device* calls of the same name (a NULL list
+// with P > 0 already refused).  The shard is in range.
+int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const RowSource& src, int n_out, int32_t* const* d_best_full,
                          uint32_t row0, int32_t* d_top5, const Top5Gather* t5, void* stream) {
     DeviceState& ds = ctx->devs[(size_t)shard];
     const PeerGroup& peers = ctx->bind[(size_t)shard];
@@ -624,24 +635,18 @@ int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& s
             return RPK_OK;
         });
     }
-    if ((!src.slots && !src.cols.req_mem) || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
+    const bool list = src.kind == RowSource::DevList;
+    if ((!list && !src.cols.req_mem) || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
     for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device: NULL output vector");
-    if (src.slots && !ds.pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_slots_device: no pod table on this shard (call rpk_pods_reset first)");
-    if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
+    if (int rc = check_select_ready(ctx, "rpk_select_slots_device", list, shard, false)) return rc;
+    if (int rc = check_select_ready(ctx, "rpk_select", false, shard)) return rc;
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
         DeviceState::Lane& ln = ds.lane[0];
-        if (src.slots) {  // the gather's compact columns: allocated on the first call of a size only
-            ln.p_req_mem.reserve(P); ln.p_req_vcpu.reserve(P); ln.p_req_ram.reserve(P); ln.p_max_price.reserve(P); ln.p_cloud.reserve(P);
-        }
+        reserve_lane(ln, P, src, false);
         SelectArgs a{};
         const bool tracked = ds.sel_scope.device_begin(st);  // the gather writes lane 0's columns: after the last select
-        if (src.slots) {
-            ctx->launches += (uint64_t)gather_pod_rows(ds, ln, P, src.slots, a, st);
-        } else {
-            const PodCols& c = src.cols;
-            a.req_mem = c.req_mem; a.req_vcpu = c.req_vcpu; a.req_ram = c.req_ram; a.max_price = c.max_price; a.cloud = c.cloud;
-        }
+        ctx->launches += (uint64_t)pod_columns(ds, ln, src, 0, P, a, st);
         a.P = P;
         for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
         a.n_out = n_out; a.row0 = row0;
@@ -657,7 +662,7 @@ int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& s
 
 // rpk_select_device_gather_top5 and rpk_select_slots_device_gather_top5: the top-5 vectors' checks, then the gather.
 // The shard is in range.
-int select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const PodSource& src, int n_out, int32_t* const* d_best_full,
+int select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const RowSource& src, int n_out, int32_t* const* d_best_full,
                               int32_t* const* d_top5_full, uint32_t row0, void* stream) {
     if (!d_best_full || !d_top5_full || n_out < 1 || n_out > RPK_MAX_GPUS)
         return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 1..8 best and top-5 vectors are required");
@@ -828,8 +833,8 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
                              const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud,
                              int n_out, int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device: shard out of range");
-    const PodSource src{PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_device: shard out of range");
+    const RowSource src{RowSource::DevCols, PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
     return select_device_gather(ctx, shard, P, src, n_out, d_best_full, row0, d_top5, nullptr, stream);
 }
 
@@ -837,8 +842,8 @@ int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int
                                   const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud, int n_out,
                                   int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: shard out of range");
-    const PodSource src{PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: shard out of range");
+    const RowSource src{RowSource::DevCols, PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
     return select_device_gather_top5(ctx, shard, P, src, n_out, d_best_full, d_top5_full, row0, stream);
 }
 
@@ -854,8 +859,9 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
     if (!ctx) return RPK_EINVAL;
     if (P == 0) return RPK_OK;
     if (!req_mem_gb || !best) return fail(ctx, RPK_EINVAL, "rpk_select: req_mem_gb and best are required");
-    for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select: no offer table uploaded (call rpk_offers_upload first)");
-    return select_host(ctx, P, PodSource{PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr}, best, top5, "rpk_select");
+    if (int rc = check_select_ready(ctx, "rpk_select", false)) return rc;
+    const RowSource rows{RowSource::HostCols, PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr};
+    return select_host(ctx, HostSelect{P, std::vector<RowSource>(ctx->devs.size(), rows), best, top5}, "rpk_select");
 }
 
 // ---- pod-requirement table -------------------------------------------------------------------------------
@@ -879,12 +885,12 @@ int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
     });
 }
 
-// slots[0, n) strictly ascending and inside the pod table (which exists): what the calls that write the table require
-static int check_pod_slots(rpk_ctx* ctx, uint32_t n, const uint32_t* slots, const char* who) {
-    const uint32_t N = ctx->devs[0].podsN;
+// slots[0, n) inside `table` (of N rows; "pod table" or "tracked table" in the message) and, with `ascending`, strictly
+// ascending: what the calls that write a table require
+static int check_slots(rpk_ctx* ctx, uint32_t n, const uint32_t* slots, uint32_t N, bool ascending, const char* who, const char* table) {
     for (uint32_t i = 0; i < n; ++i) {
-        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
-        if (i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, std::string(who) + ": slots must be strictly ascending");
+        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the " + table);
+        if (ascending && i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, std::string(who) + ": slots must be strictly ascending");
     }
     return RPK_OK;
 }
@@ -894,8 +900,8 @@ int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, c
     if (!ctx) return RPK_EINVAL;
     if (n_slots == 0) return RPK_OK;
     if (!slots || !req_mem_gb) return fail(ctx, RPK_EINVAL, "rpk_pods_seed_slots: slots and req_mem_gb are required");
-    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_seed_slots: no pod table (call rpk_pods_reset first)");
-    if (int rc = check_pod_slots(ctx, n_slots, slots, "rpk_pods_seed_slots")) return rc;
+    if (int rc = check_select_ready(ctx, "rpk_pods_seed_slots", true, -1, false)) return rc;
+    if (int rc = check_slots(ctx, n_slots, slots, ctx->devs[0].podsN, true, "rpk_pods_seed_slots", "pod table")) return rc;
     return guarded(ctx, [&]() -> int {
         // staging block: [slots : 4n][mem : 4n][vcpu : 4n][ram : 4n][max_price : 8n, 8-byte aligned][cloud : n]
         const size_t n = n_slots, o_mem = 4 * n, o_vcpu = 8 * n, o_ram = 12 * n, o_price = (16 * n + 7) & ~(size_t)7,
@@ -925,25 +931,25 @@ int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int3
     if (!ctx) return RPK_EINVAL;
     if (n_slots == 0) return RPK_OK;
     if (!slots || !best) return fail(ctx, RPK_EINVAL, "rpk_select_slots: slots and best are required");
-    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_slots: no pod table (call rpk_pods_reset first)");
-    for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select_slots: no offer table uploaded (call rpk_offers_upload first)");
-    return select_host(ctx, n_slots, PodSource{PodCols{}, slots}, best, top5, "rpk_select_slots");
+    if (int rc = check_select_ready(ctx, "rpk_select_slots", true)) return rc;
+    const std::vector<RowSource> rows(ctx->devs.size(), RowSource{RowSource::HostList, PodCols{}, slots});
+    return select_host(ctx, HostSelect{n_slots, rows, best, top5}, "rpk_select_slots");
 }
 
 int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
                                    int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: shard out of range");
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: shard out of range");
     if (n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: d_slots is required");
-    return select_device_gather(ctx, shard, n_slots, PodSource{PodCols{}, d_slots}, n_out, d_best_full, row0, d_top5, nullptr, stream);
+    return select_device_gather(ctx, shard, n_slots, RowSource{RowSource::DevList, PodCols{}, d_slots}, n_out, d_best_full, row0, d_top5, nullptr, stream);
 }
 
 int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
                                         int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: shard out of range");
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: shard out of range");
     if (n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: d_slots is required");
-    return select_device_gather_top5(ctx, shard, n_slots, PodSource{PodCols{}, d_slots}, n_out, d_best_full, d_top5_full, row0, stream);
+    return select_device_gather_top5(ctx, shard, n_slots, RowSource{RowSource::DevList, PodCols{}, d_slots}, n_out, d_best_full, d_top5_full, row0, stream);
 }
 
 int rpk_select_slots_device(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int32_t* d_best, int32_t* d_top5,
@@ -958,8 +964,8 @@ int rpk_pods_mark_pending(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
     if (!ctx) return RPK_EINVAL;
     if (n_slots == 0) return RPK_OK;
     if (!slots || !pending) return fail(ctx, RPK_EINVAL, "rpk_pods_mark_pending: slots and pending are required");
-    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_mark_pending: no pod table (call rpk_pods_reset first)");
-    if (int rc = check_pod_slots(ctx, n_slots, slots, "rpk_pods_mark_pending")) return rc;
+    if (int rc = check_select_ready(ctx, "rpk_pods_mark_pending", true, -1, false)) return rc;
+    if (int rc = check_slots(ctx, n_slots, slots, ctx->devs[0].podsN, true, "rpk_pods_mark_pending", "pod table")) return rc;
     return guarded(ctx, [&]() -> int {
         const size_t n = n_slots;  // staging block: [slots : 4n][pending : n]
         for (auto& ds : ctx->devs) {  // the table is replicated: every GPU gets every flag
@@ -998,9 +1004,9 @@ int enqueue_pending_list(DeviceState& ds, uint32_t* d_out, uint32_t* d_n, cudaSt
 
 int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out, uint32_t* d_n, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_pods_pending_list_device: shard out of range");
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_pods_pending_list_device: shard out of range");
+    if (int rc = check_select_ready(ctx, "rpk_pods_pending_list_device", true, shard, false)) return rc;
     DeviceState& ds = ctx->devs[(size_t)shard];
-    if (!ds.pods_sized) return fail(ctx, RPK_ESTATE, "rpk_pods_pending_list_device: no pod table on this shard (call rpk_pods_reset first)");
     if (!d_n || (ds.podsN > 0 && !d_slots_out)) return fail(ctx, RPK_EINVAL, "rpk_pods_pending_list_device: d_slots_out and d_n are required");
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ds.dev));
@@ -1015,8 +1021,7 @@ int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out,
 int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t* n_pending, int32_t* best, int32_t* top5) {
     if (!ctx) return RPK_EINVAL;
     if (!n_pending || (cap > 0 && !best)) return fail(ctx, RPK_EINVAL, "rpk_select_pending: n_pending and best are required");
-    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_pending: no pod table (call rpk_pods_reset first)");
-    for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select_pending: no offer table uploaded (call rpk_offers_upload first)");
+    if (int rc = check_select_ready(ctx, "rpk_select_pending", true)) return rc;
     // every GPU compacts its own replica of the flags: the table is replicated and the order ascending, so the lists are
     // identical, and each GPU then gathers its shard of the rows from its own copy.  The count lands in mapped pinned
     // memory, so the one synchronise that the list's length costs needs no copy behind it.
@@ -1049,9 +1054,9 @@ int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t
         });
         if (rc != RPK_OK) return rc;
     }
-    PodSource src{};
-    src.pending = true;
-    rc = select_host(ctx, n, src, best, top5, "rpk_select_pending");
+    HostSelect sel{n, {}, best, top5};
+    for (auto& ds : ctx->devs) sel.src.push_back(RowSource{RowSource::DevList, PodCols{}, ds.pt_list.p});
+    rc = select_host(ctx, sel, "rpk_select_pending");
     if (slots_out) {
         const int rc2 = guarded(ctx, [&]() -> int {
             RPK_CUDA(cudaSetDevice(d0.dev));
@@ -1105,8 +1110,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
     if (!ctx) return RPK_EINVAL;
     if (!n_pending || !n_reselected || !n_changed || (cap > 0 && (!slots_out || !best || !top5)))
         return fail(ctx, RPK_EINVAL, "rpk_select_pending_changed: n_pending, n_reselected, n_changed and, with cap > 0, slots_out, best and top5 are required");
-    if (!ctx->devs[0].pods_sized) return fail(ctx, RPK_ESTATE, "rpk_select_pending_changed: no pod table (call rpk_pods_reset first)");
-    for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_select_pending_changed: no offer table uploaded (call rpk_offers_upload first)");
+    if (int rc = check_select_ready(ctx, "rpk_select_pending_changed", true)) return rc;
     const int n = (int)ctx->devs.size();
     const uint32_t N = ctx->devs[0].podsN, gen = ctx->offer_gen;
     std::vector<uint32_t> pend((size_t)n, 0), stale((size_t)n, 0);
@@ -1157,12 +1161,9 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
     return guarded(ctx, [&]() -> int {
         for (int s = 0; s < n; ++s) {  // lane 0's buffers, sized on the calling thread
             DeviceState& ds = ctx->devs[(size_t)s];
-            const uint32_t k = stale[(size_t)s];
-            if (!k) continue;
+            if (!stale[(size_t)s]) continue;
             RPK_CUDA(cudaSetDevice(ds.dev));
-            DeviceState::Lane& ln = ds.lane[0];
-            ln.p_req_mem.reserve(k); ln.p_req_vcpu.reserve(k); ln.p_req_ram.reserve(k); ln.p_max_price.reserve(k); ln.p_cloud.reserve(k);
-            ln.top5.reserve((size_t)k * RPK_TOPK);
+            reserve_lane(ds.lane[0], stale[(size_t)s], RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
         }
         ctx->workers.run(n, [&](int s) {
             DeviceState& ds = ctx->devs[(size_t)s];
@@ -1173,7 +1174,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             DeviceState::Lane& ln = ds.lane[0];
             ds.res_ready = false;  // until the diff has stored every reselected row
             SelectArgs a{};
-            launches[(size_t)s] += (uint64_t)gather_pod_rows(ds, ln, k, ds.r_list.p, a, ds.stream);
+            launches[(size_t)s] += (uint64_t)pod_columns(ds, ln, RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, 0, k, a, ds.stream);
             a.P = k; a.best_out[0] = ds.r_best.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = ln.top5.p;
             launches[(size_t)s] += (uint64_t)enqueue_select(ds, ln, a, ds.stream);
             const ResultRows m = result_rows(ds, true);
@@ -1217,7 +1218,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
 
 int rpk_ipc_alloc(rpk_ctx* ctx, int shard, size_t bytes, void** d_ptr, unsigned char handle_out[64]) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size() || !d_ptr || !handle_out || bytes == 0) return fail(ctx, RPK_EINVAL, "rpk_ipc_alloc: bad argument");
+    if (bad_shard(ctx, shard) || !d_ptr || !handle_out || bytes == 0) return fail(ctx, RPK_EINVAL, "rpk_ipc_alloc: bad argument");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handle is 64 bytes");
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)shard].dev));
@@ -1236,7 +1237,7 @@ int rpk_ipc_alloc(rpk_ctx* ctx, int shard, size_t bytes, void** d_ptr, unsigned 
 
 int rpk_ipc_open(rpk_ctx* ctx, int shard, const unsigned char handle[64], void** d_peer_ptr) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size() || !handle || !d_peer_ptr) return fail(ctx, RPK_EINVAL, "rpk_ipc_open: bad argument");
+    if (bad_shard(ctx, shard) || !handle || !d_peer_ptr) return fail(ctx, RPK_EINVAL, "rpk_ipc_open: bad argument");
     return guarded(ctx, [&]() -> int {
         RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)shard].dev));
         cudaIpcMemHandle_t h;
@@ -1277,7 +1278,7 @@ int rpk_ipc_free(rpk_ctx* ctx, int shard, void* d_ptr) {
 
 int rpk_peer_fence(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int my_rank, uint32_t epoch, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size() || n < 1 || n > RPK_MAX_GPUS || !d_flags || my_rank < 0 || my_rank >= n)
+    if (bad_shard(ctx, shard) || n < 1 || n > RPK_MAX_GPUS || !d_flags || my_rank < 0 || my_rank >= n)
         return fail(ctx, RPK_EINVAL, "rpk_peer_fence: bad argument");
     for (int r = 0; r < n; ++r) if (!d_flags[r]) return fail(ctx, RPK_EINVAL, "rpk_peer_fence: NULL flag array");
     DeviceState& ds = ctx->devs[(size_t)shard];
@@ -1293,7 +1294,7 @@ int rpk_peer_fence(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int
 
 int rpk_peer_bind(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int my_rank) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size() || n < 0 || n > RPK_MAX_GPUS || (n > 0 && (!d_flags || my_rank < 0 || my_rank >= n)))
+    if (bad_shard(ctx, shard) || n < 0 || n > RPK_MAX_GPUS || (n > 0 && (!d_flags || my_rank < 0 || my_rank >= n)))
         return fail(ctx, RPK_EINVAL, "rpk_peer_bind: bad argument");
     for (int r = 0; r < n; ++r) if (!d_flags[r]) return fail(ctx, RPK_EINVAL, "rpk_peer_bind: NULL flag array");
     PeerGroup& b = ctx->bind[(size_t)shard];
@@ -1306,14 +1307,14 @@ int rpk_peer_bind(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int 
 
 int rpk_peer_inline_wait(rpk_ctx* ctx, int shard, int on) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_peer_inline_wait: shard out of range");
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_peer_inline_wait: shard out of range");
     ctx->bind[(size_t)shard].inline_wait = on ? 1 : 0;
     return RPK_OK;
 }
 
 int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size() || (what & ~3u) || !what) return fail(ctx, RPK_EINVAL, "rpk_peer_wait: bad argument");
+    if (bad_shard(ctx, shard) || (what & ~3u) || !what) return fail(ctx, RPK_EINVAL, "rpk_peer_wait: bad argument");
     if (ctx->bind[(size_t)shard].n == 0) return fail(ctx, RPK_ESTATE, "rpk_peer_wait: no flags bound (rpk_peer_bind)");
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {
@@ -1325,7 +1326,7 @@ int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream) {
 
 /* test / integration hook: device pointer of GPU `shard`'s copy of the last full assignment vector */
 const int32_t* rpk_best_device_ptr(const rpk_ctx* ctx, int shard) {
-    if (!ctx || shard < 0 || (size_t)shard >= ctx->devs.size()) return nullptr;
+    if (!ctx || bad_shard(ctx, shard)) return nullptr;
     return ctx->devs[(size_t)shard].best_full.p;
 }
 
@@ -1396,7 +1397,7 @@ int rpk_status_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
     if (!slots || !records) return fail(ctx, RPK_EINVAL, "rpk_status_seed_slots: slots and records are required");
     if (!ctx->devs[0].status_sized) return fail(ctx, RPK_ESTATE, "rpk_status_seed_slots: no tracked table (call rpk_status_reset first)");
     const uint32_t N = ctx->devs[0].statusN;
-    for (uint32_t i = 0; i < n_slots; ++i) if (slots[i] >= N) return fail(ctx, RPK_EINVAL, "rpk_status_seed_slots: slot index outside the tracked table");
+    if (int rc = check_slots(ctx, n_slots, slots, N, false, "rpk_status_seed_slots", "tracked table")) return rc;
     return guarded(ctx, [&]() -> int {
         const int n = (int)ctx->devs.size();
         for (int s = 0; s < n; ++s) {  // a handful of slots: every GPU gets the list and keeps the ones of its shard
@@ -1425,10 +1426,7 @@ int rpk_status_diff_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
     if (!slots || !records || !changed_idx) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slots, records and changed_idx are required");
     if (!ctx->devs[0].status_sized) return fail(ctx, RPK_ESTATE, "rpk_status_diff_slots: no tracked table (call rpk_status_reset first)");
     const uint32_t N = ctx->devs[0].statusN;
-    for (uint32_t i = 0; i < n_slots; ++i) {
-        if (slots[i] >= N) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slot index outside the tracked table");
-        if (i > 0 && slots[i] <= slots[i - 1]) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slots must be strictly ascending");
-    }
+    if (int rc = check_slots(ctx, n_slots, slots, N, true, "rpk_status_diff_slots", "tracked table")) return rc;
     StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
     h.slots = slots; h.n_slots = n_slots;
     return guarded(ctx, [&]() -> int { run_host(ctx, nullptr, &h, false); return RPK_OK; });
@@ -1443,10 +1441,11 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
              uint32_t stride, uint32_t* changed_idx, uint16_t* changed_code, uint32_t* n_changed) {
     if (!ctx) return RPK_EINVAL;
     if (P > 0 && (!req_mem_gb || !best)) return fail(ctx, RPK_EINVAL, "rpk_tick: req_mem_gb and best are required");
-    if (P > 0) for (auto& ds : ctx->devs) if (!ds.offers_ready) return fail(ctx, RPK_ESTATE, "rpk_tick: no offer table uploaded (call rpk_offers_upload first)");
+    if (P > 0) { if (int rc = check_select_ready(ctx, "rpk_tick", false)) return rc; }
     const StatusHostArgs h{N, records, stride, changed_idx, changed_code, n_changed, nullptr, true};
     if (int rc = check_sweep(ctx, h, "rpk_tick")) return rc;
-    const HostSelect sel{P, PodSource{PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr}, best, top5};
+    const RowSource rows{RowSource::HostCols, PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr};
+    const HostSelect sel{P, std::vector<RowSource>(ctx->devs.size(), rows), best, top5};
     return guarded(ctx, [&]() -> int { run_host(ctx, P > 0 ? &sel : nullptr, &h, true); return RPK_OK; });
 }
 
@@ -1456,7 +1455,7 @@ int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records,
                   uint32_t* const* d_xchg, uint32_t cap, int my_rank, void* stream, const uint32_t* d_slots = nullptr, uint32_t col_n = 0) {
     // d_slots: N is the list's length, and the column (col_n rows) holds global slots [idx_base, idx_base + col_n)
     if (!ctx) return RPK_EINVAL;
-    if (shard < 0 || (size_t)shard >= ctx->devs.size()) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: shard out of range");
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: shard out of range");
     if (int rc = check_stride(ctx, stride)) return rc;
     if (N > 0 && (!d_records || !d_hash_prev)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: NULL column");
     if (n_out == 0 && N > 0 && !d_changed_idx) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: d_changed_idx is NULL");
