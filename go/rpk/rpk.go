@@ -282,6 +282,37 @@ func (e *Engine) PodsPendingListDevice(shard int, dSlotsOut, dN, stream unsafe.P
 	return nil
 }
 
+// ResultsXchgBytes is the size of one exchange buffer of SelectPendingChangedGather for nRanks ranks of capacity
+// capacity: counts, then per rank slot[capacity], best[capacity], top5[5*capacity] (uint32 words), plus 16 bytes.
+func ResultsXchgBytes(nRanks, capacity int) int {
+	return int(C.rpk_results_xchg_bytes(C.int(nRanks), C.uint32_t(capacity)))
+}
+
+// SelectPendingChangedGather is SelectPendingChanged for one process per GPU: rank myRank of len(dXchg) reselects the
+// pending slots of its own range and writes its changed rows into region myRank of every rank's exchange buffer (device
+// pointers, peers' mapped with rpk_ipc_open; each ResultsXchgBytes bytes, 16-byte aligned), then signals the bound flag
+// group (rpk_peer_wait what = 4 closes the step).  It synchronises stream once and returns with the rest enqueued on it.
+func (e *Engine) SelectPendingChangedGather(shard, myRank int, dXchg []unsafe.Pointer, capacity int, stream unsafe.Pointer) (nPending, nReselected int, err error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	n := len(dXchg)
+	if n == 0 || n > C.RPK_MAX_GPUS {
+		return 0, 0, fmt.Errorf("rpk: %d exchange buffers, 1..%d ranks", n, C.RPK_MAX_GPUS)
+	}
+	// the pointer array lives in C memory: device addresses are not Go pointers, but cgo must not see a Go slice of them
+	arr := (*[C.RPK_MAX_GPUS]*C.uint32_t)(C.malloc(C.size_t(C.RPK_MAX_GPUS) * C.size_t(unsafe.Sizeof(uintptr(0)))))
+	defer C.free(unsafe.Pointer(arr))
+	for i, p := range dXchg {
+		arr[i] = (*C.uint32_t)(p)
+	}
+	var np, nr C.uint32_t
+	rc := C.rpk_select_pending_changed_gather(e.ctx, C.int(shard), C.int(n), C.int(myRank), &arr[0], C.uint32_t(capacity), &np, &nr, stream)
+	if rc != C.RPK_OK {
+		return int(np), int(nr), lastError(e.ctx, rc)
+	}
+	return int(np), int(nr), nil
+}
+
 // StatusDiff is the batched predicate of updateAllPodStatuses (kubelet.go:870-873): records holds one
 // fixed slot per tracked pod (see EncodeStatusRecord); the indices of the slots whose (status, ports)
 // pair differs from the previous sweep come back ascending.

@@ -33,7 +33,8 @@
  *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_pods_reset,
  *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
  *     rpk_select_pending_changed, the _device call
- *     rpk_pods_pending_list_device, and rpk_tick with P > 0.  Status scope: rpk_status_diff,
+ *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host), and rpk_tick
+ *     with P > 0.  Status scope: rpk_status_diff,
  *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset and
  *     rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
  *     capture neither waits nor is waited for (keep each captured entry point on one stream), and the library does
@@ -285,6 +286,38 @@ int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slot
  * they are at replay time. */
 int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out, uint32_t* d_n, void* stream);
 
+/* rpk_select_pending_changed for one-process-per-GPU callers: each rank reselects the pending slots of its own range and
+ * sends only its changed rows to every rank, over the exchange buffers and the bound flags.
+ *   - Owned range: rank my_rank of n_ranks owns slots [lo, hi) of the pod table, the range GPU my_rank of an n_ranks-GPU
+ *     ctx owns in rpk_select_pending_changed (boundaries on 16-slot units), so the ranks' ranges tile the table in rank
+ *     order; a range may be empty.  Every rank keeps the whole pod table and the flags (every rank seeds and marks the
+ *     same rows, as for rpk_select_slots_device_gather); a rank's stored results cover its own range only.
+ *   - Semantics: exactly rpk_select_pending_changed restricted to [lo, hi): the same stale rule, one select with top-5,
+ *     the same diff, and each reported result becomes the slot's stored result.  *n_pending and *n_reselected count the
+ *     rank's own slots.  Counts as one select in rpk_stats when it reselects anything.
+ *   - Exchange: the rank's changed rows, ascending by slot, land in region my_rank of every buffer d_xchg[0..n_ranks)
+ *     (peer-mapped like the assignment vectors; each rpk_results_xchg_bytes(n_ranks, cap) bytes, 16-byte aligned).  A
+ *     buffer in uint32 words: [0, 8) the count per source rank; from word 8, region r = r * 7 * cap words on: slot[cap],
+ *     best[cap], top5[5 * cap] (best is top5[0]).  Entries past a region's count are not written.  The regions of all
+ *     ranks concatenated in rank order are rpk_select_pending_changed's slots_out / best / top5, bit for bit.
+ *   - Signal: with flags bound (rpk_peer_bind) the CTA that finishes last signals the pending results epoch (word 34 of
+ *     the rank's own array, flag words 16 + my_rank) after a system-scope fence; rpk_peer_wait(what = 4) or the inline
+ *     wait makes every region readable.  A rank with nothing to reselect, or an empty range, still writes its count 0
+ *     into every buffer and signals.
+ *   - RPK_EINVAL, before anything is enqueued and without signalling: n_ranks outside 1..8, my_rank outside [0, n_ranks),
+ *     a NULL or misaligned buffer, a NULL count pointer, or cap < hi - lo (every rank must hold its worst case, so no
+ *     refusal can come after the stale step while peers wait).  RPK_ESTATE, the same way: no pod table or no offer table
+ *     on GPU `shard`, or stored results made for another range since the last rpk_pods_reset (another my_rank or
+ *     n_ranks, or rpk_select_pending_changed on the same ctx with another range).
+ *   - Ordering: select scope.  The call waits on the host for the scope's last device call, synchronises `stream` once
+ *     after the stale step (the select needs the row count on the host), and returns with the gather, select, diff,
+ *     push and signal enqueued on `stream`.  NOT graph-capturable.  A rank's first call after rpk_pods_reset (and a call
+ *     that grows the select scratch) synchronises the device, so a host thread that drives several ranks turns the
+ *     inline wait on only after each rank has made one call, as rpk_peer_inline_wait says. */
+size_t rpk_results_xchg_bytes(int n_ranks, uint32_t cap);
+int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg, uint32_t cap,
+                                      uint32_t* n_pending, uint32_t* n_reselected, void* stream);
+
 /* Cross-process peer vectors for one-process-per-GPU callers (torchrun-style): allocate a plain cudaMalloc
  * buffer on GPU `shard` and export its 64-byte CUDA IPC handle; another process opens the handle and gets a
  * device pointer it can pass in d_best_full[] of rpk_select_device_gather (peer access over NVLink is
@@ -310,9 +343,10 @@ int rpk_peer_fence(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int
  * the warp that pushes the last block of the slice (or a one-warp kernel behind the copy kernel on the small-batch
  * paths, or behind nothing for an empty shard) bumps the rank's select epoch (word 32 of its own array) and stores it
  * into word `my_rank` of every peer's array, after a system-scope fence.  rpk_status_diff_device_gather does the same
- * with the status epoch (word 33, flag words 8 + my_rank).  rpk_peer_wait enqueues the other half: one warp that
- * spins until every rank's flag shows this rank's own current epoch (what: bit 0 = select, bit 1 = status sweep;
- * all ranks of a group must issue the same sequence of gathers).  Launches carry no per-call value, so a step can be
+ * with the status epoch (word 33, flag words 8 + my_rank), and rpk_select_pending_changed_gather with the pending
+ * results epoch (word 34, flag words 16 + my_rank).  rpk_peer_wait enqueues the other half: one warp that
+ * spins until every rank's flag shows this rank's own current epoch (what: bit 0 = select, bit 1 = status sweep,
+ * bit 2 = pending results; all ranks of a group must issue the same sequence of gathers).  Launches carry no per-call value, so a step can be
  * captured in a CUDA graph and replayed.  Do not mix rpk_peer_fence and the bound mode on the same arrays (both use
  * words 0..7 and 32).
  * Ordering given: a peer's results are visible after the wait.  NOT given: once rank A has passed the wait of step e it

@@ -9,7 +9,7 @@ Contents: ``csrc/`` (CUDA kernels + the C-ABI of ``include/rpk.h``), ``lib/librp
 ``host/`` (C++ mirror of the reference's Provider surface for this path).
 """
 from . import _ffi, synth  # noqa: F401
-from .engine import Engine  # noqa: F401
+from .engine import Engine, results_region  # noqa: F401
 from ._ffi import RpkError  # noqa: F401
 
-__all__ = ["Engine", "RpkError", "synth"]
+__all__ = ["Engine", "RpkError", "results_region", "synth"]

@@ -16,6 +16,8 @@
 //                   number and the number of pending slots (rpk_select_pending_changed, before its select)
 //   k_pod_result_diff  over the rows that select returned: store each row's result and write the rows whose list changed,
 //                   ascending, to the host (rpk_select_pending_changed, after its select)
+//   k_pod_result_diff_xchg  the same, the changed rows written into region my_rank of every rank's exchange buffer, then
+//                   a peer signal (rpk_select_pending_changed_gather)
 // The host entry points check every slot against the table's N before its upload.  The device entry points cannot, so
 // an entry outside [0, N) is defined here: the seed skips it, and the gather writes a row with cloud byte kCloudNone,
 // which every select path finishes as "neither cloud" (runpod_client.go:469-475): -1 and five -1.  No caller input
@@ -100,8 +102,8 @@ __device__ __forceinline__ uint32_t count_flags(const uint4& v) {
     return (uint32_t)(__popc(__vcmpne4(v.x, 0u)) + __popc(__vcmpne4(v.y, 0u)) + __popc(__vcmpne4(v.z, 0u)) + __popc(__vcmpne4(v.w, 0u))) >> 3;
 }
 
-// The compaction itself, shared by the three kernels that turn 16-item units into an ascending list: k_pod_pending (units
-// of the flag column), k_pod_stale (units of a GPU's owned slots) and k_pod_result_diff (units of the reselected rows).
+// The compaction itself, shared by the kernels that turn 16-item units into an ascending list: k_pod_pending (units of
+// the flag column), k_pod_stale (units of a GPU's owned slots) and k_pod_result_diff[_xchg] (units of the reselected rows).
 // The policy Pol says what a unit holds:
 //   V none()                        a unit past the CTA's share
 //   V load(u)                       pass 1's view of unit u
@@ -111,7 +113,9 @@ __device__ __forceinline__ uint32_t count_flags(const uint4& v) {
 //   uint32_t count(V), bool keep(V, k), uint32_t id(u, k), emit(i, id)   pass 2: list entry i := id of kept item k of u
 //   set_count(n)                    the list's length (the last CTA in unit order)
 //   cta_total(Count)                the CTA's pass-1 total, once per CTA
+//   fence()                         every thread, after its last emit and before its CTA counts as finished
 //   last()                          thread 0 of the CTA that finishes last, after every other CTA is done
+//   last_warp()                     warp 0 of that CTA, after last()
 template <class Pol>
 __device__ __forceinline__ void compact_units(Pol& p, uint32_t n_units, unsigned long long* tile_state, uint32_t* ticket) {
     using V = typename Pol::V;
@@ -176,7 +180,7 @@ __device__ __forceinline__ void compact_units(Pol& p, uint32_t n_units, unsigned
         at += round;
         __syncthreads();  // the tile and the warp sums are rewritten by the next round
     }
-    __threadfence();
+    p.fence();
     __syncthreads();
     if (tid == 0) s_last = atomicAdd(ticket + 1, 1u) == n_ctas - 1 ? 1u : 0u;
     __syncthreads();
@@ -184,6 +188,7 @@ __device__ __forceinline__ void compact_units(Pol& p, uint32_t n_units, unsigned
     // last CTA to finish: every look-back is over -- clean the state for the next call
     for (uint32_t i = tid; i < n_ctas; i += kPendThreads) tile_state[i] = 0ull;
     if (tid == 0) { ticket[0] = 0u; ticket[1] = 0u; p.last(); }
+    if (warp == 0) p.last_warp();
 }
 
 // k_pod_pending's units: 16 flag bytes, slot 16 u + k in byte k
@@ -204,7 +209,9 @@ struct FlagUnits {
     __device__ __forceinline__ void emit(uint32_t i, uint32_t id) const { a.out[i] = id; }
     __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
     __device__ __forceinline__ void cta_total(Count) const {}
+    __device__ __forceinline__ void fence() const { __threadfence(); }
     __device__ __forceinline__ void last() const {}
+    __device__ __forceinline__ void last_warp() const {}
 };
 
 __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_pending(PendingArgs a, uint32_t n_units) {
@@ -281,7 +288,9 @@ struct StaleUnits {
     __device__ __forceinline__ void emit(uint32_t i, uint32_t id) const { a.out[i] = id; }
     __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
     __device__ __forceinline__ void cta_total(Count total) const { atomicAdd(a.ticket + 2, (uint32_t)(total >> 32)); }
+    __device__ __forceinline__ void fence() const { __threadfence(); }
     __device__ __forceinline__ void last() const { *a.n_pending = atomicExch(a.ticket + 2, 0u); }
+    __device__ __forceinline__ void last_warp() const {}
 };
 
 __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_stale(StaleArgs a, uint32_t n_units) {
@@ -328,12 +337,46 @@ struct DiffUnits {
     }
     __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
     __device__ __forceinline__ void cta_total(Count) const {}
+    __device__ __forceinline__ void fence() const { __threadfence(); }
     __device__ __forceinline__ void last() const {}
+    __device__ __forceinline__ void last_warp() const {}
 };
 
 __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff(ResultDiffArgs a, uint32_t n_units) {
     DiffUnits p{a};
     compact_units(p, n_units, a.tile_state, a.ticket);
+}
+
+// The exchange form (rpk_select_pending_changed_gather): the same units and stores, but each changed row goes into
+// region my_rank of every rank's buffer (peer stores over NVLink) and the count into word my_rank of each.  The stores
+// are made visible system-wide before a CTA counts as finished, so the CTA that finishes last can signal the results
+// epoch: a peer past its wait reads every region.
+struct DiffXchgUnits : DiffUnits {
+    const ResultXchgArgs& x;
+    __device__ __forceinline__ void emit(uint32_t i, uint32_t row) const {  // best is the list's first entry
+        const int32_t* t = a.top5 + (size_t)row * RPK_TOPK;
+        const uint32_t s = a.list[row];
+        int32_t v[RPK_TOPK];
+#pragma unroll
+        for (int q = 0; q < RPK_TOPK; ++q) v[q] = t[q];
+        for (int o = 0; o < x.n_out; ++o) {
+            uint32_t* r = x.region[o];
+            r[i] = s; r[x.cap + i] = (uint32_t)v[0];
+            uint32_t* r5 = r + 2 * (size_t)x.cap + (size_t)i * RPK_TOPK;
+#pragma unroll
+            for (int q = 0; q < RPK_TOPK; ++q) r5[q] = (uint32_t)v[q];
+        }
+    }
+    __device__ __forceinline__ void set_count(uint32_t n) const { for (int o = 0; o < x.n_out; ++o) *x.count[o] = n; }
+    __device__ __forceinline__ void fence() const { __threadfence_system(); }
+    __device__ __forceinline__ void last_warp() const {
+        if (x.peers.n > 0) signal_peers(x.peers, kFlagResults, kFlagResultsCtr, 0, x.peers.inline_wait != 0);
+    }
+};
+
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff_xchg(ResultXchgArgs x, uint32_t n_units) {
+    DiffXchgUnits p{{x.d}, x};
+    compact_units(p, n_units, x.d.tile_state, x.d.ticket);
 }
 
 int launch_pod_fill(const PodRows& t, uint8_t* pending, uint32_t N, int sm_count, cudaStream_t st) {
@@ -396,6 +439,13 @@ int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t s
     if (a.n == 0) return 0;
     const uint32_t n_units = (a.n + kPendUnit - 1) / kPendUnit;
     k_pod_result_diff<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st) {
+    const uint32_t n_units = (x.d.n + kPendUnit - 1) / kPendUnit;  // no rows: one CTA publishes the count and signals
+    k_pod_result_diff_xchg<<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, n_units);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

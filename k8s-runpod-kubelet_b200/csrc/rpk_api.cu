@@ -868,7 +868,7 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
 
 int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
     if (!ctx) return RPK_EINVAL;
-    for (auto& ds : ctx->devs) ds.pods_sized = ds.res_ready = false;  // a failure below leaves no table rather than a mix of sizes
+    for (auto& ds : ctx->devs) ds.pods_sized = ds.res_ready = ds.res_bound = false;  // a failure below leaves no table rather than a mix of sizes
     return guarded(ctx, [&]() -> int {
         for (auto& ds : ctx->devs) {
             RPK_CUDA(cudaSetDevice(ds.dev));
@@ -1091,6 +1091,14 @@ void reserve_results(DeviceState& ds, uint32_t lo, uint32_t hi) {
     RPK_CUDA(cudaMemset(ds.r_gen.p, 0, ds.r_gen.cap * sizeof(uint32_t)));
     RPK_CUDA(cudaDeviceSynchronize());
     ds.res_ready = true;
+    ds.res_bound = true; ds.res_lo = lo; ds.res_hi = hi;
+}
+
+// RPK_ESTATE when ds's stored results were made for another owned range than [lo, hi) since the last rpk_pods_reset:
+// their offsets, and possibly their size, belong to that range
+int check_results_range(rpk_ctx* ctx, const DeviceState& ds, uint32_t lo, uint32_t hi, const char* who) {
+    if (!ds.res_bound || (ds.res_lo == lo && ds.res_hi == hi)) return RPK_OK;
+    return fail(ctx, RPK_ESTATE, std::string(who) + ": the stored results of this GPU were made for another slot range (call rpk_pods_reset first)");
 }
 
 // The counts in mapped memory (the device's view with d = true), and the changed rows: in r_out (d = true), or their host
@@ -1103,6 +1111,48 @@ ResultRows result_rows(DeviceState& ds, bool d) {
     int32_t* b = d ? ds.r_out.p : reinterpret_cast<int32_t*>(ds.h_res.h + 64);
     return ResultRows{counts, reinterpret_cast<uint32_t*>(b), b + cap, b + 2 * cap};
 }
+
+// The stale step of ds over its owned slots [lo, hi): k_pod_stale lists the stale pending slots in r_list, and their
+// number and the number of owned pending slots land in the mapped counts (zeroed here; read them after synchronising
+// st).  The caller has waited for the select scope.  Returns the kernels launched.
+int enqueue_stale(DeviceState& ds, uint32_t lo, uint32_t hi, uint32_t gen, cudaStream_t st) {
+    reserve_results(ds, lo, hi);
+    reserve_compaction_state(ds);
+    const ResultRows m = result_rows(ds, true);
+    StaleArgs a{};
+    a.flags = ds.pt_pending.p; a.t = ds.pods_table(); a.N = ds.podsN; a.u_lo = lo / 16; a.r = ds.results(); a.gen = gen;
+    a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = m.counts; a.n_pending = m.counts + 1;
+    a.tile_state = ds.pt_state.p; a.ticket = ds.pt_ticket.p;
+    const ResultRows h = result_rows(ds, false);
+    reinterpret_cast<volatile uint32_t*>(h.counts)[0] = 0u; reinterpret_cast<volatile uint32_t*>(h.counts)[1] = 0u;
+    return launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, st);
+}
+
+// The reselect of the k stale rows enqueue_stale listed (lane 0's buffers sized for them): the gather, one select with
+// top-5, and the diff that stores each row's result and writes the changed rows to the mapped outputs (x null) or, in
+// its exchange form, to the buffers x names (x->d is filled here).  The exchange form runs with k = 0 too.  Returns the
+// kernels launched.
+int enqueue_reselect(DeviceState& ds, uint32_t k, uint32_t lo, uint32_t gen, cudaStream_t st, ResultXchgArgs* x = nullptr) {
+    DeviceState::Lane& ln = ds.lane[0];
+    const RowSource list{RowSource::DevList, PodCols{}, ds.r_list.p};
+    int launches = 0;
+    if (k) {
+        SelectArgs a{};
+        launches += pod_columns(ds, ln, list, 0, k, a, st);
+        a.P = k; a.best_out[0] = ds.r_best.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = ln.top5.p;
+        launches += enqueue_select(ds, ln, a, st);
+    }
+    const ResultRows m = result_rows(ds, true);
+    ResultDiffArgs d{};
+    d.list = ds.r_list.p; d.n = k;
+    d.cols = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p}; d.top5 = ln.top5.p;
+    d.r = ds.results(); d.r_lo = lo; d.gen = gen; d.mask = ds.r_mask.p;
+    d.out_slot = m.slot; d.out_best = m.best; d.out_top5 = m.top5; d.n_out = m.counts;
+    d.tile_state = ds.pt_state.p; d.ticket = ds.pt_ticket.p;
+    if (!x) return launches + launch_pod_result_diff(d, ds.sm_count, st);
+    x->d = d;
+    return launches + launch_pod_result_xchg(*x, ds.sm_count, st);
+}
 }  // namespace
 
 int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, uint32_t* n_reselected, uint32_t* slots_out,
@@ -1113,6 +1163,10 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
     if (int rc = check_select_ready(ctx, "rpk_select_pending_changed", true)) return rc;
     const int n = (int)ctx->devs.size();
     const uint32_t N = ctx->devs[0].podsN, gen = ctx->offer_gen;
+    for (int s = 0; s < n; ++s) {
+        uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
+        if (int rc = check_results_range(ctx, ctx->devs[(size_t)s], lo, hi, "rpk_select_pending_changed")) return rc;
+    }
     std::vector<uint32_t> pend((size_t)n, 0), stale((size_t)n, 0);
     std::vector<uint64_t> launches((size_t)n, 0);
     // 1. every GPU lists the stale pending slots of its own range (the flags and the table are replicated); both counts
@@ -1123,16 +1177,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();
-            reserve_results(ds, lo, hi);
-            reserve_compaction_state(ds);
-            const ResultRows m = result_rows(ds, true);
-            StaleArgs a{};
-            a.flags = ds.pt_pending.p; a.t = ds.pods_table(); a.N = N; a.u_lo = lo / 16; a.r = ds.results(); a.gen = gen;
-            a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = m.counts; a.n_pending = m.counts + 1;
-            a.tile_state = ds.pt_state.p; a.ticket = ds.pt_ticket.p;
-            const ResultRows h = result_rows(ds, false);
-            reinterpret_cast<volatile uint32_t*>(h.counts)[0] = 0u; reinterpret_cast<volatile uint32_t*>(h.counts)[1] = 0u;
-            launches[(size_t)s] += (uint64_t)launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, ds.stream);
+            launches[(size_t)s] += (uint64_t)enqueue_stale(ds, lo, hi, gen, ds.stream);
         }
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
@@ -1171,22 +1216,11 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             if (!k) return;
             uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
             RPK_CUDA(cudaSetDevice(ds.dev));
-            DeviceState::Lane& ln = ds.lane[0];
             ds.res_ready = false;  // until the diff has stored every reselected row
-            SelectArgs a{};
-            launches[(size_t)s] += (uint64_t)pod_columns(ds, ln, RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, 0, k, a, ds.stream);
-            a.P = k; a.best_out[0] = ds.r_best.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = ln.top5.p;
-            launches[(size_t)s] += (uint64_t)enqueue_select(ds, ln, a, ds.stream);
-            const ResultRows m = result_rows(ds, true);
-            ResultDiffArgs d{};
-            d.list = ds.r_list.p; d.n = k;
-            d.cols = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p}; d.top5 = ln.top5.p;
-            d.r = ds.results(); d.r_lo = lo; d.gen = gen; d.mask = ds.r_mask.p;
-            d.out_slot = m.slot; d.out_best = m.best; d.out_top5 = m.top5; d.n_out = m.counts;
-            d.tile_state = ds.pt_state.p; d.ticket = ds.pt_ticket.p;
-            launches[(size_t)s] += (uint64_t)launch_pod_result_diff(d, ds.sm_count, ds.stream);
+            launches[(size_t)s] += (uint64_t)enqueue_reselect(ds, k, lo, gen, ds.stream);
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
             ds.res_ready = true;
+            const ResultRows m = result_rows(ds, true);
             const ResultRows h = result_rows(ds, false);
             const uint32_t c = *reinterpret_cast<volatile uint32_t*>(h.counts);
             if (c) {
@@ -1210,6 +1244,56 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
         }
         *n_changed = at;
         count_select(ctx, R, ctx->devs[0].G);
+        return RPK_OK;
+    });
+}
+
+size_t rpk_results_xchg_bytes(int n_ranks, uint32_t cap) {
+    if (n_ranks < 1 || n_ranks > RPK_MAX_GPUS) return 0;
+    return (8 + (size_t)n_ranks * cap * (2 + RPK_TOPK)) * 4 + 16;
+}
+
+// Every refusal comes before the first launch, and cap >= hi - lo bounds what the diff can write: once the stale step
+// has run, the call always finishes with its count and its signal, so no peer is left waiting.
+int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg, uint32_t cap,
+                                      uint32_t* n_pending, uint32_t* n_reselected, void* stream) {
+    static const char* who = "rpk_select_pending_changed_gather";
+    if (!ctx) return RPK_EINVAL;
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, std::string(who) + ": shard out of range");
+    if (n_ranks < 1 || n_ranks > RPK_MAX_GPUS || my_rank < 0 || my_rank >= n_ranks || !d_xchg || !n_pending || !n_reselected)
+        return fail(ctx, RPK_EINVAL, std::string(who) + ": n_ranks in 1..8, my_rank in [0, n_ranks), d_xchg, n_pending and n_reselected are required");
+    for (int o = 0; o < n_ranks; ++o)
+        if (!d_xchg[o] || ((uintptr_t)d_xchg[o] & 15)) return fail(ctx, RPK_EINVAL, std::string(who) + ": NULL or not 16-byte aligned exchange buffer");
+    if (int rc = check_select_ready(ctx, who, true, shard)) return rc;
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    uint32_t lo, hi; result_range(ds.podsN, n_ranks, my_rank, &lo, &hi);
+    if (cap < hi - lo) return fail(ctx, RPK_EINVAL, std::string(who) + ": cap is below the number of slots the rank owns");
+    if (int rc = check_results_range(ctx, ds, lo, hi, who)) return rc;
+    const uint32_t gen = ctx->offer_gen;
+    return guarded(ctx, [&]() -> int {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+        ds.sel_scope.host_wait();
+        uint64_t launches = (uint64_t)enqueue_stale(ds, lo, hi, gen, st);
+        RPK_CUDA(cudaStreamSynchronize(st));  // the select needs the row count on the host
+        const volatile uint32_t* c = result_rows(ds, false).counts;
+        const uint32_t k = c[0];
+        *n_pending = c[1]; *n_reselected = k;
+        if (k) reserve_lane(ds.lane[0], k, RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
+        ResultXchgArgs x{};
+        x.n_out = n_ranks; x.cap = cap;
+        for (int o = 0; o < n_ranks; ++o) {  // buffer o: [counts : 8 words][region r: slot[cap], best[cap], top5[5 cap]]...
+            x.region[o] = d_xchg[o] + 8 + (size_t)my_rank * (2 + RPK_TOPK) * cap;
+            x.count[o] = d_xchg[o] + my_rank;
+        }
+        x.peers = ctx->bind[(size_t)shard];
+        x.peers.my_rank = my_rank;  // the diff fills and signals under the rank the call names
+        ds.res_ready = false;       // until the diff is enqueued behind the select
+        launches += (uint64_t)enqueue_reselect(ds, k, lo, gen, st, &x);
+        ds.res_ready = true;
+        ds.sel_scope.device_end(st, true);
+        ctx->launches += launches;
+        if (k) count_select(ctx, k, ds.G);
         return RPK_OK;
     });
 }
@@ -1314,7 +1398,7 @@ int rpk_peer_inline_wait(rpk_ctx* ctx, int shard, int on) {
 
 int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard) || (what & ~3u) || !what) return fail(ctx, RPK_EINVAL, "rpk_peer_wait: bad argument");
+    if (bad_shard(ctx, shard) || (what & ~7u) || !what) return fail(ctx, RPK_EINVAL, "rpk_peer_wait: bad argument");
     if (ctx->bind[(size_t)shard].n == 0) return fail(ctx, RPK_ESTATE, "rpk_peer_wait: no flags bound (rpk_peer_bind)");
     DeviceState& ds = ctx->devs[(size_t)shard];
     return guarded(ctx, [&]() -> int {

@@ -63,14 +63,15 @@ enum : uint32_t { kHdrRowsDone = 32, kHdrPushed = 64, kHdrGroupRows = 96, kHdrGr
                   kHdrCursors = kHdrGroupWork + kMaxGroups };
 
 // A peer group's flag arrays (rpk_peer_bind, rpk_peer_fence): flags[r] is rank r's array of >= 64 words; n = 0: none.
-// Word layout (rpk.h): a rank's epochs as seen by rank r sit at word kFlagSelect + my_rank / kFlagStatus + my_rank of
-// r's array; each rank counts its own epochs in kFlagSelectCtr / kFlagStatusCtr of its own array.
+// Word layout (rpk.h): a rank's epochs as seen by rank r sit at word kFlagSelect + my_rank / kFlagStatus + my_rank /
+// kFlagResults + my_rank of r's array; each rank counts its own epochs in kFlagSelectCtr / kFlagStatusCtr /
+// kFlagResultsCtr of its own array.
 struct PeerGroup {
     uint32_t* flags[RPK_MAX_GPUS];
     int n, my_rank;
     int inline_wait;  // the signalling warp also waits for every peer's signal (rpk_peer_inline_wait)
 };
-enum : uint32_t { kFlagSelect = 0, kFlagStatus = 8, kFlagSelectCtr = 32, kFlagStatusCtr = 33 };
+enum : uint32_t { kFlagSelect = 0, kFlagStatus = 8, kFlagResults = 16, kFlagSelectCtr = 32, kFlagStatusCtr = 33, kFlagResultsCtr = 34 };
 
 // One warp signals the group: epoch 0 bumps the rank's own counter word `ctr` and uses the new value (the launch then
 // carries no per-call value and can be replayed from a CUDA graph), any other epoch is used as given and leaves `ctr`
@@ -265,7 +266,8 @@ uint32_t select_tiles_max(uint32_t P, int rows_per_warp);
 int pick_rows_per_warp(uint32_t P, int sm_count);
 int launch_status_diff(const StatusArgs& a, int sm_count, cudaStream_t st);
 // one warp behind the stream's earlier work: signal the group's select words (epoch 0: self-counting), with `wait` also
-// wait for every rank's signal; what: bit 0 = wait for the select epoch, bit 1 = the status epoch
+// wait for every rank's signal; what: bit 0 = wait for the select epoch, bit 1 = the status epoch, bit 2 = the pending
+// results epoch
 int launch_peer_signal(const PeerGroup& g, uint32_t epoch, bool wait, cudaStream_t st);
 int launch_peer_wait(const PeerGroup& g, uint32_t what, cudaStream_t st);
 // persistent bit-sliced select (select_persist.cu)
@@ -320,8 +322,20 @@ struct ResultDiffArgs {
     uint32_t* n_out;                   // their number (mapped host memory)
     unsigned long long* tile_state; uint32_t* ticket;  // as StaleArgs
 };
+// The diff's exchange form (rpk_select_pending_changed_gather): the changed rows go into region my_rank of every buffer
+// instead (d.out_* and d.n_out unused), the count into word my_rank of each, and the CTA that finishes last signals the
+// results epoch.  Region of a buffer of capacity cap: [slot : cap][best : cap][top5 : 5 cap] words.
+struct ResultXchgArgs {
+    ResultDiffArgs d;
+    int n_out; uint32_t cap;
+    uint32_t* region[RPK_MAX_GPUS];  // region my_rank of buffer o
+    uint32_t* count[RPK_MAX_GPUS];   // word my_rank of buffer o
+    PeerGroup peers;                 // bound flags (n = 0: none), my_rank from the call
+};
 int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
 int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st);
+// launches even when x.d.n = 0: the count 0 still goes out and the peers are still signalled
+int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
@@ -448,6 +462,9 @@ struct DeviceState {
     DevBuf<uint32_t> r_gen, r_list; DevBuf<uint16_t> r_mask;
     PinnedBuf h_res;
     bool res_ready = false;
+    // the owned range [res_lo, res_hi) the stored results were made for, set by the first call after rpk_pods_reset
+    // (res_bound); a call over another range is refused
+    bool res_bound = false; uint32_t res_lo = 0, res_hi = 0;
     StoredResults results() { return StoredResults{r_mem.p, r_vcpu.p, r_ram.p, r_max_price.p, r_cloud.p, r_gen.p, r_top5.p}; }
     PodRows pods_table() { return PodRows{pt_mem.p, pt_vcpu.p, pt_ram.p, pt_max_price.p, pt_cloud.p}; }
     ~DeviceState();

@@ -651,6 +651,7 @@ __global__ void k_peer_wait(PeerGroup g, uint32_t what) {
     if ((int)lane < g.n) {
         if (what & 1u) { const uint32_t e = mine[kFlagSelectCtr]; while ((int32_t)(mine[kFlagSelect + lane] - e) < 0) __nanosleep(32); }
         if (what & 2u) { const uint32_t e = mine[kFlagStatusCtr]; while ((int32_t)(mine[kFlagStatus + lane] - e) < 0) __nanosleep(32); }
+        if (what & 4u) { const uint32_t e = mine[kFlagResultsCtr]; while ((int32_t)(mine[kFlagResults + lane] - e) < 0) __nanosleep(32); }
         __threadfence_system();
     }
 }

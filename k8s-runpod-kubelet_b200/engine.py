@@ -58,6 +58,22 @@ def _changed_list(cap: int, want_codes: bool):
     return ptrs, lambda: (idx[: n.value].copy(), codes[: n.value].copy() if want_codes else None)
 
 
+def results_region(words, n_ranks: int, cap: int, rank: int):
+    """Region ``rank`` of a ``select_pending_changed_gather`` exchange buffer -> (slots uint32[n], best int32[n],
+    top5 int32[n, 5]), n = the region's count.  ``words`` is the buffer (a torch tensor on any device, or a numpy
+    array) as 32-bit words, at least ``results_xchg_bytes(n_ranks, cap) // 4`` of them."""
+    if not isinstance(words, np.ndarray):
+        words = words.cpu().numpy()
+    w = np.ascontiguousarray(words).view(np.int32)
+    if not 0 <= rank < n_ranks or len(w) < 8 + n_ranks * cap * 7:
+        raise ValueError(f"results_region: rank {rank} of {n_ranks}, or a buffer of {len(w)} words for capacity {cap}")
+    n = int(w[rank])
+    if not 0 <= n <= cap:
+        raise ValueError(f"results_region: count {n} of region {rank} is outside [0, {cap}]")
+    r = w[8 + rank * 7 * cap:]
+    return r[:n].view(np.uint32).copy(), r[cap:cap + n].copy(), r[2 * cap:2 * cap + 5 * n].reshape(n, 5).copy()
+
+
 class Engine:
     """One ``rpk_ctx``.  ``n_gpus > 1`` = one process driving several GPUs (the Go kubelet's shape)."""
 
@@ -244,6 +260,22 @@ class Engine:
             raise err
         k = n_c.value
         return n_p.value, n_r.value, slots[:k], best[:k], top5[:k]
+
+    def results_xchg_bytes(self, n_ranks: int, cap: int) -> int:
+        """bytes of one exchange buffer of ``select_pending_changed_gather`` (rpk_results_xchg_bytes)"""
+        return int(self._lib.rpk_results_xchg_bytes(n_ranks, cap))
+
+    def select_pending_changed_gather(self, xchg_ptrs, cap: int, my_rank: int, shard: int = 0, stream=None):
+        """``select_pending_changed`` over the slots rank ``my_rank`` of ``len(xchg_ptrs)`` owns: its changed rows land in
+        region ``my_rank`` of every exchange buffer (raw device pointers, peers' included; read one with
+        ``results_region``), enqueued on ``stream`` behind one synchronise of it (rpk_select_pending_changed_gather).
+        -> (n_pending, n_reselected) of the rank's slots."""
+        n_ranks, xchg = _ptr_array(xchg_ptrs)
+        n_p, n_r = C.c_uint32(0), C.c_uint32(0)
+        self._check(self._lib.rpk_select_pending_changed_gather(
+            self._ctx, shard, n_ranks, my_rank, xchg, cap, C.cast(C.byref(n_p), C.c_void_p), C.cast(C.byref(n_r), C.c_void_p),
+            self._stream(stream, shard)))
+        return n_p.value, n_r.value
 
     def pods_pending_list_device(self, d_slots_out, d_n, shard: int = 0, stream=None):
         """The pending slot ids, ascending, into ``d_slots_out`` (a torch CUDA tensor with one element per slot of the

@@ -9,5 +9,6 @@ if _ROOT not in sys.path:
 _pkg = importlib.import_module("k8s-runpod-kubelet_b200")
 Engine = _pkg.Engine
 RpkError = _pkg.RpkError
+results_region = _pkg.results_region
 synth = _pkg.synth
 _ffi = _pkg._ffi

@@ -56,6 +56,31 @@ if not ONLY_MULTI:
     eng.upload_offers(offers)
     n_p, n_r, sl, _, _ = eng.select_pending_changed(len(pend))
     assert n_r == len(pend) and len(sl) == 0
+    # the same three calls in the exchange form (k_pod_result_diff_xchg) on a second ctx with the same table: one rank,
+    # one local buffer, a bound one-rank flag group; its region must equal the host call's rows
+    import torch  # noqa: E402
+    eg = rpk.Engine(1)
+    eg.upload_offers(offers)
+    eg.pods_reset(200_000)
+    eg.pods_seed_slots(np.arange(200_000, dtype=np.uint32), pods_t)
+    eg.pods_mark_pending(np.arange(200_000, dtype=np.uint32), flags)
+    xbuf = torch.full((eg.results_xchg_bytes(1, 200_000) // 4,), -9, dtype=torch.int32, device="cuda")
+    fl = torch.zeros(64, dtype=torch.int32, device="cuda")
+    eg.peer_bind([fl.data_ptr()], 0)
+    eg.peer_inline_wait(True)
+    got = []
+    for upload in (False, False, True):  # a first call, a steady call, a call after an offer upload
+        if upload:
+            eg.upload_offers(offers)
+        n_p, n_r = eg.select_pending_changed_gather([xbuf.data_ptr()], 200_000, 0)
+        torch.cuda.synchronize()
+        assert n_p == len(pend)
+        got.append((n_r, rpk.results_region(xbuf, 1, 200_000, 0)))
+    (r0, (s0, b0, t0)), (r1, (s1, _, _)), (r2, (s2, _, _)) = got
+    assert r0 == len(pend) and np.array_equal(s0, pend) and np.array_equal(b0, best) and np.array_equal(t0, t5)
+    assert r1 == 0 and len(s1) == 0 and r2 == len(pend) and len(s2) == 0
+    assert int(fl[16].item()) == 3 and int(fl[34].item()) == 3
+    eg.close()
 for stride in () if ONLY_MULTI else (16, 32, 64):
     tab = oracle.StatusTable(30_000, stride)
     e2 = rpk.Engine(1)
