@@ -136,6 +136,28 @@ inline void shard_range(uint32_t total, int n, int s, uint32_t* lo, uint32_t* hi
 
 bool bad_shard(const rpk_ctx* ctx, int shard) { return shard < 0 || (size_t)shard >= ctx->devs.size(); }
 
+// A device entry point on GPU `shard` (in range, its arguments checked), by the ordering rule of rpk.h: under guarded,
+// with the device set, prep(ds) sizes buffers and makes the refusals that need the device (nonzero: its code, and nothing
+// is enqueued); then run(ds, st) enqueues the call on st, the caller's stream or, when NULL, the shard's own, after the
+// last device call of `scope` and recorded as its last one (no scope: neither).
+template <typename Prep, typename Run>
+int device_call(rpk_ctx* ctx, int shard, void* stream, ScratchScope DeviceState::*scope, Prep&& prep, Run&& run) {
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    return guarded(ctx, [&]() -> int {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        if (int rc = prep(ds)) return rc;
+        const cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+        const bool tracked = scope && (ds.*scope).device_begin(st);
+        run(ds, st);
+        if (scope) (ds.*scope).device_end(st, tracked);
+        return RPK_OK;
+    });
+}
+template <typename Run>
+int device_call(rpk_ctx* ctx, int shard, void* stream, ScratchScope DeviceState::*scope, Run&& run) {
+    return device_call(ctx, shard, stream, scope, [](DeviceState&) { return RPK_OK; }, run);
+}
+
 // Where the rows of a select come from.  Host sources (rpk_select, rpk_tick: columns; rpk_select_slots: a list) become
 // device sources by their upload.  Device sources are on the selecting GPU (rpk_select_device*: columns;
 // rpk_select_slots_device*: a list; rpk_select_pending*: the list k_pod_pending or k_pod_stale left there).
@@ -617,72 +639,60 @@ int check_select_ready(rpk_ctx* ctx, const char* who, bool needs_pod_table, int 
     return RPK_OK;
 }
 
-// rpk_select_device_gather, and rpk_select_device_gather_top5 with t5 (its own arguments checked, a.top5 then points
-// into the local top-5 vector); with a device list, the rpk_select_slots_device* calls of the same name (a NULL list
-// with P > 0 already refused).  The shard is in range.
-int select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const RowSource& src, int n_out, int32_t* const* d_best_full,
-                         uint32_t row0, int32_t* d_top5, const Top5Gather* t5, void* stream) {
-    DeviceState& ds = ctx->devs[(size_t)shard];
-    const PeerGroup& peers = ctx->bind[(size_t)shard];
-    cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
-    if (P == 0) {  // nothing to select, but a bound gather still tells its peers that this (empty) shard is done
-        if (n_out <= 1 || peers.n == 0) return RPK_OK;
-        return guarded(ctx, [&]() -> int {
-            RPK_CUDA(cudaSetDevice(ds.dev));
-            const bool tracked = ds.sel_scope.device_begin(st);  // orders the epoch counter after the last gather's
-            ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
-            ds.sel_scope.device_end(st, tracked);
-            return RPK_OK;
-        });
-    }
+// The six rpk_select*_device* calls (`who` names the one called; src is a device list for the rpk_select_slots_device*
+// calls): the select of P rows into d_best_full[0, n_out) from row row0 on and into d_top5, or, with gather_top5 (the
+// _top5 calls), the select whose top-5 lists are gathered into d_top5_full[0, n_out).  The top-5 call finds its local
+// top-5 vector before the other refusals, and an empty one still looks it up.
+int select_device(rpk_ctx* ctx, const char* who, int shard, uint32_t P, const RowSource& src, int n_out, int32_t* const* d_best_full,
+                  uint32_t row0, int32_t* d_top5, bool gather_top5, int32_t* const* d_top5_full, void* stream) {
+    if (!ctx) return RPK_EINVAL;
+    const std::string w(who);
     const bool list = src.kind == RowSource::DevList;
-    if ((!list && !src.cols.req_mem) || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, "rpk_select_device: req_mem_gb and 1..8 output vectors are required");
-    for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device: NULL output vector");
-    if (int rc = check_select_ready(ctx, "rpk_select_slots_device", list, shard, false)) return rc;
-    if (int rc = check_select_ready(ctx, "rpk_select", false, shard)) return rc;
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        DeviceState::Lane& ln = ds.lane[0];
-        reserve_lane(ln, P, src, false);
-        SelectArgs a{};
-        const bool tracked = ds.sel_scope.device_begin(st);  // the gather writes lane 0's columns: after the last select
-        ctx->launches += (uint64_t)pod_columns(ds, ln, src, 0, P, a, st);
-        a.P = P;
-        for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
-        a.n_out = n_out; a.row0 = row0;
-        a.top5 = t5 ? t5->out[t5->self_out] + (size_t)RPK_TOPK * row0 : d_top5;
-        a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
-        if (n_out > 1) a.peers = peers;
-        ctx->launches += (uint64_t)enqueue_select(ds, ln, a, st, t5);
-        ds.sel_scope.device_end(st, tracked);
-        count_select(ctx, P, ds.G);
-        return RPK_OK;
-    });
-}
-
-// rpk_select_device_gather_top5 and rpk_select_slots_device_gather_top5: the top-5 vectors' checks, then the gather.
-// The shard is in range.
-int select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const RowSource& src, int n_out, int32_t* const* d_best_full,
-                              int32_t* const* d_top5_full, uint32_t row0, void* stream) {
-    if (!d_best_full || !d_top5_full || n_out < 1 || n_out > RPK_MAX_GPUS)
-        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 1..8 best and top-5 vectors are required");
-    for (int o = 0; o < n_out; ++o)
-        if (!d_best_full[o] || !d_top5_full[o]) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: NULL output vector");
-    if ((uint64_t)P * RPK_TOPK > UINT32_MAX) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: 5*P does not fit in uint32_t");
-    if (!same_phase(n_out, d_top5_full))
-        return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: the top-5 vectors differ in 16-byte phase");
-    DeviceState& ds = ctx->devs[(size_t)shard];
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, w + ": shard out of range");
+    if (list && P > 0 && !src.slots) return fail(ctx, RPK_EINVAL, w + ": d_slots is required");
     Top5Gather t5{};
-    const int rc = guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        t5.self_out = local_vector(ctx, shard, ds.dev, n_out, d_top5_full);
-        return RPK_OK;
-    });
-    if (rc != RPK_OK) return rc;
-    if (t5.self_out < 0) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: no top-5 vector lives on GPU `shard`");
-    for (int o = 0; o < n_out; ++o) t5.out[o] = d_top5_full[o];
-    t5.n_out = n_out;
-    return select_device_gather(ctx, shard, P, src, n_out, d_best_full, row0, nullptr, &t5, stream);
+    if (gather_top5) {
+        if (!d_best_full || !d_top5_full || n_out < 1 || n_out > RPK_MAX_GPUS) return fail(ctx, RPK_EINVAL, w + ": 1..8 best and top-5 vectors are required");
+        for (int o = 0; o < n_out; ++o) if (!d_best_full[o] || !d_top5_full[o]) return fail(ctx, RPK_EINVAL, w + ": NULL output vector");
+        if ((uint64_t)P * RPK_TOPK > UINT32_MAX) return fail(ctx, RPK_EINVAL, w + ": 5*P does not fit in uint32_t");
+        if (!same_phase(n_out, d_top5_full)) return fail(ctx, RPK_EINVAL, w + ": the top-5 vectors differ in 16-byte phase");
+        for (int o = 0; o < n_out; ++o) t5.out[o] = d_top5_full[o];
+        t5.n_out = n_out;
+    }
+    const PeerGroup& peers = ctx->bind[(size_t)shard];
+    // P = 0: nothing to select, but a bound gather still tells its peers that this (empty) shard is done, after the
+    // last gather's epoch counter
+    const bool signal = P == 0 && n_out > 1 && peers.n > 0;
+    if (P == 0 && !signal && !gather_top5) return RPK_OK;
+    return device_call(ctx, shard, stream, P > 0 || signal ? &DeviceState::sel_scope : nullptr,
+        [&](DeviceState& ds) -> int {
+            if (gather_top5 && (t5.self_out = local_vector(ctx, shard, ds.dev, n_out, d_top5_full)) < 0)
+                return fail(ctx, RPK_EINVAL, w + ": no top-5 vector lives on GPU `shard`");
+            if (P == 0) return RPK_OK;
+            if ((!list && !src.cols.req_mem) || !d_best_full || n_out < 1 || n_out > RPK_MAX_GPUS)
+                return fail(ctx, RPK_EINVAL, w + (list ? ": " : ": req_mem_gb and ") + "1..8 output vectors are required");
+            for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, w + ": NULL output vector");
+            if (int rc = check_select_ready(ctx, who, list, shard)) return rc;
+            reserve_lane(ds.lane[0], P, src, false);
+            return RPK_OK;
+        },
+        [&](DeviceState& ds, cudaStream_t st) {
+            if (P == 0) {
+                if (signal) ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
+                return;
+            }
+            DeviceState::Lane& ln = ds.lane[0];  // the gather writes lane 0's columns: after the last select
+            SelectArgs a{};
+            ctx->launches += (uint64_t)pod_columns(ds, ln, src, 0, P, a, st);
+            a.P = P;
+            for (int o = 0; o < n_out; ++o) a.best_out[o] = d_best_full[o];
+            a.n_out = n_out; a.row0 = row0;
+            a.top5 = gather_top5 ? t5.out[t5.self_out] + (size_t)RPK_TOPK * row0 : d_top5;
+            a.self_out = find_local_vector(ctx, shard, ds.dev, n_out, d_best_full);
+            if (n_out > 1) a.peers = peers;
+            ctx->launches += (uint64_t)enqueue_select(ds, ln, a, st, gather_top5 ? &t5 : nullptr);
+            count_select(ctx, P, ds.G);
+        });
 }
 
 }  // namespace
@@ -832,26 +842,23 @@ int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int
 int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
                              const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud,
                              int n_out, int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
-    if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_device: shard out of range");
     const RowSource src{RowSource::DevCols, PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
-    return select_device_gather(ctx, shard, P, src, n_out, d_best_full, row0, d_top5, nullptr, stream);
+    return select_device(ctx, "rpk_select_device_gather", shard, P, src, n_out, d_best_full, row0, d_top5, false, nullptr, stream);
 }
 
 int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
                                   const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud, int n_out,
                                   int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
-    if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_device_gather_top5: shard out of range");
     const RowSource src{RowSource::DevCols, PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
-    return select_device_gather_top5(ctx, shard, P, src, n_out, d_best_full, d_top5_full, row0, stream);
+    return select_device(ctx, "rpk_select_device_gather_top5", shard, P, src, n_out, d_best_full, row0, nullptr, true, d_top5_full, stream);
 }
 
 int rpk_select_device(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
                       const int32_t* d_req_ram_gb, const double* d_max_price, const uint8_t* d_cloud, int32_t* d_best,
                       int32_t* d_top5, void* stream) {
     int32_t* outs[1] = {d_best};
-    return rpk_select_device_gather(ctx, shard, P, d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud, 1, outs, 0, d_top5, stream);
+    const RowSource src{RowSource::DevCols, PodCols{d_req_mem_gb, d_req_vcpu, d_req_ram_gb, d_max_price, d_cloud}, nullptr};
+    return select_device(ctx, "rpk_select_device", shard, P, src, 1, outs, 0, d_top5, false, nullptr, stream);
 }
 
 int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t* req_vcpu, const int32_t* req_ram_gb,
@@ -938,24 +945,21 @@ int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int3
 
 int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
                                    int32_t* const* d_best_full, uint32_t row0, int32_t* d_top5, void* stream) {
-    if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: shard out of range");
-    if (n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device: d_slots is required");
-    return select_device_gather(ctx, shard, n_slots, RowSource{RowSource::DevList, PodCols{}, d_slots}, n_out, d_best_full, row0, d_top5, nullptr, stream);
+    const RowSource src{RowSource::DevList, PodCols{}, d_slots};
+    return select_device(ctx, "rpk_select_slots_device_gather", shard, n_slots, src, n_out, d_best_full, row0, d_top5, false, nullptr, stream);
 }
 
 int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
                                         int32_t* const* d_best_full, int32_t* const* d_top5_full, uint32_t row0, void* stream) {
-    if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: shard out of range");
-    if (n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_select_slots_device_gather_top5: d_slots is required");
-    return select_device_gather_top5(ctx, shard, n_slots, RowSource{RowSource::DevList, PodCols{}, d_slots}, n_out, d_best_full, d_top5_full, row0, stream);
+    const RowSource src{RowSource::DevList, PodCols{}, d_slots};
+    return select_device(ctx, "rpk_select_slots_device_gather_top5", shard, n_slots, src, n_out, d_best_full, row0, nullptr, true, d_top5_full, stream);
 }
 
 int rpk_select_slots_device(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int32_t* d_best, int32_t* d_top5,
                             void* stream) {
     int32_t* outs[1] = {d_best};
-    return rpk_select_slots_device_gather(ctx, shard, n_slots, d_slots, 1, outs, 0, d_top5, stream);
+    const RowSource src{RowSource::DevList, PodCols{}, d_slots};
+    return select_device(ctx, "rpk_select_slots_device", shard, n_slots, src, 1, outs, 0, d_top5, false, nullptr, stream);
 }
 
 // ---- pending set of the pod table ---------------------------------------------------------------------------
@@ -1008,13 +1012,9 @@ int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out,
     if (int rc = check_select_ready(ctx, "rpk_pods_pending_list_device", true, shard, false)) return rc;
     DeviceState& ds = ctx->devs[(size_t)shard];
     if (!d_n || (ds.podsN > 0 && !d_slots_out)) return fail(ctx, RPK_EINVAL, "rpk_pods_pending_list_device: d_slots_out and d_n are required");
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
-        const bool tracked = ds.sel_scope.device_begin(st);  // the look-back state is the shard's: after the last list
+    // the look-back state is the shard's: after the last list
+    return device_call(ctx, shard, stream, &DeviceState::sel_scope, [&](DeviceState&, cudaStream_t st) {
         ctx->launches += (uint64_t)enqueue_pending_list(ds, d_slots_out, d_n, st);
-        ds.sel_scope.device_end(st, tracked);
-        return RPK_OK;
     });
 }
 
@@ -1270,9 +1270,7 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
     if (cap < hi - lo) return fail(ctx, RPK_EINVAL, std::string(who) + ": cap is below the number of slots the rank owns");
     if (int rc = check_results_range(ctx, ds, lo, hi, who)) return rc;
     const uint32_t gen = ctx->offer_gen;
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
+    return device_call(ctx, shard, stream, nullptr, [&](DeviceState&, cudaStream_t st) {
         ds.sel_scope.host_wait();
         uint64_t launches = (uint64_t)enqueue_stale(ds, lo, hi, gen, st);
         RPK_CUDA(cudaStreamSynchronize(st));  // the select needs the row count on the host
@@ -1294,7 +1292,6 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
         ds.sel_scope.device_end(st, true);
         ctx->launches += launches;
         if (k) count_select(ctx, k, ds.G);
-        return RPK_OK;
     });
 }
 
@@ -1304,8 +1301,7 @@ int rpk_ipc_alloc(rpk_ctx* ctx, int shard, size_t bytes, void** d_ptr, unsigned 
     if (!ctx) return RPK_EINVAL;
     if (bad_shard(ctx, shard) || !d_ptr || !handle_out || bytes == 0) return fail(ctx, RPK_EINVAL, "rpk_ipc_alloc: bad argument");
     static_assert(sizeof(cudaIpcMemHandle_t) == 64, "CUDA IPC handle is 64 bytes");
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)shard].dev));
+    return device_call(ctx, shard, nullptr, nullptr, [&](DeviceState&, cudaStream_t) {
         void* p = nullptr;
         RPK_CUDA(cudaMalloc(&p, bytes));
         RPK_CUDA(cudaMemset(p, 0, bytes));
@@ -1315,22 +1311,19 @@ int rpk_ipc_alloc(rpk_ctx* ctx, int shard, size_t bytes, void** d_ptr, unsigned 
         memcpy(handle_out, &h, 64);
         ctx->ipc_owned.emplace_back(shard, p);
         *d_ptr = p;
-        return RPK_OK;
     });
 }
 
 int rpk_ipc_open(rpk_ctx* ctx, int shard, const unsigned char handle[64], void** d_peer_ptr) {
     if (!ctx) return RPK_EINVAL;
     if (bad_shard(ctx, shard) || !handle || !d_peer_ptr) return fail(ctx, RPK_EINVAL, "rpk_ipc_open: bad argument");
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)shard].dev));
+    return device_call(ctx, shard, nullptr, nullptr, [&](DeviceState&, cudaStream_t) {
         cudaIpcMemHandle_t h;
         memcpy(&h, handle, 64);
         void* p = nullptr;
         RPK_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
         ctx->ipc_mapped.emplace_back(shard, p);
         *d_peer_ptr = p;
-        return RPK_OK;
     });
 }
 
@@ -1343,21 +1336,13 @@ static int drop_entry(std::vector<std::pair<int, void*>>& v, int shard, void* p)
 int rpk_ipc_close(rpk_ctx* ctx, int shard, void* d_peer_ptr) {
     if (!ctx) return RPK_EINVAL;
     if (!drop_entry(ctx->ipc_mapped, shard, d_peer_ptr)) return fail(ctx, RPK_EINVAL, "rpk_ipc_close: pointer was not opened by this ctx");
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)shard].dev));
-        RPK_CUDA(cudaIpcCloseMemHandle(d_peer_ptr));
-        return RPK_OK;
-    });
+    return device_call(ctx, shard, nullptr, nullptr, [&](DeviceState&, cudaStream_t) { RPK_CUDA(cudaIpcCloseMemHandle(d_peer_ptr)); });
 }
 
 int rpk_ipc_free(rpk_ctx* ctx, int shard, void* d_ptr) {
     if (!ctx) return RPK_EINVAL;
     if (!drop_entry(ctx->ipc_owned, shard, d_ptr)) return fail(ctx, RPK_EINVAL, "rpk_ipc_free: pointer was not allocated by this ctx");
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ctx->devs[(size_t)shard].dev));
-        RPK_CUDA(cudaFree(d_ptr));
-        return RPK_OK;
-    });
+    return device_call(ctx, shard, nullptr, nullptr, [&](DeviceState&, cudaStream_t) { RPK_CUDA(cudaFree(d_ptr)); });
 }
 
 int rpk_peer_fence(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int my_rank, uint32_t epoch, void* stream) {
@@ -1365,14 +1350,11 @@ int rpk_peer_fence(rpk_ctx* ctx, int shard, int n, uint32_t* const* d_flags, int
     if (bad_shard(ctx, shard) || n < 1 || n > RPK_MAX_GPUS || !d_flags || my_rank < 0 || my_rank >= n)
         return fail(ctx, RPK_EINVAL, "rpk_peer_fence: bad argument");
     for (int r = 0; r < n; ++r) if (!d_flags[r]) return fail(ctx, RPK_EINVAL, "rpk_peer_fence: NULL flag array");
-    DeviceState& ds = ctx->devs[(size_t)shard];
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
+    return device_call(ctx, shard, stream, nullptr, [&](DeviceState&, cudaStream_t st) {
         PeerGroup g{};
         for (int r = 0; r < n; ++r) g.flags[r] = d_flags[r];
         g.n = n; g.my_rank = my_rank;
-        ctx->launches += (uint64_t)launch_peer_signal(g, epoch, true, stream ? (cudaStream_t)stream : ds.stream);
-        return RPK_OK;
+        ctx->launches += (uint64_t)launch_peer_signal(g, epoch, true, st);
     });
 }
 
@@ -1400,11 +1382,8 @@ int rpk_peer_wait(rpk_ctx* ctx, int shard, unsigned what, void* stream) {
     if (!ctx) return RPK_EINVAL;
     if (bad_shard(ctx, shard) || (what & ~7u) || !what) return fail(ctx, RPK_EINVAL, "rpk_peer_wait: bad argument");
     if (ctx->bind[(size_t)shard].n == 0) return fail(ctx, RPK_ESTATE, "rpk_peer_wait: no flags bound (rpk_peer_bind)");
-    DeviceState& ds = ctx->devs[(size_t)shard];
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        ctx->launches += (uint64_t)launch_peer_wait(ctx->bind[(size_t)shard], what, stream ? (cudaStream_t)stream : ds.stream);
-        return RPK_OK;
+    return device_call(ctx, shard, stream, nullptr, [&](DeviceState&, cudaStream_t st) {
+        ctx->launches += (uint64_t)launch_peer_wait(ctx->bind[(size_t)shard], what, st);
     });
 }
 
@@ -1416,8 +1395,8 @@ const int32_t* rpk_best_device_ptr(const rpk_ctx* ctx, int shard) {
 
 // ---- status --------------------------------------------------------------------------------------------
 
-static int check_stride(rpk_ctx* ctx, uint32_t stride) {
-    if (stride < 16 || stride > 256 || (stride & 15)) return fail(ctx, RPK_EINVAL, "status stride must be a multiple of 16 in [16, 256]");
+static int check_stride(rpk_ctx* ctx, uint32_t stride, const char* who) {
+    if (stride < 16 || stride > 256 || (stride & 15)) return fail(ctx, RPK_EINVAL, std::string(who) + ": status stride must be a multiple of 16 in [16, 256]");
     return RPK_OK;
 }
 
@@ -1444,7 +1423,7 @@ namespace {
 // point in the messages).  The first sweep of a ctx sizes the tracked table to its N.
 int check_sweep(rpk_ctx* ctx, const StatusHostArgs& h, const char* who) {
     const std::string w(who);
-    if (int rc = check_stride(ctx, h.stride)) return rc;
+    if (int rc = check_stride(ctx, h.stride, who)) return rc;
     if (h.N > 0 && !h.records) return fail(ctx, RPK_EINVAL, w + ": records is NULL");
     if (h.report && (!h.n_changed || (h.N > 0 && !h.changed_idx))) return fail(ctx, RPK_EINVAL, w + ": changed_idx and n_changed are required");
     if (!ctx->devs[0].status_sized) { if (int rc = rpk_status_reset(ctx, h.N)) return rc; }
@@ -1452,9 +1431,9 @@ int check_sweep(rpk_ctx* ctx, const StatusHostArgs& h, const char* who) {
     return RPK_OK;
 }
 
-int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
+int status_host(rpk_ctx* ctx, const StatusHostArgs& h, const char* who) {
     if (!ctx) return RPK_EINVAL;
-    if (int rc = check_sweep(ctx, h, "rpk_status_diff")) return rc;
+    if (int rc = check_sweep(ctx, h, who)) return rc;
     return guarded(ctx, [&]() -> int { run_host(ctx, nullptr, &h, false); return RPK_OK; });
 }
 
@@ -1462,21 +1441,21 @@ int status_host(rpk_ctx* ctx, const StatusHostArgs& h) {
 
 int rpk_status_diff(rpk_ctx* ctx, uint32_t N, const uint8_t* records, uint32_t stride, uint32_t* changed_idx,
                     uint32_t* n_changed, uint64_t* hashes_out) {
-    return status_host(ctx, StatusHostArgs{N, records, stride, changed_idx, nullptr, n_changed, hashes_out, true});
+    return status_host(ctx, StatusHostArgs{N, records, stride, changed_idx, nullptr, n_changed, hashes_out, true}, "rpk_status_diff");
 }
 
 int rpk_status_diff_codes(rpk_ctx* ctx, uint32_t N, const uint8_t* records, uint32_t stride, uint32_t* changed_idx,
                           uint16_t* changed_code, uint32_t* n_changed, uint64_t* hashes_out) {
-    return status_host(ctx, StatusHostArgs{N, records, stride, changed_idx, changed_code, n_changed, hashes_out, true});
+    return status_host(ctx, StatusHostArgs{N, records, stride, changed_idx, changed_code, n_changed, hashes_out, true}, "rpk_status_diff_codes");
 }
 
 int rpk_status_seed(rpk_ctx* ctx, uint32_t N, const uint8_t* records, uint32_t stride) {
-    return status_host(ctx, StatusHostArgs{N, records, stride, nullptr, nullptr, nullptr, nullptr, false});
+    return status_host(ctx, StatusHostArgs{N, records, stride, nullptr, nullptr, nullptr, nullptr, false}, "rpk_status_seed");
 }
 
 int rpk_status_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* records, uint32_t stride) {
     if (!ctx) return RPK_EINVAL;
-    if (int rc = check_stride(ctx, stride)) return rc;
+    if (int rc = check_stride(ctx, stride, "rpk_status_seed_slots")) return rc;
     if (n_slots == 0) return RPK_OK;
     if (!slots || !records) return fail(ctx, RPK_EINVAL, "rpk_status_seed_slots: slots and records are required");
     if (!ctx->devs[0].status_sized) return fail(ctx, RPK_ESTATE, "rpk_status_seed_slots: no tracked table (call rpk_status_reset first)");
@@ -1504,7 +1483,7 @@ int rpk_status_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
 int rpk_status_diff_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, const uint8_t* records, uint32_t stride,
                           uint32_t* changed_idx, uint16_t* changed_code, uint32_t* n_changed) {
     if (!ctx) return RPK_EINVAL;
-    if (int rc = check_stride(ctx, stride)) return rc;
+    if (int rc = check_stride(ctx, stride, "rpk_status_diff_slots")) return rc;
     if (!n_changed) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: n_changed is required");
     if (n_slots == 0) { *n_changed = 0; return RPK_OK; }
     if (!slots || !records || !changed_idx) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots: slots, records and changed_idx are required");
@@ -1534,69 +1513,78 @@ int rpk_tick(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t*
 }
 
 namespace {
-int status_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride, uint64_t* d_hash_prev,
-                  uint32_t idx_base, uint32_t* d_changed_idx, uint16_t* d_changed_code, uint32_t* d_n_changed, int n_out,
-                  uint32_t* const* d_xchg, uint32_t cap, int my_rank, void* stream, const uint32_t* d_slots = nullptr, uint32_t col_n = 0) {
-    // d_slots: N is the list's length, and the column (col_n rows) holds global slots [idx_base, idx_base + col_n)
+// The arguments of a device sweep, the device counterpart of StatusHostArgs.  list (the rpk_status_diff_slots_device*
+// calls): slots[0, N) lists global slot ids, and the hash column (col_n rows) holds global slots [idx_base, idx_base +
+// col_n).  gather (the _gather calls): the changed list goes into region my_rank of the n_out exchange buffers, of cap
+// entries per rank; with n_out = 0 the call sweeps as the calls without an exchange do.
+struct StatusDeviceArgs {
+    uint32_t N; const uint8_t* records; uint32_t stride; uint64_t* hash_prev; uint32_t idx_base;
+    uint32_t* changed_idx; uint16_t* changed_code; uint32_t* n_changed;
+    bool list; const uint32_t* slots; uint32_t col_n;
+    bool gather; int n_out; uint32_t* const* xchg; uint32_t cap; int my_rank;
+};
+
+// The five rpk_status_diff*_device* calls (`who` names the one called)
+int status_device(rpk_ctx* ctx, const char* who, int shard, const StatusDeviceArgs& d, void* stream) {
     if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: shard out of range");
-    if (int rc = check_stride(ctx, stride)) return rc;
-    if (N > 0 && (!d_records || !d_hash_prev)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: NULL column");
-    if (n_out == 0 && N > 0 && !d_changed_idx) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: d_changed_idx is NULL");
-    if (!d_n_changed) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: d_n_changed is NULL");
-    if (((uintptr_t)d_records | (uintptr_t)d_hash_prev) & 15) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device: d_records and d_hash_prev must be 16-byte aligned");
-    if (n_out < 0 || n_out > RPK_MAX_GPUS || (n_out > 0 && (!d_xchg || my_rank < 0 || my_rank >= n_out || N > cap)))
-        return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: bad exchange arguments (N must fit the per-rank capacity)");
-    for (int o = 0; o < n_out; ++o) if (!d_xchg[o]) return fail(ctx, RPK_EINVAL, "rpk_status_diff_device_gather: NULL exchange buffer");
-    if (d_slots == nullptr && col_n != 0) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: d_slots is NULL");
-    if ((uint64_t)idx_base + col_n > (1ull << 32)) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: idx_base + N exceeds the slot range");
-    DeviceState& ds = ctx->devs[(size_t)shard];
-    return guarded(ctx, [&]() -> int {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        const bool codes = d_changed_code || n_out > 0;
-        reserve_sweep_scratch(ds, N, codes);
-        StatusArgs a{};
-        a.records = d_records; a.stride = stride; a.N = N; a.hash_prev = d_hash_prev; a.hash_out = nullptr;
-        a.changed_idx = d_changed_idx; a.changed_code = d_changed_code; a.n_changed = d_n_changed; a.idx_base = idx_base;
-        sweep_scratch_args(ds, codes, a);
-        a.n_out = n_out;
-        a.slots = d_slots; a.col_n = col_n;
-        for (int o = 0; o < n_out; ++o) {  // rank o's buffer: [counts : 8 words][n_out index regions of cap][n_out code regions of cap u16]
-            uint32_t* base = d_xchg[o];
-            a.out_count[o] = base;
-            a.out_idx[o] = base + 8 + (size_t)my_rank * cap;
-            a.out_code[o] = reinterpret_cast<uint16_t*>(base + 8 + (size_t)n_out * cap) + (size_t)my_rank * cap;
-        }
-        if (n_out > 0) a.peers = ctx->bind[(size_t)shard];
-        a.peers.my_rank = my_rank;  // the sweep fills and signals under the rank its call names
-        cudaStream_t st = stream ? (cudaStream_t)stream : ds.stream;
-        const bool tracked = ds.status_scope.device_begin(st);
-        ds.status_dirty = true;
-        ctx->launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
-        ds.status_dirty = false;
-        ds.status_scope.device_end(st, tracked);
-        ctx->stats.status_calls += 1; ctx->stats.status_records += N;
-        return RPK_OK;
-    });
+    const std::string w(who);
+    if (d.list && d.N > 0 && !d.slots) return fail(ctx, RPK_EINVAL, w + ": d_slots is NULL");
+    if (d.list && d.gather && d.n_out < 1) return fail(ctx, RPK_EINVAL, w + ": n_ranks must be 1..8");
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, w + ": shard out of range");
+    if (int rc = check_stride(ctx, d.stride, who)) return rc;
+    if (d.N > 0 && (!d.records || !d.hash_prev)) return fail(ctx, RPK_EINVAL, w + ": NULL column");
+    if (d.n_out == 0 && d.N > 0 && !d.changed_idx) return fail(ctx, RPK_EINVAL, w + ": d_changed_idx is NULL");
+    if (!d.n_changed) return fail(ctx, RPK_EINVAL, w + ": d_n_changed is NULL");
+    if (((uintptr_t)d.records | (uintptr_t)d.hash_prev) & 15) return fail(ctx, RPK_EINVAL, w + ": d_records and d_hash_prev must be 16-byte aligned");
+    if (d.n_out < 0 || d.n_out > RPK_MAX_GPUS || (d.n_out > 0 && (!d.xchg || d.my_rank < 0 || d.my_rank >= d.n_out || d.N > d.cap)))
+        return fail(ctx, RPK_EINVAL, w + ": bad exchange arguments (N must fit the per-rank capacity)");
+    for (int o = 0; o < d.n_out; ++o) if (!d.xchg[o]) return fail(ctx, RPK_EINVAL, w + ": NULL exchange buffer");
+    const uint32_t col_n = d.N > 0 ? d.col_n : 0;  // an empty list sweeps as an empty table does
+    if ((uint64_t)d.idx_base + col_n > (1ull << 32)) return fail(ctx, RPK_EINVAL, w + ": idx_base + N exceeds the slot range");
+    const bool codes = d.changed_code || d.n_out > 0;
+    return device_call(ctx, shard, stream, &DeviceState::status_scope,
+        [&](DeviceState& ds) { reserve_sweep_scratch(ds, d.N, codes); return RPK_OK; },
+        [&](DeviceState& ds, cudaStream_t st) {
+            StatusArgs a{};
+            a.records = d.records; a.stride = d.stride; a.N = d.N; a.hash_prev = d.hash_prev; a.hash_out = nullptr;
+            a.changed_idx = d.changed_idx; a.changed_code = d.changed_code; a.n_changed = d.n_changed; a.idx_base = d.idx_base;
+            sweep_scratch_args(ds, codes, a);
+            a.n_out = d.n_out;
+            a.slots = d.N > 0 ? d.slots : nullptr; a.col_n = col_n;
+            for (int o = 0; o < d.n_out; ++o) {  // rank o's buffer: [counts : 8 words][n_out index regions of cap][n_out code regions of cap u16]
+                uint32_t* base = d.xchg[o];
+                a.out_count[o] = base;
+                a.out_idx[o] = base + 8 + (size_t)d.my_rank * d.cap;
+                a.out_code[o] = reinterpret_cast<uint16_t*>(base + 8 + (size_t)d.n_out * d.cap) + (size_t)d.my_rank * d.cap;
+            }
+            if (d.n_out > 0) a.peers = ctx->bind[(size_t)shard];
+            a.peers.my_rank = d.my_rank;  // the sweep fills and signals under the rank its call names
+            ds.status_dirty = true;
+            ctx->launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
+            ds.status_dirty = false;
+            ctx->stats.status_calls += 1; ctx->stats.status_records += d.N;
+        });
 }
 }  // namespace
 
 int rpk_status_diff_device(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                            uint64_t* d_hash_prev, uint32_t* d_changed_idx, uint32_t* d_n_changed, void* stream) {
-    return status_device(ctx, shard, N, d_records, stride, d_hash_prev, 0, d_changed_idx, nullptr, d_n_changed, 0, nullptr, 0, 0, stream);
+    return status_device(ctx, "rpk_status_diff_device", shard,
+                         StatusDeviceArgs{N, d_records, stride, d_hash_prev, 0, d_changed_idx, nullptr, d_n_changed}, stream);
 }
 
 int rpk_status_diff_device_codes(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                                  uint64_t* d_hash_prev, uint32_t* d_changed_idx, uint16_t* d_changed_code, uint32_t* d_n_changed, void* stream) {
-    return status_device(ctx, shard, N, d_records, stride, d_hash_prev, 0, d_changed_idx, d_changed_code, d_n_changed, 0, nullptr, 0, 0, stream);
+    return status_device(ctx, "rpk_status_diff_device_codes", shard,
+                         StatusDeviceArgs{N, d_records, stride, d_hash_prev, 0, d_changed_idx, d_changed_code, d_n_changed}, stream);
 }
 
 int rpk_status_diff_slots_device(rpk_ctx* ctx, int shard, uint32_t N, uint32_t idx_base, uint32_t n_slots,
                                  const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* d_hash_prev,
                                  uint32_t* d_changed_idx, uint16_t* d_changed_code, uint32_t* d_n_changed, void* stream) {
-    if (ctx && n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device: d_slots is NULL");
-    return status_device(ctx, shard, n_slots, d_records, stride, d_hash_prev, idx_base, d_changed_idx, d_changed_code, d_n_changed,
-                         0, nullptr, 0, 0, stream, n_slots > 0 ? d_slots : nullptr, n_slots > 0 ? N : 0);
+    return status_device(ctx, "rpk_status_diff_slots_device", shard,
+                         StatusDeviceArgs{n_slots, d_records, stride, d_hash_prev, idx_base, d_changed_idx, d_changed_code, d_n_changed,
+                                          true, d_slots, N}, stream);
 }
 
 size_t rpk_xchg_bytes(int n_ranks, uint32_t cap) { return (size_t)(8 + (size_t)n_ranks * cap) * 4 + (size_t)n_ranks * cap * 2 + 16; }
@@ -1604,7 +1592,9 @@ size_t rpk_xchg_bytes(int n_ranks, uint32_t cap) { return (size_t)(8 + (size_t)n
 int rpk_status_diff_device_gather(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                                   uint64_t* d_hash_prev, uint32_t idx_base, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,
                                   int my_rank, uint32_t* d_n_changed, void* stream) {
-    return status_device(ctx, shard, N, d_records, stride, d_hash_prev, idx_base, nullptr, nullptr, d_n_changed, n_ranks, d_xchg, cap, my_rank, stream);
+    return status_device(ctx, "rpk_status_diff_device_gather", shard,
+                         StatusDeviceArgs{N, d_records, stride, d_hash_prev, idx_base, nullptr, nullptr, d_n_changed,
+                                          false, nullptr, 0, true, n_ranks, d_xchg, cap, my_rank}, stream);
 }
 
 // n_slots bounds what a region receives (list order is not checked on the device), so it is what must fit the capacity
@@ -1612,10 +1602,9 @@ int rpk_status_diff_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t N, uin
                                         const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride,
                                         uint64_t* d_hash_prev, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,
                                         int my_rank, uint32_t* d_n_changed, void* stream) {
-    if (ctx && n_slots > 0 && !d_slots) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device_gather: d_slots is NULL");
-    if (ctx && n_ranks < 1) return fail(ctx, RPK_EINVAL, "rpk_status_diff_slots_device_gather: n_ranks must be 1..8");
-    return status_device(ctx, shard, n_slots, d_records, stride, d_hash_prev, idx_base, nullptr, nullptr, d_n_changed, n_ranks,
-                         d_xchg, cap, my_rank, stream, n_slots > 0 ? d_slots : nullptr, n_slots > 0 ? N : 0);
+    return status_device(ctx, "rpk_status_diff_slots_device_gather", shard,
+                         StatusDeviceArgs{n_slots, d_records, stride, d_hash_prev, idx_base, nullptr, nullptr, d_n_changed,
+                                          true, d_slots, N, true, n_ranks, d_xchg, cap, my_rank}, stream);
 }
 
 int rpk_stats_get(const rpk_ctx* ctx, rpk_stats* out) {
