@@ -117,17 +117,42 @@ func u8p(s []uint8) *C.uint8_t {
 func (e *Engine) UploadOffers(o *Offers) error {
 	e.mu.Lock()
 	defer e.mu.Unlock()
+	_, err := e.installOffers(o, nil)
+	return err
+}
+
+// installOffers passes the six columns to rpk_offers_upload (n == nil) or rpk_offers_refresh; e.mu is held.
+func (e *Engine) installOffers(o *Offers, n *C.uint32_t) (uint32, error) {
 	g := len(o.MemoryInGb)
 	if len(o.SecurePrice) != g || len(o.CommunityPrice) != g || len(o.Flags) != g {
-		return fmt.Errorf("rpk: offer columns differ in length")
+		return 0, fmt.Errorf("rpk: offer columns differ in length")
 	}
-	rc := C.rpk_offers_upload(e.ctx, C.uint32_t(g), i32p(o.MemoryInGb), i32p(o.VCPU), i32p(o.RAMGb),
-		f64p(o.SecurePrice), f64p(o.CommunityPrice), u8p(o.Flags))
+	var rc C.int
+	if n == nil {
+		rc = C.rpk_offers_upload(e.ctx, C.uint32_t(g), i32p(o.MemoryInGb), i32p(o.VCPU), i32p(o.RAMGb),
+			f64p(o.SecurePrice), f64p(o.CommunityPrice), u8p(o.Flags))
+	} else {
+		rc = C.rpk_offers_refresh(e.ctx, C.uint32_t(g), i32p(o.MemoryInGb), i32p(o.VCPU), i32p(o.RAMGb),
+			f64p(o.SecurePrice), f64p(o.CommunityPrice), u8p(o.Flags), n)
+	}
 	if rc != C.RPK_OK {
-		return lastError(e.ctx, rc)
+		return 0, lastError(e.ctx, rc)
 	}
 	e.g = g
-	return nil
+	if n == nil {
+		return 0, nil
+	}
+	return uint32(*n), nil
+}
+
+// RefreshOffers is UploadOffers for a table that mostly equals the resident one: the stored pending results
+// (SelectPendingChanged) that no changed offer can reach stay valid.  It returns the number of offers that
+// changed, or math.MaxUint32 when the stored results were invalidated wholesale (rpk.h, rpk_offers_refresh).
+func (e *Engine) RefreshOffers(o *Offers) (uint32, error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	var n C.uint32_t
+	return e.installOffers(o, &n)
 }
 
 // Select evaluates GetGPUTypes (runpod_client.go:465-509) for every pod of the batch at once.

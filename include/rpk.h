@@ -30,7 +30,7 @@
  *     pod table and the select scratch) and the status scope (the sweep scratch).  A _device call issued on another
  *     stream than the last _device call of its scope first waits for that call, so any streams may be used.  A host
  *     call waits for the last _device call of its scopes before it touches anything, and returns after its own work is
- *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_pods_reset,
+ *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset,
  *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
  *     rpk_select_pending_changed, the _device call
  *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host), and rpk_tick
@@ -121,6 +121,22 @@ void rpk_host_free(void* p);
 int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu, const int32_t* ram_gb,
                       const double* secure_price, const double* community_price, const uint8_t* flags);
 
+/* Offers a refresh remembers as changed between two wholesale invalidations of the pending results (below). */
+#define RPK_OFFERS_DELTA_MAX 16
+
+/* rpk_offers_upload for a table that is mostly the one already resident: the same arguments, argument rules, refusals,
+ * installed table and views.  The one difference is what happens to the results rpk_select_pending_changed[_gather]
+ * stored.  When a table with the same G is resident, every GPU compares the new columns with it, offer by offer and bit
+ * for bit (-0.0 and 0.0 differ), and the changed offers join the ctx's change window: one entry per offer, at the
+ * generation of its latest change.  A stored result then stays valid unless a changed offer can reach its row (the rule
+ * under rpk_select_pending_changed).  *n_offers_changed (nullable) receives the number of offers that differ, or
+ * UINT32_MAX when the stored results are invalidated wholesale instead, as after rpk_offers_upload: no table resident,
+ * another G, or a window that would hold more than RPK_OFFERS_DELTA_MAX offers.  The window is cleared then, and by
+ * every rpk_offers_upload.  An identical table changes nothing (*n_offers_changed = 0).  Select scope, host call. */
+int rpk_offers_refresh(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu, const int32_t* ram_gb,
+                       const double* secure_price, const double* community_price, const uint8_t* flags,
+                       uint32_t* n_offers_changed);
+
 /* ---- selection: P pods x G offers ----------------------------------------------------------------- */
 
 /* For pod row p: feasible(g) = cloud ok && price > 0 && price < max_price[p] && mem_gb[g] >= req_mem_gb[p]
@@ -188,7 +204,14 @@ int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t
  *     sends the whole list); best is top5[0].
  *   - Reselected: a pending slot with no reported result, whose five columns differ bit for bit from the ones its
  *     reported result came from, or whose result predates the last rpk_offers_upload (an upload of an identical table
- *     included).  No other pending slot is recomputed.  *n_reselected counts them.
+ *     included) or the last wholesale invalidation of rpk_offers_refresh.  After that, a result that predates a refresh
+ *     is reselected only when an offer c the window says changed since the result was made reaches the row: c is in the
+ *     reported list L, or c is feasible for the row under the current table (rpk_select's predicate) and L has fewer
+ *     than five entries or (price(c), c) < (price(L[4]), L[4]) in the row's cloud.  Otherwise the list under the current
+ *     table is L, exactly.  No other pending slot is recomputed.  *n_reselected counts them.
+ *   - A pending slot whose result predates a refresh and that no changed offer reaches has its result marked current,
+ *     so later calls do not test it again; this happens on the cap refusal below too, and is not observable: the
+ *     stored list is R(s).
  *   - Reported, ascending by slot: every reselected slot whose R(s) differs from its reported result, or that has none.
  *     Row i is slots_out[i], best[i], top5[5i, 5i+5); *n_changed <= *n_reselected rows.  Each reported R(s) becomes the
  *     slot's reported result.  A caller that applies every report to a mirror kept per SLOT holds R(s) for every pending
@@ -200,7 +223,7 @@ int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t
  *     (capacities cap, cap and 5*cap); else RPK_EINVAL.  No pod table or no offer table: RPK_ESTATE.  Both before
  *     anything is enqueued.
  *   - More than cap slots to reselect: RPK_EINVAL with *n_pending and *n_reselected written, nothing else written, no
- *     stored result changed, nothing counted; retry with cap = *n_reselected.
+ *     stored list changed (only the marking above), nothing counted; retry with cap = *n_reselected.
  *   - Counts as one select in rpk_stats (offer_scores += n_reselected * G) when it reselects anything; a call that
  *     reselects nothing counts no select.  Select scope, host call.
  *   - Multi-GPU ctx: the stored results are sharded by slot range (GPU k owns a contiguous range, its boundaries on
@@ -292,7 +315,8 @@ int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out,
  *     ctx owns in rpk_select_pending_changed (boundaries on 16-slot units), so the ranks' ranges tile the table in rank
  *     order; a range may be empty.  Every rank keeps the whole pod table and the flags (every rank seeds and marks the
  *     same rows, as for rpk_select_slots_device_gather); a rank's stored results cover its own range only.
- *   - Semantics: exactly rpk_select_pending_changed restricted to [lo, hi): the same stale rule, one select with top-5,
+ *   - Semantics: exactly rpk_select_pending_changed restricted to [lo, hi): the same stale rule (with the reach rule of
+ *     rpk_offers_refresh against this ctx's change window, and the same marking of unreached results), one select with top-5,
  *     the same diff, and each reported result becomes the slot's stored result.  *n_pending and *n_reselected count the
  *     rank's own slots.  Counts as one select in rpk_stats when it reselects anything.
  *   - Exchange: the rank's changed rows, ascending by slot, land in region my_rank of every buffer d_xchg[0..n_ranks)

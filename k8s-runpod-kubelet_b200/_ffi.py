@@ -37,6 +37,7 @@ ABI = {
     "rpk_host_alloc": (_p, [_size]),
     "rpk_host_free": (None, [_p]),
     "rpk_offers_upload": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
+    "rpk_offers_refresh": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_select": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_pods_reset": (_int, [_p, _u32]),
     "rpk_pods_seed_slots": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),

@@ -214,6 +214,41 @@ __global__ void k_offer_slices(const uint32_t* __restrict__ bmT, uint32_t* __res
     bmM[i] = sp[m * kSubStride] & sp[other * kSubStride];
 }
 
+// ---- refresh: which offers changed ---------------------------------------------------------------------------
+// One thread per offer, the prices compared as bit patterns (NaN equals itself, -0.0 differs from 0.0).  A warp claims
+// the places of its changed offers with one atomic; the CTA that finishes last publishes the count and the listed indices
+// to the mapped output and clears the state words for the next call.
+__global__ void __launch_bounds__(256) k_offer_diff(OfferDiffArgs a) {
+    __shared__ uint32_t s_last;
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
+    bool ch = false;
+    if (i < a.in.G)
+        ch = a.was.mem[i] != a.in.mem[i] || a.was.vcpu[i] != a.in.vcpu[i] || a.was.ram[i] != a.in.ram[i] ||
+             __double_as_longlong(a.was.secure_price[i]) != __double_as_longlong(a.in.secure_price[i]) ||
+             __double_as_longlong(a.was.community_price[i]) != __double_as_longlong(a.in.community_price[i]) ||
+             a.was.flags[i] != a.in.flags[i];
+    const uint32_t m = __ballot_sync(0xFFFFFFFFu, ch);
+    uint32_t base = 0;
+    if (lane == 0 && m) base = atomicAdd(a.state, (uint32_t)__popc(m));
+    base = __shfl_sync(0xFFFFFFFFu, base, 0) + (uint32_t)__popc(m & ((1u << lane) - 1u));
+    if (ch && base < RPK_OFFERS_DELTA_MAX) a.idx[base] = i;
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) s_last = atomicAdd(a.state + 1, 1u) == gridDim.x - 1 ? 1u : 0u;
+    __syncthreads();
+    if (!s_last) return;
+    const uint32_t n = __ldcg(a.state);
+    for (uint32_t k = threadIdx.x; k < n && k < RPK_OFFERS_DELTA_MAX; k += blockDim.x) a.out[1 + k] = __ldcg(a.idx + k);
+    if (threadIdx.x == 0) { a.out[0] = n; a.state[0] = 0u; a.state[1] = 0u; }
+}
+
+int launch_offer_diff(const OfferDiffArgs& a, cudaStream_t st) {
+    if (a.in.G == 0) return 0;
+    k_offer_diff<<<(a.in.G + 255) / 256, 256, 0, st>>>(a);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
+}
+
 static uint32_t bitlen(uint32_t x) { uint32_t b = 0; while (x) { ++b; x >>= 1; } return b ? b : 1; }
 
 int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st) {

@@ -14,6 +14,8 @@
 //                   check and no upload stand before the gather.
 //   k_pod_stale     of one GPU's owned slots: the ascending list of the pending slots whose stored result is stale, their
 //                   number and the number of pending slots (rpk_select_pending_changed, before its select)
+//   k_pod_stale_reach  the same against a non-empty change window of rpk_offers_refresh: a result older than the
+//                   current table is stale only below the floor or when a changed offer reaches the row
 //   k_pod_result_diff  over the rows that select returned: store each row's result and write the rows whose list changed,
 //                   ascending, to the host (rpk_select_pending_changed, after its select)
 //   k_pod_result_diff_xchg  the same, the changed rows written into region my_rank of every rank's exchange buffer, then
@@ -103,8 +105,10 @@ __device__ __forceinline__ uint32_t count_flags(const uint4& v) {
 }
 
 // The compaction itself, shared by the kernels that turn 16-item units into an ascending list: k_pod_pending (units of
-// the flag column), k_pod_stale (units of a GPU's owned slots) and k_pod_result_diff[_xchg] (units of the reselected rows).
+// the flag column), k_pod_stale[_reach] (units of a GPU's owned slots) and k_pod_result_diff[_xchg] (units of the
+// reselected rows).
 // The policy Pol says what a unit holds:
+//   prepare(c_lo, c_hi)             every thread, once the CTA's share [c_lo, c_hi) is known, before pass 1
 //   V none()                        a unit past the CTA's share
 //   V load(u)                       pass 1's view of unit u
 //   V reload(u)                     pass 2's view of unit u (the thread that loaded u in pass 1: u - c_lo is the same
@@ -129,6 +133,7 @@ __device__ __forceinline__ void compact_units(Pol& p, uint32_t n_units, unsigned
     __syncthreads();
     const uint32_t cid = s_id, n_ctas = gridDim.x;
     const uint32_t c_lo = (uint32_t)((unsigned long long)n_units * cid / n_ctas), c_hi = (uint32_t)((unsigned long long)n_units * (cid + 1) / n_ctas);
+    p.prepare(c_lo, c_hi);
     // ---- pass 1: the CTA's count -> its offset among the CTAs ----
     Count mine = 0;
     for (uint32_t u0 = c_lo + tid; u0 < c_hi; u0 += 4 * kPendThreads) {
@@ -212,6 +217,7 @@ struct FlagUnits {
     __device__ __forceinline__ void fence() const { __threadfence(); }
     __device__ __forceinline__ void last() const {}
     __device__ __forceinline__ void last_warp() const {}
+    __device__ __forceinline__ void prepare(uint32_t, uint32_t) const {}
 };
 
 __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_pending(PendingArgs a, uint32_t n_units) {
@@ -291,11 +297,93 @@ struct StaleUnits {
     __device__ __forceinline__ void fence() const { __threadfence(); }
     __device__ __forceinline__ void last() const { *a.n_pending = atomicExch(a.ticket + 2, 0u); }
     __device__ __forceinline__ void last_warp() const {}
+    __device__ __forceinline__ void prepare(uint32_t, uint32_t) const {}
 };
 
 __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_stale(StaleArgs a, uint32_t n_units) {
     StaleUnits p{a};
     compact_units(p, n_units, a.tile_state, a.ticket);
+}
+
+// The change window of k_pod_stale_reach, staged once per CTA: entry e is offer idx[e], changed at generation gen[e]
+// (newest first), with its columns in the current table
+struct WindowStage {
+    uint32_t idx[RPK_OFFERS_DELTA_MAX], gen[RPK_OFFERS_DELTA_MAX];
+    int32_t mem[RPK_OFFERS_DELTA_MAX], vcpu[RPK_OFFERS_DELTA_MAX], ram[RPK_OFFERS_DELTA_MAX];
+    double sp[RPK_OFFERS_DELTA_MAX], cp[RPK_OFFERS_DELTA_MAX];
+    uint8_t flags[RPK_OFFERS_DELTA_MAX];
+};
+
+// k_pod_stale_reach's units: k_pod_stale's, after a pre-pass over the CTA's share (prepare) that marks current every
+// pending slot whose stored result is older than the current generation, not below the floor, made from the table
+// row's columns, and reached by no window entry newer than it (rpk.h, rpk_select_pending_changed): its list is the
+// row's list under the current table.  Pass 1 then keeps exactly the slots k_pod_stale keeps, and later calls skip the
+// marked slots.  The pre-pass runs before pass 1's four loads are in flight, so the two never share registers; a thread
+// marks the units it loads in pass 1 (u - c_lo the same modulo kPendThreads), so no barrier stands between them.
+struct StaleReachUnits : StaleUnits {
+    const StaleReachArgs& x;
+    const WindowStage& w;
+    // some window entry newer than generation rg reaches the row of global slot s, whose stored list sits at owned index j
+    __device__ __forceinline__ bool reached(uint32_t s, uint32_t j, uint32_t rg) const {
+        uint32_t n = 0;  // the entries newer than rg: a prefix of the window
+        while (n < x.n_win && w.gen[n] > rg) ++n;
+        const int32_t* l = a.r.top5 + (size_t)j * RPK_TOPK;
+        for (int q = 0; q < RPK_TOPK; ++q) {  // rule 1: an entry of the list changed
+            const int32_t lq = l[q];
+            for (uint32_t e = 0; e < n; ++e)
+                if ((int32_t)w.idx[e] == lq) return true;
+        }
+        const uint8_t cloud = a.t.cloud[s];
+        if (cloud > RPK_CLOUD_COMMUNITY) return false;  // nothing is feasible
+        const int32_t mem = a.t.mem[s], vcpu = a.t.vcpu[s], ram = a.t.ram[s], l4 = l[4];
+        const double mx = a.t.max_price[s];
+        const double* price = cloud ? w.cp : w.sp;
+        const double p4 = l4 >= 0 ? (cloud ? x.cp : x.sp)[l4] : 0.0;  // L[4] did not change: its price is the one it was listed at
+        const uint8_t bit = cloud ? (uint8_t)RPK_FLAG_COMMUNITY_CLOUD : (uint8_t)RPK_FLAG_SECURE_CLOUD;
+        for (uint32_t e = 0; e < n; ++e) {  // rule 2: a changed offer is feasible, and L is short or it comes before L[4]
+            const double p = price[e];
+            const int32_t c = (int32_t)w.idx[e];
+            if ((w.flags[e] & bit) && p > 0.0 && p < mx && w.mem[e] >= mem && w.vcpu[e] >= vcpu && w.ram[e] >= ram &&
+                (l4 < 0 || p < p4 || (p == p4 && c < l4)))
+                return true;
+        }
+        return false;
+    }
+    __device__ __forceinline__ void prepare(uint32_t c_lo, uint32_t c_hi) const {
+        for (uint32_t u = c_lo + threadIdx.x; u < c_hi; u += kPendThreads) {
+            const uint32_t g = a.u_lo + u, j = u * kPendUnit, s = g * kPendUnit;
+            const uint32_t pm = nonzero_bytes16(load_flags(a.flags, g, a.N));
+            if (!pm) continue;
+            uint32_t test = 0;  // pending, older than the current generation, not below the floor
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+                const uint4 v = reinterpret_cast<const uint4*>(a.r.gen + j)[q];
+                test |= ((uint32_t)(v.x != a.gen && v.x >= x.floor) | (uint32_t)(v.y != a.gen && v.y >= x.floor) << 1 |
+                         (uint32_t)(v.z != a.gen && v.z >= x.floor) << 2 | (uint32_t)(v.w != a.gen && v.w >= x.floor) << 3) << (4 * q);
+            }
+            for (test &= pm; test; test &= test - 1) {
+                const uint32_t k = (uint32_t)__ffs(test) - 1;
+                if (a.t.mem[s + k] != a.r.mem[j + k] || a.t.vcpu[s + k] != a.r.vcpu[j + k] || a.t.ram[s + k] != a.r.ram[j + k] ||
+                    __double_as_longlong(a.t.max_price[s + k]) != __double_as_longlong(a.r.max_price[j + k]) ||
+                    a.t.cloud[s + k] != a.r.cloud[j + k] || reached(s + k, j + k, a.r.gen[j + k]))
+                    continue;
+                a.r.gen[j + k] = a.gen;
+            }
+        }
+    }
+};
+
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_stale_reach(StaleReachArgs x, uint32_t n_units) {
+    __shared__ WindowStage w;
+    for (uint32_t e = threadIdx.x; e < x.n_win; e += kPendThreads) {
+        const uint2 en = x.win[e];
+        w.idx[e] = en.x; w.gen[e] = en.y;
+        w.mem[e] = x.mem[en.x]; w.vcpu[e] = x.vcpu[en.x]; w.ram[e] = x.ram[en.x];
+        w.sp[e] = x.sp[en.x]; w.cp[e] = x.cp[en.x]; w.flags[e] = x.flags[en.x];
+    }
+    __syncthreads();
+    StaleReachUnits p{{x.s}, x, w};
+    compact_units(p, n_units, x.s.tile_state, x.s.ticket);
 }
 
 // k_pod_result_diff's units: 16 reselected rows.  Pass 1 compares each row's new list with the stored one (a slot never
@@ -340,6 +428,7 @@ struct DiffUnits {
     __device__ __forceinline__ void fence() const { __threadfence(); }
     __device__ __forceinline__ void last() const {}
     __device__ __forceinline__ void last_warp() const {}
+    __device__ __forceinline__ void prepare(uint32_t, uint32_t) const {}
 };
 
 __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff(ResultDiffArgs a, uint32_t n_units) {
@@ -431,6 +520,13 @@ int launch_pod_pending(const PendingArgs& a, int sm_count, cudaStream_t st) {
 int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st) {
     if (n_units == 0) return 0;
     k_pod_stale<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_pod_stale_reach(const StaleReachArgs& a, uint32_t n_units, int sm_count, cudaStream_t st) {
+    if (n_units == 0) return 0;
+    k_pod_stale_reach<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

@@ -81,7 +81,11 @@ struct rpk_ctx {
     std::string err;
     rpk_stats stats;
     uint64_t launches = 0;
-    uint32_t offer_gen = 0;  // rpk_offers_upload calls so far, skipping 0: the generation stored with a pending result
+    // the offer-table generation stored with a pending result: bumped by every upload and by every refresh that changes
+    // an offer, skipping 0.  Results below offer_floor are stale; window (offer index, generation of its latest change;
+    // newest first) lists the offers changed since offer_floor.  Empty window: offer_floor == offer_gen.
+    uint32_t offer_gen = 0, offer_floor = 0;
+    std::vector<uint2> window;
     explicit rpk_ctx(int n_gpus) : devs((size_t)n_gpus), bind((size_t)n_gpus) {}
 };
 
@@ -788,21 +792,67 @@ void rpk_destroy(rpk_ctx* ctx) {
     cudaGetLastError();
 }
 
-int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu, const int32_t* ram_gb,
-                      const double* secure_price, const double* community_price, const uint8_t* flags) {
-    if (!ctx) return RPK_EINVAL;
-    if (G > 0 && (!mem_gb || !secure_price || !community_price || !flags))
-        return fail(ctx, RPK_EINVAL, "rpk_offers_upload: mem_gb, secure_price, community_price and flags are required");
-    if (G > (1u << 26)) return fail(ctx, RPK_EINVAL, "rpk_offers_upload: G above 2^26 offers is not supported");
-    if (has_int32_max(mem_gb, G) || has_int32_max(vcpu, G) || has_int32_max(ram_gb, G))
-        return fail(ctx, RPK_EINVAL, "rpk_offers_upload: offer columns must be < INT32_MAX (requests saturate there)");
-    // every stored pending result is stale from here on; after 2^32 uploads the generations start over, and so do
-    // the stored results
+namespace {
+// Every stored pending result is stale from here on: a new generation becomes the floor and the window is cleared.
+// After 2^32 generations they start over, and so do the stored results.
+void invalidate_results(rpk_ctx* ctx) {
     if (++ctx->offer_gen == 0) {
         ctx->offer_gen = 1;
         for (auto& ds : ctx->devs) ds.res_ready = false;
     }
-    return guarded(ctx, [&]() -> int {
+    ctx->offer_floor = ctx->offer_gen;
+    ctx->window.clear();
+}
+
+// The changed offers the refresh's diffs listed (each GPU diffed its own replica) join the window at a new generation,
+// newest first, and the window goes to every GPU.  Returns the number of changed offers, or UINT32_MAX after a wholesale
+// invalidation: too many changes for the window.
+uint32_t merge_window(rpk_ctx* ctx) {
+    std::vector<uint32_t> changed;
+    for (auto& ds : ctx->devs) {
+        const volatile uint32_t* o = reinterpret_cast<const volatile uint32_t*>(ds.h_delta.h);
+        const uint32_t n = o[0];
+        if (n > RPK_OFFERS_DELTA_MAX) { invalidate_results(ctx); return UINT32_MAX; }
+        for (uint32_t k = 0; k < n; ++k) changed.push_back((uint32_t)o[1 + k]);
+    }
+    std::sort(changed.begin(), changed.end());
+    changed.erase(std::unique(changed.begin(), changed.end()), changed.end());
+    if (changed.empty()) return 0;
+    const uint32_t gen = ctx->offer_gen + 1;
+    if (gen == 0) { invalidate_results(ctx); return UINT32_MAX; }
+    std::vector<uint2> w;
+    for (uint32_t c : changed) w.push_back(make_uint2(c, gen));
+    for (const uint2& e : ctx->window)
+        if (!std::binary_search(changed.begin(), changed.end(), e.x)) w.push_back(e);
+    if (w.size() > RPK_OFFERS_DELTA_MAX) { invalidate_results(ctx); return UINT32_MAX; }
+    ctx->offer_gen = gen;
+    ctx->window.swap(w);
+    for (auto& ds : ctx->devs) {  // on the GPU's stream, finished before the call returns: every reader comes later
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        ds.win.reserve(RPK_OFFERS_DELTA_MAX);
+        RPK_CUDA(cudaMemcpyAsync(ds.win.p, ctx->window.data(), ctx->window.size() * sizeof(uint2), cudaMemcpyHostToDevice, ds.stream));
+        RPK_CUDA(cudaStreamSynchronize(ds.stream));
+    }
+    return (uint32_t)changed.size();
+}
+
+// rpk_offers_upload (refresh false) and rpk_offers_refresh: one ingest.  A refresh of a table with the resident G
+// uploads the new columns next to the resident ones, diffs the two and installs the new ones; everything else is the
+// upload, which invalidates the stored results wholesale.
+int install_offers(rpk_ctx* ctx, const char* who, bool refresh, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu,
+                   const int32_t* ram_gb, const double* secure_price, const double* community_price, const uint8_t* flags,
+                   uint32_t* n_offers_changed) {
+    if (!ctx) return RPK_EINVAL;
+    if (G > 0 && (!mem_gb || !secure_price || !community_price || !flags))
+        return fail(ctx, RPK_EINVAL, std::string(who) + ": mem_gb, secure_price, community_price and flags are required");
+    if (G > (1u << 26)) return fail(ctx, RPK_EINVAL, std::string(who) + ": G above 2^26 offers is not supported");
+    if (has_int32_max(mem_gb, G) || has_int32_max(vcpu, G) || has_int32_max(ram_gb, G))
+        return fail(ctx, RPK_EINVAL, std::string(who) + ": offer columns must be < INT32_MAX (requests saturate there)");
+    bool diff = refresh;
+    for (const auto& ds : ctx->devs) diff = diff && ds.offers_ready && ds.G == G;
+    if (!diff) invalidate_results(ctx);
+    uint32_t changed = UINT32_MAX;
+    const int rc = guarded(ctx, [&]() -> int {
         for (auto& ds : ctx->devs) {
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();  // a device select may still read the views rewritten below
@@ -816,27 +866,62 @@ int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int
                 else if (!strcmp(fk, "bitmap_price")) ds.force_kind = 6;    // ... through the persistent kernel, table staged by price
             }
             const size_t n = G ? G : 1;
-            ds.raw_mem.reserve(n); ds.raw_vcpu.reserve(n); ds.raw_ram.reserve(n); ds.raw_sp.reserve(n); ds.raw_cp.reserve(n); ds.raw_flags.reserve(n);
+            // the new columns go to raw_* (upload) or new_* (diff); after the diff new_* become raw_*
+            DevBuf<int32_t>& c_mem = diff ? ds.new_mem : ds.raw_mem; DevBuf<int32_t>& c_vcpu = diff ? ds.new_vcpu : ds.raw_vcpu;
+            DevBuf<int32_t>& c_ram = diff ? ds.new_ram : ds.raw_ram; DevBuf<double>& c_sp = diff ? ds.new_sp : ds.raw_sp;
+            DevBuf<double>& c_cp = diff ? ds.new_cp : ds.raw_cp; DevBuf<uint8_t>& c_flags = diff ? ds.new_flags : ds.raw_flags;
+            c_mem.reserve(n); c_vcpu.reserve(n); c_ram.reserve(n); c_sp.reserve(n); c_cp.reserve(n); c_flags.reserve(n);
             if (G) {
-                RPK_CUDA(cudaMemcpyAsync(ds.raw_mem.p, mem_gb, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
-                if (vcpu) RPK_CUDA(cudaMemcpyAsync(ds.raw_vcpu.p, vcpu, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
-                else RPK_CUDA(cudaMemsetAsync(ds.raw_vcpu.p, 0, (size_t)G * 4, ds.stream));
-                if (ram_gb) RPK_CUDA(cudaMemcpyAsync(ds.raw_ram.p, ram_gb, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
-                else RPK_CUDA(cudaMemsetAsync(ds.raw_ram.p, 0, (size_t)G * 4, ds.stream));
-                RPK_CUDA(cudaMemcpyAsync(ds.raw_sp.p, secure_price, (size_t)G * 8, cudaMemcpyHostToDevice, ds.stream));
-                RPK_CUDA(cudaMemcpyAsync(ds.raw_cp.p, community_price, (size_t)G * 8, cudaMemcpyHostToDevice, ds.stream));
-                RPK_CUDA(cudaMemcpyAsync(ds.raw_flags.p, flags, (size_t)G, cudaMemcpyHostToDevice, ds.stream));
+                RPK_CUDA(cudaMemcpyAsync(c_mem.p, mem_gb, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
+                if (vcpu) RPK_CUDA(cudaMemcpyAsync(c_vcpu.p, vcpu, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
+                else RPK_CUDA(cudaMemsetAsync(c_vcpu.p, 0, (size_t)G * 4, ds.stream));
+                if (ram_gb) RPK_CUDA(cudaMemcpyAsync(c_ram.p, ram_gb, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
+                else RPK_CUDA(cudaMemsetAsync(c_ram.p, 0, (size_t)G * 4, ds.stream));
+                RPK_CUDA(cudaMemcpyAsync(c_sp.p, secure_price, (size_t)G * 8, cudaMemcpyHostToDevice, ds.stream));
+                RPK_CUDA(cudaMemcpyAsync(c_cp.p, community_price, (size_t)G * 8, cudaMemcpyHostToDevice, ds.stream));
+                RPK_CUDA(cudaMemcpyAsync(c_flags.p, flags, (size_t)G, cudaMemcpyHostToDevice, ds.stream));
+            }
+            if (diff) {
+                if (!ds.delta_state.p) {  // zero between calls: the diff's last CTA clears it again
+                    ds.delta_state.reserve(2); ds.delta_idx.reserve(RPK_OFFERS_DELTA_MAX);
+                    RPK_CUDA(cudaMemsetAsync(ds.delta_state.p, 0, ds.delta_state.cap * sizeof(uint32_t), ds.stream));
+                }
+                ds.h_delta.reserve(4 * (1 + RPK_OFFERS_DELTA_MAX));
+                *reinterpret_cast<volatile uint32_t*>(ds.h_delta.h) = 0u;
+                const OfferDiffArgs da{OfferIngest{G, ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p},
+                                       OfferIngest{G, c_mem.p, c_vcpu.p, c_ram.p, c_sp.p, c_cp.p, c_flags.p},
+                                       ds.delta_state.p, ds.delta_idx.p, reinterpret_cast<uint32_t*>(ds.h_delta.d)};
+                ctx->launches += (uint64_t)launch_offer_diff(da, ds.stream);
+                ds.raw_mem.swap(ds.new_mem); ds.raw_vcpu.swap(ds.new_vcpu); ds.raw_ram.swap(ds.new_ram);
+                ds.raw_sp.swap(ds.new_sp); ds.raw_cp.swap(ds.new_cp); ds.raw_flags.swap(ds.new_flags);
             }
             OfferIngest in{G, ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p};
             ctx->launches += (uint64_t)launch_offer_ingest(ds, in, ds.stream);
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
         }
+        if (diff) changed = merge_window(ctx);
         const DeviceState& d0 = ctx->devs[0];
         ctx->stats.select_kernel_kind = d0.pk.bm_words ? 4u : d0.pk.bits ? (d0.pk.pos_bits ? 3u : 2u) : 1u;
         ctx->stats.distinct_mem = d0.D[0]; ctx->stats.distinct_vcpu = d0.D[1]; ctx->stats.distinct_ram = d0.D[2];
         ctx->stats.packed_bits = d0.pk.bits;
         return RPK_OK;
     });
+    if (rc != RPK_OK && diff) invalidate_results(ctx);  // the table may be half new
+    if (rc == RPK_OK && n_offers_changed) *n_offers_changed = changed;
+    return rc;
+}
+}  // namespace
+
+int rpk_offers_upload(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu, const int32_t* ram_gb,
+                      const double* secure_price, const double* community_price, const uint8_t* flags) {
+    return install_offers(ctx, "rpk_offers_upload", false, G, mem_gb, vcpu, ram_gb, secure_price, community_price, flags, nullptr);
+}
+
+int rpk_offers_refresh(rpk_ctx* ctx, uint32_t G, const int32_t* mem_gb, const int32_t* vcpu, const int32_t* ram_gb,
+                       const double* secure_price, const double* community_price, const uint8_t* flags,
+                       uint32_t* n_offers_changed) {
+    return install_offers(ctx, "rpk_offers_refresh", true, G, mem_gb, vcpu, ram_gb, secure_price, community_price, flags,
+                          n_offers_changed);
 }
 
 int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb, const int32_t* d_req_vcpu,
@@ -1114,18 +1199,22 @@ ResultRows result_rows(DeviceState& ds, bool d) {
 
 // The stale step of ds over its owned slots [lo, hi): k_pod_stale lists the stale pending slots in r_list, and their
 // number and the number of owned pending slots land in the mapped counts (zeroed here; read them after synchronising
-// st).  The caller has waited for the select scope.  Returns the kernels launched.
-int enqueue_stale(DeviceState& ds, uint32_t lo, uint32_t hi, uint32_t gen, cudaStream_t st) {
+// st).  While the ctx's change window is not empty, k_pod_stale_reach takes k_pod_stale's place.  The caller has waited
+// for the select scope.  Returns the kernels launched.
+int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi, cudaStream_t st) {
     reserve_results(ds, lo, hi);
     reserve_compaction_state(ds);
     const ResultRows m = result_rows(ds, true);
     StaleArgs a{};
-    a.flags = ds.pt_pending.p; a.t = ds.pods_table(); a.N = ds.podsN; a.u_lo = lo / 16; a.r = ds.results(); a.gen = gen;
+    a.flags = ds.pt_pending.p; a.t = ds.pods_table(); a.N = ds.podsN; a.u_lo = lo / 16; a.r = ds.results(); a.gen = ctx->offer_gen;
     a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = m.counts; a.n_pending = m.counts + 1;
     a.tile_state = ds.pt_state.p; a.ticket = ds.pt_ticket.p;
     const ResultRows h = result_rows(ds, false);
     reinterpret_cast<volatile uint32_t*>(h.counts)[0] = 0u; reinterpret_cast<volatile uint32_t*>(h.counts)[1] = 0u;
-    return launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, st);
+    if (ctx->window.empty()) return launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, st);
+    const StaleReachArgs x{a, ctx->offer_floor, ds.win.p, (uint32_t)ctx->window.size(),
+                           ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p};
+    return launch_pod_stale_reach(x, (hi - lo + 15) / 16, ds.sm_count, st);
 }
 
 // The reselect of the k stale rows enqueue_stale listed (lane 0's buffers sized for them): the gather, one select with
@@ -1177,7 +1266,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();
-            launches[(size_t)s] += (uint64_t)enqueue_stale(ds, lo, hi, gen, ds.stream);
+            launches[(size_t)s] += (uint64_t)enqueue_stale(ctx, ds, lo, hi, ds.stream);
         }
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
@@ -1272,7 +1361,7 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
     const uint32_t gen = ctx->offer_gen;
     return device_call(ctx, shard, stream, nullptr, [&](DeviceState&, cudaStream_t st) {
         ds.sel_scope.host_wait();
-        uint64_t launches = (uint64_t)enqueue_stale(ds, lo, hi, gen, st);
+        uint64_t launches = (uint64_t)enqueue_stale(ctx, ds, lo, hi, st);
         RPK_CUDA(cudaStreamSynchronize(st));  // the select needs the row count on the host
         const volatile uint32_t* c = result_rows(ds, false).counts;
         const uint32_t k = c[0];

@@ -4,6 +4,7 @@
 #include <stdint.h>
 
 #include <string>
+#include <utility>
 #include <vector>
 
 #include "rpk.h"
@@ -256,6 +257,11 @@ struct OfferIngest {   // raw device columns in, views out
 
 struct DeviceState;
 int launch_offer_ingest(DeviceState& ds, const OfferIngest& in, cudaStream_t st);
+// rpk_offers_refresh: the offers whose six columns differ bit for bit between `was` and `in` (same G).  Their number
+// and the first RPK_OFFERS_DELTA_MAX of their indices, in no particular order, land in out[0] and out[1, ...) (mapped
+// host memory) once the stream has run the kernel.  state: [2] words, zero between calls (the last CTA clears them).
+struct OfferDiffArgs { OfferIngest was, in; uint32_t* state; uint32_t* idx; uint32_t* out; };
+int launch_offer_diff(const OfferDiffArgs& a, cudaStream_t st);
 struct PersistPlan;
 // The top-5 lists' all-gather (rpk_select_device_gather_top5): the top-5 kernel writes out[self_out] (SelectArgs::top5
 // points into it at 5 * row0), and the finished slice [5 * row0, 5 * (row0 + P)) is pushed into the other vectors.
@@ -332,7 +338,17 @@ struct ResultXchgArgs {
     uint32_t* count[RPK_MAX_GPUS];   // word my_rank of buffer o
     PeerGroup peers;                 // bound flags (n = 0: none), my_rank from the call
 };
+// The stale step against a change window (rpk_offers_refresh): a result is also stale below the floor generation, or
+// when a window entry newer than it reaches its row (rpk.h); one that nothing reaches gets generation s.gen.  win holds
+// n_win (offer index, generation) pairs, newest first; the six raw columns are the current table's.
+struct StaleReachArgs {
+    StaleArgs s;
+    uint32_t floor;
+    const uint2* win; uint32_t n_win;
+    const int32_t* mem; const int32_t* vcpu; const int32_t* ram; const double* sp; const double* cp; const uint8_t* flags;
+};
 int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
+int launch_pod_stale_reach(const StaleReachArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
 int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st);
 // launches even when x.d.n = 0: the count 0 still goes out and the peers are still signalled
 int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st);
@@ -355,6 +371,7 @@ struct DevBuf {  // grow-only device buffer, freed by its destructor
         RPK_CUDA(cudaMalloc(&p, want * sizeof(T)));
         cap = want;
     }
+    void swap(DevBuf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
 };
 
 struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches it at d
@@ -409,6 +426,10 @@ struct DeviceState {
     uint32_t G = 0, Gpad = 0;
     bool offers_ready = false;
     DevBuf<int32_t> raw_mem, raw_vcpu, raw_ram; DevBuf<double> raw_sp, raw_cp; DevBuf<uint8_t> raw_flags;
+    // rpk_offers_refresh: the new columns land here next to the resident ones and take their place after the diff; the
+    // diff's state words and index list, its mapped output, and the change window's device copy
+    DevBuf<int32_t> new_mem, new_vcpu, new_ram; DevBuf<double> new_sp, new_cp; DevBuf<uint8_t> new_flags;
+    DevBuf<uint32_t> delta_state, delta_idx; PinnedBuf h_delta; DevBuf<uint2> win;
     DevBuf<unsigned long long> sort_keys; DevBuf<uint32_t> sort_vals;
     DevBuf<uint32_t> v_packed[2]; DevBuf<uint32_t> v_bitmap[2]; DevBuf<uint32_t> v_bitmapT[2]; DevBuf<uint32_t> v_bitmapM[2]; uint32_t nsub = 0; DevBuf<int4> v_wide[2]; DevBuf<double> v_price[2]; DevBuf<int32_t> v_perm[2];
     DevBuf<int32_t> distinct[3]; DevBuf<uint32_t> dcount;

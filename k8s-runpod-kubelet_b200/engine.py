@@ -167,13 +167,27 @@ class Engine:
         return int(self._lib.rpk_launch_count(self._ctx))
 
     # -- offers --------------------------------------------------------------------------------------
-    def upload_offers(self, offers: dict):
+    @staticmethod
+    def _offer_cols(offers: dict):
+        """the offer table -> (G, pointers of its six columns), as rpk_offers_upload and rpk_offers_refresh take them"""
         G = int(offers["mem_gb"].shape[0])
-        self._check(self._lib.rpk_offers_upload(
-            self._ctx, G, _np_ptr(offers["mem_gb"], np.int32, G, "mem_gb"), _np_ptr(offers.get("vcpu"), np.int32, G, "vcpu"),
-            _np_ptr(offers.get("ram_gb"), np.int32, G, "ram_gb"), _np_ptr(offers["secure_price"], np.float64, G, "secure_price"),
-            _np_ptr(offers["community_price"], np.float64, G, "community_price"), _np_ptr(offers["flags"], np.uint8, G, "flags")))
+        return G, [_np_ptr(offers["mem_gb"], np.int32, G, "mem_gb"), _np_ptr(offers.get("vcpu"), np.int32, G, "vcpu"),
+                   _np_ptr(offers.get("ram_gb"), np.int32, G, "ram_gb"), _np_ptr(offers["secure_price"], np.float64, G, "secure_price"),
+                   _np_ptr(offers["community_price"], np.float64, G, "community_price"), _np_ptr(offers["flags"], np.uint8, G, "flags")]
+
+    def upload_offers(self, offers: dict):
+        G, cols = self._offer_cols(offers)
+        self._check(self._lib.rpk_offers_upload(self._ctx, G, *cols))
         self.G = G
+
+    def refresh_offers(self, offers: dict) -> int:
+        """``upload_offers`` that keeps the stored pending results a changed offer cannot reach (rpk_offers_refresh).
+        Returns the number of offers that changed, or ``2**32 - 1`` when the stored results were invalidated wholesale."""
+        G, cols = self._offer_cols(offers)
+        n = C.c_uint32(0)
+        self._check(self._lib.rpk_offers_refresh(self._ctx, G, *cols, C.cast(C.byref(n), C.c_void_p)))
+        self.G = G
+        return int(n.value)
 
     # -- selection -----------------------------------------------------------------------------------
     def select(self, pods: dict, want_top5: bool = False, out_best=None, out_top5=None):

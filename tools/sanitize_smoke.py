@@ -56,6 +56,13 @@ if not ONLY_MULTI:
     eng.upload_offers(offers)
     n_p, n_r, sl, _, _ = eng.select_pending_changed(len(pend))
     assert n_r == len(pend) and len(sl) == 0
+    # a refresh (k_offer_diff) that changes two offers, then the reach step (k_pod_stale_reach) and a steady call
+    fresh = {k: (v.copy() if v is not None else None) for k, v in offers.items()}
+    fresh["secure_price"][:2] *= 0.5
+    assert eng.refresh_offers(fresh) == 2
+    assert 0 < eng.select_pending_changed(len(pend))[1] < len(pend), "two offers reach some rows, not every row"
+    assert eng.select_pending_changed(len(pend))[1] == 0
+    eng.upload_offers(offers)
     # the same three calls in the exchange form (k_pod_result_diff_xchg) on a second ctx with the same table: one rank,
     # one local buffer, a bound one-rank flag group; its region must equal the host call's rows
     import torch  # noqa: E402
