@@ -33,7 +33,8 @@
  *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset,
  *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
  *     rpk_select_pending_changed, the _device call
- *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host), and rpk_tick
+ *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host),
+ *     rpk_select_pending_changed_device_gather, and rpk_tick
  *     with P > 0.  Status scope: rpk_status_diff,
  *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset and
  *     rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
@@ -341,6 +342,32 @@ int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out,
 size_t rpk_results_xchg_bytes(int n_ranks, uint32_t cap);
 int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg, uint32_t cap,
                                       uint32_t* n_pending, uint32_t* n_reselected, void* stream);
+/* rpk_select_pending_changed_gather with the row count kept on the device, so the tick never waits for the host and can
+ * be captured in a CUDA graph.  Everything not listed here is as there.
+ *   - Semantics: identical.  The owned range, the stale rule (the reach rule against the ctx's change window and the
+ *     marking of unreached results included), one select with top-5, the diff, each reported result becoming the slot's
+ *     stored result, the exchange layout (rpk_results_xchg_bytes), the bound signal on the pending results epoch (word
+ *     34, flag words 16 + my_rank) and the inline wait.  The regions are bit for bit what the host-sync form writes after
+ *     the same history; the two forms may be mixed on one ctx.
+ *   - Counts: d_counts (nullable; device memory on GPU `shard`, 4-byte aligned) receives [n_pending, n_reselected] of
+ *     the rank's range.  Nothing is read back to the host.
+ *   - Refusals: every refusal of rpk_select_pending_changed_gather except the NULL count pointers, plus a d_counts that is
+ *     not 4-byte aligned (RPK_EINVAL); all before anything is enqueued and without signalling.
+ *   - Ordering: a _device call of the select scope, ordered like rpk_select_slots_device: no host wait; host calls wait for
+ *     it as for any other device call.  The kernels are sized for the rank's worst case, hi - lo rows, and read the row
+ *     count the stale step left on the device.
+ *   - Graph capture: the first call after rpk_pods_reset sizes every buffer for hi - lo rows and synchronises the device
+ *     (make it outside a capture, and before the inline wait is turned on, as for the host-sync form).  After one call
+ *     with the same (n_ranks, my_rank, cap) on a pod table of the same N, the call only enqueues launches.  A replay reads
+ *     the flags, the pod rows and the stored results as they are at replay time, so seeds and marks between replays are
+ *     picked up.  The reselected rows go to scratch of this call's own (41 bytes per owned slot, allocated by its first
+ *     call), so selects of any size on the ctx between replays leave a captured graph valid.  The offer-table generation
+ *     and change window are taken at capture: rpk_offers_upload, rpk_offers_refresh and rpk_pods_reset each invalidate a
+ *     captured graph (re-capture after them), as does a call with another range, which is refused at call time but not
+ *     at replay.
+ *   - Stats: not counted in rpk_stats (the host never learns n_reselected); rpk_launch_count counts what was enqueued. */
+int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg,
+                                             uint32_t cap, uint32_t* d_counts, void* stream);
 
 /* Cross-process peer vectors for one-process-per-GPU callers (torchrun-style): allocate a plain cudaMalloc
  * buffer on GPU `shard` and export its 64-byte CUDA IPC handle; another process opens the handle and gets a

@@ -54,6 +54,7 @@ ABI = {
     "rpk_pods_pending_list_device": (_int, [_p, _int, _p, _p, _p]),
     "rpk_results_xchg_bytes": (_size, [_int, _u32]),
     "rpk_select_pending_changed_gather": (_int, [_p, _int, _int, _int, _pp, _u32, _p, _p, _p]),
+    "rpk_select_pending_changed_device_gather": (_int, [_p, _int, _int, _int, _pp, _u32, _p, _p]),
     "rpk_ipc_alloc": (_int, [_p, _int, _size, _pp, C.c_char_p]),
     "rpk_ipc_open": (_int, [_p, _int, C.c_char_p, _pp]),
     "rpk_ipc_close": (_int, [_p, _int, _p]),

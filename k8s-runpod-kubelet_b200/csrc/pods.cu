@@ -19,7 +19,8 @@
 //   k_pod_result_diff  over the rows that select returned: store each row's result and write the rows whose list changed,
 //                   ascending, to the host (rpk_select_pending_changed, after its select)
 //   k_pod_result_diff_xchg  the same, the changed rows written into region my_rank of every rank's exchange buffer, then
-//                   a peer signal (rpk_select_pending_changed_gather)
+//                   a peer signal (rpk_select_pending_changed_gather; with the row count read on the device,
+//                   rpk_select_pending_changed_device_gather)
 // The host entry points check every slot against the table's N before its upload.  The device entry points cannot, so
 // an entry outside [0, N) is defined here: the seed skips it, and the gather writes a row with cloud byte kCloudNone,
 // which every select path finishes as "neither cloud" (runpod_client.go:469-475): -1 and five -1.  No caller input
@@ -394,11 +395,13 @@ struct DiffUnits {
     using Count = uint32_t;
     const ResultDiffArgs& a;
     __device__ __forceinline__ V none() const { return V{0u}; }
-    __device__ __forceinline__ V load(uint32_t u) const {
+    __device__ __forceinline__ V load(uint32_t u) const { return load_n(u, a.n); }
+    // unit u of a list of n rows
+    __device__ __forceinline__ V load_n(uint32_t u, uint32_t n) const {
         uint32_t keep = 0;
         for (uint32_t k = 0; k < kPendUnit; ++k) {
             const uint32_t i = u * kPendUnit + k;
-            if (i >= a.n) break;
+            if (i >= n) break;
             const uint32_t j = a.list[i] - a.r_lo;
             const int32_t* nt = a.top5 + (size_t)i * RPK_TOPK;
             int32_t* ot = a.r.top5 + (size_t)j * RPK_TOPK;
@@ -463,9 +466,26 @@ struct DiffXchgUnits : DiffUnits {
     }
 };
 
-__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff_xchg(ResultXchgArgs x, uint32_t n_units) {
-    DiffXchgUnits p{{x.d}, x};
-    compact_units(p, n_units, x.d.tile_state, x.d.ticket);
+// ... over a list whose length n the device holds (rpk_select_pending_changed_device_gather)
+struct DiffXchgCountUnits : DiffXchgUnits {
+    uint32_t n;
+    __device__ __forceinline__ V load(uint32_t u) const { return load_n(u, n); }
+};
+
+// kDevCount: the row count is *d_n, read here, and the grid was sized for the worst case (x.d.n and n_units unused):
+// the units of the count are shared out over the whole grid, so a CTA past them publishes a zero count at once and the
+// look-back, the count stores and the last CTA's signal complete as for a launch sized for the count
+template <bool kDevCount>
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff_xchg(ResultXchgArgs x, uint32_t n_units,
+                                                                                            const uint32_t* __restrict__ d_n) {
+    if constexpr (kDevCount) {
+        const uint32_t n = *d_n;
+        DiffXchgCountUnits p{{{x.d}, x}, n};
+        compact_units(p, (n + kPendUnit - 1) / kPendUnit, x.d.tile_state, x.d.ticket);
+    } else {
+        DiffXchgUnits p{{x.d}, x};
+        compact_units(p, n_units, x.d.tile_state, x.d.ticket);
+    }
 }
 
 int launch_pod_fill(const PodRows& t, uint8_t* pending, uint32_t N, int sm_count, cudaStream_t st) {
@@ -541,7 +561,14 @@ int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t s
 
 int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st) {
     const uint32_t n_units = (x.d.n + kPendUnit - 1) / kPendUnit;  // no rows: one CTA publishes the count and signals
-    k_pod_result_diff_xchg<<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, n_units);
+    k_pod_result_diff_xchg<false><<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, n_units, nullptr);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
+}
+
+int launch_pod_result_xchg_device(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st) {
+    const uint32_t n_units = (n_max + kPendUnit - 1) / kPendUnit;
+    k_pod_result_diff_xchg<true><<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, n_units, d_n);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

@@ -219,7 +219,8 @@ int pod_columns(DeviceState& ds, DeviceState::Lane& ln, const RowSource& src, ui
 // scratch and launches on st.  A bit-sliced table takes the persistent kernel above the fused kernel's batch size and
 // the fused kernel otherwise (which also serves an empty table at any batch size).  t5: the top-5 lists' gather, if
 // any.  Returns the kernels launched.
-int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaStream_t st, const Top5Gather* t5 = nullptr) {
+// a's offer side: ds's views, G, the distinct values of the rank thresholds and the pack layout
+void offer_args(const DeviceState& ds, SelectArgs& a) {
     for (int c = 0; c < 2; ++c) {
         a.view[c].packed = ds.v_packed[c].p; a.view[c].bitmap = ds.v_bitmap[c].p; a.view[c].bitmapT = ds.v_bitmapT[c].p;
         a.view[c].bitmapM = ds.pk.slice_rows ? ds.v_bitmapM[c].p : nullptr; a.view[c].wide = ds.v_wide[c].p;
@@ -227,6 +228,10 @@ int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaSt
     }
     a.G = ds.G; a.Gpad = ds.Gpad; a.pk = ds.pk; a.nsub = ds.nsub;
     for (int d = 0; d < 3; ++d) { a.distinct[d] = ds.distinct[d].p; a.D[d] = ds.D[d]; }
+}
+
+int enqueue_select(DeviceState& ds, DeviceState::Lane& ln, SelectArgs& a, cudaStream_t st, const Top5Gather* t5 = nullptr) {
+    offer_args(ds, a);
     const uint32_t P = a.P;
     const int R = ds.pk.bm_words ? 0 : pick_rows_per_warp(P, ds.sm_count);  // rows per warp of the packed / wide kernels
     const uint32_t tiles = R ? select_tiles_max(P, R) : 0u;
@@ -1197,24 +1202,39 @@ ResultRows result_rows(DeviceState& ds, bool d) {
     return ResultRows{counts, reinterpret_cast<uint32_t*>(b), b + cap, b + 2 * cap};
 }
 
-// The stale step of ds over its owned slots [lo, hi): k_pod_stale lists the stale pending slots in r_list, and their
-// number and the number of owned pending slots land in the mapped counts (zeroed here; read them after synchronising
-// st).  While the ctx's change window is not empty, k_pod_stale_reach takes k_pod_stale's place.  The caller has waited
-// for the select scope.  Returns the kernels launched.
-int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi, cudaStream_t st) {
-    reserve_results(ds, lo, hi);
-    reserve_compaction_state(ds);
-    const ResultRows m = result_rows(ds, true);
+// The stale step of ds over its owned slots [lo, hi): k_pod_stale lists the stale pending slots in r_list, their number
+// lands in *n_out and the number of owned pending slots in *n_pending: the mapped counts by default (zeroed here; read
+// them after synchronising st), or device words (the device form; the caller zeroes them for an empty range, where
+// nothing is launched).  While the ctx's change window is not empty, k_pod_stale_reach takes k_pod_stale's place.  The
+// caller has reserved the results and waited for the select scope.  Returns the kernels launched.
+int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi, cudaStream_t st, uint32_t* n_out = nullptr,
+                  uint32_t* n_pending = nullptr) {
+    if (!n_out) {
+        const ResultRows m = result_rows(ds, true), h = result_rows(ds, false);
+        n_out = m.counts; n_pending = m.counts + 1;
+        reinterpret_cast<volatile uint32_t*>(h.counts)[0] = 0u; reinterpret_cast<volatile uint32_t*>(h.counts)[1] = 0u;
+    }
     StaleArgs a{};
     a.flags = ds.pt_pending.p; a.t = ds.pods_table(); a.N = ds.podsN; a.u_lo = lo / 16; a.r = ds.results(); a.gen = ctx->offer_gen;
-    a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = m.counts; a.n_pending = m.counts + 1;
+    a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = n_out; a.n_pending = n_pending;
     a.tile_state = ds.pt_state.p; a.ticket = ds.pt_ticket.p;
-    const ResultRows h = result_rows(ds, false);
-    reinterpret_cast<volatile uint32_t*>(h.counts)[0] = 0u; reinterpret_cast<volatile uint32_t*>(h.counts)[1] = 0u;
     if (ctx->window.empty()) return launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, st);
     const StaleReachArgs x{a, ctx->offer_floor, ds.win.p, (uint32_t)ctx->window.size(),
                            ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p};
     return launch_pod_stale_reach(x, (hi - lo + 15) / 16, ds.sm_count, st);
+}
+
+// The diff of k reselected rows of ds (the list in r_list, their columns and top-5 lists in ln's buffers) against the
+// stored results of the owned slots from lo on, the changed rows to the mapped outputs
+ResultDiffArgs diff_args(DeviceState& ds, const DeviceState::Lane& ln, uint32_t k, uint32_t lo, uint32_t gen) {
+    const ResultRows m = result_rows(ds, true);
+    ResultDiffArgs d{};
+    d.list = ds.r_list.p; d.n = k;
+    d.cols = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p}; d.top5 = ln.top5.p;
+    d.r = ds.results(); d.r_lo = lo; d.gen = gen; d.mask = ds.r_mask.p;
+    d.out_slot = m.slot; d.out_best = m.best; d.out_top5 = m.top5; d.n_out = m.counts;
+    d.tile_state = ds.pt_state.p; d.ticket = ds.pt_ticket.p;
+    return d;
 }
 
 // The reselect of the k stale rows enqueue_stale listed (lane 0's buffers sized for them): the gather, one select with
@@ -1231,13 +1251,7 @@ int enqueue_reselect(DeviceState& ds, uint32_t k, uint32_t lo, uint32_t gen, cud
         a.P = k; a.best_out[0] = ds.r_best.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = ln.top5.p;
         launches += enqueue_select(ds, ln, a, st);
     }
-    const ResultRows m = result_rows(ds, true);
-    ResultDiffArgs d{};
-    d.list = ds.r_list.p; d.n = k;
-    d.cols = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p}; d.top5 = ln.top5.p;
-    d.r = ds.results(); d.r_lo = lo; d.gen = gen; d.mask = ds.r_mask.p;
-    d.out_slot = m.slot; d.out_best = m.best; d.out_top5 = m.top5; d.n_out = m.counts;
-    d.tile_state = ds.pt_state.p; d.ticket = ds.pt_ticket.p;
+    const ResultDiffArgs d = diff_args(ds, ln, k, lo, gen);
     if (!x) return launches + launch_pod_result_diff(d, ds.sm_count, st);
     x->d = d;
     return launches + launch_pod_result_xchg(*x, ds.sm_count, st);
@@ -1266,6 +1280,8 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();
+            reserve_results(ds, lo, hi);
+            reserve_compaction_state(ds);
             launches[(size_t)s] += (uint64_t)enqueue_stale(ctx, ds, lo, hi, ds.stream);
         }
         for (int s = 0; s < n; ++s) {
@@ -1342,45 +1358,110 @@ size_t rpk_results_xchg_bytes(int n_ranks, uint32_t cap) {
     return (8 + (size_t)n_ranks * cap * (2 + RPK_TOPK)) * 4 + 16;
 }
 
-// Every refusal comes before the first launch, and cap >= hi - lo bounds what the diff can write: once the stale step
-// has run, the call always finishes with its count and its signal, so no peer is left waiting.
+namespace {
+// The refusals of rpk_select_pending_changed_gather and its device form, in order (`who` names the call; args_ok: its
+// own pointer arguments, refused with the n_ranks / my_rank message `required`).  On RPK_OK [*lo, *hi) is the rank's
+// owned range.  Every refusal comes before the first launch, and cap >= hi - lo bounds what the diff can write: once the
+// stale step has run, the call always finishes with its count and its signal, so no peer is left waiting.
+int check_results_gather(rpk_ctx* ctx, const char* who, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg, uint32_t cap,
+                         bool args_ok, const char* required, uint32_t* lo, uint32_t* hi) {
+    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, std::string(who) + ": shard out of range");
+    if (n_ranks < 1 || n_ranks > RPK_MAX_GPUS || my_rank < 0 || my_rank >= n_ranks || !d_xchg || !args_ok)
+        return fail(ctx, RPK_EINVAL, std::string(who) + ": " + required);
+    for (int o = 0; o < n_ranks; ++o)
+        if (!d_xchg[o] || ((uintptr_t)d_xchg[o] & 15)) return fail(ctx, RPK_EINVAL, std::string(who) + ": NULL or not 16-byte aligned exchange buffer");
+    if (int rc = check_select_ready(ctx, who, true, shard)) return rc;
+    const DeviceState& ds = ctx->devs[(size_t)shard];
+    result_range(ds.podsN, n_ranks, my_rank, lo, hi);
+    if (cap < *hi - *lo) return fail(ctx, RPK_EINVAL, std::string(who) + ": cap is below the number of slots the rank owns");
+    return check_results_range(ctx, ds, *lo, *hi, who);
+}
+
+// The exchange of rank my_rank: buffer o is [counts : 8 words][region r: slot[cap], best[cap], top5[5 cap]]...; the diff
+// fills and signals under the rank the call names (x.d is the caller's)
+ResultXchgArgs results_xchg(const rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg, uint32_t cap) {
+    ResultXchgArgs x{};
+    x.n_out = n_ranks; x.cap = cap;
+    for (int o = 0; o < n_ranks; ++o) {
+        x.region[o] = d_xchg[o] + 8 + (size_t)my_rank * (2 + RPK_TOPK) * cap;
+        x.count[o] = d_xchg[o] + my_rank;
+    }
+    x.peers = ctx->bind[(size_t)shard];
+    x.peers.my_rank = my_rank;
+    return x;
+}
+}  // namespace
+
 int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg, uint32_t cap,
                                       uint32_t* n_pending, uint32_t* n_reselected, void* stream) {
     static const char* who = "rpk_select_pending_changed_gather";
     if (!ctx) return RPK_EINVAL;
-    if (bad_shard(ctx, shard)) return fail(ctx, RPK_EINVAL, std::string(who) + ": shard out of range");
-    if (n_ranks < 1 || n_ranks > RPK_MAX_GPUS || my_rank < 0 || my_rank >= n_ranks || !d_xchg || !n_pending || !n_reselected)
-        return fail(ctx, RPK_EINVAL, std::string(who) + ": n_ranks in 1..8, my_rank in [0, n_ranks), d_xchg, n_pending and n_reselected are required");
-    for (int o = 0; o < n_ranks; ++o)
-        if (!d_xchg[o] || ((uintptr_t)d_xchg[o] & 15)) return fail(ctx, RPK_EINVAL, std::string(who) + ": NULL or not 16-byte aligned exchange buffer");
-    if (int rc = check_select_ready(ctx, who, true, shard)) return rc;
+    uint32_t lo, hi;
+    if (int rc = check_results_gather(ctx, who, shard, n_ranks, my_rank, d_xchg, cap, n_pending && n_reselected,
+                                      "n_ranks in 1..8, my_rank in [0, n_ranks), d_xchg, n_pending and n_reselected are required", &lo, &hi))
+        return rc;
     DeviceState& ds = ctx->devs[(size_t)shard];
-    uint32_t lo, hi; result_range(ds.podsN, n_ranks, my_rank, &lo, &hi);
-    if (cap < hi - lo) return fail(ctx, RPK_EINVAL, std::string(who) + ": cap is below the number of slots the rank owns");
-    if (int rc = check_results_range(ctx, ds, lo, hi, who)) return rc;
     const uint32_t gen = ctx->offer_gen;
     return device_call(ctx, shard, stream, nullptr, [&](DeviceState&, cudaStream_t st) {
         ds.sel_scope.host_wait();
+        reserve_results(ds, lo, hi);
+        reserve_compaction_state(ds);
         uint64_t launches = (uint64_t)enqueue_stale(ctx, ds, lo, hi, st);
         RPK_CUDA(cudaStreamSynchronize(st));  // the select needs the row count on the host
         const volatile uint32_t* c = result_rows(ds, false).counts;
         const uint32_t k = c[0];
         *n_pending = c[1]; *n_reselected = k;
         if (k) reserve_lane(ds.lane[0], k, RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
-        ResultXchgArgs x{};
-        x.n_out = n_ranks; x.cap = cap;
-        for (int o = 0; o < n_ranks; ++o) {  // buffer o: [counts : 8 words][region r: slot[cap], best[cap], top5[5 cap]]...
-            x.region[o] = d_xchg[o] + 8 + (size_t)my_rank * (2 + RPK_TOPK) * cap;
-            x.count[o] = d_xchg[o] + my_rank;
-        }
-        x.peers = ctx->bind[(size_t)shard];
-        x.peers.my_rank = my_rank;  // the diff fills and signals under the rank the call names
+        ResultXchgArgs x = results_xchg(ctx, shard, n_ranks, my_rank, d_xchg, cap);
         ds.res_ready = false;       // until the diff is enqueued behind the select
         launches += (uint64_t)enqueue_reselect(ds, k, lo, gen, st, &x);
         ds.res_ready = true;
         ds.sel_scope.device_end(st, true);
         ctx->launches += launches;
         if (k) count_select(ctx, k, ds.G);
+    });
+}
+
+// The same tick with the row count kept on the device: the stale step writes it to r_dn, the reselect kernel and the
+// diff read it there and are sized for the rank's worst case, hi - lo rows, so nothing waits for the host.  Every buffer
+// is sized in prep for that worst case: after one call the call only enqueues.  The reselected rows' columns and lists
+// go to r_lane, which no other call grows, so a select of any size on the ctx cannot free what a captured graph writes.
+int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg,
+                                             uint32_t cap, uint32_t* d_counts, void* stream) {
+    static const char* who = "rpk_select_pending_changed_device_gather";
+    if (!ctx) return RPK_EINVAL;
+    uint32_t lo, hi;
+    if (int rc = check_results_gather(ctx, who, shard, n_ranks, my_rank, d_xchg, cap, ((uintptr_t)d_counts & 3) == 0,
+                                      "n_ranks in 1..8, my_rank in [0, n_ranks) and d_xchg are required, d_counts 4-byte aligned", &lo, &hi))
+        return rc;
+    DeviceState& ds = ctx->devs[(size_t)shard];
+    const uint32_t gen = ctx->offer_gen;
+    const auto prep = [&](DeviceState&) {
+        reserve_results(ds, lo, hi);
+        reserve_compaction_state(ds);
+        ds.r_dn.reserve(2);
+        reserve_lane(ds.r_lane, std::max<uint32_t>(hi - lo, 1u), RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
+        return RPK_OK;
+    };
+    return device_call(ctx, shard, stream, &DeviceState::sel_scope, prep, [&](DeviceState&, cudaStream_t st) {
+        uint32_t* dn = ds.r_dn.p;  // [n_pending, n_reselected]
+        uint64_t launches = 0;
+        ds.res_ready = false;  // until every launch is enqueued
+        if (hi > lo) launches += (uint64_t)enqueue_stale(ctx, ds, lo, hi, st, dn + 1, dn);
+        else RPK_CUDA(cudaMemsetAsync(dn, 0, 2 * sizeof(uint32_t), st));  // an empty range: no stale step
+        ReselectArgs r{};
+        offer_args(ds, r.s);
+        const DeviceState::Lane& ln = ds.r_lane;
+        r.s.top5 = ln.top5.p;
+        r.t = ds.pods_table();
+        r.out = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
+        r.list = ds.r_list.p; r.dn = dn; r.counts = d_counts;
+        launches += (uint64_t)launch_pod_reselect(r, hi - lo, ds.sm_count, st);
+        ResultXchgArgs x = results_xchg(ctx, shard, n_ranks, my_rank, d_xchg, cap);
+        x.d = diff_args(ds, ds.r_lane, 0, lo, gen);
+        launches += (uint64_t)launch_pod_result_xchg_device(x, dn + 1, hi - lo, ds.sm_count, st);
+        ds.res_ready = true;
+        ctx->launches += launches;
     });
 }
 

@@ -347,11 +347,27 @@ struct StaleReachArgs {
     const uint2* win; uint32_t n_win;
     const int32_t* mem; const int32_t* vcpu; const int32_t* ram; const double* sp; const double* cp; const uint8_t* flags;
 };
+// The reselect of the device form (rpk_select_pending_changed_device_gather, select.cu): rows [0, dn[1]) of list, the
+// count the stale step left on the device.  Row i's five columns go to out, its top-5 list to s.top5 (s: the offer views,
+// G, the rank thresholds' distinct values and pk, as enqueue_select fills them).  counts (nullable) := dn[0, 2).
+struct ReselectArgs {
+    SelectArgs s;
+    PodRows t;              // the pod table
+    PodRows out;            // row i: the columns the list entry's row holds
+    const uint32_t* list;   // the reselected slots
+    const uint32_t* dn;     // [n_pending, n_reselected], written by the stale step
+    uint32_t* counts;       // nullable: the caller's copy of dn
+};
+// a few waves sized for the worst case of n_max rows, the count read on the device; launches for n_max = 0 too
+int launch_pod_reselect(const ReselectArgs& r, uint32_t n_max, int sm_count, cudaStream_t st);
 int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
 int launch_pod_stale_reach(const StaleReachArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
 int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st);
 // launches even when x.d.n = 0: the count 0 still goes out and the peers are still signalled
 int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st);
+// the same with the row count read from d_n on the device (x.d.n unused): the grid is sized for n_max rows, the worst
+// case; the CTAs past the count publish a zero count at once
+int launch_pod_result_xchg_device(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
@@ -481,6 +497,9 @@ struct DeviceState {
     // (rpk_pods_reset, a failed call)
     DevBuf<int32_t> r_mem, r_vcpu, r_ram, r_top5, r_best, r_out; DevBuf<double> r_max_price; DevBuf<uint8_t> r_cloud;
     DevBuf<uint32_t> r_gen, r_list; DevBuf<uint16_t> r_mask;
+    // rpk_select_pending_changed_device_gather: [n_pending, n_reselected] of the stale step, and the reselected rows'
+    // columns and top-5 lists (its own buffers, sized once for the owned range: a captured call keeps pointing at them)
+    DevBuf<uint32_t> r_dn; Lane r_lane;
     PinnedBuf h_res;
     bool res_ready = false;
     // the owned range [res_lo, res_hi) the stored results were made for, set by the first call after rpk_pods_reset

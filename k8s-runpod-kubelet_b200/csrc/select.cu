@@ -13,11 +13,14 @@
 //                     applies price < maxPrice to the winner (the bound is a prefix of the sorted order) and stores
 //                     the offer index into every peer's assignment vector (the fused all-gather).
 //   k_select_top5*    optional: the whole <=5 gpuTypeIds list per row (runpod_client.go:502-509).
+//   k_pod_reselect_top5  the pending results' device form: gather + thresholds + top-5 over a list whose length is
+//                     read on the device (rpk_select_pending_changed_device_gather)
 //   k_gather_push     several output vectors: copies the finished slice to the peers (a second launch copies the top-5
 //                     lists' slice for rpk_select_device_gather_top5); k_peer_signal (select_persist.cu) then signals a
 //                     bound peer group.
 #include <math_constants.h>
 
+#include <algorithm>
 #include <cstdlib>
 #include <cstring>
 
@@ -372,60 +375,49 @@ __global__ void __launch_bounds__(kCtaThreads, 2) k_select_wide(SelectArgs a, ui
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// top-5: "Take up to 5 GPUs" (runpod_client.go:502-509).  One warp per pod row walks the sorted view in
-// ascending price order, ballots feasibility over 32 positions at a time and stops after five hits or at
-// the first position whose price is not < maxPrice (everything after it is at least as expensive).
+// top-5: "Take up to 5 GPUs" (runpod_client.go:502-509).  The two walks below are the rule, once: the top-5 kernels
+// and the pending results' reselect (k_pod_reselect_top5) call them.
 // ---------------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_select_top5(SelectArgs a) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
-    const uint32_t Gc = ((a.G + kChunk - 1) / kChunk) * kChunk;
-    for (uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < a.P; p += nwarps) {
-        const uint8_t c = a.cloud ? a.cloud[p] : (uint8_t)RPK_CLOUD_SECURE;
-        if (c > 1) continue;  // filled by k_pod_prep
-        const int32_t qm = a.req_mem[p], qv = a.req_vcpu ? a.req_vcpu[p] : 0, qr = a.req_ram ? a.req_ram[p] : 0;
-        const double mx = a.max_price ? a.max_price[p] : RPK_DEFAULT_MAX_PRICE;
-        const int4* __restrict__ wide = a.view[c].wide;
-        const double* __restrict__ price = a.view[c].price;
-        int cnt = 0;
-        for (uint32_t base = 0; base < Gc && cnt < RPK_TOPK; base += 32) {
-            const int4 o = wide[base + lane];
-            const bool price_ok = price[base + lane] < mx;  // NaN (unavailable / padding) fails
-            const bool f = price_ok && o.x >= qm && o.y >= qv && o.z >= qr;
-            uint32_t mask = __ballot_sync(0xFFFFFFFFu, f);
-            const bool stop = __ballot_sync(0xFFFFFFFFu, !price_ok) != 0;
-            while (mask && cnt < RPK_TOPK) {
-                const int b = __ffs(mask) - 1;
-                const int idx = __shfl_sync(0xFFFFFFFFu, o.w, b);
-                if (lane == 0) a.top5[(size_t)p * RPK_TOPK + cnt] = idx;
-                ++cnt;
-                mask &= mask - 1;
-            }
-            if (stop) break;
+// One warp per pod row (every lane passes the same row) walks the wide view of cloud c in ascending price order,
+// ballots feasibility over 32 positions at a time and stops after five hits or at the first position whose price is
+// not < mx (everything after it is at least as expensive).  Lane 0 writes row p of a.top5, -1 padded.  Gc: G rounded up to
+// kChunk; lane: threadIdx.x & 31.
+__device__ __forceinline__ void top5_walk_wide(const SelectArgs& a, uint8_t c, uint32_t lane, uint32_t Gc, int32_t qm, int32_t qv,
+                                               int32_t qr, double mx, uint32_t p) {
+    const int4* __restrict__ wide = a.view[c].wide;
+    const double* __restrict__ price = a.view[c].price;
+    int cnt = 0;
+    for (uint32_t base = 0; base < Gc && cnt < RPK_TOPK; base += 32) {
+        const int4 o = wide[base + lane];
+        const bool price_ok = price[base + lane] < mx;  // NaN (unavailable / padding) fails
+        const bool f = price_ok && o.x >= qm && o.y >= qv && o.z >= qr;
+        uint32_t mask = __ballot_sync(0xFFFFFFFFu, f);
+        const bool stop = __ballot_sync(0xFFFFFFFFu, !price_ok) != 0;
+        while (mask && cnt < RPK_TOPK) {
+            const int b = __ffs(mask) - 1;
+            const int idx = __shfl_sync(0xFFFFFFFFu, o.w, b);
+            if (lane == 0) a.top5[(size_t)p * RPK_TOPK + cnt] = idx;
+            ++cnt;
+            mask &= mask - 1;
         }
-        if (lane == 0) for (int k = cnt; k < RPK_TOPK; ++k) a.top5[(size_t)p * RPK_TOPK + k] = -1;
+        if (stop) break;
     }
+    if (lane == 0) for (int k = cnt; k < RPK_TOPK; ++k) a.top5[(size_t)p * RPK_TOPK + k] = -1;
 }
 
-// top-5 on the bit-sliced view: one lane per pod row.  The price bound is a prefix of the sorted view (binary
-// search for its length), inside it the row's three masks give 32 positions per step; the walk stops at five hits.
+// One lane per pod row on the bit-sliced view (its price, bitmap and perm arrays): o1 / o2 / o3 are the row's three mask
+// words (its rank thresholds), mx its price bound.  The bound is a prefix of the sorted view (binary search for its
+// length), inside it the row's three masks give 32 positions per step; the walk stops at five hits.  Writes out[0, 5),
+// -1 padded.  The views come in as restrict parameters: that keeps the load kinds the top-5 kernel had with its own
+// restrict locals (price and perm through the read-only path, the masks not).
 template <int STRIDE>
-__global__ void __launch_bounds__(256) k_select_top5_bitmap(SelectArgs a) {
-    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
-    if (p >= a.P) return;
-    const uint8_t c = a.cloud ? a.cloud[p] : (uint8_t)RPK_CLOUD_SECURE;
-    if (c > 1) return;  // filled by k_pod_prep
-    const uint32_t w = a.rw[p];
-    const uint32_t o1 = w & 0xFFu, o2 = (w >> 8) & 0xFFu, o3 = (w >> 16) & 0xFFu;
-    const double mx = a.max_price ? a.max_price[p] : RPK_DEFAULT_MAX_PRICE;
-    const double* __restrict__ price = a.view[c].price;
-    const uint32_t* __restrict__ bm = a.view[c].bitmap;
-    const int32_t* __restrict__ perm = a.view[c].perm;
-    uint32_t lo = 0, hi = a.G;  // number of positions with price < mx (NaN = unavailable sorts last and fails)
+__device__ __forceinline__ void top5_walk_bitmap(const double* __restrict__ price, const uint32_t* __restrict__ bm,
+                                                 const int32_t* __restrict__ perm, uint32_t G, uint32_t o1, uint32_t o2,
+                                                 uint32_t o3, double mx, int32_t* out) {
+    uint32_t lo = 0, hi = G;  // number of positions with price < mx (NaN = unavailable sorts last and fails)
     while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (price[mid] < mx) lo = mid + 1; else hi = mid; }
     const uint32_t cut = lo;
     int cnt = 0;
-    int32_t* out = a.top5 + (size_t)p * RPK_TOPK;
     for (uint32_t base = 0; base < cut && cnt < RPK_TOPK; base += 32) {
         const uint32_t* row = bm + (size_t)(base >> 5) * STRIDE;
         uint32_t m = row[o1] & row[o2] & row[o3];
@@ -436,6 +428,77 @@ __global__ void __launch_bounds__(256) k_select_top5_bitmap(SelectArgs a) {
         }
     }
     for (; cnt < RPK_TOPK; ++cnt) out[cnt] = -1;
+}
+
+__global__ void __launch_bounds__(256) k_select_top5(SelectArgs a) {
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t nwarps = (gridDim.x * blockDim.x) >> 5;
+    const uint32_t Gc = ((a.G + kChunk - 1) / kChunk) * kChunk;
+    for (uint32_t p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; p < a.P; p += nwarps) {
+        const uint8_t c = a.cloud ? a.cloud[p] : (uint8_t)RPK_CLOUD_SECURE;
+        if (c > 1) continue;  // filled by k_pod_prep
+        const int32_t qm = a.req_mem[p], qv = a.req_vcpu ? a.req_vcpu[p] : 0, qr = a.req_ram ? a.req_ram[p] : 0;
+        const double mx = a.max_price ? a.max_price[p] : RPK_DEFAULT_MAX_PRICE;
+        top5_walk_wide(a, c, lane, Gc, qm, qv, qr, mx, p);
+    }
+}
+
+template <int STRIDE>
+__global__ void __launch_bounds__(256) k_select_top5_bitmap(SelectArgs a) {
+    const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= a.P) return;
+    const uint8_t c = a.cloud ? a.cloud[p] : (uint8_t)RPK_CLOUD_SECURE;
+    if (c > 1) return;  // filled by k_pod_prep
+    const uint32_t w = a.rw[p];
+    const uint32_t o1 = w & 0xFFu, o2 = (w >> 8) & 0xFFu, o3 = (w >> 16) & 0xFFu;
+    const double mx = a.max_price ? a.max_price[p] : RPK_DEFAULT_MAX_PRICE;
+    top5_walk_bitmap<STRIDE>(a.view[c].price, a.view[c].bitmap, a.view[c].perm, a.G, o1, o2, o3, mx, a.top5 + (size_t)p * RPK_TOPK);
+}
+
+// The reselect of rpk_select_pending_changed_device_gather: rows [0, n) of r.list, n = r.dn[1] as the stale step left
+// it on the device, so the launch is sized for the worst case and needs no count on the host.  Row i gathers its slot's
+// five columns into r.out (the columns the diff stores with the result) and writes its top-5 list to r.s.top5 -- what
+// the host-sync form's gather, select and top-5 kernel leave there, bit for bit; best is not needed (it is top5[0]).
+// STRIDE 32 / 64: the bit-sliced view, one lane per row, the rank thresholds computed here as the select kernels compute
+// them.  STRIDE 0: the wide view (tables without pk.bm_words), one warp per row, which compares the raw columns.  A row
+// whose cloud byte is above 1 gets five -1.  Grid-stride: the grid is a few waves whatever the count.
+template <int STRIDE>
+__global__ void __launch_bounds__(256) k_pod_reselect_top5(ReselectArgs r) {
+    const SelectArgs& a = r.s;
+    if (r.counts && blockIdx.x == 0 && threadIdx.x == 0) { r.counts[0] = r.dn[0]; r.counts[1] = r.dn[1]; }
+    const uint32_t n = r.dn[1];
+    constexpr uint32_t kRowThreads = STRIDE ? 1u : 32u;
+    const uint32_t step = gridDim.x * blockDim.x / kRowThreads;
+    for (uint32_t i = (blockIdx.x * blockDim.x + threadIdx.x) / kRowThreads; i < n; i += step) {
+        const uint32_t s = r.list[i];
+        const int32_t mem = r.t.mem[s], vcpu = r.t.vcpu[s], ram = r.t.ram[s];
+        const double mx = r.t.max_price[s];
+        const uint8_t c = r.t.cloud[s];
+        if (STRIDE || (threadIdx.x & 31) == 0) {
+            r.out.mem[i] = mem; r.out.vcpu[i] = vcpu; r.out.ram[i] = ram; r.out.max_price[i] = mx; r.out.cloud[i] = c;
+            if (c > 1) for (int k = 0; k < RPK_TOPK; ++k) a.top5[(size_t)i * RPK_TOPK + k] = -1;
+        }
+        if (c > 1) continue;
+        if constexpr (STRIDE != 0) {
+            const uint32_t o1 = lower_bound_i32(a.distinct[0], a.D[0], mem);
+            const uint32_t o2 = a.pk.bm_off_vcpu + lower_bound_i32(a.distinct[1], a.D[1], vcpu);
+            const uint32_t o3 = a.pk.bm_off_ram + lower_bound_i32(a.distinct[2], a.D[2], ram);
+            top5_walk_bitmap<STRIDE>(a.view[c].price, a.view[c].bitmap, a.view[c].perm, a.G, o1, o2, o3, mx,
+                                     a.top5 + (size_t)i * RPK_TOPK);
+        } else {
+            top5_walk_wide(a, c, threadIdx.x & 31, ((a.G + kChunk - 1) / kChunk) * kChunk, mem, vcpu, ram, mx, i);
+        }
+    }
+}
+
+int launch_pod_reselect(const ReselectArgs& r, uint32_t n_max, int sm_count, cudaStream_t st) {
+    const uint32_t rows_per_cta = r.s.pk.bm_words ? 256u : 8u;
+    const uint32_t blocks = std::max<uint32_t>(1u, std::min<uint32_t>((n_max + rows_per_cta - 1) / rows_per_cta, (uint32_t)sm_count * 8));
+    if (!r.s.pk.bm_words) k_pod_reselect_top5<0><<<blocks, 256, 0, st>>>(r);
+    else if (r.s.pk.bm_stride == 64) k_pod_reselect_top5<64><<<blocks, 256, 0, st>>>(r);
+    else k_pod_reselect_top5<32><<<blocks, 256, 0, st>>>(r);
+    RPK_CUDA(cudaGetLastError());
+    return 1;
 }
 
 // ---------------------------------------------------------------------------------------------------------

@@ -21,7 +21,7 @@ _DEV_DTYPES = {
     "cloud": ("uint8",), "d_best": ("int32",), "d_top5": ("int32",), "d_records": ("uint8",),
     "d_hash_prev": ("int64", "uint64"), "d_changed_idx": ("int32", "uint32"), "d_changed_code": ("int16", "uint16"),
     "d_n_changed": ("int32", "uint32"), "d_slots": ("int32", "uint32"), "d_slots_out": ("int32", "uint32"),
-    "d_n": ("int32", "uint32"),
+    "d_n": ("int32", "uint32"), "d_counts": ("int32", "uint32"),
 }
 
 
@@ -290,6 +290,16 @@ class Engine:
             self._ctx, shard, n_ranks, my_rank, xchg, cap, C.cast(C.byref(n_p), C.c_void_p), C.cast(C.byref(n_r), C.c_void_p),
             self._stream(stream, shard)))
         return n_p.value, n_r.value
+
+    def select_pending_changed_device_gather(self, xchg_ptrs, cap: int, my_rank: int, d_counts=None, shard: int = 0, stream=None):
+        """``select_pending_changed_gather`` with the row count kept on the device: everything is enqueued on ``stream``
+        and nothing is synchronised, so after one call of the same ``(cap, my_rank, len(xchg_ptrs))`` the call can be
+        captured in a CUDA graph (rpk_select_pending_changed_device_gather).  ``d_counts`` (a torch CUDA tensor of at
+        least two int32 / uint32 on the shard's GPU, or None) receives [n_pending, n_reselected] of the rank's slots."""
+        n_ranks, xchg = _ptr_array(xchg_ptrs)
+        self._check(self._lib.rpk_select_pending_changed_device_gather(
+            self._ctx, shard, n_ranks, my_rank, xchg, cap, self._dev_ptr(d_counts, "d_counts", shard, at_least=2),
+            self._stream(stream, shard)))
 
     def pods_pending_list_device(self, d_slots_out, d_n, shard: int = 0, stream=None):
         """The pending slot ids, ascending, into ``d_slots_out`` (a torch CUDA tensor with one element per slot of the

@@ -88,6 +88,30 @@ if not ONLY_MULTI:
     assert r1 == 0 and len(s1) == 0 and r2 == len(pend) and len(s2) == 0
     assert int(fl[16].item()) == 3 and int(fl[34].item()) == 3
     eg.close()
+    # the device form (k_pod_stale, k_pod_reselect_top5, the device-count k_pod_result_diff_xchg): one eager call that
+    # reports every pending slot, then one replay of a captured steady call
+    ed = rpk.Engine(1)
+    ed.upload_offers(offers)
+    ed.pods_reset(200_000)
+    ed.pods_seed_slots(np.arange(200_000, dtype=np.uint32), pods_t)
+    ed.pods_mark_pending(np.arange(200_000, dtype=np.uint32), flags)
+    xbuf.fill_(-9)
+    fl.zero_()
+    cnt = torch.zeros(2, dtype=torch.int32, device="cuda")
+    ed.peer_bind([fl.data_ptr()], 0)
+    ed.select_pending_changed_device_gather([xbuf.data_ptr()], 200_000, 0, d_counts=cnt)
+    torch.cuda.synchronize()
+    s0, b0, t0 = rpk.results_region(xbuf, 1, 200_000, 0)
+    assert cnt.tolist() == [len(pend), len(pend)] and np.array_equal(s0, pend) and np.array_equal(b0, best) and np.array_equal(t0, t5)
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph, capture_error_mode="thread_local"):
+        ed.select_pending_changed_device_gather([xbuf.data_ptr()], 200_000, 0, d_counts=cnt)
+    graph.replay()
+    torch.cuda.synchronize()
+    assert cnt.tolist() == [len(pend), 0] and len(rpk.results_region(xbuf, 1, 200_000, 0)[0]) == 0
+    assert int(fl[16].item()) == 2 and int(fl[34].item()) == 2
+    del graph
+    ed.close()
 for stride in () if ONLY_MULTI else (16, 32, 64):
     tab = oracle.StatusTable(30_000, stride)
     e2 = rpk.Engine(1)
