@@ -124,3 +124,87 @@ def test_special_prices_flags_and_clouds():
     _, l = oracle.select(offers, pods)
     assert (l == -1).all()
     assert not model.reached(change(rng, offers, 10), pods, l, np.arange(10)).any(), "nothing reaches a row of neither cloud"
+
+
+# ---- Generations: the rule over whole histories ----------------------------------------------------------------------
+def seeded(rng, N, G):
+    offers = table(rng, G)
+    gm = model.Generations(N)
+    gm.upload(offers)
+    pods = rows(rng, N)
+    gm.seed(np.arange(N), pods)
+    return gm, offers
+
+
+def test_window_arithmetic():
+    rng = np.random.default_rng(3)
+    gm, offers = seeded(rng, 10, 40)
+    assert gm.refresh(offers) == 0 and gm.gen == 1, "an identical refresh bumps nothing"
+
+    def bump(t, gs):
+        new = {k: v.copy() for k, v in t.items()}
+        new["mem_gb"][gs] += 1
+        return new
+
+    a = bump(offers, np.arange(8))
+    assert gm.refresh(a) == 8
+    b = bump(a, np.arange(8, 16))
+    assert gm.refresh(b) == 8 and len(gm.window) == 16 and [e[1] for e in gm.window] == [3] * 8 + [2] * 8
+    c = bump(b, [3])
+    assert gm.refresh(c) == 1 and len(gm.window) == 16 and gm.window[0] == (3, 4), "an offer changed twice holds one entry"
+    d = bump(c, [20])
+    assert gm.refresh(d) == model.WHOLESALE and gm.window == [] and gm.floor == gm.gen == 5, "17 offers: wholesale"
+    assert gm.refresh(bump(d, np.arange(17))) == model.WHOLESALE, "17 in one refresh: wholesale"
+    assert gm.refresh({k: v[:39] for k, v in d.items()}) == model.WHOLESALE, "another G: wholesale"
+    fresh = model.Generations(4)
+    assert fresh.refresh(offers) == model.WHOLESALE and fresh.floor == 1, "no resident table: wholesale"
+
+
+def oracle_lists(gm):
+    pend = gm.pending_slots()
+    return pend, oracle.select(gm.offers, gm.rows(pend))[1] if len(pend) else np.zeros((0, 5), np.int32)
+
+
+@pytest.mark.parametrize("seed", range(8))
+def test_random_histories_keep_every_unreselected_list(seed):
+    """refreshes of 1-17 offers (some changed again), uploads, identical and changed seeds, marks and unmarks across
+    refreshes, and ticks: after every tick each pending slot the model does not reselect holds the oracle's list"""
+    rng = np.random.default_rng(2000 + seed)
+    N, G = 3000, int(rng.integers(17, 60))
+    gm, offers = seeded(rng, N, G)
+    gm.mark(np.arange(N), rng.random(N) < 0.5)
+    kept = hit_total = 0
+    ops = {"refresh": 0, "wholesale": 0}
+    for stp in range(60):
+        op = rng.choice(["refresh", "refresh", "refresh", "upload", "seed", "mark", "tick", "tick", "tick"])
+        if op == "refresh":
+            k = int(rng.integers(1, 18))
+            new = change(rng, gm.offers, k)
+            if rng.random() < 0.3 and gm.window:  # one more change to an offer the window already holds
+                g = gm.window[-1][0]
+                new["mem_gb"][g] ^= np.int32(1)
+            n = gm.refresh(new)
+            ops["refresh"] += 1
+            ops["wholesale"] += n == model.WHOLESALE
+            assert n == model.WHOLESALE or n == len(model.changed_offers(offers, new))
+            offers = new
+        elif op == "upload":
+            gm.upload(change(rng, gm.offers, 2) if rng.random() < 0.5 else gm.offers)
+            offers = gm.offers
+        elif op == "seed":
+            sl = np.sort(rng.choice(N, int(rng.integers(1, 400)), replace=False))
+            gm.seed(sl, gm.rows(sl) if rng.random() < 0.4 else rows(rng, len(sl)))
+        elif op == "mark":
+            sl = np.sort(rng.choice(N, int(rng.integers(1, 800)), replace=False))
+            gm.mark(sl, rng.random(len(sl)) < 0.5)
+        else:
+            pend, want = oracle_lists(gm)
+            before = gm.top5[pend].copy()
+            hit = gm.tick(want)
+            keep = ~np.isin(pend, hit)
+            bad = np.flatnonzero(keep & (before != want).any(axis=1))
+            assert not len(bad), f"step {stp}: slots {pend[bad[:8]].tolist()} keep a stale list"
+            assert np.array_equal(gm.top5[pend], want)
+            kept += int(keep.sum())
+            hit_total += len(hit)
+    assert kept and hit_total and ops["refresh"] > ops["wholesale"], (kept, hit_total, ops)
