@@ -1,6 +1,7 @@
 """Restatement of the persistent select's launch plan: ``class_dims`` and ``persist_plan`` in
-k8s-runpod-kubelet_b200/csrc/select_persist.cu, with the constants of rpk_internal.cuh, the bitmapM condition of
-``launch_offer_ingest`` (offers.cu) and the host entry point's row sub-batches (``sub_batch_rows``, rpk_api.cu).
+k8s-runpod-kubelet_b200/csrc/select_persist.cu, with the constants of rpk_internal.cuh, the view layout
+``launch_offer_ingest`` (offers.cu) picks from the distinct counts (``layout``, which includes the bitmapM condition)
+and the host entry point's row sub-batches (``sub_batch_rows``, rpk_api.cu).
 
 The GPU tests assert through it which regime each case reaches, so a change to a constant that moves a case off its
 regime fails the case instead of quietly testing something else."""
@@ -14,10 +15,49 @@ PWARPS, RPI = 16, 64                   # warps per 512-thread CTA; rows per item
 STAGE_MAX = 220 * 1024                 # persist_plan's stage cap
 FUSED_ROWS_MAX, SMALL_BATCH = 16384, 4096  # kFusedRowsMax, kSmallBatch
 SUB_BATCH_ROWS = 131072                # kSubBatchRows (x1, x2, x3, then x4)
+POS_BITS = 14                          # kPosBits: position-in-segment bits of a packed_pos word (kSegPacked = 2^14)
+# RPK_FORCE_KERNEL values as install_offers (rpk_api.cu) reads them; any other string is the automatic choice
+FORCE_KINDS = {"generic": 1, "packed": 2, "packed_pos": 3, "bitmap": 4, "bitmap_grouped": 5, "bitmap_price": 6}
+KIND_NAMES = {1: "generic", 2: "packed", 3: "packed_pos", 4: "bitmap"}  # rpk_stats.select_kernel_kind
 
 
 def cdiv(a, b):
     return -(-a // b)
+
+
+def bitlen(x):
+    """offers.cu's bitlen: the bits of x, at least 1"""
+    return max(int(x).bit_length(), 1)
+
+
+def layout(D, force=None):
+    """the offer views launch_offer_ingest builds for distinct counts D = [mem, vcpu, ram] under RPK_FORCE_KERNEL
+    `force` (None: the automatic choice).  The packed word holds mem rank' + 1 in [0, D0] against thresholds up to
+    D0 + 1, and vcpu / ram ranks against thresholds up to D, each field with a guard bit; it exists when the fields
+    total 32 bits or less, and carries the 14-bit position in its segment when they total 18 or less.  The bit-sliced
+    view has one mask word per threshold, (D0 + 1) + (D1 + 1) + (D2 + 1) of them, in rows of 32 or 64 words, and
+    per-mem-threshold slices when the class key keeps the mem threshold (and the table is not empty).
+    kind is rpk_stats.select_kernel_kind: 4 bitmap, 3 packed_pos, 2 packed, 1 generic."""
+    k = FORCE_KINDS.get(force, 0)
+    b1, b2, b3 = bitlen(D[0] + 1), bitlen(D[1]), bitlen(D[2])
+    bits = b1 + b2 + b3 + 3
+    if bits > 32:
+        bits = 0
+    pos_bits = POS_BITS if bits and bits + POS_BITS <= 32 else 0
+    bm_words = (D[0] + 1) + (D[1] + 1) + (D[2] + 1)
+    if bm_words > BM_MAX_STRIDE:
+        bm_words = 0
+    if k == 1:
+        bits = pos_bits = bm_words = 0
+    elif k == 2:
+        pos_bits = bm_words = 0
+    elif k == 3:
+        bm_words = 0
+    kind = 4 if bm_words else 3 if pos_bits else 2 if bits else 1
+    return SimpleNamespace(kind=kind, name=KIND_NAMES[kind], packed_bits=bits, pos_bits=pos_bits, bm_words=bm_words,
+                           bm_stride=(32 if bm_words <= 32 else 64) if bm_words else 0,
+                           slice=bool(bm_words) and D[0] > 0 and class_dims(D)[3],
+                           no_fused=k >= 5, no_slice=k == 6)
 
 
 def distinct(offers):

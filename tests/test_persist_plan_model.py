@@ -75,6 +75,71 @@ def test_unknown_cloud_has_no_queue():
     assert model.queues(pl, [np.arange(13)] * 3, pods) == 0
 
 
+def test_layout_packed_boundaries():
+    """field widths bitlen(D0 + 1), bitlen(D1), bitlen(D2) plus three guards: 18 bits keep the position field, 19 drop
+    it, 32 are packed, 33 generic; each field steps where its highest threshold (D0 + 1 for mem, D for vcpu / ram)
+    needs one more bit.  Every case has more than 64 mask words, so packed is the automatic choice."""
+    cases = {  # D: (kind, packed_bits)
+        (62, 15, 31): (3, 18),   # 6 + 4 + 5 + 3
+        (63, 15, 31): (2, 19),   # mem threshold 64: 7 bits
+        (62, 16, 31): (2, 19),   # vcpu threshold 16: 5 bits
+        (62, 15, 32): (2, 19),   # ram threshold 32: 6 bits
+        (64, 15, 31): (2, 19),
+        (61, 15, 31): (3, 18),
+        (30, 63, 7): (3, 17),
+        (30, 64, 7): (3, 18),
+        (14, 7, 127): (3, 17),
+        (14, 7, 128): (3, 18),
+        (1022, 1023, 511): (2, 32),  # 10 + 10 + 9 + 3
+        (1023, 1023, 511): (1, 0),   # mem threshold 1024: 11 bits
+        (1022, 1024, 511): (1, 0),
+        (1022, 1023, 512): (1, 0),
+        (1021, 1023, 511): (2, 32),
+    }
+    for D, (kind, bits) in cases.items():
+        L = model.layout(list(D))
+        assert sum(D) + 3 > model.BM_MAX_STRIDE and L.bm_words == 0 and L.bm_stride == 0, D
+        assert (L.kind, L.packed_bits) == (kind, bits), (D, L)
+        assert L.pos_bits == (model.POS_BITS if kind == 3 else 0), D
+
+
+def test_layout_bitmap_boundaries():
+    """mask words (D0 + 1) + (D1 + 1) + (D2 + 1): rows of 32 words up to 32, 64 up to 64, no bit-sliced view at 65;
+    per-mem-threshold slices while 2 * Dm1 * Dv1 * Dr1 <= 4096"""
+    L = model.layout([15, 7, 7])
+    assert (L.kind, L.bm_words, L.bm_stride, L.slice, L.packed_bits, L.pos_bits) == (4, 32, 32, True, 14, 14)
+    L = model.layout([16, 7, 7])
+    assert (L.kind, L.bm_words, L.bm_stride, L.slice) == (4, 33, 64, True)
+    L = model.layout([47, 7, 7])
+    assert (L.kind, L.bm_words, L.bm_stride, L.slice) == (4, 64, 64, False)
+    L = model.layout([48, 7, 7])
+    assert (L.kind, L.bm_words, L.bm_stride, L.packed_bits) == (3, 0, 0, 6 + 3 + 3 + 3)
+    assert model.layout([31, 7, 7]).slice and not model.layout([32, 7, 7]).slice
+    assert model.layout([0, 0, 0]).kind == 4 and not model.layout([0, 0, 0]).slice  # empty table: no sub-range
+
+
+def test_layout_forced():
+    """RPK_FORCE_KERNEL removes views, never adds one: packed_pos drops the bit-sliced view, packed also the position,
+    generic every rank view; bitmap_grouped / bitmap_price keep the views and route every batch through the
+    persistent kernel (bitmap_price without the slices); an unknown value is the automatic choice"""
+    bm, pos, packed, generic = [15, 7, 7], [62, 15, 31], [63, 15, 31], [1022, 1023, 512]
+    want = {  # (D, force): kind
+        (0, None): 4, (0, "packed_pos"): 3, (0, "packed"): 2, (0, "generic"): 1, (0, "bitmap"): 4,
+        (0, "bitmap_grouped"): 4, (0, "bitmap_price"): 4, (0, "no-such-kernel"): 4,
+        (1, None): 3, (1, "packed_pos"): 3, (1, "packed"): 2, (1, "generic"): 1, (1, "bitmap_grouped"): 3,
+        (2, None): 2, (2, "packed_pos"): 2, (2, "packed"): 2, (2, "generic"): 1,
+        (3, None): 1, (3, "packed_pos"): 1, (3, "packed"): 1, (3, "bitmap"): 1,
+    }
+    tables = [bm, pos, packed, generic]
+    for (t, force), kind in want.items():
+        assert model.layout(tables[t], force).kind == kind, (tables[t], force)
+    assert model.layout(bm, "packed").packed_bits == 14 and model.layout(bm, "packed").pos_bits == 0
+    assert model.layout(bm, "generic").packed_bits == 0
+    g, p = model.layout(bm, "bitmap_grouped"), model.layout(bm, "bitmap_price")
+    assert g.no_fused and not g.no_slice and p.no_fused and p.no_slice and g.slice and p.slice
+    assert not model.layout(bm, "bitmap").no_fused
+
+
 def test_tune_parsing():
     assert model.tune_from_env("stagekb=4") == (4, 0, 0)
     assert model.tune_from_env("pdl=off,ipw=64,k0ctas=3") == (0, 64, 3)
