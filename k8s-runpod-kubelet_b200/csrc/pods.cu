@@ -13,13 +13,13 @@
 //                   over and rpk_pods_pending_list_device returns.  The list is in range by construction, so no host
 //                   check and no upload stand before the gather.
 //   k_pod_stale     of one GPU's owned slots: the ascending list of the pending slots whose stored result is stale, their
-//                   number and the number of pending slots (rpk_select_pending_changed, before its select)
+//                   number and the number of pending slots (rpk_select_pending_changed*, before the reselect)
 //   k_pod_stale_reach  the same against a non-empty change window of rpk_offers_refresh: a result older than the
 //                   current table is stale only below the floor or when a changed offer reaches the row
-//   k_pod_result_diff  over the rows that select returned: store each row's result and write the rows whose list changed,
-//                   ascending, to the host (rpk_select_pending_changed, after its select)
-//   k_pod_result_diff_xchg  the same, the changed rows written into region my_rank of every rank's exchange buffer, then
-//                   a peer signal (rpk_select_pending_changed_gather; with the row count read on the device,
+//   k_pod_result_diff_xchg  over the rows k_pod_reselect_top5 returned, their number read on the device: store each
+//                   row's result and write the rows whose list changed, ascending, into one region per output (the
+//                   host call: its device copy of the rows; the one-process-per-GPU forms: region my_rank of every
+//                   rank's exchange buffer), then a peer signal if a group is bound (rpk_select_pending_changed[_gather],
 //                   rpk_select_pending_changed_device_gather)
 // The host entry points check every slot against the table's N before its upload.  The device entry points cannot, so
 // an entry outside [0, N) is defined here: the seed skips it, and the gather writes a row with cloud byte kCloudNone,
@@ -106,8 +106,8 @@ __device__ __forceinline__ uint32_t count_flags(const uint4& v) {
 }
 
 // The compaction itself, shared by the kernels that turn 16-item units into an ascending list: k_pod_pending (units of
-// the flag column), k_pod_stale[_reach] (units of a GPU's owned slots) and k_pod_result_diff[_xchg] (units of the
-// reselected rows).
+// the flag column), k_pod_stale[_reach] (units of a GPU's owned slots) and k_pod_result_diff_xchg (units of the reselected
+// rows).
 // The policy Pol says what a unit holds:
 //   prepare(c_lo, c_hi)             every thread, once the CTA's share [c_lo, c_hi) is known, before pass 1
 //   V none()                        a unit past the CTA's share
@@ -387,17 +387,20 @@ __global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_stale
     compact_units(p, n_units, x.s.tile_state, x.s.ticket);
 }
 
-// k_pod_result_diff's units: 16 reselected rows.  Pass 1 compares each row's new list with the stored one (a slot never
-// reported has none, and differs), stores the row's result -- its list, the columns the gather took it from and the
-// offer-table generation -- and leaves the changed bits in mask[u]; pass 2 writes the changed rows out.
-struct DiffUnits {
+// k_pod_result_diff_xchg's units: 16 reselected rows of the n the stale step listed.  Pass 1 compares each row's new
+// list with the stored one (a slot never reported has none, and differs), stores the row's result -- its list, the
+// columns the reselect took it from and the offer-table generation -- and leaves the changed bits in mask[u]; pass 2
+// writes each changed row into every output region (peer stores over NVLink for an exchange buffer) and the last CTA in
+// unit order writes the count into every count word.  The stores are made visible system-wide before a CTA counts as
+// finished, so the CTA that finishes last can signal the results epoch: a peer past its wait reads every region.
+struct DiffXchgUnits {
     struct V { uint32_t keep; };
     using Count = uint32_t;
     const ResultDiffArgs& a;
+    const ResultXchgArgs& x;
+    uint32_t n;
     __device__ __forceinline__ V none() const { return V{0u}; }
-    __device__ __forceinline__ V load(uint32_t u) const { return load_n(u, a.n); }
-    // unit u of a list of n rows
-    __device__ __forceinline__ V load_n(uint32_t u, uint32_t n) const {
+    __device__ __forceinline__ V load(uint32_t u) const {
         uint32_t keep = 0;
         for (uint32_t k = 0; k < kPendUnit; ++k) {
             const uint32_t i = u * kPendUnit + k;
@@ -422,31 +425,6 @@ struct DiffUnits {
     __device__ __forceinline__ uint32_t id(uint32_t u, uint32_t k) const { return u * kPendUnit + k; }
     __device__ __forceinline__ void emit(uint32_t i, uint32_t row) const {  // best is the list's first entry
         const int32_t* t = a.top5 + (size_t)row * RPK_TOPK;
-        a.out_slot[i] = a.list[row]; a.out_best[i] = t[0];
-#pragma unroll
-        for (int q = 0; q < RPK_TOPK; ++q) a.out_top5[(size_t)i * RPK_TOPK + q] = t[q];
-    }
-    __device__ __forceinline__ void set_count(uint32_t n) const { *a.n_out = n; }
-    __device__ __forceinline__ void cta_total(Count) const {}
-    __device__ __forceinline__ void fence() const { __threadfence(); }
-    __device__ __forceinline__ void last() const {}
-    __device__ __forceinline__ void last_warp() const {}
-    __device__ __forceinline__ void prepare(uint32_t, uint32_t) const {}
-};
-
-__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff(ResultDiffArgs a, uint32_t n_units) {
-    DiffUnits p{a};
-    compact_units(p, n_units, a.tile_state, a.ticket);
-}
-
-// The exchange form (rpk_select_pending_changed_gather): the same units and stores, but each changed row goes into
-// region my_rank of every rank's buffer (peer stores over NVLink) and the count into word my_rank of each.  The stores
-// are made visible system-wide before a CTA counts as finished, so the CTA that finishes last can signal the results
-// epoch: a peer past its wait reads every region.
-struct DiffXchgUnits : DiffUnits {
-    const ResultXchgArgs& x;
-    __device__ __forceinline__ void emit(uint32_t i, uint32_t row) const {  // best is the list's first entry
-        const int32_t* t = a.top5 + (size_t)row * RPK_TOPK;
         const uint32_t s = a.list[row];
         int32_t v[RPK_TOPK];
 #pragma unroll
@@ -460,32 +438,22 @@ struct DiffXchgUnits : DiffUnits {
         }
     }
     __device__ __forceinline__ void set_count(uint32_t n) const { for (int o = 0; o < x.n_out; ++o) *x.count[o] = n; }
+    __device__ __forceinline__ void cta_total(Count) const {}
     __device__ __forceinline__ void fence() const { __threadfence_system(); }
+    __device__ __forceinline__ void last() const {}
     __device__ __forceinline__ void last_warp() const {
         if (x.peers.n > 0) signal_peers(x.peers, kFlagResults, kFlagResultsCtr, 0, x.peers.inline_wait != 0);
     }
+    __device__ __forceinline__ void prepare(uint32_t, uint32_t) const {}
 };
 
-// ... over a list whose length n the device holds (rpk_select_pending_changed_device_gather)
-struct DiffXchgCountUnits : DiffXchgUnits {
-    uint32_t n;
-    __device__ __forceinline__ V load(uint32_t u) const { return load_n(u, n); }
-};
-
-// kDevCount: the row count is *d_n, read here, and the grid was sized for the worst case (x.d.n and n_units unused):
-// the units of the count are shared out over the whole grid, so a CTA past them publishes a zero count at once and the
-// look-back, the count stores and the last CTA's signal complete as for a launch sized for the count
-template <bool kDevCount>
-__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff_xchg(ResultXchgArgs x, uint32_t n_units,
-                                                                                            const uint32_t* __restrict__ d_n) {
-    if constexpr (kDevCount) {
-        const uint32_t n = *d_n;
-        DiffXchgCountUnits p{{{x.d}, x}, n};
-        compact_units(p, (n + kPendUnit - 1) / kPendUnit, x.d.tile_state, x.d.ticket);
-    } else {
-        DiffXchgUnits p{{x.d}, x};
-        compact_units(p, n_units, x.d.tile_state, x.d.ticket);
-    }
+// The row count is *d_n, read here, and the grid was sized for the worst case: the units of the count are shared out
+// over the whole grid, so a CTA past them publishes a zero count at once and the look-back, the count stores and the
+// last CTA's signal complete as for a launch sized for the count
+__global__ void __launch_bounds__(kPendThreads, 1024 / kPendThreads) k_pod_result_diff_xchg(ResultXchgArgs x, const uint32_t* __restrict__ d_n) {
+    const uint32_t n = *d_n;
+    DiffXchgUnits p{x.d, x, n};
+    compact_units(p, (n + kPendUnit - 1) / kPendUnit, x.d.tile_state, x.d.ticket);
 }
 
 int launch_pod_fill(const PodRows& t, uint8_t* pending, uint32_t N, int sm_count, cudaStream_t st) {
@@ -551,24 +519,9 @@ int launch_pod_stale_reach(const StaleReachArgs& a, uint32_t n_units, int sm_cou
     return 1;
 }
 
-int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st) {
-    if (a.n == 0) return 0;
-    const uint32_t n_units = (a.n + kPendUnit - 1) / kPendUnit;
-    k_pod_result_diff<<<compact_grid(n_units, sm_count), kPendThreads, 0, st>>>(a, n_units);
-    RPK_CUDA(cudaGetLastError());
-    return 1;
-}
-
-int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st) {
-    const uint32_t n_units = (x.d.n + kPendUnit - 1) / kPendUnit;  // no rows: one CTA publishes the count and signals
-    k_pod_result_diff_xchg<false><<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, n_units, nullptr);
-    RPK_CUDA(cudaGetLastError());
-    return 1;
-}
-
-int launch_pod_result_xchg_device(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st) {
-    const uint32_t n_units = (n_max + kPendUnit - 1) / kPendUnit;
-    k_pod_result_diff_xchg<true><<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, n_units, d_n);
+int launch_pod_result_xchg(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st) {
+    const uint32_t n_units = (n_max + kPendUnit - 1) / kPendUnit;  // no rows: one CTA publishes the count and signals
+    k_pod_result_diff_xchg<<<std::max<uint32_t>(compact_grid(n_units, sm_count), 1u), kPendThreads, 0, st>>>(x, d_n);
     RPK_CUDA(cudaGetLastError());
     return 1;
 }

@@ -1171,12 +1171,14 @@ void result_range(uint32_t N, int n, int s, uint32_t* lo, uint32_t* hi) {
 }
 
 // The stored results of ds's owned slots [lo, hi), allocated on the first call after a reset with every generation 0
-// (nothing reported), and the scratch and mapped output of a call that reselects all of them.  The caller has waited.
+// (nothing reported), and the scratch and mapped output of a call that reselects all of them.  The owned range is fixed
+// until the next reset (check_results_range), so no later call grows r_lane.  The caller has waited.
 void reserve_results(DeviceState& ds, uint32_t lo, uint32_t hi) {
     if (ds.res_ready) return;
     const size_t n = ((size_t)(hi - lo) + 15) / 16 * 16 + 16;  // whole units: k_pod_stale loads 16 slots at a time
     ds.r_mem.reserve(n); ds.r_vcpu.reserve(n); ds.r_ram.reserve(n); ds.r_max_price.reserve(n); ds.r_cloud.reserve(n);
-    ds.r_gen.reserve(n); ds.r_top5.reserve(n * RPK_TOPK); ds.r_best.reserve(n); ds.r_list.reserve(n); ds.r_mask.reserve(n / 16 + 1);
+    ds.r_gen.reserve(n); ds.r_top5.reserve(n * RPK_TOPK); ds.r_list.reserve(n); ds.r_mask.reserve(n / 16 + 1); ds.r_dn.reserve(2);
+    reserve_lane(ds.r_lane, std::max<uint32_t>(hi - lo, 1u), RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
     ds.r_out.reserve(n * (2 + RPK_TOPK)); ds.h_res.reserve(64 + ds.r_out.cap * 4);  // result_rows: the same layout
     RPK_CUDA(cudaMemset(ds.r_gen.p, 0, ds.r_gen.cap * sizeof(uint32_t)));
     RPK_CUDA(cudaDeviceSynchronize());
@@ -1191,9 +1193,10 @@ int check_results_range(rpk_ctx* ctx, const DeviceState& ds, uint32_t lo, uint32
     return fail(ctx, RPK_ESTATE, std::string(who) + ": the stored results of this GPU were made for another slot range (call rpk_pods_reset first)");
 }
 
-// The counts in mapped memory (the device's view with d = true), and the changed rows: in r_out (d = true), or their host
-// copy in h_res (false).  The rows go back in three copies of the length the count says: written to mapped memory
-// straight from the kernel, row by row, they cost 9 ms at 1M changed rows on an H100 (4- and 20-byte PCIe writes).
+// The counts in mapped memory (the device's view with d = true): [n_pending, n_reselected] as the stale step left them
+// in r_dn, then the diff's count of changed rows.  The changed rows: in r_out (d = true), or their host copy in h_res
+// (false).  The rows go back in three copies of the length the count says: written to mapped memory straight from the
+// kernel, row by row, they cost 9 ms at 1M changed rows on an H100 (4- and 20-byte PCIe writes).
 struct ResultRows { uint32_t* counts; uint32_t* slot; int32_t* best; int32_t* top5; };
 ResultRows result_rows(DeviceState& ds, bool d) {
     const size_t cap = ds.r_out.cap / (2 + RPK_TOPK);
@@ -1202,21 +1205,18 @@ ResultRows result_rows(DeviceState& ds, bool d) {
     return ResultRows{counts, reinterpret_cast<uint32_t*>(b), b + cap, b + 2 * cap};
 }
 
-// The stale step of ds over its owned slots [lo, hi): k_pod_stale lists the stale pending slots in r_list, their number
-// lands in *n_out and the number of owned pending slots in *n_pending: the mapped counts by default (zeroed here; read
-// them after synchronising st), or device words (the device form; the caller zeroes them for an empty range, where
-// nothing is launched).  While the ctx's change window is not empty, k_pod_stale_reach takes k_pod_stale's place.  The
-// caller has reserved the results and waited for the select scope.  Returns the kernels launched.
-int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi, cudaStream_t st, uint32_t* n_out = nullptr,
-                  uint32_t* n_pending = nullptr) {
-    if (!n_out) {
-        const ResultRows m = result_rows(ds, true), h = result_rows(ds, false);
-        n_out = m.counts; n_pending = m.counts + 1;
-        reinterpret_cast<volatile uint32_t*>(h.counts)[0] = 0u; reinterpret_cast<volatile uint32_t*>(h.counts)[1] = 0u;
+// The stale step of ds over its owned slots [lo, hi): k_pod_stale lists the stale pending slots in r_list and writes
+// [n_pending, n_reselected] to r_dn (zeroed here for an empty range, where nothing is launched).  While the ctx's change
+// window is not empty, k_pod_stale_reach takes k_pod_stale's place.  The caller has reserved the results and waited for
+// the select scope.  Returns the kernels launched.
+int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi, cudaStream_t st) {
+    if (hi == lo) {
+        RPK_CUDA(cudaMemsetAsync(ds.r_dn.p, 0, 2 * sizeof(uint32_t), st));
+        return 0;
     }
     StaleArgs a{};
     a.flags = ds.pt_pending.p; a.t = ds.pods_table(); a.N = ds.podsN; a.u_lo = lo / 16; a.r = ds.results(); a.gen = ctx->offer_gen;
-    a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = n_out; a.n_pending = n_pending;
+    a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = ds.r_dn.p + 1; a.n_pending = ds.r_dn.p;
     a.tile_state = ds.pt_state.p; a.ticket = ds.pt_ticket.p;
     if (ctx->window.empty()) return launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, st);
     const StaleReachArgs x{a, ctx->offer_floor, ds.win.p, (uint32_t)ctx->window.size(),
@@ -1224,37 +1224,35 @@ int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi,
     return launch_pod_stale_reach(x, (hi - lo + 15) / 16, ds.sm_count, st);
 }
 
-// The diff of k reselected rows of ds (the list in r_list, their columns and top-5 lists in ln's buffers) against the
-// stored results of the owned slots from lo on, the changed rows to the mapped outputs
-ResultDiffArgs diff_args(DeviceState& ds, const DeviceState::Lane& ln, uint32_t k, uint32_t lo, uint32_t gen) {
-    const ResultRows m = result_rows(ds, true);
-    ResultDiffArgs d{};
-    d.list = ds.r_list.p; d.n = k;
-    d.cols = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p}; d.top5 = ln.top5.p;
-    d.r = ds.results(); d.r_lo = lo; d.gen = gen; d.mask = ds.r_mask.p;
-    d.out_slot = m.slot; d.out_best = m.best; d.out_top5 = m.top5; d.n_out = m.counts;
-    d.tile_state = ds.pt_state.p; d.ticket = ds.pt_ticket.p;
-    return d;
+// The host-sync forms' read of the stale step's counts: r_dn is copied into the mapped block behind it, and read there
+// once st has been synchronised
+void copy_stale_counts(DeviceState& ds, cudaStream_t st) {
+    RPK_CUDA(cudaMemcpyAsync(result_rows(ds, false).counts, ds.r_dn.p, 2 * sizeof(uint32_t), cudaMemcpyDeviceToHost, st));
 }
 
-// The reselect of the k stale rows enqueue_stale listed (lane 0's buffers sized for them): the gather, one select with
-// top-5, and the diff that stores each row's result and writes the changed rows to the mapped outputs (x null) or, in
-// its exchange form, to the buffers x names (x->d is filled here).  The exchange form runs with k = 0 too.  Returns the
-// kernels launched.
-int enqueue_reselect(DeviceState& ds, uint32_t k, uint32_t lo, uint32_t gen, cudaStream_t st, ResultXchgArgs* x = nullptr) {
-    DeviceState::Lane& ln = ds.lane[0];
-    const RowSource list{RowSource::DevList, PodCols{}, ds.r_list.p};
+// The reselect of the rows enqueue_stale listed, whose number the kernels read from r_dn on the device, sized for n_max
+// rows: the count the host read (host_count), or the owned range's worst case.  k_pod_reselect_top5 writes their
+// columns and top-5 lists to r_lane (and r_dn to d_counts, if not null); the diff stores each row's result and writes
+// the changed rows where x says (x.d is filled here).  With a host count of 0 only the diff runs, which still publishes
+// the count 0 and signals.  Returns the kernels launched.
+int enqueue_reselect(DeviceState& ds, uint32_t n_max, bool host_count, uint32_t lo, uint32_t gen, ResultXchgArgs& x,
+                     uint32_t* d_counts, cudaStream_t st) {
+    const DeviceState::Lane& ln = ds.r_lane;
+    const PodRows cols{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
     int launches = 0;
-    if (k) {
-        SelectArgs a{};
-        launches += pod_columns(ds, ln, list, 0, k, a, st);
-        a.P = k; a.best_out[0] = ds.r_best.p; a.n_out = 1; a.self_out = 0; a.row0 = 0; a.top5 = ln.top5.p;
-        launches += enqueue_select(ds, ln, a, st);
+    if (n_max || !host_count) {
+        ReselectArgs r{};
+        offer_args(ds, r.s);
+        r.s.top5 = ln.top5.p;
+        r.t = ds.pods_table(); r.out = cols;
+        r.list = ds.r_list.p; r.dn = ds.r_dn.p; r.counts = d_counts;
+        launches += launch_pod_reselect(r, n_max, ds.sm_count, st);
     }
-    const ResultDiffArgs d = diff_args(ds, ln, k, lo, gen);
-    if (!x) return launches + launch_pod_result_diff(d, ds.sm_count, st);
-    x->d = d;
-    return launches + launch_pod_result_xchg(*x, ds.sm_count, st);
+    ResultDiffArgs& d = x.d;
+    d.list = ds.r_list.p; d.cols = cols; d.top5 = ln.top5.p;
+    d.r = ds.results(); d.r_lo = lo; d.gen = gen; d.mask = ds.r_mask.p;
+    d.tile_state = ds.pt_state.p; d.ticket = ds.pt_ticket.p;
+    return launches + launch_pod_result_xchg(x, ds.r_dn.p + 1, n_max, ds.sm_count, st);
 }
 }  // namespace
 
@@ -1273,7 +1271,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
     std::vector<uint32_t> pend((size_t)n, 0), stale((size_t)n, 0);
     std::vector<uint64_t> launches((size_t)n, 0);
     // 1. every GPU lists the stale pending slots of its own range (the flags and the table are replicated); both counts
-    //    land in mapped memory, so the one synchronise needs no copy behind it
+    //    are copied into mapped memory ahead of the one synchronise
     int rc = guarded(ctx, [&]() -> int {
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
@@ -1283,13 +1281,14 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             reserve_results(ds, lo, hi);
             reserve_compaction_state(ds);
             launches[(size_t)s] += (uint64_t)enqueue_stale(ctx, ds, lo, hi, ds.stream);
+            copy_stale_counts(ds, ds.stream);
         }
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
             RPK_CUDA(cudaSetDevice(ds.dev));
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
             const volatile uint32_t* c = result_rows(ds, false).counts;
-            stale[(size_t)s] = c[0]; pend[(size_t)s] = c[1];
+            pend[(size_t)s] = c[0]; stale[(size_t)s] = c[1];
         }
         return RPK_OK;
     });
@@ -1305,29 +1304,25 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
         for (int s = 0; s < n; ++s) ctx->launches += launches[(size_t)s];
         return RPK_OK;
     }
-    // 3. every GPU gathers, selects and diffs its stale rows on its own thread, in one select over the list (lane 0's
-    //    scratch); the count of changed rows lands in mapped memory, the rows themselves come back in copies of that
+    // 3. every GPU reselects and diffs its stale rows on its own thread; the diff writes the changed rows to r_out, as one
+    //    region without peers, and their count to mapped memory; the rows themselves come back in copies of that
     //    length, and they are copied out in GPU order, which is ascending
     return guarded(ctx, [&]() -> int {
-        for (int s = 0; s < n; ++s) {  // lane 0's buffers, sized on the calling thread
-            DeviceState& ds = ctx->devs[(size_t)s];
-            if (!stale[(size_t)s]) continue;
-            RPK_CUDA(cudaSetDevice(ds.dev));
-            reserve_lane(ds.lane[0], stale[(size_t)s], RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
-        }
         ctx->workers.run(n, [&](int s) {
             DeviceState& ds = ctx->devs[(size_t)s];
             const uint32_t k = stale[(size_t)s];
             if (!k) return;
             uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
             RPK_CUDA(cudaSetDevice(ds.dev));
-            ds.res_ready = false;  // until the diff has stored every reselected row
-            launches[(size_t)s] += (uint64_t)enqueue_reselect(ds, k, lo, gen, ds.stream);
-            RPK_CUDA(cudaStreamSynchronize(ds.stream));
-            ds.res_ready = true;
             const ResultRows m = result_rows(ds, true);
             const ResultRows h = result_rows(ds, false);
-            const uint32_t c = *reinterpret_cast<volatile uint32_t*>(h.counts);
+            ResultXchgArgs x{};
+            x.n_out = 1; x.cap = (uint32_t)(ds.r_out.cap / (2 + RPK_TOPK)); x.region[0] = m.slot; x.count[0] = m.counts + 2;
+            ds.res_ready = false;  // until the diff has stored every reselected row
+            launches[(size_t)s] += (uint64_t)enqueue_reselect(ds, k, true, lo, gen, x, nullptr, ds.stream);
+            RPK_CUDA(cudaStreamSynchronize(ds.stream));
+            ds.res_ready = true;
+            const uint32_t c = reinterpret_cast<volatile uint32_t*>(h.counts)[2];
             if (c) {
                 RPK_CUDA(cudaMemcpyAsync(h.slot, m.slot, (size_t)c * 4, cudaMemcpyDeviceToHost, ds.stream));
                 RPK_CUDA(cudaMemcpyAsync(h.best, m.best, (size_t)c * 4, cudaMemcpyDeviceToHost, ds.stream));
@@ -1341,7 +1336,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             ctx->launches += launches[(size_t)s];
             if (!stale[(size_t)s]) continue;
             const ResultRows h = result_rows(ds, false);
-            const uint32_t c = *reinterpret_cast<volatile uint32_t*>(h.counts);
+            const uint32_t c = reinterpret_cast<volatile uint32_t*>(h.counts)[2];
             memcpy(slots_out + at, h.slot, (size_t)c * 4);
             memcpy(best + at, h.best, (size_t)c * 4);
             memcpy(top5 + (size_t)at * RPK_TOPK, h.top5, (size_t)c * 4 * RPK_TOPK);
@@ -1407,14 +1402,14 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
         reserve_results(ds, lo, hi);
         reserve_compaction_state(ds);
         uint64_t launches = (uint64_t)enqueue_stale(ctx, ds, lo, hi, st);
-        RPK_CUDA(cudaStreamSynchronize(st));  // the select needs the row count on the host
+        copy_stale_counts(ds, st);
+        RPK_CUDA(cudaStreamSynchronize(st));  // the reselect is sized for the row count the host reads
         const volatile uint32_t* c = result_rows(ds, false).counts;
-        const uint32_t k = c[0];
-        *n_pending = c[1]; *n_reselected = k;
-        if (k) reserve_lane(ds.lane[0], k, RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
+        const uint32_t k = c[1];
+        *n_pending = c[0]; *n_reselected = k;
         ResultXchgArgs x = results_xchg(ctx, shard, n_ranks, my_rank, d_xchg, cap);
-        ds.res_ready = false;       // until the diff is enqueued behind the select
-        launches += (uint64_t)enqueue_reselect(ds, k, lo, gen, st, &x);
+        ds.res_ready = false;       // until the diff is enqueued behind the reselect
+        launches += (uint64_t)enqueue_reselect(ds, k, true, lo, gen, x, nullptr, st);
         ds.res_ready = true;
         ds.sel_scope.device_end(st, true);
         ctx->launches += launches;
@@ -1422,10 +1417,10 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
     });
 }
 
-// The same tick with the row count kept on the device: the stale step writes it to r_dn, the reselect kernel and the
-// diff read it there and are sized for the rank's worst case, hi - lo rows, so nothing waits for the host.  Every buffer
-// is sized in prep for that worst case: after one call the call only enqueues.  The reselected rows' columns and lists
-// go to r_lane, which no other call grows, so a select of any size on the ctx cannot free what a captured graph writes.
+// The same tick with the row count kept on the device: the reselect and the diff are sized for the rank's worst case,
+// hi - lo rows, so nothing waits for the host.  Every buffer is sized in prep for that worst case: after one call the
+// call only enqueues.  The reselected rows' columns and lists go to r_lane, which no select grows, so a select of any
+// size on the ctx cannot free what a captured graph writes.
 int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_ranks, int my_rank, uint32_t* const* d_xchg,
                                              uint32_t cap, uint32_t* d_counts, void* stream) {
     static const char* who = "rpk_select_pending_changed_device_gather";
@@ -1439,27 +1434,13 @@ int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_rank
     const auto prep = [&](DeviceState&) {
         reserve_results(ds, lo, hi);
         reserve_compaction_state(ds);
-        ds.r_dn.reserve(2);
-        reserve_lane(ds.r_lane, std::max<uint32_t>(hi - lo, 1u), RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
         return RPK_OK;
     };
     return device_call(ctx, shard, stream, &DeviceState::sel_scope, prep, [&](DeviceState&, cudaStream_t st) {
-        uint32_t* dn = ds.r_dn.p;  // [n_pending, n_reselected]
-        uint64_t launches = 0;
         ds.res_ready = false;  // until every launch is enqueued
-        if (hi > lo) launches += (uint64_t)enqueue_stale(ctx, ds, lo, hi, st, dn + 1, dn);
-        else RPK_CUDA(cudaMemsetAsync(dn, 0, 2 * sizeof(uint32_t), st));  // an empty range: no stale step
-        ReselectArgs r{};
-        offer_args(ds, r.s);
-        const DeviceState::Lane& ln = ds.r_lane;
-        r.s.top5 = ln.top5.p;
-        r.t = ds.pods_table();
-        r.out = PodRows{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
-        r.list = ds.r_list.p; r.dn = dn; r.counts = d_counts;
-        launches += (uint64_t)launch_pod_reselect(r, hi - lo, ds.sm_count, st);
+        uint64_t launches = (uint64_t)enqueue_stale(ctx, ds, lo, hi, st);
         ResultXchgArgs x = results_xchg(ctx, shard, n_ranks, my_rank, d_xchg, cap);
-        x.d = diff_args(ds, ds.r_lane, 0, lo, gen);
-        launches += (uint64_t)launch_pod_result_xchg_device(x, dn + 1, hi - lo, ds.sm_count, st);
+        launches += (uint64_t)enqueue_reselect(ds, hi - lo, false, lo, gen, x, d_counts, st);
         ds.res_ready = true;
         ctx->launches += launches;
     });

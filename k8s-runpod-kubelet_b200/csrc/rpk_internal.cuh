@@ -314,23 +314,22 @@ struct StaleArgs {
     StoredResults r; uint32_t gen;   // stored results of the owned slots, the ctx's offer-table generation
     uint16_t* mask;                  // [units] scratch: the kept slots of each unit, from pass 1 to pass 2
     uint32_t* out;                   // the stale slot ids, ascending
-    uint32_t* n_out;                 // their number (mapped host memory)
-    uint32_t* n_pending;             // the owned pending slots (mapped host memory)
+    uint32_t* n_out;                 // their number (device memory)
+    uint32_t* n_pending;             // the owned pending slots (device memory)
     unsigned long long* tile_state;  // look-back state: pending_state_words entries; zero between calls
     uint32_t* ticket;                // [3] scheduling ticket, finished CTAs, pending count; zero between calls
 };
 struct ResultDiffArgs {
-    const uint32_t* list; uint32_t n;  // the reselected slots, ascending
-    PodRows cols; const int32_t* top5; // row i: the columns the gather took and the select's top-5 list
+    const uint32_t* list;              // the reselected slots, ascending
+    PodRows cols; const int32_t* top5; // row i: the columns the reselect took and its top-5 list
     StoredResults r; uint32_t r_lo, gen;
     uint16_t* mask;                    // [units] scratch, as StaleArgs::mask
-    uint32_t* out_slot; int32_t* out_best; int32_t* out_top5;  // the changed rows, ascending
-    uint32_t* n_out;                   // their number (mapped host memory)
     unsigned long long* tile_state; uint32_t* ticket;  // as StaleArgs
 };
-// The diff's exchange form (rpk_select_pending_changed_gather): the changed rows go into region my_rank of every buffer
-// instead (d.out_* and d.n_out unused), the count into word my_rank of each, and the CTA that finishes last signals the
-// results epoch.  Region of a buffer of capacity cap: [slot : cap][best : cap][top5 : 5 cap] words.
+// Where the diff writes: the changed rows, ascending, into each of n_out regions, their count into each count word,
+// and the CTA that finishes last signals the results epoch when peers are bound.  The host call has one region, its
+// device copy of the rows, and one count word in mapped memory; the one-process-per-GPU forms write region my_rank and
+// word my_rank of every rank's exchange buffer.  Region of capacity cap: [slot : cap][best : cap][top5 : 5 cap] words.
 struct ResultXchgArgs {
     ResultDiffArgs d;
     int n_out; uint32_t cap;
@@ -347,8 +346,8 @@ struct StaleReachArgs {
     const uint2* win; uint32_t n_win;
     const int32_t* mem; const int32_t* vcpu; const int32_t* ram; const double* sp; const double* cp; const uint8_t* flags;
 };
-// The reselect of the device form (rpk_select_pending_changed_device_gather, select.cu): rows [0, dn[1]) of list, the
-// count the stale step left on the device.  Row i's five columns go to out, its top-5 list to s.top5 (s: the offer views,
+// The reselect of the pending results (rpk_select_pending_changed*, select.cu): rows [0, dn[1]) of list, the count the
+// stale step left on the device.  Row i's five columns go to out, its top-5 list to s.top5 (s: the offer views,
 // G, the rank thresholds' distinct values and pk, as enqueue_select fills them).  counts (nullable) := dn[0, 2).
 struct ReselectArgs {
     SelectArgs s;
@@ -362,12 +361,10 @@ struct ReselectArgs {
 int launch_pod_reselect(const ReselectArgs& r, uint32_t n_max, int sm_count, cudaStream_t st);
 int launch_pod_stale(const StaleArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
 int launch_pod_stale_reach(const StaleReachArgs& a, uint32_t n_units, int sm_count, cudaStream_t st);
-int launch_pod_result_diff(const ResultDiffArgs& a, int sm_count, cudaStream_t st);
-// launches even when x.d.n = 0: the count 0 still goes out and the peers are still signalled
-int launch_pod_result_xchg(const ResultXchgArgs& x, int sm_count, cudaStream_t st);
-// the same with the row count read from d_n on the device (x.d.n unused): the grid is sized for n_max rows, the worst
-// case; the CTAs past the count publish a zero count at once
-int launch_pod_result_xchg_device(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st);
+// the diff of the *d_n reselected rows, the count read on the device: the grid is sized for n_max rows, the worst case,
+// and the CTAs past the count publish a zero count at once.  Launches for n_max = 0 too: the count 0 still goes out and
+// the peers are still signalled
+int launch_pod_result_xchg(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
 
@@ -490,15 +487,14 @@ struct DeviceState {
     PinnedBuf h_pending;                   // rpk_select_pending: the list's length, written by the kernel
     cudaStream_t pending_stream = nullptr; // rpk_select_pending: the list's copy to the caller, beside the select
     uint32_t podsN = 0; bool pods_sized = false;
-    // pending results (rpk_select_pending_changed), allocated on its first call: the stored results of the owned slots,
-    // the stale list, its rows' best (the select needs a vector), the per-unit masks, the changed rows (r_out:
-    // [slots : cap][best : cap][top5 : 5 cap]) and their host copy behind the counts the kernels write
-    // (h_res: [counts : 64 bytes][the r_out layout]).  res_ready: allocated for this table and not cleared since
-    // (rpk_pods_reset, a failed call)
-    DevBuf<int32_t> r_mem, r_vcpu, r_ram, r_top5, r_best, r_out; DevBuf<double> r_max_price; DevBuf<uint8_t> r_cloud;
+    // pending results (rpk_select_pending_changed*), allocated on the first call after a reset: the stored results of the
+    // owned slots, the stale list, the per-unit masks, [n_pending, n_reselected] of the stale step (r_dn), the reselected
+    // rows' columns and top-5 lists (r_lane: sized once for the owned range, so a captured device-form call keeps
+    // pointing at them), the host call's changed rows (r_out: [slots : cap][best : cap][top5 : 5 cap]) and their host
+    // copy behind the counts (h_res: [r_dn's copy, the changed count : 64 bytes][the r_out layout]).  res_ready:
+    // allocated for this table and not cleared since (rpk_pods_reset, a failed call)
+    DevBuf<int32_t> r_mem, r_vcpu, r_ram, r_top5, r_out; DevBuf<double> r_max_price; DevBuf<uint8_t> r_cloud;
     DevBuf<uint32_t> r_gen, r_list; DevBuf<uint16_t> r_mask;
-    // rpk_select_pending_changed_device_gather: [n_pending, n_reselected] of the stale step, and the reselected rows'
-    // columns and top-5 lists (its own buffers, sized once for the owned range: a captured call keeps pointing at them)
     DevBuf<uint32_t> r_dn; Lane r_lane;
     PinnedBuf h_res;
     bool res_ready = false;

@@ -13,8 +13,8 @@
 //                     applies price < maxPrice to the winner (the bound is a prefix of the sorted order) and stores
 //                     the offer index into every peer's assignment vector (the fused all-gather).
 //   k_select_top5*    optional: the whole <=5 gpuTypeIds list per row (runpod_client.go:502-509).
-//   k_pod_reselect_top5  the pending results' device form: gather + thresholds + top-5 over a list whose length is
-//                     read on the device (rpk_select_pending_changed_device_gather)
+//   k_pod_reselect_top5  the pending results' reselect: gather + thresholds + top-5 over a list whose length is read
+//                     on the device (rpk_select_pending_changed, _gather and _device_gather)
 //   k_gather_push     several output vectors: copies the finished slice to the peers (a second launch copies the top-5
 //                     lists' slice for rpk_select_device_gather_top5); k_peer_signal (select_persist.cu) then signals a
 //                     bound peer group.
@@ -455,10 +455,10 @@ __global__ void __launch_bounds__(256) k_select_top5_bitmap(SelectArgs a) {
     top5_walk_bitmap<STRIDE>(a.view[c].price, a.view[c].bitmap, a.view[c].perm, a.G, o1, o2, o3, mx, a.top5 + (size_t)p * RPK_TOPK);
 }
 
-// The reselect of rpk_select_pending_changed_device_gather: rows [0, n) of r.list, n = r.dn[1] as the stale step left
-// it on the device, so the launch is sized for the worst case and needs no count on the host.  Row i gathers its slot's
-// five columns into r.out (the columns the diff stores with the result) and writes its top-5 list to r.s.top5 -- what
-// the host-sync form's gather, select and top-5 kernel leave there, bit for bit; best is not needed (it is top5[0]).
+// The reselect of rpk_select_pending_changed*: rows [0, n) of r.list, n = r.dn[1] as the stale step left it on the
+// device, so the launch may be sized for a worst case and needs no count on the host.  Row i gathers its slot's five
+// columns into r.out (the columns the diff stores with the result) and writes its top-5 list to r.s.top5 -- what
+// k_pod_gather, a select and its top-5 kernel leave for the same rows, bit for bit; best is not needed (it is top5[0]).
 // STRIDE 32 / 64: the bit-sliced view, one lane per row, the rank thresholds computed here as the select kernels compute
 // them.  STRIDE 0: the wide view (tables without pk.bm_words), one warp per row, which compares the raw columns.  A row
 // whose cloud byte is above 1 gets five -1.  Grid-stride: the grid is a few waves whatever the count.

@@ -5,9 +5,10 @@ On one GPU the ranks of a group are separate one-GPU ctxs on device 0, each boun
 called in turn with the inline wait off; then the device is synchronised.  Every rank has a twin ctx with the same history
 that calls the host-sync form (rpk_select_pending_changed_gather) on buffers and flags of its own, and a reference ctx calls
 rpk_select_pending_changed.  After each step the device form's buffers, flag words and counts must equal the twins' bit for
-bit, and the regions concatenated in rank order must equal the reference's output.  Every buffer and count vector is
-sentinel-filled between guard words before a call and compared whole.  The two-GPU case at the end runs the real group over
-NVLink (skipped on one GPU)."""
+bit, the regions concatenated in rank order must equal the reference's output, and the reference's reported rows must equal
+rpk_select_slots on the same ctx, which runs no reselect kernel.  Every buffer and count vector is sentinel-filled between
+guard words before a call and compared whole.  The two-GPU case at the end runs the real group over NVLink (skipped on one
+GPU)."""
 import contextlib
 import ctypes as C
 import os
@@ -144,6 +145,9 @@ class Twins:
         got = [np.concatenate([p[i] for p in parts]) for i in range(3)]
         assert np.array_equal(got[0], slots), f"{what}: concatenated slots differ from rpk_select_pending_changed"
         assert np.array_equal(got[1], best) and np.array_equal(got[2], top5.reshape(-1, 5)), f"{what}: best / top5 differ"
+        if len(slots):  # an independent reference: rpk_select_slots runs the gather, select and top-5 kernels, no reselect
+            sb, st = self.ref.select_slots(slots, want_top5=True)
+            assert np.array_equal(best, sb) and np.array_equal(top5.reshape(-1, 5), st), f"{what}: reported rows differ from rpk_select_slots"
         return n_p, n_r, slots
 
 

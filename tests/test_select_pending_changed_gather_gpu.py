@@ -5,8 +5,8 @@ On one GPU the ranks of a group are separate one-GPU ctxs on device 0 with the s
 the group's flag arrays; their exchange buffers and flag arrays are torch tensors on device 0.  No kernel here waits for
 another rank: the ranks are called in turn with the inline wait off, then the device is synchronised.  A reference ctx
 with the same history calls rpk_select_pending_changed, and the regions concatenated in rank order must equal its output
-bit for bit.  Every buffer is sentinel-filled between guard words before a call and compared whole, so a store past a
-region's count shows.  The two-GPU cases at the end run the real group over NVLink (skipped on one GPU)."""
+bit for bit; its reported rows must equal rpk_select_slots on the same ctx, which runs no reselect kernel.  Every buffer
+is sentinel-filled between guard words before a call and compared whole, so a store past a region's count shows.  The two-GPU cases at the end run the real group over NVLink (skipped on one GPU)."""
 import ctypes as C
 
 import numpy as np
@@ -109,6 +109,9 @@ class Group:
         got = [np.concatenate([p[i] for p in parts]) for i in range(3)]
         assert np.array_equal(got[0], slots), f"{what}: concatenated slots differ from rpk_select_pending_changed"
         assert np.array_equal(got[1], best) and np.array_equal(got[2], top5.reshape(-1, 5)), f"{what}: best / top5 differ"
+        if len(slots):  # an independent reference: rpk_select_slots runs the gather, select and top-5 kernels, no reselect
+            sb, st = self.ref.select_slots(slots, want_top5=True)
+            assert np.array_equal(best, sb) and np.array_equal(top5.reshape(-1, 5), st), f"{what}: reported rows differ from rpk_select_slots"
         want = self.expected_buffer(slots, best, top5)
         for o, b in enumerate(bufs):
             if not np.array_equal(b, want):
@@ -170,8 +173,8 @@ def test_ranks_equal_the_host_call(n, N):
 
 
 def test_stats_and_launches():
-    """a call that reselects counts one select (offer_scores += n_reselected * G); a steady call counts none and is two
-    launches (the stale step, and the diff that publishes the zero count and signals)"""
+    """a call that reselects counts one select (offer_scores += n_reselected * G) and is three launches; a steady call
+    counts none and is two launches (the stale step, and the diff that publishes the zero count and signals)"""
     N = 20_001
     g = Group(1, N)
     try:
@@ -180,10 +183,11 @@ def test_stats_and_launches():
         e.pods_reset(N)
         e.pods_seed_slots(np.arange(N, dtype=np.uint32), rpk.synth.make_pods(N))
         e.pods_mark_pending(np.arange(0, N, 3, dtype=np.uint32), np.ones(len(range(0, N, 3)), np.uint8))
-        s0 = e.stats()
+        s0, c0 = e.stats(), e.launch_count()
         n_p, n_r = e.select_pending_changed_gather(g.ptrs, g.cap, 0)
         s1 = e.stats()
         assert n_r == n_p == len(range(0, N, 3))
+        assert e.launch_count() == c0 + 3, "a reselecting call is three launches (stale step, reselect, diff)"
         assert s1["select_calls"] == s0["select_calls"] + 1 and s1["offer_scores"] == s0["offer_scores"] + n_r * G
         c0 = e.launch_count()
         assert e.select_pending_changed_gather(g.ptrs, g.cap, 0) == (n_p, 0)

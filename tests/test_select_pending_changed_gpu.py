@@ -85,8 +85,10 @@ def test_first_call_reports_every_pending_slot_then_nothing(name, force):
             pend = np.arange(TRACKED, dtype=np.uint32)
         mark_only(eng, TRACKED, pend)
         m = Mirror(TRACKED)
+        c0 = eng.launch_count()
         n_p, n_r, slots, _, _ = step(eng, m, len(pend))
         assert n_p == n_r == len(slots) == len(pend) and np.array_equal(slots, pend), f"{name} {force}: the first call reports every pending slot"
+        assert eng.launch_count() == c0 + 3, "a reselecting call is three launches per GPU (stale step, reselect, diff)"
         check_mirror(f"{name} force={force}", eng, m, pend, eb[pend], et[pend])
         for cap in (len(pend), 0):  # a steady call needs no capacity
             s0, c0 = eng.stats(), eng.launch_count()

@@ -47,8 +47,8 @@ if not ONLY_MULTI:
         assert np.array_equal(sl, np.flatnonzero(flags)), n
         ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, n_threads=8)
         assert np.array_equal(best, ob) and np.array_equal(t5, ot), n
-    # the pending results (k_pod_stale, k_pod_result_diff): a first call reports every pending slot, a steady call
-    # nothing, a call after an offer upload reselects every pending slot
+    # the pending results (k_pod_stale, k_pod_reselect_top5, k_pod_result_diff_xchg): a first call reports every pending
+    # slot, a steady call nothing, a call after an offer upload reselects every pending slot
     pend = np.flatnonzero(flags)
     n_p, n_r, sl, best, t5 = eng.select_pending_changed(len(pend))
     assert n_r == len(pend) and np.array_equal(sl, pend)
@@ -63,7 +63,7 @@ if not ONLY_MULTI:
     assert 0 < eng.select_pending_changed(len(pend))[1] < len(pend), "two offers reach some rows, not every row"
     assert eng.select_pending_changed(len(pend))[1] == 0
     eng.upload_offers(offers)
-    # the same three calls in the exchange form (k_pod_result_diff_xchg) on a second ctx with the same table: one rank,
+    # the same three calls in the exchange form on a second ctx with the same table: one rank,
     # one local buffer, a bound one-rank flag group; its region must equal the host call's rows
     import torch  # noqa: E402
     eg = rpk.Engine(1)
@@ -88,7 +88,7 @@ if not ONLY_MULTI:
     assert r1 == 0 and len(s1) == 0 and r2 == len(pend) and len(s2) == 0
     assert int(fl[16].item()) == 3 and int(fl[34].item()) == 3
     eg.close()
-    # the device form (k_pod_stale, k_pod_reselect_top5, the device-count k_pod_result_diff_xchg): one eager call that
+    # the device form (the same kernels, the row count never read on the host): one eager call that
     # reports every pending slot, then one replay of a captured steady call
     ed = rpk.Engine(1)
     ed.upload_offers(offers)
