@@ -26,11 +26,13 @@
  *   - "host" entry points take host pointers (pageable or pinned; pinned from rpk_host_alloc is faster);
  *     "_device" entry points take device pointers on the shard's GPU and enqueue on the given stream
  *     without synchronising it.
- *   - Ordering.  The calls on one shard share ctx-owned buffers in two scopes: the select scope (the offer table, the
- *     pod table and the select scratch) and the status scope (the sweep scratch).  A _device call issued on another
- *     stream than the last _device call of its scope first waits for that call, so any streams may be used.  A host
- *     call waits for the last _device call of its scopes before it touches anything, and returns after its own work is
- *     done; the caller needs no synchronise between the two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset,
+ *   - Ordering.  The calls on one shard are ordered in two scopes: the select scope (the offer table and the pod table,
+ *     which host and _device calls share, and the _device selects' scratch) and the status scope (the _device sweeps'
+ *     scratch).  Host calls have select and sweep scratch of their own ("Graph capture" below).  A _device call issued
+ *     on another stream than the last _device call of its scope first waits for that call, so any streams may be used.
+ *     A host call waits for the last _device call of its scopes before it touches anything, so host and _device calls
+ *     of one scope never overlap, and returns after its own work is done; the caller needs no synchronise between the
+ *     two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset,
  *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
  *     rpk_select_pending_changed, the _device call
  *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host),
@@ -41,6 +43,24 @@
  *     capture neither waits nor is waited for (keep each captured entry point on one stream), and the library does
  *     not see replays of a captured graph: a caller that replays a captured device step orders its host calls after
  *     the replay itself.
+ *   - Graph capture.  After one call of a given size a _device call only enqueues launches, so it can be captured in a
+ *     CUDA graph and replayed.  The graph keeps every ctx-owned device buffer the call handed its kernels
+ *     (rpk_test_capture_buffers lists them) and the values the call read at capture.  Host calls have scratch of their
+ *     own, and the _device calls of a shard share one select scratch and one sweep scratch that only _device calls size.
+ *     A capture of a _device call on shard s stays valid across:
+ *       - every host call, of any size, on any shard (rpk_select, rpk_select_slots, rpk_select_pending*, the host
+ *         sweeps, rpk_tick, rpk_status_reset, ...);
+ *       - the seeds and marks: rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_status_seed, rpk_status_seed_slots (a
+ *         replay reads the rows, flags and hashes as they are at replay time);
+ *       - _device calls on s that need no more scratch than the calls made on s before the capture.
+ *     It is invalidated by (capture again after them, after one call outside the capture):
+ *       - a _device call on s that needs more scratch: a select of more rows, or a sweep of more records or list
+ *         entries, than any before (the scratch grows and frees the buffers the graph points at);
+ *       - rpk_offers_upload and rpk_offers_refresh (new views and columns; G, the layout and the change window are
+ *         copied at capture);
+ *       - rpk_pods_reset, for the calls that read the pod table or the flags (rpk_select_slots_device*,
+ *         rpk_pods_pending_list_device, rpk_select_pending_changed_device_gather);
+ *       - rpk_peer_bind and rpk_peer_inline_wait, for the bound gathers (the group is copied at capture).
  */
 #ifndef RPK_H_
 #define RPK_H_
@@ -248,7 +268,7 @@ int rpk_select_device(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_
  * a peer-written vector.  All vectors must share the slice's 16-byte alignment (same offset from cudaMalloc'ed
  * bases); if none of them lives on GPU `shard`, or the alignments differ, every result is stored into all
  * vectors directly from the select epilogue instead (slower, same result).  After one call of a given size the
- * function only enqueues launches, so it can be captured in a CUDA graph. */
+ * function only enqueues launches, so it can be captured in a CUDA graph ("Graph capture" at the top). */
 int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb,
                              const int32_t* d_req_vcpu, const int32_t* d_req_ram_gb, const double* d_max_price,
                              const uint8_t* d_cloud, int n_out, int32_t* const* d_best_full, uint32_t row0,
@@ -268,7 +288,8 @@ int rpk_select_device_gather(rpk_ctx* ctx, int shard, uint32_t P, const int32_t*
  *     peer and on word 32).  P == 0 signals and writes nothing.
  *   - RPK_EINVAL, before anything is enqueued and without signalling: no top-5 vector on GPU `shard`, top-5 vectors of
  *     different 16-byte phase, a NULL vector pointer, n_out outside 1..8, or 5*P beyond uint32_t.
- *   - After one call of a given size the function only enqueues launches (CUDA-graph capturable). */
+ *   - After one call of a given size the function only enqueues launches (CUDA-graph capturable: "Graph capture" at the
+ *     top). */
 int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int32_t* d_req_mem_gb,
                                   const int32_t* d_req_vcpu, const int32_t* d_req_ram_gb, const double* d_max_price,
                                   const uint8_t* d_cloud, int n_out, int32_t* const* d_best_full,
@@ -288,10 +309,10 @@ int rpk_select_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t P, const int
  *   - No pod table or no offer table on GPU `shard`: RPK_ESTATE.  d_slots NULL with n_slots > 0: RPK_EINVAL.  Both
  *     before anything is enqueued.
  *   - Counts as one select in rpk_stats (offer_scores += n_slots * G).  One gather kernel runs ahead of the select.
- *   - After one call of a given size the call only enqueues launches, so it can be captured in a CUDA graph.  A replay
- *     reads the table as it is at replay time, so seeds between replays are picked up (the caller orders a seed after
- *     a replay still in flight; the library does not see replays).  rpk_pods_reset invalidates a captured graph: the
- *     graph keeps the old N and possibly buffers the reset freed. */
+ *   - After one call of a given size the call only enqueues launches, so it can be captured in a CUDA graph ("Graph
+ *     capture" at the top).  A replay reads the table as it is at replay time, so seeds between replays are picked up
+ *     (the caller orders a seed after a replay still in flight; the library does not see replays).  rpk_pods_reset
+ *     invalidates a captured graph: the graph keeps the old N and possibly buffers the reset freed. */
 int rpk_select_slots_device(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int32_t* d_best,
                             int32_t* d_top5, void* stream);
 int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,
@@ -306,8 +327,8 @@ int rpk_select_slots_device_gather_top5(rpk_ctx* ctx, int shard, uint32_t n_slot
  * Enqueued on `stream`, no synchronisation; select scope, device call (ordered like rpk_select_slots_device).  The
  * select kernels take no device-side row count: the caller reads *d_n (or knows it from its own mirror of the flags)
  * and passes it as n_slots, with the list, to rpk_select_slots_device[_gather[_top5]].  No pod table: RPK_ESTATE; NULL
- * output: RPK_EINVAL; both before anything is enqueued.  Graph-capturable after one call; a replay reads the flags as
- * they are at replay time. */
+ * output: RPK_EINVAL; both before anything is enqueued.  Graph-capturable after one call ("Graph capture" at the top); a
+ * replay reads the flags as they are at replay time. */
 int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out, uint32_t* d_n, void* stream);
 
 /* rpk_select_pending_changed for one-process-per-GPU callers: each rank reselects the pending slots of its own range and
@@ -361,7 +382,8 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
  *     with the same (n_ranks, my_rank, cap) on a pod table of the same N, the call only enqueues launches.  A replay reads
  *     the flags, the pod rows and the stored results as they are at replay time, so seeds and marks between replays are
  *     picked up.  The reselected rows go to scratch of this call's own (41 bytes per owned slot, allocated by its first
- *     call), so selects of any size on the ctx between replays leave a captured graph valid.  The offer-table generation
+ *     call), so selects of any size on the ctx between replays leave a captured graph valid ("Graph capture" at the
+ *     top).  The offer-table generation
  *     and change window are taken at capture: rpk_offers_upload, rpk_offers_refresh and rpk_pods_reset each invalidate a
  *     captured graph (re-capture after them), as does a call with another range, which is refused at call time but not
  *     at replay.
@@ -415,6 +437,14 @@ int rpk_peer_inline_wait(rpk_ctx* ctx, int shard, int on);
 /* Device pointer of GPU `shard`'s copy of the full assignment vector written by the last rpk_select or rpk_select_slots
  * (ctx-owned; every GPU of the ctx holds the whole vector after the call). */
 const int32_t* rpk_best_device_ptr(const rpk_ctx* ctx, int shard);
+
+/* Test hook: the ctx-owned device buffers a _device call on GPU `shard` passes to its kernels, as pointers (NULL: not
+ * allocated), in a fixed order: the device select lane (16), the device sweep scratch (5), the two offer views (7
+ * each), the distinct values (3), the raw offer columns (6) and the change window, the pod table and its flags (6), the
+ * compaction state (2), the stored pending results (10) and their reselect lane (16).  *n receives the count; the first
+ * min(cap, *n) go to ptrs.  A call that leaves every one of them in place leaves a captured graph valid ("Graph
+ * capture" at the top).  RPK_EINVAL for a NULL ctx or n, a bad shard, or cap > 0 with NULL ptrs. */
+int rpk_test_capture_buffers(const rpk_ctx* ctx, int shard, const void** ptrs, size_t cap, size_t* n);
 
 /* ---- status sweep diff ------------------------------------------------------------------------------ */
 
@@ -473,7 +503,8 @@ int rpk_status_diff_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots,
  * all be handed the same global list.  Enqueued on `stream`, no synchronisation, graph-capturable after one call
  * of the size.  d_records and d_hash_prev 16-byte aligned (else RPK_EINVAL); d_changed_idx capacity n_slots.  Order
  * is a precondition here (not checked): with a list that is not strictly ascending the changed list is unspecified,
- * but no memory outside d_hash_prev[0, N) and the outputs is touched. */
+ * but no memory outside d_hash_prev[0, N) and the outputs is touched.  "Graph capture" at the top says which calls keep
+ * a capture valid. */
 int rpk_status_diff_slots_device(rpk_ctx* ctx, int shard, uint32_t N, uint32_t idx_base, uint32_t n_slots,
                                  const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride,
                                  uint64_t* d_hash_prev, uint32_t* d_changed_idx, uint16_t* d_changed_code,
@@ -508,7 +539,7 @@ int rpk_status_diff_device_codes(rpk_ctx* ctx, int shard, uint32_t N, const uint
  * With flags bound (rpk_peer_bind) the CTA that finishes last signals the status epoch; rpk_peer_wait(what = 2) on
  * every rank makes all regions readable.  Every stride of rpk_status_diff (16..256), so a table that
  * Provider::WidenRecords has widened for a long status string keeps the exchange.  A rank with N = 0 still publishes
- * its zero count and signals.  Graph-capturable after one call of the size. */
+ * its zero count and signals.  Graph-capturable after one call of the size ("Graph capture" at the top). */
 size_t rpk_xchg_bytes(int n_ranks, uint32_t cap);
 int rpk_status_diff_device_gather(rpk_ctx* ctx, int shard, uint32_t N, const uint8_t* d_records, uint32_t stride,
                                   uint64_t* d_hash_prev, uint32_t idx_base, int n_ranks, uint32_t* const* d_xchg, uint32_t cap,

@@ -64,6 +64,7 @@ ABI = {
     "rpk_peer_wait": (_int, [_p, _int, C.c_uint, _p]),
     "rpk_peer_inline_wait": (_int, [_p, _int, _int]),
     "rpk_best_device_ptr": (_p, [_p, _int]),
+    "rpk_test_capture_buffers": (_int, [_p, _int, _pp, _size, C.POINTER(C.c_size_t)]),
     "rpk_status_diff": (_int, [_p, _u32, _p, _u32, _p, _p, _p]),
     "rpk_status_diff_codes": (_int, [_p, _u32, _p, _u32, _p, _p, _p, _p]),
     "rpk_status_seed": (_int, [_p, _u32, _p, _u32]),

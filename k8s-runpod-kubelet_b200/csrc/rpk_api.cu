@@ -461,28 +461,28 @@ bool enqueue_select_shard(rpk_ctx* ctx, int s, const HostSelect& sel, uint64_t* 
     return ok;
 }
 
-// Scratch of a sweep over N records (or list entries) on ds: the look-back state and tickets -- zero between calls by
-// construction, zeroed here when (re)allocated -- and the per-warp index stage, its code stage (`codes`) and the
-// per-unit counts.
-void reserve_sweep_scratch(DeviceState& ds, uint32_t N, bool codes) {
+// Scratch w of a sweep over N records (or list entries) on a GPU of sm_count SMs: the look-back state and tickets --
+// zero between calls by construction, zeroed here when (re)allocated -- and the per-warp index stage, its code stage
+// (`codes`) and the per-unit counts.
+void reserve_sweep_scratch(DeviceState::SweepScratch& w, int sm_count, uint32_t N, bool codes) {
     const uint32_t cap = N ? N : 1;
-    const size_t need = status_state_words(ds.sm_count);
-    if (need > ds.s_tile_state.cap || !ds.s_misc.p || ds.status_dirty) {
-        ds.s_tile_state.reserve(need);
-        ds.s_misc.reserve(64);
-        RPK_CUDA(cudaMemset(ds.s_tile_state.p, 0, ds.s_tile_state.cap * sizeof(unsigned long long)));
-        RPK_CUDA(cudaMemset(ds.s_misc.p, 0, ds.s_misc.cap * sizeof(uint32_t)));
+    const size_t need = status_state_words(sm_count);
+    if (need > w.tile_state.cap || !w.misc.p || w.dirty) {
+        w.tile_state.reserve(need);
+        w.misc.reserve(64);
+        RPK_CUDA(cudaMemset(w.tile_state.p, 0, w.tile_state.cap * sizeof(unsigned long long)));
+        RPK_CUDA(cudaMemset(w.misc.p, 0, w.misc.cap * sizeof(uint32_t)));
         RPK_CUDA(cudaDeviceSynchronize());
-        ds.status_dirty = false;
+        w.dirty = false;
     }
-    ds.s_stage_idx.reserve(cap + 64); ds.s_unit_cnt.reserve(cap / 32 + 2);
-    if (codes) ds.s_stage_code.reserve(cap + 64);
+    w.stage_idx.reserve(cap + 64); w.unit_cnt.reserve(cap / 32 + 2);
+    if (codes) w.stage_code.reserve(cap + 64);
 }
 
 // the StatusArgs fields of the scratch reserve_sweep_scratch sized
-void sweep_scratch_args(const DeviceState& ds, bool codes, StatusArgs& a) {
-    a.tile_state = ds.s_tile_state.p; a.tile_counter = ds.s_misc.p;
-    a.stage_idx = ds.s_stage_idx.p; a.stage_code = codes ? ds.s_stage_code.p : nullptr; a.unit_cnt = ds.s_unit_cnt.p;
+void sweep_scratch_args(const DeviceState::SweepScratch& w, bool codes, StatusArgs& a) {
+    a.tile_state = w.tile_state.p; a.tile_counter = w.misc.p;
+    a.stage_idx = w.stage_idx.p; a.stage_code = codes ? w.stage_code.p : nullptr; a.unit_cnt = w.unit_cnt.p;
 }
 
 struct StatusHostArgs {
@@ -517,7 +517,7 @@ void reserve_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h) {
     ds.s_records.reserve((size_t)cap * h.stride);
     if (h.slots) ds.s_seed_slots.reserve(cap);
     if (h.hashes_out) ds.s_hash_out.reserve(cap);
-    reserve_sweep_scratch(ds, Ns, h.changed_code != nullptr);
+    reserve_sweep_scratch(ds.sweep, ds.sm_count, Ns, h.changed_code != nullptr);
     ds.h_changed.reserve(h.report ? (size_t)cap * (h.changed_code ? 6 : 4) + 64 : 64);
 }
 
@@ -543,11 +543,11 @@ void enqueue_status_shard(rpk_ctx* ctx, int s, const StatusHostArgs& h, cudaStre
     a.changed_idx = h.report ? m_idx : nullptr; a.n_changed = h.report ? m_count : nullptr;
     a.changed_code = h.report && h.changed_code ? m_code : nullptr;
     a.idx_base = lo;
-    sweep_scratch_args(ds, h.changed_code != nullptr, a);
+    sweep_scratch_args(ds.sweep, h.changed_code != nullptr, a);
     if (h.slots) { a.slots = ds.s_seed_slots.p; a.col_n = sp.hi - sp.lo; }
-    ds.status_dirty = true;
+    ds.sweep.dirty = true;
     if (Ns) *launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
-    ds.status_dirty = false;
+    ds.sweep.dirty = false;
     RPK_CUDA(cudaEventRecord(ds.ev[2], st));
     if (h.hashes_out && Ns) RPK_CUDA(cudaMemcpyAsync(h.hashes_out + lo, ds.s_hash_out.p, (size_t)Ns * 8, cudaMemcpyDeviceToHost, st));
     RPK_CUDA(cudaEventRecord(ds.ev[3], st));
@@ -682,7 +682,7 @@ int select_device(rpk_ctx* ctx, const char* who, int shard, uint32_t P, const Ro
                 return fail(ctx, RPK_EINVAL, w + (list ? ": " : ": req_mem_gb and ") + "1..8 output vectors are required");
             for (int o = 0; o < n_out; ++o) if (!d_best_full[o]) return fail(ctx, RPK_EINVAL, w + ": NULL output vector");
             if (int rc = check_select_ready(ctx, who, list, shard)) return rc;
-            reserve_lane(ds.lane[0], P, src, false);
+            reserve_lane(ds.dev_lane, P, src, false);
             return RPK_OK;
         },
         [&](DeviceState& ds, cudaStream_t st) {
@@ -690,7 +690,7 @@ int select_device(rpk_ctx* ctx, const char* who, int shard, uint32_t P, const Ro
                 if (signal) ctx->launches += (uint64_t)launch_peer_signal(peers, 0, peers.inline_wait != 0, st);
                 return;
             }
-            DeviceState::Lane& ln = ds.lane[0];  // the gather writes lane 0's columns: after the last select
+            DeviceState::Lane& ln = ds.dev_lane;  // the gather writes the lane's columns: after the last device select
             SelectArgs a{};
             ctx->launches += (uint64_t)pod_columns(ds, ln, src, 0, P, a, st);
             a.P = P;
@@ -1544,6 +1544,32 @@ const int32_t* rpk_best_device_ptr(const rpk_ctx* ctx, int shard) {
     return ctx->devs[(size_t)shard].best_full.p;
 }
 
+/* test hook: the ctx-owned device buffers a _device call on `shard` hands its kernels, in a fixed order */
+int rpk_test_capture_buffers(const rpk_ctx* ctx, int shard, const void** ptrs, size_t cap, size_t* n) {
+    if (!ctx || bad_shard(ctx, shard) || !n || (cap > 0 && !ptrs)) return RPK_EINVAL;
+    const DeviceState& ds = ctx->devs[(size_t)shard];
+    std::vector<const void*> v;
+    const auto lane = [&v](const DeviceState::Lane& ln) {
+        v.insert(v.end(), {ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p, ln.p_slots.p, ln.top5.p,
+                           ln.rw.p, ln.order.p, ln.pos.p, ln.ctrs.p, ln.key.p, ln.ord_rw.p, ln.hist.p, ln.k0_base.p, ln.hdr.p});
+    };
+    lane(ds.dev_lane);
+    const DeviceState::SweepScratch& w = ds.dev_sweep;
+    v.insert(v.end(), {w.tile_state.p, w.misc.p, w.stage_idx.p, w.stage_code.p, w.unit_cnt.p});
+    for (int c = 0; c < 2; ++c)
+        v.insert(v.end(), {ds.v_packed[c].p, ds.v_bitmap[c].p, ds.v_bitmapT[c].p, ds.v_bitmapM[c].p, ds.v_wide[c].p, ds.v_price[c].p,
+                           ds.v_perm[c].p});
+    v.insert(v.end(), {ds.distinct[0].p, ds.distinct[1].p, ds.distinct[2].p, ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p,
+                       ds.raw_cp.p, ds.raw_flags.p, ds.win.p});
+    v.insert(v.end(), {ds.pt_mem.p, ds.pt_vcpu.p, ds.pt_ram.p, ds.pt_max_price.p, ds.pt_cloud.p, ds.pt_pending.p, ds.pt_state.p, ds.pt_ticket.p});
+    v.insert(v.end(), {ds.r_mem.p, ds.r_vcpu.p, ds.r_ram.p, ds.r_max_price.p, ds.r_cloud.p, ds.r_gen.p, ds.r_top5.p, ds.r_list.p,
+                       ds.r_mask.p, ds.r_dn.p});
+    lane(ds.r_lane);
+    *n = v.size();
+    for (size_t i = 0; i < v.size() && i < cap; ++i) ptrs[i] = v[i];
+    return RPK_OK;
+}
+
 // ---- status --------------------------------------------------------------------------------------------
 
 static int check_stride(rpk_ctx* ctx, uint32_t stride, const char* who) {
@@ -1694,12 +1720,12 @@ int status_device(rpk_ctx* ctx, const char* who, int shard, const StatusDeviceAr
     if ((uint64_t)d.idx_base + col_n > (1ull << 32)) return fail(ctx, RPK_EINVAL, w + ": idx_base + N exceeds the slot range");
     const bool codes = d.changed_code || d.n_out > 0;
     return device_call(ctx, shard, stream, &DeviceState::status_scope,
-        [&](DeviceState& ds) { reserve_sweep_scratch(ds, d.N, codes); return RPK_OK; },
+        [&](DeviceState& ds) { reserve_sweep_scratch(ds.dev_sweep, ds.sm_count, d.N, codes); return RPK_OK; },
         [&](DeviceState& ds, cudaStream_t st) {
             StatusArgs a{};
             a.records = d.records; a.stride = d.stride; a.N = d.N; a.hash_prev = d.hash_prev; a.hash_out = nullptr;
             a.changed_idx = d.changed_idx; a.changed_code = d.changed_code; a.n_changed = d.n_changed; a.idx_base = d.idx_base;
-            sweep_scratch_args(ds, codes, a);
+            sweep_scratch_args(ds.dev_sweep, codes, a);
             a.n_out = d.n_out;
             a.slots = d.N > 0 ? d.slots : nullptr; a.col_n = col_n;
             for (int o = 0; o < d.n_out; ++o) {  // rank o's buffer: [counts : 8 words][n_out index regions of cap][n_out code regions of cap u16]
@@ -1710,9 +1736,9 @@ int status_device(rpk_ctx* ctx, const char* who, int shard, const StatusDeviceAr
             }
             if (d.n_out > 0) a.peers = ctx->bind[(size_t)shard];
             a.peers.my_rank = d.my_rank;  // the sweep fills and signals under the rank its call names
-            ds.status_dirty = true;
+            ds.dev_sweep.dirty = true;
             ctx->launches += (uint64_t)launch_status_diff(a, ds.sm_count, st);
-            ds.status_dirty = false;
+            ds.dev_sweep.dirty = false;
             ctx->stats.status_calls += 1; ctx->stats.status_records += d.N;
         });
 }

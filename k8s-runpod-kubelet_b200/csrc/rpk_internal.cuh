@@ -406,8 +406,9 @@ struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches i
     }
 };
 
-// Buffers that a shard's host and device entry points share, and the last device call that used them: the ordering rule
-// of rpk.h.  Inside a stream capture a device call neither waits nor records (an event recorded outside a capture cannot
+// One ordering scope of a shard (rpk.h, "Ordering"): the buffers its device entry points share -- the device select
+// scratch with the offer and pod tables, which host calls also write, or the device sweep scratch -- and the last device
+// call that used them.  Host calls wait for that call before they start.  Inside a stream capture a device call neither waits nor records (an event recorded outside a capture cannot
 // be waited on inside it), so a captured step keeps each entry point on one stream, as bench.py does.
 struct ScratchScope {
     cudaStream_t last = nullptr;  // the stream of the last device call outside a capture
@@ -450,9 +451,9 @@ struct DeviceState {
     PackLayout pk = {};
     int force_kind = 0;  // RPK_FORCE_KERNEL (tests): 0 auto, 1 generic, 2 packed+select, 3 packed+pos, 4 bit-sliced,
                          // 5 / 6 every batch of a non-empty table through the persistent / price-staged persistent kernel
-    // select scratch.  The host entry point pipelines row sub-batches over four lanes (stream + staging +
+    // select scratch.  The host entry points pipeline row sub-batches over four lanes (stream + staging +
     // scratch each) so that the H2D of one sub-batch, the kernels of another and the D2H of a third overlap;
-    // the device entry points use lane 0's scratch on the caller's stream.
+    // the device entry points use dev_lane's scratch on the caller's stream.
     struct Lane {
         cudaStream_t stream = nullptr;
         cudaEvent_t done = nullptr;
@@ -466,17 +467,27 @@ struct DeviceState {
     };
     static constexpr int kLanes = 4;  // one per sub-batch of a 1M-row call: no upload ever waits for a kernel to free its buffers
     Lane lane[kLanes];
+    // the rpk_select*_device* calls' scratch (no stream of its own): only device calls size it, so no host call of any
+    // size frees what a captured device call points at (rpk.h, "Graph capture")
+    Lane dev_lane;
     DevBuf<int32_t> best_full;
     // small-batch (latency) path: one pinned staging block in, one out
     PinnedBuf h_small; DevBuf<unsigned char> d_small_in; DevBuf<int32_t> d_small_out;
     // status
-    DevBuf<uint8_t> s_records; DevBuf<uint64_t> s_hash_prev, s_hash_out; DevBuf<uint32_t> s_misc;
-    DevBuf<unsigned long long> s_tile_state; DevBuf<uint32_t> s_stage_idx; DevBuf<uint16_t> s_stage_code; DevBuf<uint32_t> s_unit_cnt;
+    DevBuf<uint8_t> s_records; DevBuf<uint64_t> s_hash_prev, s_hash_out;
+    // a sweep's scratch: the look-back state and the ticket words (zero between calls by construction), the per-warp index
+    // and code stages and the per-unit counts.  The host sweeps and rpk_tick use `sweep`; the rpk_status_diff*_device*
+    // calls use `dev_sweep`, which only they size, as dev_lane above
+    struct SweepScratch {
+        DevBuf<unsigned long long> tile_state; DevBuf<uint32_t> misc;
+        DevBuf<uint32_t> stage_idx; DevBuf<uint16_t> stage_code; DevBuf<uint32_t> unit_cnt;
+        bool dirty = false;  // a launch failed midway: re-zero the look-back state before the next one
+    };
+    SweepScratch sweep, dev_sweep;
     DevBuf<uint32_t> s_seed_slots; DevBuf<uint8_t> s_seed_recs;  // slot lists of rpk_status_seed_slots and rpk_status_diff_slots
     PinnedBuf h_changed;                   // the host sweep's changed list: count, indices, codes
     cudaStream_t status_stream = nullptr;  // rpk_tick: the sweep next to the selection
-    ScratchScope sel_scope, status_scope;  // the offer views, the pod table and lane 0; the sweep scratch
-    bool status_dirty = false;             // a status launch failed midway: re-zero the look-back state before the next one
+    ScratchScope sel_scope, status_scope;  // the offer views, the pod table and dev_lane; dev_sweep
     uint32_t statusN = 0; bool status_sized = false;
     // pod-requirement table (rpk_pods_reset): the five columns of podsN slots, the whole table on every GPU of the ctx
     DevBuf<int32_t> pt_mem, pt_vcpu, pt_ram; DevBuf<double> pt_max_price; DevBuf<uint8_t> pt_cloud;

@@ -399,6 +399,15 @@ class Engine:
     def best_device_ptr(self, shard: int = 0) -> int:
         return int(self._lib.rpk_best_device_ptr(self._ctx, shard) or 0)
 
+    def capture_buffers(self, shard: int = 0) -> list:
+        """The ctx-owned device buffers a device call on ``shard`` hands its kernels, as addresses (0: not allocated), in
+        rpk_test_capture_buffers' order."""
+        n = C.c_size_t(0)
+        self._check(self._lib.rpk_test_capture_buffers(self._ctx, shard, None, 0, C.byref(n)))
+        ptrs = (C.c_void_p * max(n.value, 1))()
+        self._check(self._lib.rpk_test_capture_buffers(self._ctx, shard, ptrs, n.value, C.byref(n)))
+        return [int(p or 0) for p in ptrs[:n.value]]
+
     # -- status sweep --------------------------------------------------------------------------------
     def status_reset(self, N: int):
         self._check(self._lib.rpk_status_reset(self._ctx, N))
