@@ -190,6 +190,17 @@ func (e *Engine) PodsReset(n int) error {
 	return nil
 }
 
+// PodsGrow grows the device pod table to n slots, keeping every row, pending flag and stored result; the new slots get
+// the columns of a pod with no annotations and are not pending (rpk_pods_grow).
+func (e *Engine) PodsGrow(n int) error {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if rc := C.rpk_pods_grow(e.ctx, C.uint32_t(n)); rc != C.RPK_OK {
+		return lastError(e.ctx, rc)
+	}
+	return nil
+}
+
 // PodsSeedSlots writes row slots[i] of the pod table from row i of p (slots strictly ascending; nil optional columns
 // take Select's defaults).  processPendingPods (kubelet.go:747-814) seeds only the rows whose columns changed.
 func (e *Engine) PodsSeedSlots(slots []uint32, p *Pods) error {
@@ -364,6 +375,16 @@ func (e *Engine) StatusSeed(records []byte, stride int) error {
 	defer e.mu.Unlock()
 	rc := C.rpk_status_seed(e.ctx, C.uint32_t(len(records)/stride), u8p(records), C.uint32_t(stride))
 	if rc != C.RPK_OK {
+		return lastError(e.ctx, rc)
+	}
+	return nil
+}
+
+// StatusGrow grows the tracked table to n slots, keeping every hash; the new slots are never seen (rpk_status_grow).
+func (e *Engine) StatusGrow(n int) error {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	if rc := C.rpk_status_grow(e.ctx, C.uint32_t(n)); rc != C.RPK_OK {
 		return lastError(e.ctx, rc)
 	}
 	return nil

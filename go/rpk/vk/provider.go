@@ -15,6 +15,7 @@ package vk
 import (
 	"context"
 	"fmt"
+	"math"
 	"sort"
 	"strings"
 	"sync"
@@ -68,7 +69,7 @@ type Provider struct {
 	api     RunPodAPI
 	engine  *rpk.Engine
 	offers  *rpk.Offers
-	maxPods int
+	maxPods int // slot capacity, doubled by growSlots when every slot is taken (podsMutex)
 
 	podsMutex sync.RWMutex // kubelet.go:38-45
 	pods      map[string]*v1.Pod
@@ -128,13 +129,19 @@ func key(pod *v1.Pod) string { return fmt.Sprintf("%s-%s", pod.Namespace, pod.Na
 // CreatePod -- kubelet.go:384-418.
 func (p *Provider) CreatePod(ctx context.Context, pod *v1.Pod) error {
 	k := key(pod)
-	p.podsMutex.Lock()
-	info, ok := p.podStatus[k]
-	if !ok {
-		if len(p.freeSlots) == 0 {
-			p.podsMutex.Unlock()
-			return fmt.Errorf("provider pod capacity exceeded")
+	var info *InstanceInfo
+	var ok bool
+	for {
+		p.podsMutex.Lock()
+		if info, ok = p.podStatus[k]; ok || len(p.freeSlots) > 0 {
+			break
 		}
+		p.podsMutex.Unlock()
+		if err := p.growSlots(); err != nil { // podsMutex released: it is never held with the engine's lock
+			return err
+		}
+	}
+	if !ok {
 		info = &InstanceInfo{slot: p.freeSlots[len(p.freeSlots)-1]}
 		p.freeSlots = p.freeSlots[:len(p.freeSlots)-1]
 	}
@@ -149,6 +156,49 @@ func (p *Provider) CreatePod(ctx context.Context, pod *v1.Pod) error {
 	// previous state of THIS slot only: a whole-table seed would adopt other pods' pending changes as "previous"
 	_ = p.engine.StatusSeedSlots([]uint32{info.slot}, one, stride)
 	p.deployBatch([]string{k}) // errors are logged and swallowed: kubelet.go:406-415
+	return nil
+}
+
+// growSlots doubles the slot capacity when no slot is free.  Both device tables grow in place, keeping every row,
+// pending flag, stored result and hash (PodsGrow, StatusGrow); then the seed mirror follows under seedMutex and the
+// pod-side mirrors under podsMutex, and the new slots are freed last, so no slot at or above the old capacity is handed
+// out before both tables and every mirror cover it.  sweepMutex is taken first, as a sweep takes it.  Slots never move
+// and the slices only grow.  New status slots need no seed: CreatePod seeds the slot it takes.
+func (p *Provider) growSlots() error {
+	p.sweepMutex.Lock()
+	defer p.sweepMutex.Unlock()
+	p.podsMutex.RLock()
+	n0, free := p.maxPods, len(p.freeSlots)
+	p.podsMutex.RUnlock()
+	if free > 0 {
+		return nil // another goroutine grew the table meanwhile
+	}
+	n := 2 * n0
+	if n < n0+1 {
+		n = n0 + 1
+	}
+	if n > math.MaxUint32 {
+		return fmt.Errorf("provider pod capacity exceeded")
+	}
+	if err := p.engine.PodsGrow(n); err != nil {
+		return err
+	}
+	if err := p.engine.StatusGrow(n); err != nil {
+		return err
+	}
+	p.seedMutex.Lock()
+	for s := n0; s < n; s++ {
+		p.seededMem, p.seededCld = append(p.seededMem, 16), append(p.seededCld, rpk.CloudSecure)
+	}
+	p.seedMutex.Unlock()
+	p.podsMutex.Lock()
+	defer p.podsMutex.Unlock()
+	p.records = append(p.records, make([]byte, (n-n0)*stride)...)
+	p.slotKey = append(p.slotKey, make([]string, n-n0)...)
+	for s := n; s > n0; s-- {
+		p.freeSlots = append(p.freeSlots, uint32(s-1))
+	}
+	p.maxPods = n
 	return nil
 }
 

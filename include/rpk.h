@@ -32,14 +32,14 @@
  *     on another stream than the last _device call of its scope first waits for that call, so any streams may be used.
  *     A host call waits for the last _device call of its scopes before it touches anything, so host and _device calls
  *     of one scope never overlap, and returns after its own work is done; the caller needs no synchronise between the
- *     two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset,
+ *     two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset, rpk_pods_grow,
  *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
  *     rpk_select_pending_changed, the _device call
  *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host),
  *     rpk_select_pending_changed_device_gather, and rpk_tick
  *     with P > 0.  Status scope: rpk_status_diff,
- *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset and
- *     rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
+ *     rpk_status_diff_codes, rpk_status_seed, rpk_status_diff_slots and rpk_tick.  rpk_status_reset, rpk_status_grow
+ *     and rpk_status_seed_slots touch only buffers no _device call uses and do not wait.  A _device call inside a stream
  *     capture neither waits nor is waited for (keep each captured entry point on one stream), and the library does
  *     not see replays of a captured graph: a caller that replays a captured device step orders its host calls after
  *     the replay itself.
@@ -49,7 +49,7 @@
  *     own, and the _device calls of a shard share one select scratch and one sweep scratch that only _device calls size.
  *     A capture of a _device call on shard s stays valid across:
  *       - every host call, of any size, on any shard (rpk_select, rpk_select_slots, rpk_select_pending*, the host
- *         sweeps, rpk_tick, rpk_status_reset, ...);
+ *         sweeps, rpk_tick, rpk_status_reset, rpk_status_grow, ...);
  *       - the seeds and marks: rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_status_seed, rpk_status_seed_slots (a
  *         replay reads the rows, flags and hashes as they are at replay time);
  *       - _device calls on s that need no more scratch than the calls made on s before the capture.
@@ -58,8 +58,9 @@
  *         entries, than any before (the scratch grows and frees the buffers the graph points at);
  *       - rpk_offers_upload and rpk_offers_refresh (new views and columns; G, the layout and the change window are
  *         copied at capture);
- *       - rpk_pods_reset, for the calls that read the pod table or the flags (rpk_select_slots_device*,
- *         rpk_pods_pending_list_device, rpk_select_pending_changed_device_gather);
+ *       - rpk_pods_reset and rpk_pods_grow, for the calls that read the pod table or the flags
+ *         (rpk_select_slots_device*, rpk_pods_pending_list_device, rpk_select_pending_changed_device_gather): N is an
+ *         argument of their kernels, so a grow invalidates them even when no buffer moves;
  *       - rpk_peer_bind and rpk_peer_inline_wait, for the bound gathers (the group is copied at capture).
  */
 #ifndef RPK_H_
@@ -185,6 +186,23 @@ int rpk_select(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_
  * from, an offer-table generation and the five list entries), about 36 bytes of device scratch and 28 bytes of pinned
  * host memory for the rows it returns, all allocated by its first call, so callers that never use it pay nothing. */
 int rpk_pods_reset(rpk_ctx* ctx, uint32_t N);
+/* Grow the pod table from its N0 slots to N >= N0 on every GPU of the ctx, keeping what it holds, so a caller whose
+ * pods outgrow the table need not reset it (and reselect and report every pending slot on the next tick).
+ *   - Slots [0, N0) keep their rows and pending flags bit for bit; slots [N0, N) get what rpk_pods_reset(N) gives them
+ *     (the columns of a pod with no annotations, not pending).
+ *   - The results rpk_select_pending_changed stored are kept.  On a multi-GPU ctx each GPU's owned range moves with N,
+ *     and each stored result moves to its slot's new owner (a peer copy).  A ctx grown from N0 to N therefore returns from
+ *     every later call what a ctx reset at N with the same history returns: growing reselects and reports nothing.
+ *   - Results made by rpk_select_pending_changed_gather or its device form for another range than
+ *     rpk_select_pending_changed's (n_ranks above the ctx's GPUs) are cleared, as rpk_pods_reset clears them: the other
+ *     ranks' results live in other processes.  Each rank's next call binds its new range and reports every pending slot
+ *     of it once.  With n_ranks = the ctx's GPUs (a one-GPU ctx with n_ranks = 1) the results are kept.
+ *   - N < N0: RPK_EINVAL; no pod table: RPK_ESTATE; N == N0: RPK_OK and nothing is touched.  A failed allocation:
+ *     RPK_ENOMEM and the ctx as it was (every GPU's buffers are allocated before anything is copied).
+ *   - Select scope, host call: waits for the scope's last _device call first.  Invalidates captured graphs as
+ *     rpk_pods_reset does ("Graph capture" at the top).  A grow within the 25 % of spare capacity the table keeps
+ *     allocates nothing. */
+int rpk_pods_grow(rpk_ctx* ctx, uint32_t N);
 /* Row slots[i] := element i of each column.  Columns may be NULL exactly where rpk_select's may, with the same defaults
  * (req_mem_gb is required).  slots must be strictly ascending and < N of the pod table (else RPK_EINVAL, nothing
  * written; no pod table: RPK_ESTATE).  Rows not listed are not touched.  Every GPU of the ctx gets the rows.
@@ -239,7 +257,8 @@ int rpk_select_pending(rpk_ctx* ctx, uint32_t cap, uint32_t* slots_out, uint32_t
  *     slot afterwards.
  *   - Stored results outlive the pending flag: a slot that leaves the set and comes back with the same columns and offer
  *     table is not reported again, and a slot reused by another pod needs nothing special (the result depends on the
- *     columns only).  rpk_pods_reset clears them all; no other call reads or writes them.
+ *     columns only).  rpk_pods_reset clears them all and rpk_pods_grow moves them with their slots; no other call reads
+ *     or writes them.
  *   - *n_pending, *n_reselected and *n_changed are always required; with cap > 0 so are slots_out, best and top5
  *     (capacities cap, cap and 5*cap); else RPK_EINVAL.  No pod table or no offer table: RPK_ESTATE.  Both before
  *     anything is enqueued.
@@ -353,8 +372,8 @@ int rpk_pods_pending_list_device(rpk_ctx* ctx, int shard, uint32_t* d_slots_out,
  *   - RPK_EINVAL, before anything is enqueued and without signalling: n_ranks outside 1..8, my_rank outside [0, n_ranks),
  *     a NULL or misaligned buffer, a NULL count pointer, or cap < hi - lo (every rank must hold its worst case, so no
  *     refusal can come after the stale step while peers wait).  RPK_ESTATE, the same way: no pod table or no offer table
- *     on GPU `shard`, or stored results made for another range since the last rpk_pods_reset (another my_rank or
- *     n_ranks, or rpk_select_pending_changed on the same ctx with another range).
+ *     on GPU `shard`, or stored results made for another range since the last rpk_pods_reset or rpk_pods_grow (another
+ *     my_rank or n_ranks, or rpk_select_pending_changed on the same ctx with another range).
  *   - Ordering: select scope.  The call waits on the host for the scope's last device call, synchronises `stream` once
  *     after the stale step (the select needs the row count on the host), and returns with the gather, select, diff,
  *     push and signal enqueued on `stream`.  NOT graph-capturable.  A rank's first call after rpk_pods_reset (and a call
@@ -511,6 +530,12 @@ int rpk_status_diff_slots_device(rpk_ctx* ctx, int shard, uint32_t N, uint32_t i
                                  uint32_t* d_n_changed, void* stream);
 /* Forget all previous hashes and (re)size the table to N slots: every slot reports changed next time. */
 int rpk_status_reset(rpk_ctx* ctx, uint32_t N);
+/* Grow the tracked table from its N0 slots to N >= N0, keeping every hash: slots [0, N0) report only real changes on the
+ * next sweep, slots [N0, N) are never seen (hash 0), as after rpk_status_reset(N).  On a multi-GPU ctx the hashes move
+ * with the shard boundaries.  The whole-table host sweeps and rpk_tick then take N.  N < N0: RPK_EINVAL; no tracked
+ * table: RPK_ESTATE; N == N0: RPK_OK, nothing touched; a failed allocation: RPK_ENOMEM, the table as it was.  Like
+ * rpk_status_reset it touches no buffer a _device call uses and does not wait. */
+int rpk_status_grow(rpk_ctx* ctx, uint32_t N);
 
 /* One tick: rpk_select (P rows; P = 0 skips it) and rpk_status_diff_codes (N slots) enqueued together -- the two are
  * independent (processPendingPods kubelet.go:747-814, updateAllPodStatuses :816-974), so the sweep's upload follows the

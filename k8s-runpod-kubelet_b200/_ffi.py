@@ -40,6 +40,7 @@ ABI = {
     "rpk_offers_refresh": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_select": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p, _p]),
     "rpk_pods_reset": (_int, [_p, _u32]),
+    "rpk_pods_grow": (_int, [_p, _u32]),
     "rpk_pods_seed_slots": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
     "rpk_select_slots": (_int, [_p, _u32, _p, _p, _p]),
     "rpk_pods_mark_pending": (_int, [_p, _u32, _p, _p]),
@@ -72,6 +73,7 @@ ABI = {
     "rpk_status_diff_slots": (_int, [_p, _u32, _p, _p, _u32, _p, _p, _p]),
     "rpk_status_diff_slots_device": (_int, [_p, _int, _u32, _u32, _u32, _p, _p, _u32, _p, _p, _p, _p, _p]),
     "rpk_status_reset": (_int, [_p, _u32]),
+    "rpk_status_grow": (_int, [_p, _u32]),
     "rpk_tick": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p, _p, _u32, _p, _u32, _p, _p, _p]),
     "rpk_status_diff_device": (_int, [_p, _int, _u32, _p, _u32, _p, _p, _p, _p]),
     "rpk_status_diff_device_codes": (_int, [_p, _int, _u32, _p, _u32, _p, _p, _p, _p, _p]),

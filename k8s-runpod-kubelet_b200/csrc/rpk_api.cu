@@ -1172,8 +1172,9 @@ void result_range(uint32_t N, int n, int s, uint32_t* lo, uint32_t* hi) {
 
 // The stored results of ds's owned slots [lo, hi), allocated on the first call after a reset with every generation 0
 // (nothing reported), and the scratch and mapped output of a call that reselects all of them.  The owned range is fixed
-// until the next reset (check_results_range), so no later call grows r_lane.  The caller has waited.
-void reserve_results(DeviceState& ds, uint32_t lo, uint32_t hi) {
+// until the next reset (check_results_range) or grow, so no other call grows r_lane.  [lo, hi) is range my_rank of
+// n_ranks (result_range).  The caller has waited.
+void reserve_results(DeviceState& ds, uint32_t lo, uint32_t hi, int n_ranks, int my_rank) {
     if (ds.res_ready) return;
     const size_t n = ((size_t)(hi - lo) + 15) / 16 * 16 + 16;  // whole units: k_pod_stale loads 16 slots at a time
     ds.r_mem.reserve(n); ds.r_vcpu.reserve(n); ds.r_ram.reserve(n); ds.r_max_price.reserve(n); ds.r_cloud.reserve(n);
@@ -1183,7 +1184,7 @@ void reserve_results(DeviceState& ds, uint32_t lo, uint32_t hi) {
     RPK_CUDA(cudaMemset(ds.r_gen.p, 0, ds.r_gen.cap * sizeof(uint32_t)));
     RPK_CUDA(cudaDeviceSynchronize());
     ds.res_ready = true;
-    ds.res_bound = true; ds.res_lo = lo; ds.res_hi = hi;
+    ds.res_bound = true; ds.res_lo = lo; ds.res_hi = hi; ds.res_ranks = n_ranks; ds.res_rank = my_rank;
 }
 
 // RPK_ESTATE when ds's stored results were made for another owned range than [lo, hi) since the last rpk_pods_reset:
@@ -1278,7 +1279,7 @@ int rpk_select_pending_changed(rpk_ctx* ctx, uint32_t cap, uint32_t* n_pending, 
             uint32_t lo, hi; result_range(N, n, s, &lo, &hi);
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();
-            reserve_results(ds, lo, hi);
+            reserve_results(ds, lo, hi, n, s);
             reserve_compaction_state(ds);
             launches[(size_t)s] += (uint64_t)enqueue_stale(ctx, ds, lo, hi, ds.stream);
             copy_stale_counts(ds, ds.stream);
@@ -1399,7 +1400,7 @@ int rpk_select_pending_changed_gather(rpk_ctx* ctx, int shard, int n_ranks, int 
     const uint32_t gen = ctx->offer_gen;
     return device_call(ctx, shard, stream, nullptr, [&](DeviceState&, cudaStream_t st) {
         ds.sel_scope.host_wait();
-        reserve_results(ds, lo, hi);
+        reserve_results(ds, lo, hi, n_ranks, my_rank);
         reserve_compaction_state(ds);
         uint64_t launches = (uint64_t)enqueue_stale(ctx, ds, lo, hi, st);
         copy_stale_counts(ds, st);
@@ -1432,7 +1433,7 @@ int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_rank
     DeviceState& ds = ctx->devs[(size_t)shard];
     const uint32_t gen = ctx->offer_gen;
     const auto prep = [&](DeviceState&) {
-        reserve_results(ds, lo, hi);
+        reserve_results(ds, lo, hi, n_ranks, my_rank);
         reserve_compaction_state(ds);
         return RPK_OK;
     };
@@ -1444,6 +1445,138 @@ int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_rank
         ds.res_ready = true;
         ctx->launches += launches;
     });
+}
+
+// ---- growing the tables ---------------------------------------------------------------------------------------
+
+namespace {
+struct SlotRange { uint32_t lo, hi; };
+
+// A column sharded by slot range (`bytes` per slot) moves from the old ranges `was` to the new ones `now`: every slot
+// of was[s] is copied from src[s] into dst[d] of the shard d whose new range holds it, on d's stream (a peer copy
+// between GPUs).  A shard whose column is the one it had (same buffer, same first slot) keeps its slots in place; its
+// new range then holds all of them, as a range with the same first slot only grows.
+void move_slots(rpk_ctx* ctx, const std::vector<SlotRange>& was, const std::vector<SlotRange>& now,
+                const std::vector<const void*>& src, const std::vector<void*>& dst, size_t bytes) {
+    const size_t n = ctx->devs.size();
+    for (size_t d = 0; d < n; ++d) {
+        DeviceState& dd = ctx->devs[d];
+        RPK_CUDA(cudaSetDevice(dd.dev));
+        for (size_t s = 0; s < n; ++s) {
+            const uint32_t lo = std::max(was[s].lo, now[d].lo), hi = std::min(was[s].hi, now[d].hi);
+            if (lo >= hi || src[s] == dst[d]) continue;
+            RPK_CUDA(cudaMemcpyPeerAsync(static_cast<char*>(dst[d]) + (size_t)(lo - now[d].lo) * bytes, dd.dev,
+                                         static_cast<const char*>(src[s]) + (size_t)(lo - was[s].lo) * bytes, ctx->devs[s].dev,
+                                         (size_t)(hi - lo) * bytes, dd.stream));
+        }
+    }
+}
+
+void sync_all(rpk_ctx* ctx) {
+    for (auto& ds : ctx->devs) {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        RPK_CUDA(cudaStreamSynchronize(ds.stream));
+    }
+}
+}  // namespace
+
+int rpk_pods_grow(rpk_ctx* ctx, uint32_t N) {
+    static const char* who = "rpk_pods_grow";
+    if (!ctx) return RPK_EINVAL;
+    if (int rc = check_select_ready(ctx, who, true, -1, false)) return rc;
+    const uint32_t N0 = ctx->devs[0].podsN;
+    if (N < N0) return fail(ctx, RPK_EINVAL, std::string(who) + ": N is below the pod table's size (a table only grows)");
+    if (N == N0) return RPK_OK;
+    const int n = (int)ctx->devs.size();
+    // The stored results move with their slots when every GPU holds the range rpk_select_pending_changed gives it.  Any
+    // other results were made for the range of a one-process-per-GPU rank, whose peers' results live in other processes:
+    // they are cleared, as rpk_pods_reset clears them.
+    bool move_results = true;
+    for (int s = 0; s < n; ++s) {
+        const DeviceState& ds = ctx->devs[(size_t)s];
+        move_results = move_results && ds.res_ready && ds.res_bound && ds.res_ranks == n && ds.res_rank == s;
+    }
+    std::vector<SlotRange> was((size_t)n), now((size_t)n);
+    for (int s = 0; s < n; ++s) {
+        result_range(N0, n, s, &was[(size_t)s].lo, &was[(size_t)s].hi);
+        result_range(N, n, s, &now[(size_t)s].lo, &now[(size_t)s].hi);
+    }
+    struct Bufs {
+        Grow<int32_t> mem, vcpu, ram; Grow<double> max_price; Grow<uint8_t> cloud, pending; Grow<uint32_t> list;
+        Grow<int32_t> r_mem, r_vcpu, r_ram, r_top5; Grow<double> r_max_price; Grow<uint8_t> r_cloud; Grow<uint32_t> r_gen;
+        Grow<uint32_t> r_list; Grow<uint16_t> r_mask; Grow<int32_t> r_out;
+        Grow<int32_t> l_mem, l_vcpu, l_ram, l_top5; Grow<double> l_max_price; Grow<uint8_t> l_cloud;
+        PinnedBuf h_res;
+    };
+    std::vector<std::unique_ptr<Bufs>> g;
+    const int rc = guarded(ctx, [&]() -> int {
+        // 1. every GPU's new buffers, before anything changes
+        for (int s = 0; s < n; ++s) {
+            DeviceState& ds = ctx->devs[(size_t)s];
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ds.sel_scope.host_wait();  // a device select may still gather from the table
+            g.emplace_back(new Bufs());
+            Bufs& b = *g.back();
+            b.mem.alloc(ds.pt_mem, N); b.vcpu.alloc(ds.pt_vcpu, N); b.ram.alloc(ds.pt_ram, N);
+            b.max_price.alloc(ds.pt_max_price, N); b.cloud.alloc(ds.pt_cloud, N); b.pending.alloc(ds.pt_pending, N);
+            b.list.alloc(ds.pt_list, ds.pt_list.p ? N : 0);
+            if (!move_results) continue;
+            // the sizes reserve_results gives a range; a range whose first slot moves gets new columns
+            const SlotRange r = now[(size_t)s];
+            const bool moved = r.lo != was[(size_t)s].lo;
+            const size_t m = ((size_t)(r.hi - r.lo) + 15) / 16 * 16 + 16, rows = std::max<uint32_t>(r.hi - r.lo, 1u);
+            b.r_mem.alloc(ds.r_mem, m, moved); b.r_vcpu.alloc(ds.r_vcpu, m, moved); b.r_ram.alloc(ds.r_ram, m, moved);
+            b.r_max_price.alloc(ds.r_max_price, m, moved); b.r_cloud.alloc(ds.r_cloud, m, moved);
+            b.r_gen.alloc(ds.r_gen, m, moved); b.r_top5.alloc(ds.r_top5, m * RPK_TOPK, moved);
+            b.r_list.alloc(ds.r_list, m); b.r_mask.alloc(ds.r_mask, m / 16 + 1);
+            DeviceState::Lane& ln = ds.r_lane;
+            b.l_mem.alloc(ln.p_req_mem, rows); b.l_vcpu.alloc(ln.p_req_vcpu, rows); b.l_ram.alloc(ln.p_req_ram, rows);
+            b.l_max_price.alloc(ln.p_max_price, rows); b.l_cloud.alloc(ln.p_cloud, rows); b.l_top5.alloc(ln.top5, rows * RPK_TOPK);
+            b.r_out.alloc(ds.r_out, m * (2 + RPK_TOPK));
+            if (64 + b.r_out.dst_cap() * 4 > ds.h_res.cap) b.h_res.reserve(64 + b.r_out.dst_cap() * 4);
+        }
+        // 2. the rows and flags of [0, N0) stay, [N0, N) become reset rows (k_pod_fill on the new part alone); the stored
+        //    results go to their new owners, and every owned slot without one has generation 0
+        for (int s = 0; s < n; ++s) {
+            DeviceState& ds = ctx->devs[(size_t)s];
+            Bufs& b = *g[(size_t)s];
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            b.mem.keep(N0, ds.stream); b.vcpu.keep(N0, ds.stream); b.ram.keep(N0, ds.stream);
+            b.max_price.keep(N0, ds.stream); b.cloud.keep(N0, ds.stream); b.pending.keep(N0, ds.stream);
+            const PodRows fresh_rows{b.mem.dst() + N0, b.vcpu.dst() + N0, b.ram.dst() + N0, b.max_price.dst() + N0, b.cloud.dst() + N0};
+            ctx->launches += (uint64_t)launch_pod_fill(fresh_rows, b.pending.dst() + N0, N - N0, ds.sm_count, ds.stream);
+            if (!move_results) continue;
+            const size_t kept = b.r_gen.dst() == ds.r_gen.p ? was[(size_t)s].hi - was[(size_t)s].lo : 0;
+            RPK_CUDA(cudaMemsetAsync(b.r_gen.dst() + kept, 0, (b.r_gen.dst_cap() - kept) * sizeof(uint32_t), ds.stream));
+        }
+        if (move_results) {
+            std::vector<const void*> src((size_t)n);
+            std::vector<void*> dst((size_t)n);
+            const auto column = [&](auto buf, size_t bytes) {  // buf: a Grow member of Bufs
+                for (int s = 0; s < n; ++s) { src[(size_t)s] = ((*g[(size_t)s]).*buf).b->p; dst[(size_t)s] = ((*g[(size_t)s]).*buf).dst(); }
+                move_slots(ctx, was, now, src, dst, bytes);
+            };
+            column(&Bufs::r_mem, 4); column(&Bufs::r_vcpu, 4); column(&Bufs::r_ram, 4); column(&Bufs::r_max_price, 8);
+            column(&Bufs::r_cloud, 1); column(&Bufs::r_gen, 4); column(&Bufs::r_top5, 4 * RPK_TOPK);
+        }
+        sync_all(ctx);
+        // 3. the new buffers and sizes take effect together
+        for (int s = 0; s < n; ++s) {
+            DeviceState& ds = ctx->devs[(size_t)s];
+            Bufs& b = *g[(size_t)s];
+            b.mem.commit(); b.vcpu.commit(); b.ram.commit(); b.max_price.commit(); b.cloud.commit(); b.pending.commit(); b.list.commit();
+            ds.podsN = N;
+            if (!move_results) { ds.res_ready = ds.res_bound = false; continue; }
+            b.r_mem.commit(); b.r_vcpu.commit(); b.r_ram.commit(); b.r_max_price.commit(); b.r_cloud.commit(); b.r_gen.commit();
+            b.r_top5.commit(); b.r_list.commit(); b.r_mask.commit(); b.r_out.commit();
+            b.l_mem.commit(); b.l_vcpu.commit(); b.l_ram.commit(); b.l_max_price.commit(); b.l_cloud.commit(); b.l_top5.commit();
+            if (b.h_res.h) ds.h_res.swap(b.h_res);
+            ds.res_lo = now[(size_t)s].lo; ds.res_hi = now[(size_t)s].hi;
+        }
+        return RPK_OK;
+    });
+    if (rc != RPK_OK) ctx->err = std::string(who) + ": " + ctx->err;
+    return rc;
 }
 
 // ---- cross-process peer vectors (CUDA IPC) ---------------------------------------------------------------
@@ -1592,6 +1725,50 @@ int rpk_status_reset(rpk_ctx* ctx, uint32_t N) {
         }
         return RPK_OK;
     });
+}
+
+int rpk_status_grow(rpk_ctx* ctx, uint32_t N) {
+    static const char* who = "rpk_status_grow";
+    if (!ctx) return RPK_EINVAL;
+    if (!ctx->devs[0].status_sized) return fail(ctx, RPK_ESTATE, std::string(who) + ": no tracked table (call rpk_status_reset first)");
+    const uint32_t N0 = ctx->devs[0].statusN;
+    if (N < N0) return fail(ctx, RPK_EINVAL, std::string(who) + ": N is below the tracked table's size (a table only grows)");
+    if (N == N0) return RPK_OK;
+    const int n = (int)ctx->devs.size();
+    std::vector<SlotRange> was((size_t)n), now((size_t)n);
+    for (int s = 0; s < n; ++s) {
+        shard_range(N0, n, s, &was[(size_t)s].lo, &was[(size_t)s].hi);
+        shard_range(N, n, s, &now[(size_t)s].lo, &now[(size_t)s].hi);
+    }
+    std::vector<std::unique_ptr<Grow<uint64_t>>> g;
+    const int rc = guarded(ctx, [&]() -> int {
+        // 1. every GPU's new column, before anything changes; a shard whose first slot moves gets a new one
+        for (int s = 0; s < n; ++s) {
+            DeviceState& ds = ctx->devs[(size_t)s];
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            g.emplace_back(new Grow<uint64_t>());
+            g.back()->alloc(ds.s_hash_prev, std::max<uint32_t>(now[(size_t)s].hi - now[(size_t)s].lo, 1u), now[(size_t)s].lo != was[(size_t)s].lo);
+        }
+        // 2. every new slot is never seen (hash 0), the hashes of [0, N0) go to their new shards
+        std::vector<const void*> src((size_t)n);
+        std::vector<void*> dst((size_t)n);
+        for (int s = 0; s < n; ++s) {
+            DeviceState& ds = ctx->devs[(size_t)s];
+            const Grow<uint64_t>& b = *g[(size_t)s];
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            const size_t kept = b.dst() == ds.s_hash_prev.p ? was[(size_t)s].hi - was[(size_t)s].lo : 0;
+            const size_t m = std::max<uint32_t>(now[(size_t)s].hi - now[(size_t)s].lo, 1u);
+            RPK_CUDA(cudaMemsetAsync(b.dst() + kept, 0, (m - kept) * sizeof(uint64_t), ds.stream));
+            src[(size_t)s] = ds.s_hash_prev.p; dst[(size_t)s] = b.dst();
+        }
+        move_slots(ctx, was, now, src, dst, sizeof(uint64_t));
+        sync_all(ctx);
+        // 3. the new columns and the size take effect together
+        for (int s = 0; s < n; ++s) { g[(size_t)s]->commit(); ctx->devs[(size_t)s].statusN = N; }
+        return RPK_OK;
+    });
+    if (rc != RPK_OK) ctx->err = std::string(who) + ": " + ctx->err;
+    return rc;
 }
 
 namespace {

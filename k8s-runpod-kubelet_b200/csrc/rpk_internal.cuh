@@ -387,6 +387,24 @@ struct DevBuf {  // grow-only device buffer, freed by its destructor
     void swap(DevBuf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
 };
 
+// One buffer of a grow (rpk_pods_grow, rpk_status_grow).  The replacement of a buffer whose capacity is short (with
+// `always`: of the buffer whatever its capacity) is allocated for every GPU before anything is copied or resized, so a
+// refused allocation frees what was allocated and leaves the ctx as it was.  commit() puts it in place once every copy
+// is done; the old buffer is freed with the Grow.
+template <typename T>
+struct Grow {
+    DevBuf<T>* b = nullptr;
+    DevBuf<T> fresh;
+    void alloc(DevBuf<T>& buf, size_t n, bool always = false) { b = &buf; if (always || n > buf.cap) fresh.reserve(n); }
+    T* dst() const { return fresh.p ? fresh.p : b->p; }
+    size_t dst_cap() const { return fresh.p ? fresh.cap : b->cap; }
+    // the first n elements stay as they are
+    void keep(size_t n, cudaStream_t st) const {
+        if (fresh.p && n) RPK_CUDA(cudaMemcpyAsync(fresh.p, b->p, n * sizeof(T), cudaMemcpyDeviceToDevice, st));
+    }
+    void commit() { if (fresh.p) b->swap(fresh); }
+};
+
 struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches it at d
     unsigned char* h = nullptr;
     unsigned char* d = nullptr;
@@ -404,6 +422,7 @@ struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches i
         RPK_CUDA(cudaHostGetDevicePointer((void**)&d, h, 0));
         cap = want;
     }
+    void swap(PinnedBuf& o) { std::swap(h, o.h); std::swap(d, o.d); std::swap(cap, o.cap); }
 };
 
 // One ordering scope of a shard (rpk.h, "Ordering"): the buffers its device entry points share -- the device select
@@ -510,8 +529,9 @@ struct DeviceState {
     PinnedBuf h_res;
     bool res_ready = false;
     // the owned range [res_lo, res_hi) the stored results were made for, set by the first call after rpk_pods_reset
-    // (res_bound); a call over another range is refused
-    bool res_bound = false; uint32_t res_lo = 0, res_hi = 0;
+    // (res_bound), and the (n_ranks, my_rank) it was computed from (rpk_select_pending_changed: the ctx's GPUs and the
+    // shard); a call over another range is refused
+    bool res_bound = false; uint32_t res_lo = 0, res_hi = 0; int res_ranks = 0, res_rank = 0;
     StoredResults results() { return StoredResults{r_mem.p, r_vcpu.p, r_ram.p, r_max_price.p, r_cloud.p, r_gen.p, r_top5.p}; }
     PodRows pods_table() { return PodRows{pt_mem.p, pt_vcpu.p, pt_ram.p, pt_max_price.p, pt_cloud.p}; }
     ~DeviceState();

@@ -208,6 +208,12 @@ class Engine:
         self._check(self._lib.rpk_pods_reset(self._ctx, N))
         self._pods_n = N  # the capacity pods_pending_list_device requires of its output
 
+    def pods_grow(self, N: int):
+        """Grow the pod table to N slots, keeping every row, pending flag and stored result; the new slots are reset rows
+        (rpk_pods_grow)."""
+        self._check(self._lib.rpk_pods_grow(self._ctx, N))
+        self._pods_n = N
+
     def pods_seed_slots(self, slots: np.ndarray, pods: dict):
         """Row slots[i] := row i of the host columns ``pods`` (as ``select`` takes them; slots strictly ascending)."""
         n = int(pods["req_mem_gb"].shape[0])
@@ -411,6 +417,10 @@ class Engine:
     # -- status sweep --------------------------------------------------------------------------------
     def status_reset(self, N: int):
         self._check(self._lib.rpk_status_reset(self._ctx, N))
+
+    def status_grow(self, N: int):
+        """Grow the tracked table to N slots, keeping every hash; the new slots are never seen (rpk_status_grow)."""
+        self._check(self._lib.rpk_status_grow(self._ctx, N))
 
     def status_seed(self, records: np.ndarray):
         N, stride = records.shape

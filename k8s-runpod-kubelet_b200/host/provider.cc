@@ -363,10 +363,42 @@ void Provider::StopTickers() {
 }
 
 uint32_t Provider::AllocSlot() {
-    if (free_slots_.empty()) throw std::runtime_error("provider pod capacity exceeded");
     uint32_t s = free_slots_.back();
     free_slots_.pop_back();
     return s;
+}
+
+// No free slot is left: double the capacity.  Both device tables grow in place, keeping every row, pending flag, stored
+// result and hash (rpk_pods_grow, rpk_status_grow); then the engine-side mirrors follow under engine_mutex_ and the
+// pod-side mirrors under pods_mutex_, and the new slots join free_slots_ last, so no slot at or above the old capacity
+// is handed out before both tables and every mirror cover it.  sweep_mutex_ is taken first, as the sweep takes it, so
+// WidenRecords' whole-table seed never meets a half-grown table.  Slots never move and the vectors only grow, so a tick
+// already running keeps valid slot indices.  New status slots need no seed: CreatePod seeds the slot it takes.
+void Provider::GrowSlots() {
+    std::lock_guard<std::mutex> sweep_guard(sweep_mutex_);
+    uint32_t n0;
+    {
+        std::lock_guard<std::mutex> g(pods_mutex_);
+        if (!free_slots_.empty()) return;  // another thread grew the table meanwhile
+        n0 = max_pods_;
+    }
+    const uint64_t want = std::max<uint64_t>(2ull * n0, (uint64_t)n0 + 1);
+    if (want > UINT32_MAX) throw std::runtime_error("provider pod capacity exceeded");
+    const uint32_t n = (uint32_t)want;
+    {
+        std::lock_guard<std::mutex> g(engine_mutex_);
+        if (rpk_pods_grow(ctx_, n) != RPK_OK || rpk_status_grow(ctx_, n) != RPK_OK) throw std::runtime_error(rpk_last_error(ctx_));
+        seeded_.req_mem_gb.resize(n, 16); seeded_.req_vcpu.resize(n, 0); seeded_.req_ram_gb.resize(n, 0);
+        seeded_.max_price.resize(n, DefaultMaxPrice); seeded_.cloud.resize(n, RPK_CLOUD_SECURE);
+        marked_.resize(n, 0);
+        lists_.resize((size_t)n * RPK_TOPK, -1);
+    }
+    std::lock_guard<std::mutex> g(pods_mutex_);
+    records_.resize((size_t)n * stride_, 0);
+    slot_key_.resize(n);
+    want_pending_.resize(n, 0);
+    for (uint32_t s = n; s > n0; --s) free_slots_.push_back(s - 1);
+    max_pods_ = n;
 }
 
 bool Provider::IsPending(const Pod& pod) {
@@ -404,19 +436,25 @@ void Provider::SeedSlot(uint32_t slot) {
 std::string Provider::CreatePod(const PodPtr& pod) {
     const std::string key = Key(pod->ns, pod->name);
     uint32_t slot;
-    {
-        std::lock_guard<std::mutex> g(pods_mutex_);
-        auto it = pods_.find(key);
-        Tracked t;
-        t.slot = it != pods_.end() ? it->second.slot : AllocSlot();
-        t.pod = std::make_shared<Pod>(*pod);  // DeepCopy
-        t.info.PodName = pod->name; t.info.Namespace = pod->ns; t.info.Status = PodStarting;
-        t.info.CreationTime = now_; t.info.RequestedPorts = GetRequestedPorts(*pod); t.info.PortsExposed = false;
-        slot_key_[t.slot] = key;
-        EncodeStatusRecord(&records_[(size_t)t.slot * stride_], stride_, t.info.Status, t.info.PortsExposed);
-        slot = t.slot;
-        TrackPending(slot, IsPending(*t.pod));
-        pods_[key] = std::move(t);
+    for (;;) {
+        {
+            std::lock_guard<std::mutex> g(pods_mutex_);
+            auto it = pods_.find(key);
+            if (it != pods_.end() || !free_slots_.empty()) {
+                Tracked t;
+                t.slot = it != pods_.end() ? it->second.slot : AllocSlot();
+                t.pod = std::make_shared<Pod>(*pod);  // DeepCopy
+                t.info.PodName = pod->name; t.info.Namespace = pod->ns; t.info.Status = PodStarting;
+                t.info.CreationTime = now_; t.info.RequestedPorts = GetRequestedPorts(*pod); t.info.PortsExposed = false;
+                slot_key_[t.slot] = key;
+                EncodeStatusRecord(&records_[(size_t)t.slot * stride_], stride_, t.info.Status, t.info.PortsExposed);
+                slot = t.slot;
+                TrackPending(slot, IsPending(*t.pod));
+                pods_[key] = std::move(t);
+                break;
+            }
+        }
+        GrowSlots();  // with pods_mutex_ released (it is never held with engine_mutex_), then take a slot again
     }
     SeedSlot(slot);  // previous state for the sweep = what InstanceInfo says now, for this slot only
     DeployBatch({key});  // errors are logged and swallowed: kubelet.go:406-415
@@ -425,20 +463,27 @@ std::string Provider::CreatePod(const PodPtr& pod) {
 
 // UpdatePod -- kubelet.go:421-432
 std::string Provider::UpdatePod(const PodPtr& pod) {
-    std::lock_guard<std::mutex> g(pods_mutex_);
-    auto it = pods_.find(Key(pod->ns, pod->name));
-    if (it == pods_.end()) {  // the reference inserts into p.pods without an InstanceInfo; mirror the visible part
-        Tracked t;
-        t.slot = AllocSlot();
-        t.pod = std::make_shared<Pod>(*pod);
-        slot_key_[t.slot] = Key(pod->ns, pod->name);
-        TrackPending(t.slot, IsPending(*t.pod));
-        pods_[Key(pod->ns, pod->name)] = std::move(t);
-    } else {
-        it->second.pod = std::make_shared<Pod>(*pod);
-        TrackPending(it->second.slot, IsPending(*pod));  // a changed phase or RunPod id
+    for (;;) {
+        {
+            std::lock_guard<std::mutex> g(pods_mutex_);
+            auto it = pods_.find(Key(pod->ns, pod->name));
+            if (it != pods_.end()) {
+                it->second.pod = std::make_shared<Pod>(*pod);
+                TrackPending(it->second.slot, IsPending(*pod));  // a changed phase or RunPod id
+                return "";
+            }
+            if (!free_slots_.empty()) {  // the reference inserts into p.pods without an InstanceInfo; mirror the visible part
+                Tracked t;
+                t.slot = AllocSlot();
+                t.pod = std::make_shared<Pod>(*pod);
+                slot_key_[t.slot] = Key(pod->ns, pod->name);
+                TrackPending(t.slot, IsPending(*t.pod));
+                pods_[Key(pod->ns, pod->name)] = std::move(t);
+                return "";
+            }
+        }
+        GrowSlots();  // as in CreatePod
     }
-    return "";
 }
 
 // DeletePod -- kubelet.go:621-651

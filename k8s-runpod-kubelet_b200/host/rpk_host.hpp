@@ -165,7 +165,8 @@ struct ProviderOptions {
 
 class Provider {
 public:
-    // n_gpus GPUs behind one rpk ctx; throws std::runtime_error when the engine cannot start (no CPU fallback)
+    // n_gpus GPUs behind one rpk ctx; throws std::runtime_error when the engine cannot start (no CPU fallback).  max_pods
+    // is the initial slot capacity: when every slot is taken, CreatePod and UpdatePod double it (GrowSlots)
     Provider(std::shared_ptr<RunPodAPI> api, int n_gpus = 1, uint32_t max_pods = 1024, ProviderOptions opt = ProviderOptions());
     ~Provider();
 
@@ -213,7 +214,8 @@ private:
     static bool IsPending(const Pod& pod);       // processPendingPods' predicate (kubelet.go:752, :768)
     void TrackPending(uint32_t slot, bool pending);  // pods_mutex_ held: the slot's wanted flag, queued for the next tick
     void Notify(const PodPtr& pod);
-    uint32_t AllocSlot();
+    uint32_t AllocSlot();                        // pods_mutex_ held, free_slots_ not empty
+    void GrowSlots();                            // no lock held: double the slot capacity (sweep_mutex_, then the others)
     void SeedSlot(uint32_t slot);                // device previous state of ONE slot := records_[slot]
     void WidenRecords(uint32_t stride);          // re-encode every slot at a wider stride (sweeps are excluded by sweep_mutex_)
     void StartTicker(double interval_s, std::function<void()> body);
@@ -226,7 +228,7 @@ private:
     std::map<std::string, std::string> deleted_pods_;  // "ns/name" -> RunPod id (kubelet.go:628)
     std::function<void(const PodPtr&)> notify_;
     std::vector<GPUType> offers_;
-    std::vector<uint8_t> records_;      // max_pods x stride_: what InstanceInfo says per slot (pods_mutex_)
+    std::vector<uint8_t> records_;      // max_pods_ x stride_: what InstanceInfo says per slot (pods_mutex_)
     uint32_t stride_ = 16;              // every RunPod status fits 16 bytes; widened (32 .. 256) if an API string does not
     uint32_t want_stride_ = 16;
     std::vector<std::thread> tickers_;
@@ -234,7 +236,7 @@ private:
     uint64_t host_compares_ = 0;
     std::vector<uint32_t> free_slots_;
     std::vector<std::string> slot_key_;
-    uint32_t max_pods_;
+    uint32_t max_pods_;                 // slot capacity (pods_mutex_; changed by GrowSlots, which also holds sweep_mutex_)
     PodColumnsSoA seeded_;              // max_pods rows: what the device pod table holds per slot (engine_mutex_)
     std::vector<uint8_t> want_pending_; // max_pods flags: the slot's pod is Pending without a RunPod id (pods_mutex_)
     std::vector<uint32_t> pending_dirty_;  // slots whose wanted flag changed since the last tick took them (pods_mutex_)

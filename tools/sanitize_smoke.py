@@ -87,6 +87,10 @@ if not ONLY_MULTI:
     assert r0 == len(pend) and np.array_equal(s0, pend) and np.array_equal(b0, best) and np.array_equal(t0, t5)
     assert r1 == 0 and len(s1) == 0 and r2 == len(pend) and len(s2) == 0
     assert int(fl[16].item()) == 3 and int(fl[34].item()) == 3
+    # a grow (k_pod_fill on the new slots alone, the one-rank results copied: their range is the host call's) reselects
+    # nothing
+    eg.pods_grow(200_000 + 4099)
+    assert eg.select_pending_changed(len(pend))[1] == 0
     eg.close()
     # the device form (the same kernels, the row count never read on the host): one eager call that
     # reports every pending slot, then one replay of a captured steady call
