@@ -176,6 +176,14 @@ class StatusTable:
         self.prev = np.zeros((N, self.stride), np.uint8)
         self.has_prev = np.zeros(N, np.uint8)
 
+    def grow(self, N: int) -> None:
+        """rpk_status_grow: slots [self.N, N) are appended, never seen; every other slot keeps its state"""
+        assert N >= self.N
+        prev, has_prev = self.prev, self.has_prev
+        self.reset(N)
+        self.prev[: len(prev)] = prev
+        self.has_prev[: len(has_prev)] = has_prev
+
     def prev_hashes(self) -> np.ndarray:
         """the device's previous-hash column for this state: the record hash of a seen slot, 0 for a slot never seen"""
         return np.where(self.has_prev != 0, record_hashes(self.prev), np.uint64(0))

@@ -84,6 +84,19 @@ class Generations:
         self.res_gen = np.zeros(N, np.int64)
         self.top5 = np.full((N, 5), -1, np.int32)
 
+    def grow(self, N, keep_results=True):
+        """rpk_pods_grow: slots [self.N, N) get reset rows, no flag and no stored result; every other slot keeps its row,
+        flag and stored result.  keep_results=False drops every stored result, as a grow does on a ctx whose results
+        were made for the range of a one-process-per-GPU rank."""
+        assert N >= self.N
+        N0, old = self.N, (self.cols, self.res_cols, self.pending, self.res_gen, self.top5)
+        self.reset(N)
+        for k in POD_COLS:
+            self.cols[k][:N0], self.res_cols[k][:N0] = old[0][k], old[1][k]
+        self.pending[:N0] = old[2]
+        if keep_results:
+            self.res_gen[:N0], self.top5[:N0] = old[3], old[4]
+
     def _wholesale(self):
         self.gen += 1
         self.floor = self.gen
