@@ -112,6 +112,19 @@ def queues(pl, dist, pods):
     return len(np.unique(grp)) * pl.S
 
 
+def iterations_per_cta(pl, n_queues):
+    """stages the busiest CTA loads in one call: with more queues than CTAs, CTA b serves queues b, b + grid, ...;
+    otherwise every CTA keeps one queue"""
+    return cdiv(n_queues, pl.grid) if n_queues > pl.grid else min(n_queues, 1)
+
+
+def copy_groups(pl, s):
+    """copy groups (bulk copies on their own mbarrier, at most kCopyGroups = 8) that load stage s"""
+    nsubs = min(pl.per, pl.nsub - s * pl.per)
+    gs = cdiv(nsubs, min(pl.per, 8))
+    return cdiv(nsubs, gs)
+
+
 def host_sub_batches(P):
     """row counts of the host entry point's sub-batches on one GPU (sub_batch_rows); P <= SMALL_BATCH is one call"""
     out, j = [], 0
