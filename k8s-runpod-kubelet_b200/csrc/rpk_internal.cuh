@@ -222,6 +222,7 @@ struct Tune {
     int stage_kb = 0;            // stagekb=: persistent select's stage cap (0: 220 KB)
     int items_per_warp = 0;      // ipw=: persistent select's items per warp (0: 4)
     int k0ctas = 0;              // k0ctas=: CTAs of the persistent select's class sort (0: four per SM)
+    int grid_tiles = 0;          // gridtiles=: row tiles per launch of the packed / wide grid (0: as many as gridDim.x takes)
 };
 Tune read_tune();
 

@@ -151,12 +151,12 @@ __device__ __forceinline__ void finish_tile(const SelectArgs& a, const TileInfo&
 //                so that a lower one overwrites.
 // ---------------------------------------------------------------------------------------------------------
 template <int R, bool kPos>
-__global__ void __launch_bounds__(kCtaThreads, 3) k_select_packed(SelectArgs a, uint32_t S, uint32_t seg_len) {
+__global__ void __launch_bounds__(kCtaThreads, 3) k_select_packed(SelectArgs a, uint32_t S, uint32_t seg_len, uint32_t tile0) {
     extern __shared__ __align__(128) uint32_t s_off[];
     __shared__ __align__(8) uint64_t s_bar;
     __shared__ int s_last;
     constexpr uint32_t RPC = kWarpsPerCta * R;
-    const uint32_t tile = blockIdx.x / S, seg = blockIdx.x - tile * S;
+    const uint32_t lt = blockIdx.x / S, seg = blockIdx.x - lt * S, tile = tile0 + lt;
     pdl_wait();     // k_pod_prep (counts, order, rw, pos) has completed
     pdl_trigger();  // a dependent (the peer fence) may be scheduled; it waits for this grid to complete
     const TileInfo t = decode_tile(a, tile, RPC);
@@ -324,12 +324,12 @@ __global__ void __launch_bounds__(kCtaThreads) k_select_fused(SelectArgs a, uint
 // K1 (generic): full-range int32 columns, one int4 per offer, 4 instructions per offer-score
 // ---------------------------------------------------------------------------------------------------------
 template <int R>
-__global__ void __launch_bounds__(kCtaThreads, 2) k_select_wide(SelectArgs a, uint32_t S, uint32_t seg_len) {
+__global__ void __launch_bounds__(kCtaThreads, 2) k_select_wide(SelectArgs a, uint32_t S, uint32_t seg_len, uint32_t tile0) {
     extern __shared__ __align__(128) uint32_t s_off[];
     __shared__ __align__(8) uint64_t s_bar;
     __shared__ int s_last;
     constexpr uint32_t RPC = kWarpsPerCta * R;
-    const uint32_t tile = blockIdx.x / S, seg = blockIdx.x - tile * S;
+    const uint32_t lt = blockIdx.x / S, seg = blockIdx.x - lt * S, tile = tile0 + lt;
     pdl_wait();     // k_pod_prep (counts, order, rw, pos) has completed
     pdl_trigger();  // a dependent (the peer fence) may be scheduled; it waits for this grid to complete
     const TileInfo t = decode_tile(a, tile, RPC);
@@ -542,6 +542,7 @@ static Tune parse_tune() {
     if (const char* p = strstr(e, "stagekb=")) t.stage_kb = atoi(p + 8);
     if (const char* p = strstr(e, "ipw=")) t.items_per_warp = atoi(p + 4);
     if (const char* p = strstr(e, "k0ctas=")) { const int v = atoi(p + 7); if (v > 0) t.k0ctas = v; }
+    if (const char* p = strstr(e, "gridtiles=")) { const int v = atoi(p + 10); if (v > 0) t.grid_tiles = v; }
     return t;
 }
 Tune read_tune() {
@@ -574,29 +575,42 @@ int pick_rows_per_warp(uint32_t P, int sm_count) {
     return 1;
 }
 
+// The grid is (row tile) x (offer segment), tiles * S CTAs, which passes gridDim.x's 2^31 - 1 on the largest tables and
+// batches (2^26 offers in 4096-offer segments and 2^24 rows at 128 rows per tile).  It is cut into launches of at most
+// (2^31 - 1) / S whole row tiles (RPK_TUNE gridtiles=N: at most N), each told its first tile; the tile counters, done
+// and the group counts span the launches.  Returns the launches.
 template <int R>
-static void launch_grid(const SelectArgs& a, cudaStream_t st) {
+static int launch_grid(const SelectArgs& a, cudaStream_t st) {
     static thread_local int dev_pos = -1, dev_packed = -1, dev_wide = -1;
-    const bool pdl = read_tune().pdl;
+    const Tune tune = read_tune();
+    const bool pdl = tune.pdl;
     uint32_t S, seg_len;
     const uint32_t tiles = select_tiles_max(a.P, R);
+    auto launch = [&](auto kernel, size_t smem) {
+        uint32_t per = (uint32_t)std::min<uint64_t>(tiles, (uint64_t)INT32_MAX / S);
+        if (tune.grid_tiles > 0) per = std::min(per, (uint32_t)tune.grid_tiles);
+        int n = 0;
+        for (uint32_t t0 = 0; t0 < tiles; t0 += per, ++n) {
+            const uint64_t ctas = (uint64_t)std::min(per, tiles - t0) * S;
+            launch_pdl(kernel, dim3((uint32_t)ctas), dim3(kCtaThreads), smem, st, pdl, a, S, seg_len, t0);
+        }
+        return n;
+    };
     if (a.pk.bits && a.pk.pos_bits) {
         // fixed 2^kPosBits-offer segments: the embedded positions are segment-local
         const uint32_t Gc = ((a.G + kChunk - 1) / kChunk) * kChunk;
         S = (Gc + kSegPacked - 1) / kSegPacked; if (S == 0) S = 1;
         seg_len = kSegPacked;
         allow_smem(k_select_packed<R, true>, (int)(kSegPacked * 4), &dev_pos);
-        launch_pdl(k_select_packed<R, true>, dim3(tiles * S), dim3(kCtaThreads), (size_t)kSegPacked * 4, st, pdl, a, S, seg_len);
+        return launch(k_select_packed<R, true>, (size_t)kSegPacked * 4);
     } else if (a.pk.bits) {
         seg_plan(a.G, kSegPacked, &S, &seg_len);
-        const size_t smem = (size_t)seg_len * 4;
         allow_smem(k_select_packed<R, false>, (int)(kSegPacked * 4), &dev_packed);
-        launch_pdl(k_select_packed<R, false>, dim3(tiles * S), dim3(kCtaThreads), smem, st, pdl, a, S, seg_len);
+        return launch(k_select_packed<R, false>, (size_t)seg_len * 4);
     } else {
         seg_plan(a.G, kSegWide, &S, &seg_len);
-        const size_t smem = (size_t)seg_len * 16;
         allow_smem(k_select_wide<R>, (int)(kSegWide * 16), &dev_wide);
-        launch_pdl(k_select_wide<R>, dim3(tiles * S), dim3(kCtaThreads), smem, st, pdl, a, S, seg_len);
+        return launch(k_select_wide<R>, (size_t)seg_len * 16);
     }
 }
 
@@ -666,13 +680,12 @@ static int launch_select_kernels(const SelectArgs& a, int R, const PersistPlan* 
     // counts / done / tile tickets are zero here: zeroed when allocated, and every grid kernel leaves them zero
     k_pod_prep<<<(a.P + 1023) / 1024, 1024, 0, st>>>(a); ++launches;
     switch (R) {
-        case 16: launch_grid<16>(a, st); break;
-        case 8: launch_grid<8>(a, st); break;
-        case 4: launch_grid<4>(a, st); break;
-        case 2: launch_grid<2>(a, st); break;
-        default: launch_grid<1>(a, st); break;
+        case 16: launches += launch_grid<16>(a, st); break;
+        case 8: launches += launch_grid<8>(a, st); break;
+        case 4: launches += launch_grid<4>(a, st); break;
+        case 2: launches += launch_grid<2>(a, st); break;
+        default: launches += launch_grid<1>(a, st); break;
     }
-    ++launches;
     if (a.top5) {
         const uint32_t blocks = (uint32_t)min((uint64_t)(a.P + 7) / 8, (uint64_t)sm_count * 32);
         k_select_top5<<<blocks, 256, 0, st>>>(a); ++launches;

@@ -1,7 +1,9 @@
 """Restatement of the persistent select's launch plan: ``class_dims`` and ``persist_plan`` in
 k8s-runpod-kubelet_b200/csrc/select_persist.cu, with the constants of rpk_internal.cuh, the view layout
 ``launch_offer_ingest`` (offers.cu) picks from the distinct counts (``layout``, which includes the bitmapM condition)
-and the host entry point's row sub-batches (``sub_batch_rows``, rpk_api.cu).
+the host entry point's row sub-batches (``sub_batch_rows``, rpk_api.cu), and the grid of the packed and wide kernels
+that tables without a bit-sliced view take (``pick_rows_per_warp``, ``select_tiles_max``, ``seg_plan`` and
+``launch_grid`` in select.cu).
 
 The GPU tests assert through it which regime each case reaches, so a change to a constant that moves a case off its
 regime fails the case instead of quietly testing something else."""
@@ -16,6 +18,9 @@ STAGE_MAX = 220 * 1024                 # persist_plan's stage cap
 FUSED_ROWS_MAX, SMALL_BATCH = 16384, 4096  # kFusedRowsMax, kSmallBatch
 SUB_BATCH_ROWS = 131072                # kSubBatchRows (x1, x2, x3, then x4)
 POS_BITS = 14                          # kPosBits: position-in-segment bits of a packed_pos word (kSegPacked = 2^14)
+WARPS_PER_CTA, GROUPS, CHUNK = 8, 8, 128  # kWarpsPerCta, kGroups (cloud x vcpu constrains x ram constrains), kChunk
+SEG_PACKED, SEG_WIDE = 1 << POS_BITS, 4096  # kSegPacked, kSegWide: offers staged per CTA of the packed / wide kernels
+GRID_X_MAX = 2**31 - 1                 # gridDim.x limit: launch_grid cuts larger grids into launches of whole row tiles
 # RPK_FORCE_KERNEL values as install_offers (rpk_api.cu) reads them; any other string is the automatic choice
 FORCE_KINDS = {"generic": 1, "packed": 2, "packed_pos": 3, "bitmap": 4, "bitmap_grouped": 5, "bitmap_price": 6}
 KIND_NAMES = {1: "generic", 2: "packed", 3: "packed_pos", 4: "bitmap"}  # rpk_stats.select_kernel_kind
@@ -142,16 +147,86 @@ def persistent(P, no_fused=False):
     return P > FUSED_ROWS_MAX or no_fused
 
 
+def tune_value(env, key):
+    """the number after `key` in an RPK_TUNE string, parsed like parse_tune (select.cu); 0 when absent"""
+    i = env.find(key)
+    if i < 0:
+        return 0
+    digits = ""
+    for ch in env[i + len(key):]:
+        if not ch.isdigit():
+            break
+        digits += ch
+    return int(digits or 0)
+
+
 def tune_from_env(env):
-    """(stage_kb, items_per_warp, k0ctas) of an RPK_TUNE string, parsed like parse_tune (select.cu)"""
-    def num(key):
-        i = env.find(key)
-        if i < 0:
-            return 0
-        digits = ""
-        for ch in env[i + len(key):]:
-            if not ch.isdigit():
-                break
-            digits += ch
-        return int(digits or 0)
-    return num("stagekb="), num("ipw="), num("k0ctas=")
+    """(stage_kb, items_per_warp, k0ctas) of an RPK_TUNE string"""
+    return tune_value(env, "stagekb="), tune_value(env, "ipw="), tune_value(env, "k0ctas=")
+
+
+# ---- the packed and wide kernels (kinds 3 / 2 / 1) -------------------------------------------------------------------
+def rows_per_warp(P, sm):
+    """pick_rows_per_warp: the most rows per warp (16, 8, 4, 2) that still give ~4 waves of 3 CTAs per SM, else 1"""
+    for r in (16, 8, 4, 2):
+        if cdiv(P, WARPS_PER_CTA * r) >= sm * 12:
+            return r
+    return 1
+
+
+def rows_per_warp_bounds(sm):
+    """the smallest P at which rows_per_warp reaches 2, 4, 8 and 16"""
+    return [(sm * 12 - 1) * WARPS_PER_CTA * r + 1 for r in (2, 4, 8, 16)]
+
+
+def tiles_max(P, R):
+    """select_tiles_max: row tiles of R rows per warp, every row group ending in at most one partial tile"""
+    return cdiv(P, WARPS_PER_CTA * R) + GROUPS
+
+
+def grid_segments(kind, G):
+    """(S, segment length) of the offer segments: packed_pos (3) takes fixed 2^14-offer segments, since its words carry
+    the position inside the segment; packed (2) and wide (1) split the table evenly (seg_plan) into segments of at
+    most 16 384 and 4 096 offers, each a multiple of 128"""
+    Gc = cdiv(G, CHUNK) * CHUNK
+    if kind == 3:
+        return max(cdiv(Gc, SEG_PACKED), 1), SEG_PACKED
+    assert kind in (1, 2), kind
+    S = max(cdiv(Gc, SEG_PACKED if kind == 2 else SEG_WIDE), 1)
+    return S, cdiv(cdiv(Gc, S), CHUNK) * CHUNK
+
+
+def grid_launches(P, R, S, grid_tiles=0):
+    """[(first tile, CTAs)] of launch_grid: tiles_max x S CTAs in launches of at most GRID_X_MAX // S whole tiles
+    (RPK_TUNE gridtiles=N: at most N)"""
+    tiles = tiles_max(P, R)
+    per = min(tiles, GRID_X_MAX // S)
+    if grid_tiles > 0:
+        per = min(per, grid_tiles)
+    return [(t0, min(per, tiles - t0) * S) for t0 in range(0, tiles, per)]
+
+
+def row_groups(kind, dist, pods):
+    """rows per k_pod_prep row group, cloud * 4 + (vcpu threshold > 0) * 2 + (ram threshold > 0); the generic kernel
+    (kind 1) has no rank thresholds and puts every row in group 3 or 7; rows of neither cloud join no group"""
+    P = len(pods["req_mem_gb"])
+    cloud = pods.get("cloud")
+    cloud = np.zeros(P, np.int64) if cloud is None else np.asarray(cloud).astype(np.int64)
+    if kind == 1:
+        need = np.full(P, 3, np.int64)
+    else:
+        th = [np.searchsorted(d, np.zeros(P, np.int32) if pods.get(k) is None else pods[k], side="left") > 0
+              for d, k in zip(dist[1:], ("req_vcpu", "req_ram_gb"))]
+        need = th[0] * 2 + th[1]
+    keep = cloud <= 1
+    return np.bincount(cloud[keep] * 4 + need[keep], minlength=GROUPS)
+
+
+def valid_tiles(counts, R):
+    """row tiles holding rows (decode_tile's total_tiles): tiles [0, valid_tiles) are walked, later ones return"""
+    return int(sum(cdiv(int(n), WARPS_PER_CTA * R) for n in counts))
+
+
+def top5_rows_per_pass(P, sm):
+    """rows (one warp each) of one grid-stride pass of k_select_top5: min(ceil(P / 8), 32 x sm) blocks of 8 warps"""
+    return min(cdiv(P, 8), 32 * sm) * 8

@@ -143,3 +143,67 @@ def test_layout_forced():
 def test_tune_parsing():
     assert model.tune_from_env("stagekb=4") == (4, 0, 0)
     assert model.tune_from_env("pdl=off,ipw=64,k0ctas=3") == (0, 64, 3)
+    assert model.tune_value("gridtiles=97,pdl=off", "gridtiles=") == 97 and model.tune_value("ipw=4", "gridtiles=") == 0
+
+
+def test_grid_tiles_cap():
+    """gridtiles=97 on 100k synth offers: the last tile with rows lies in a later launch than the first one at every
+    size of the capped-grid test (select_grid_child.py), for each kind's row groups"""
+    offers = rpk.synth.make_offers(100_000, correlated=True)
+    dist = model.distinct(offers)
+    pods = rpk.synth.make_pods(50_000)
+    for kind in (1, 2, 3):
+        counts = model.row_groups(kind, dist, pods)
+        assert counts.sum() == (pods["cloud"] <= 1).sum()
+        assert (np.nonzero(counts)[0] % 4 == 3).all() if kind == 1 else len(np.nonzero(counts)[0]) > 2
+        R = model.rows_per_warp(50_000, 132)
+        launches = model.grid_launches(50_000, R, model.grid_segments(kind, 100_000)[0], grid_tiles=97)
+        assert len(launches) == 33 and all(n == 97 * model.grid_segments(kind, 100_000)[0] for _, n in launches[:-1])
+        assert model.valid_tiles(counts, R) > 97 * 30
+    assert model.grid_launches(50_000, 2, 7) == [(0, model.tiles_max(50_000, 2) * 7)]
+
+
+def test_rows_per_warp_boundaries():
+    """R steps at ceil(P / (8 R)) = 12 x SMs row tiles: 25 329 / 50 657 / 101 313 / 202 625 rows with 132 SMs,
+    21 873 / 43 745 / 87 489 / 174 977 with 114; the host entry point's 1M-row sub-batches take R = 8, 16, 16, 16"""
+    for sm, bounds in ((132, [25_329, 50_657, 101_313, 202_625]), (114, [21_873, 43_745, 87_489, 174_977])):
+        assert model.rows_per_warp_bounds(sm) == bounds
+        for R, b in zip((2, 4, 8, 16), bounds):
+            assert model.rows_per_warp(b - 1, sm) == R // 2 and model.rows_per_warp(b, sm) == R, (sm, b)
+        assert [model.rows_per_warp(P, sm) for P in model.host_sub_batches(1_000_000)] == [8, 16, 16, 16]
+        assert model.rows_per_warp(1, sm) == 1 and model.rows_per_warp(2**32 // 5, sm) == 16
+    assert model.tiles_max(1, 1) == 9 and model.tiles_max(128, 16) == 9 and model.tiles_max(129, 16) == 10
+
+
+def test_grid_segments():
+    """packed_pos: 2^14-offer segments at any G; packed: seg_plan(G, 16 384), 7 x 14 336 at 100k; wide: seg_plan(G,
+    4096); every table of a multiple of 4096 offers fills its segments"""
+    assert model.grid_segments(3, 16_384) == (1, 16_384) and model.grid_segments(3, 16_385) == (2, 16_384)
+    assert model.grid_segments(3, 100_000) == (7, 16_384) and model.grid_segments(3, 0) == (1, 16_384)
+    assert model.grid_segments(2, 100_000) == (7, 14_336) and model.grid_segments(2, 16_384) == (1, 16_384)
+    assert model.grid_segments(2, 16_385) == (2, 8_320)
+    assert model.grid_segments(1, 100_000) == (25, 4_096) and model.grid_segments(1, 20_000) == (5, 4_096)
+    assert model.grid_segments(1, 4_097) == (2, 2_176) and model.grid_segments(1, 2**26) == (16_384, 4_096)
+    assert model.grid_segments(2, 2**26) == (4_096, 16_384)
+
+
+def test_grid_launches():
+    """2^26 offers in the wide kernel (S = 16 384) at R = 16: 2^24 + 2^20 + 37 rows need 2.28e9 CTAs, more than
+    gridDim.x takes; 2^25 + 2^20 rows need 4.43e9, which wraps modulo 2^32 to 134 348 800 (8200 tiles) in 32 bits.
+    They take two and three launches of whole tiles; the 1M-row bench step on 100k offers takes one."""
+    P1, P2 = 2**24 + 2**20 + 37, 2**25 + 2**20
+    S = model.grid_segments(1, 2**26)[0]
+    assert model.rows_per_warp(P1, 132) == model.rows_per_warp(P2, 114) == 16
+    t1, t2 = model.tiles_max(P1, 16), model.tiles_max(P2, 16)
+    assert t1 * S == 2_281_848_832 > model.GRID_X_MAX and (t2 * S) % 2**32 == 134_348_800 == 8200 * S
+    per = model.GRID_X_MAX // S
+    assert model.grid_launches(P1, 16, S) == [(0, per * S), (per, (t1 - per) * S)]
+    assert model.grid_launches(P2, 16, S) == [(0, per * S), (per, per * S), (2 * per, (t2 - 2 * per) * S)]
+    assert all(n <= model.GRID_X_MAX for _, n in model.grid_launches(2**32 // 5, 1, S))
+    assert sum(n for _, n in model.grid_launches(2**32 // 5, 1, S)) == model.tiles_max(2**32 // 5, 1) * S
+    assert model.grid_launches(1_000_000, 16, 7) == [(0, model.tiles_max(1_000_000, 16) * 7)]
+
+
+def test_top5_rows_per_pass():
+    assert model.top5_rows_per_pass(1_000_000, 132) == 33_792 and model.top5_rows_per_pass(1_000_000, 114) == 29_184
+    assert model.top5_rows_per_pass(5_003, 132) == 5_008 and model.top5_rows_per_pass(1, 132) == 8
