@@ -5,8 +5,9 @@ Below the big-table threshold the sweep runs one 8-warp CTA per SM (so that it f
 every warp takes one 64-slot unit until SMs * 8 * 64 slots; past that point the warps take longer runs.  At 4M slots
 the sweep switches to 1024-thread CTAs.  The boundaries are the same at every stride; they are crossed at strides 16
 and 32, and at the wide strides 48, 64 and 256, whose sweep takes the stride from its arguments (the 4M boundary at 48
-only, which keeps host memory modest).  Each size runs a host-entry sequence (seed, diff with codes and hashes, an
-unchanged diff, reset, diff), a device-entry diff of a caller-owned hash column, and an rpk_tick."""
+only, which keeps host memory modest; test_status_scale_gpu.py runs every stride 16..256 at 4M + 37 slots, with keys
+instead of host records).  Each size runs a host-entry sequence (seed, diff with codes and hashes, an unchanged diff,
+reset, diff), a device-entry diff of a caller-owned hash column, and an rpk_tick."""
 import numpy as np
 import pytest
 
