@@ -242,6 +242,61 @@ func (e *Engine) SelectSlots(slots []uint32, wantTop5 bool) (best []int32, top5 
 	return best, top5, nil
 }
 
+// Requirements an Explanation counts offers under (RPK_REQ_*).
+const (
+	ReqPrice = C.RPK_REQ_PRICE // price < max price
+	ReqMem   = C.RPK_REQ_MEM   // memory >= the request
+	ReqVCPU  = C.RPK_REQ_VCPU  // vCPUs >= the request
+	ReqRAM   = C.RPK_REQ_RAM   // RAM >= the request
+)
+
+// Explanation is rpk_explanation: why a pod row gets the GPU types it gets.  An offer is offered to the row when it
+// passes the cloud check and price > 0 in the row's cloud; NFail[r] counts the offered offers failing requirement r,
+// NOnly[r] those failing r alone, and Nearest[r] is the cheapest of those (-1: none), the offer the pod would get if
+// only r were relaxed.  Same layout as the C struct.
+type Explanation struct {
+	NFeasible  uint32
+	NUnoffered uint32
+	NFail      [4]uint32
+	NOnly      [4]uint32
+	Nearest    [4]int32
+}
+
+// Explain returns, per pod row, what rules out each offer of the resident table (rpk_explain).  Columns and defaults as
+// Select's.
+func (e *Engine) Explain(p *Pods) ([]Explanation, error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	n := len(p.ReqMemGb)
+	out := make([]Explanation, n)
+	if n == 0 {
+		return out, nil
+	}
+	rc := C.rpk_explain(e.ctx, C.uint32_t(n), i32p(p.ReqMemGb), i32p(p.ReqVCPU), i32p(p.ReqRAMGb), f64p(p.MaxPrice), u8p(p.Cloud),
+		(*C.rpk_explanation)(unsafe.Pointer(&out[0])))
+	if rc != C.RPK_OK {
+		return nil, lastError(e.ctx, rc)
+	}
+	return out, nil
+}
+
+// ExplainSlots is Explain over rows of the pod table: out[i] is what Explain returns for the row held at slots[i] (any
+// order, repeats allowed; rpk_explain_slots).
+func (e *Engine) ExplainSlots(slots []uint32) ([]Explanation, error) {
+	e.mu.Lock()
+	defer e.mu.Unlock()
+	n := len(slots)
+	out := make([]Explanation, n)
+	if n == 0 {
+		return out, nil
+	}
+	rc := C.rpk_explain_slots(e.ctx, C.uint32_t(n), (*C.uint32_t)(unsafe.Pointer(&slots[0])), (*C.rpk_explanation)(unsafe.Pointer(&out[0])))
+	if rc != C.RPK_OK {
+		return nil, lastError(e.ctx, rc)
+	}
+	return out, nil
+}
+
 // PodsMarkPending sets the pending flag of slot slots[i] to pending[i] != 0 (slots strictly ascending): the predicate of
 // processPendingPods (Phase == Pending and no runpod.io/pod-id, kubelet.go:752, :768), kept per slot on the device.
 func (e *Engine) PodsMarkPending(slots []uint32, pending []uint8) error {

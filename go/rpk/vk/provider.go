@@ -78,9 +78,10 @@ type Provider struct {
 	slotKey   []string // slot -> pod key
 	freeSlots []uint32
 
-	seedMutex sync.Mutex // the device pod table and its mirror: one deployBatch seeds and selects at a time
-	seededMem []int32    // maxPods: the columns the device pod table holds per slot
-	seededCld []uint8
+	seedMutex     sync.Mutex // the device pod table and its mirror: one deployBatch seeds and selects at a time
+	seededMem     []int32    // maxPods: the columns the device pod table holds per slot
+	seededCld     []uint8
+	unschedulable map[uint32]string // slot -> key of the pod whose last select returned no GPU type (seedMutex)
 
 	notifyMutex sync.RWMutex
 	notifyFunc  func(*v1.Pod)
@@ -94,7 +95,7 @@ func NewProvider(api RunPodAPI, nGPUs, maxPods int) (*Provider, error) {
 		return nil, fmt.Errorf("rpk engine unavailable (no CPU fallback): %w", err)
 	}
 	p := &Provider{api: api, engine: e, maxPods: maxPods, pods: map[string]*v1.Pod{}, podStatus: map[string]*InstanceInfo{},
-		records: make([]byte, maxPods*stride), slotKey: make([]string, maxPods)}
+		records: make([]byte, maxPods*stride), slotKey: make([]string, maxPods), unschedulable: map[uint32]string{}}
 	for s := maxPods; s > 0; s-- {
 		p.freeSlots = append(p.freeSlots, uint32(s-1))
 	}
@@ -357,6 +358,15 @@ func (p *Provider) deployBatch(keys []string) {
 		p.offers = offers
 	}
 	top5, err := p.seedAndSelect(slots, cols)
+	if err == nil {
+		for i, s := range slots {
+			if top5[i*rpk.TopK] < 0 {
+				p.unschedulable[s] = key(pods[i])
+			} else {
+				delete(p.unschedulable, s)
+			}
+		}
+	}
 	p.seedMutex.Unlock()
 	if err != nil {
 		return
@@ -389,6 +399,107 @@ func (p *Provider) deployBatch(keys []string) {
 		}
 		p.podsMutex.Unlock()
 	}
+}
+
+// Unschedulable is one pending pod that no GPU type fits, and why.
+type Unschedulable struct {
+	Namespace, Name string
+	Why             rpk.Explanation
+	Message         string // UnschedulableMessage
+}
+
+// ExplainUnschedulable lists the pending pods whose last select returned no GPU type, ascending by slot, with what rules
+// out each GPU type for them: one Engine.ExplainSlots over their slots.  It changes nothing the ticks do; the embedding
+// process decides what to do with the explanations (k8s Events, logs).  The C++ twin is Provider::ExplainUnschedulable.
+func (p *Provider) ExplainUnschedulable() []Unschedulable {
+	p.seedMutex.Lock()
+	slots := make([]uint32, 0, len(p.unschedulable))
+	for s := range p.unschedulable {
+		slots = append(slots, s)
+	}
+	sort.Slice(slots, func(a, b int) bool { return slots[a] < slots[b] })
+	keys, rows := make([]string, len(slots)), make([]Requirements, len(slots))
+	for i, s := range slots {
+		keys[i] = p.unschedulable[s]
+		rows[i] = Requirements{MemGb: p.seededMem[s], MaxPrice: rpk.DefaultMaxPrice, Cloud: p.seededCld[s]}
+	}
+	offers := p.offers
+	var why []rpk.Explanation
+	var err error
+	if len(slots) > 0 && offers != nil {
+		why, err = p.engine.ExplainSlots(slots)
+	}
+	p.seedMutex.Unlock()
+	if len(why) == 0 || err != nil {
+		return nil
+	}
+	var out []Unschedulable
+	p.podsMutex.RLock()
+	defer p.podsMutex.RUnlock()
+	for i, s := range slots { // only what is still that pod, still pending
+		pod, ok := p.pods[keys[i]]
+		if !ok || p.slotKey[s] != keys[i] || pod.Status.Phase != v1.PodPending || pod.Annotations[PodIDAnnotation] != "" {
+			continue
+		}
+		out = append(out, Unschedulable{Namespace: pod.Namespace, Name: pod.Name, Why: why[i],
+			Message: UnschedulableMessage(why[i], rows[i], offers)})
+	}
+	return out
+}
+
+// Requirements are the columns of one pod row a message names.
+type Requirements struct {
+	MemGb, VCPU, RAMGb int32
+	MaxPrice           float64
+	Cloud              uint8
+}
+
+// UnschedulableMessage is the scheduler-style text of one explanation, as the C++ twin builds it: "0/{G} GPU types fit: "
+// and the non-zero counts joined by ", ", then "."; then, if any nearest offer exists, " Nearest: " and one hint per
+// requirement joined by "; ", then ".".
+func UnschedulableMessage(why rpk.Explanation, r Requirements, offers *rpk.Offers) string {
+	cloud, prices := "SECURE", offers.SecurePrice
+	if r.Cloud == rpk.CloudCommunity {
+		cloud, prices = "COMMUNITY", offers.CommunityPrice
+	}
+	var parts []string
+	add := func(n uint32, format string, v interface{}) {
+		if n > 0 {
+			parts = append(parts, fmt.Sprintf(format, n, v))
+		}
+	}
+	add(why.NUnoffered, "%d not offered in %s cloud", cloud)
+	add(why.NFail[rpk.ReqPrice], "%d at or above $%.2f/hr", r.MaxPrice)
+	add(why.NFail[rpk.ReqMem], "%d under %d GB GPU memory", r.MemGb)
+	add(why.NFail[rpk.ReqVCPU], "%d under %d vCPUs", r.VCPU)
+	add(why.NFail[rpk.ReqRAM], "%d under %d GB RAM", r.RAMGb)
+	msg := fmt.Sprintf("0/%d GPU types fit: %s.", len(offers.IDs), strings.Join(parts, ", "))
+	col := func(c []int32, g int32) int32 {
+		if c == nil {
+			return 0
+		}
+		return c[g]
+	}
+	var hints []string
+	for req, g := range why.Nearest {
+		if g < 0 || int(g) >= len(offers.IDs) {
+			continue
+		}
+		switch req {
+		case rpk.ReqPrice:
+			hints = append(hints, fmt.Sprintf("%s needs a max price above $%.2f/hr", offers.IDs[g], prices[g]))
+		case rpk.ReqMem:
+			hints = append(hints, fmt.Sprintf("%s has %d GB GPU memory", offers.IDs[g], offers.MemoryInGb[g]))
+		case rpk.ReqVCPU:
+			hints = append(hints, fmt.Sprintf("%s has %d vCPUs", offers.IDs[g], col(offers.VCPU, g)))
+		case rpk.ReqRAM:
+			hints = append(hints, fmt.Sprintf("%s has %d GB RAM", offers.IDs[g], col(offers.RAMGb, g)))
+		}
+	}
+	if len(hints) > 0 {
+		msg += " Nearest: " + strings.Join(hints, "; ") + "."
+	}
+	return msg
 }
 
 // updateAllPodStatuses -- kubelet.go:816-974, batched; see the C++ mirror for the concurrency argument.

@@ -34,7 +34,7 @@
  *     of one scope never overlap, and returns after its own work is done; the caller needs no synchronise between the
  *     two.  Select scope: rpk_offers_upload, rpk_offers_refresh, rpk_pods_reset, rpk_pods_grow,
  *     rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_select, rpk_select_slots, rpk_select_pending,
- *     rpk_select_pending_changed, the _device call
+ *     rpk_select_pending_changed, rpk_explain, rpk_explain_slots, the _device call
  *     rpk_pods_pending_list_device, rpk_select_pending_changed_gather (which also waits on the host),
  *     rpk_select_pending_changed_device_gather, and rpk_tick
  *     with P > 0.  Status scope: rpk_status_diff,
@@ -48,8 +48,8 @@
  *     (rpk_test_capture_buffers lists them) and the values the call read at capture.  Host calls have scratch of their
  *     own, and the _device calls of a shard share one select scratch and one sweep scratch that only _device calls size.
  *     A capture of a _device call on shard s stays valid across:
- *       - every host call, of any size, on any shard (rpk_select, rpk_select_slots, rpk_select_pending*, the host
- *         sweeps, rpk_tick, rpk_status_reset, rpk_status_grow, ...);
+ *       - every host call, of any size, on any shard (rpk_select, rpk_select_slots, rpk_select_pending*, rpk_explain,
+ *         rpk_explain_slots, the host sweeps, rpk_tick, rpk_status_reset, rpk_status_grow, ...);
  *       - the seeds and marks: rpk_pods_seed_slots, rpk_pods_mark_pending, rpk_status_seed, rpk_status_seed_slots (a
  *         replay reads the rows, flags and hashes as they are at replay time);
  *       - _device calls on s that need no more scratch than the calls made on s before the capture.
@@ -215,6 +215,39 @@ int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, c
  * is checked just before its upload).  No pod table or no offer table: RPK_ESTATE.  Counts as one select in rpk_stats
  * (select_calls, offer_scores += n_slots * G).  n_slots == 0 is a no-op. */
 int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int32_t* best, int32_t* top5);
+
+/* ---- explaining an empty gpuTypeIds list ------------------------------------------------------------------- */
+
+/* Why a pod gets no GPU type: for one row, what rules out each offer of the resident table.  An offer is OFFERED to
+ * the row when it passes the cloud check and price > 0 in the row's cloud (a cloud byte other than SECURE or COMMUNITY
+ * offers nothing).  Four requirements are then checked on every offered offer: RPK_REQ_PRICE price < max_price (IEEE:
+ * a NaN bound fails every offer), RPK_REQ_MEM mem_gb >= req_mem_gb, RPK_REQ_VCPU vcpu >= req_vcpu and RPK_REQ_RAM
+ * ram_gb >= req_ram_gb -- rpk_select's predicate, split into its parts.  Invariants: n_unoffered + n_feasible + (the
+ * offered offers failing at least one requirement) == G; n_feasible > 0 exactly when rpk_select's best != -1, and
+ * min(n_feasible, 5) is the length of its top-5 list. */
+#define RPK_REQ_PRICE 0
+#define RPK_REQ_MEM 1
+#define RPK_REQ_VCPU 2
+#define RPK_REQ_RAM 3
+typedef struct rpk_explanation {
+    uint32_t n_feasible;   /* offered offers passing all four: what rpk_select's predicate keeps */
+    uint32_t n_unoffered;  /* G - offered */
+    uint32_t n_fail[4];    /* offered offers failing requirement r (an offer may count under several r) */
+    uint32_t n_only[4];    /* offered offers failing requirement r and no other */
+    int32_t nearest[4];    /* among the n_only[r] offers, the lowest (price in the row's cloud, offer index); -1 if
+                              n_only[r] == 0.  The offer the pod would get if only r were relaxed, whenever n_feasible == 0 */
+} rpk_explanation;
+/* out[i] for pod row i (out: P entries).  Columns, their NULL rules and defaults as rpk_select's.  P == 0 is a no-op.
+ * No offer table: RPK_ESTATE.  On a multi-GPU ctx the rows are split over the GPUs as rpk_select splits them; the result
+ * does not depend on the number of GPUs.  Select scope, host call: it waits for the scope's last _device call, and reads
+ * no stored pending result and writes no pending flag, pod row, change window or rpk_stats counter; its scratch is the
+ * host calls' own, so a captured _device graph stays valid across it. */
+int rpk_explain(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t* req_vcpu, const int32_t* req_ram_gb,
+                const double* max_price, const uint8_t* cloud, rpk_explanation* out);
+/* rpk_explain over rows of the pod table: out[i] is what rpk_explain returns for the row held at slot slots[i].  The
+ * list may be in any order and may repeat a slot.  An entry >= N of the pod table: RPK_EINVAL, before anything is
+ * enqueued.  No pod table or no offer table: RPK_ESTATE.  n_slots == 0 is a no-op.  Otherwise as rpk_explain. */
+int rpk_explain_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, rpk_explanation* out);
 
 /* The pending set: which slots processPendingPods would retry, kept in the table next to the columns, so that a tick
  * sends no list at all.  The set changes as slowly as the columns do: a pod enters it in CreatePod and leaves it when a

@@ -43,6 +43,8 @@ ABI = {
     "rpk_pods_grow": (_int, [_p, _u32]),
     "rpk_pods_seed_slots": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
     "rpk_select_slots": (_int, [_p, _u32, _p, _p, _p]),
+    "rpk_explain": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),
+    "rpk_explain_slots": (_int, [_p, _u32, _p, _p]),
     "rpk_pods_mark_pending": (_int, [_p, _u32, _p, _p]),
     "rpk_select_pending": (_int, [_p, _u32, _p, _p, _p, _p]),
     "rpk_select_pending_changed": (_int, [_p, _u32, _p, _p, _p, _p, _p, _p]),

@@ -408,6 +408,31 @@ void reserve_select(rpk_ctx* ctx, const HostSelect& sel) {
     }
 }
 
+// Rows [b0, b0 + nb) of src as a device source for pod_columns, from row *at on: a host source's rows are uploaded into
+// lane ln's buffers on st (*at = 0; a host list's slot ids must already be checked), a device source is src itself
+// (*at = b0).
+RowSource upload_rows(DeviceState::Lane& ln, const RowSource& src, uint32_t b0, uint32_t nb, cudaStream_t st, uint32_t* at) {
+    *at = 0;
+    if (src.kind == RowSource::HostList) {
+        RPK_CUDA(cudaMemcpyAsync(ln.p_slots.p, src.slots + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
+        return RowSource{RowSource::DevList, PodCols{}, ln.p_slots.p};
+    }
+    if (src.kind == RowSource::HostCols) {
+        const PodCols& pods = src.cols;
+        // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
+        auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
+            if (!col) return nullptr;
+            RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
+            return buf.p;
+        };
+        return RowSource{RowSource::DevCols,
+                         PodCols{upload(ln.p_req_mem, pods.req_mem), upload(ln.p_req_vcpu, pods.req_vcpu), upload(ln.p_req_ram, pods.req_ram),
+                                 upload(ln.p_max_price, pods.max_price), upload(ln.p_cloud, pods.cloud)}, nullptr};
+    }
+    *at = b0;
+    return src;
+}
+
 // One shard's half of the host select: row sub-batches rotate over the lanes; within a lane everything is stream
 // ordered (H2D -> kernels -> D2H), across lanes copies and kernels overlap.  ds.ev[0] / ds.ev[3] bracket it on ds.stream;
 // the caller synchronises ds.stream.  Slot ids are checked per sub-batch just before their upload: false = an entry
@@ -426,23 +451,9 @@ bool enqueue_select_shard(rpk_ctx* ctx, int s, const HostSelect& sel, uint64_t* 
         nb = sub_batch_rows(src.kind, j, hi - b0);
         DeviceState::Lane& ln = ds.lane[j % DeviceState::kLanes];
         cudaStream_t st = ln.stream;
-        RowSource dev = src; uint32_t at = b0;  // the sub-batch's device source and first row: a host source lands in the lane
-        if (src.kind == RowSource::HostList) {
-            if (!slots_below(src.slots + b0, nb, ds.podsN)) { ok = false; break; }
-            RPK_CUDA(cudaMemcpyAsync(ln.p_slots.p, src.slots + b0, (size_t)nb * 4, cudaMemcpyHostToDevice, st));
-            dev = RowSource{RowSource::DevList, PodCols{}, ln.p_slots.p}; at = 0;
-        } else if (src.kind == RowSource::HostCols) {
-            const PodCols& pods = src.cols;
-            // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
-            auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
-                if (!col) return nullptr;
-                RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
-                return buf.p;
-            };
-            dev = RowSource{RowSource::DevCols,
-                            PodCols{upload(ln.p_req_mem, pods.req_mem), upload(ln.p_req_vcpu, pods.req_vcpu), upload(ln.p_req_ram, pods.req_ram),
-                                    upload(ln.p_max_price, pods.max_price), upload(ln.p_cloud, pods.cloud)}, nullptr}; at = 0;
-        }
+        if (src.kind == RowSource::HostList && !slots_below(src.slots + b0, nb, ds.podsN)) { ok = false; break; }
+        uint32_t at;
+        const RowSource dev = upload_rows(ln, src, b0, nb, st, &at);
         SelectArgs a{};
         *launches += (uint64_t)pod_columns(ds, ln, dev, at, nb, a, st);
         a.P = nb;
@@ -702,6 +713,46 @@ int select_device(rpk_ctx* ctx, const char* who, int shard, uint32_t P, const Ro
             ctx->launches += (uint64_t)enqueue_select(ds, ln, a, st, gather_top5 ? &t5 : nullptr);
             count_select(ctx, P, ds.G);
         });
+}
+
+// rpk_explain and rpk_explain_slots once their arguments are checked (`who` names the one called): every GPU explains
+// its contiguous share of the P rows, rpk_select's split, staged in its host lane 0 as a select's rows are, and copies
+// the results into out.  A slot list is checked whole before anything is enqueued.  Counts nothing in rpk_stats.
+int explain_host(rpk_ctx* ctx, uint32_t P, const RowSource& src, rpk_explanation* out, const char* who) {
+    if (src.kind == RowSource::HostList && !slots_below(src.slots, P, ctx->devs[0].podsN))
+        return fail(ctx, RPK_EINVAL, std::string(who) + ": slot index outside the pod table");
+    return guarded(ctx, [&]() -> int {
+        const int n = (int)ctx->devs.size();
+        for (int s = 0; s < n; ++s) {  // sized from the calling thread, behind the scope's last device call
+            DeviceState& ds = ctx->devs[(size_t)s];
+            uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            ds.sel_scope.host_wait();
+            reserve_lane(ds.lane[0], std::max<uint32_t>(hi - lo, 1u), src, false);
+            ds.explain_out.reserve(std::max<uint32_t>(hi - lo, 1u));
+        }
+        std::vector<uint64_t> launches((size_t)n, 0);
+        ctx->workers.run(n, [&](int s) {
+            DeviceState& ds = ctx->devs[(size_t)s];
+            uint32_t lo, hi; shard_range(P, n, s, &lo, &hi);
+            if (lo == hi) return;
+            RPK_CUDA(cudaSetDevice(ds.dev));
+            DeviceState::Lane& ln = ds.lane[0];
+            uint32_t at;
+            const RowSource dev = upload_rows(ln, src, lo, hi - lo, ln.stream, &at);
+            SelectArgs a{};
+            launches[(size_t)s] += (uint64_t)pod_columns(ds, ln, dev, at, hi - lo, a, ln.stream);
+            ExplainArgs e{};
+            e.rows = PodCols{a.req_mem, a.req_vcpu, a.req_ram, a.max_price, a.cloud}; e.P = hi - lo;
+            for (int c = 0; c < 2; ++c) { e.wide[c] = ds.v_wide[c].p; e.price[c] = ds.v_price[c].p; }
+            e.G = ds.G; e.out = ds.explain_out.p;
+            launches[(size_t)s] += (uint64_t)launch_explain(e, ln.stream);
+            RPK_CUDA(cudaMemcpyAsync(out + lo, ds.explain_out.p, (size_t)(hi - lo) * sizeof(rpk_explanation), cudaMemcpyDeviceToHost, ln.stream));
+            RPK_CUDA(cudaStreamSynchronize(ln.stream));
+        });
+        for (uint64_t l : launches) ctx->launches += l;
+        return RPK_OK;
+    });
 }
 
 }  // namespace
@@ -1031,6 +1082,24 @@ int rpk_select_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, int3
     if (int rc = check_select_ready(ctx, "rpk_select_slots", true)) return rc;
     const std::vector<RowSource> rows(ctx->devs.size(), RowSource{RowSource::HostList, PodCols{}, slots});
     return select_host(ctx, HostSelect{n_slots, rows, best, top5}, "rpk_select_slots");
+}
+
+int rpk_explain(rpk_ctx* ctx, uint32_t P, const int32_t* req_mem_gb, const int32_t* req_vcpu, const int32_t* req_ram_gb,
+                const double* max_price, const uint8_t* cloud, rpk_explanation* out) {
+    if (!ctx) return RPK_EINVAL;
+    if (P == 0) return RPK_OK;
+    if (!req_mem_gb || !out) return fail(ctx, RPK_EINVAL, "rpk_explain: req_mem_gb and out are required");
+    if (int rc = check_select_ready(ctx, "rpk_explain", false)) return rc;
+    const RowSource rows{RowSource::HostCols, PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, nullptr};
+    return explain_host(ctx, P, rows, out, "rpk_explain");
+}
+
+int rpk_explain_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, rpk_explanation* out) {
+    if (!ctx) return RPK_EINVAL;
+    if (n_slots == 0) return RPK_OK;
+    if (!slots || !out) return fail(ctx, RPK_EINVAL, "rpk_explain_slots: slots and out are required");
+    if (int rc = check_select_ready(ctx, "rpk_explain_slots", true)) return rc;
+    return explain_host(ctx, n_slots, RowSource{RowSource::HostList, PodCols{}, slots}, out, "rpk_explain_slots");
 }
 
 int rpk_select_slots_device_gather(rpk_ctx* ctx, int shard, uint32_t n_slots, const uint32_t* d_slots, int n_out,

@@ -368,6 +368,14 @@ int launch_pod_stale_reach(const StaleReachArgs& a, uint32_t n_units, int sm_cou
 int launch_pod_result_xchg(const ResultXchgArgs& x, const uint32_t* d_n, uint32_t n_max, int sm_count, cudaStream_t st);
 int launch_status_seed_slots(uint32_t n, const uint32_t* d_slots, const uint8_t* d_records, uint32_t stride, uint64_t* hash_prev,
                              uint32_t lo, uint32_t hi, cudaStream_t st);
+// rpk_explain (explain.cu): out[i] for pod row i of the columns (req_mem required, the others nullable with rpk_select's
+// defaults) against the two cloud views wide / price of a G-offer table
+struct ExplainArgs {
+    PodCols rows; uint32_t P;
+    const int4* wide[2]; const double* price[2]; uint32_t G;
+    rpk_explanation* out;
+};
+int launch_explain(const ExplainArgs& a, cudaStream_t st);
 
 template <typename T>
 struct DevBuf {  // grow-only device buffer, freed by its destructor
@@ -506,6 +514,7 @@ struct DeviceState {
     SweepScratch sweep, dev_sweep;
     DevBuf<uint32_t> s_seed_slots; DevBuf<uint8_t> s_seed_recs;  // slot lists of rpk_status_seed_slots and rpk_status_diff_slots
     PinnedBuf h_changed;                   // the host sweep's changed list: count, indices, codes
+    DevBuf<rpk_explanation> explain_out;   // rpk_explain*: the shard's rows, copied to the caller (host-call scratch)
     cudaStream_t status_stream = nullptr;  // rpk_tick: the sweep next to the selection
     ScratchScope sel_scope, status_scope;  // the offer views, the pod table and dev_lane; dev_sweep
     uint32_t statusN = 0; bool status_sized = false;

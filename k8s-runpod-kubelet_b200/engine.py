@@ -74,6 +74,16 @@ def results_region(words, n_ranks: int, cap: int, rank: int):
     return r[:n].view(np.uint32).copy(), r[cap:cap + n].copy(), r[2 * cap:2 * cap + 5 * n].reshape(n, 5).copy()
 
 
+EXPLAIN_WORDS = 14  # uint32 words of one rpk_explanation
+
+
+def explanation_fields(raw):
+    """rpk_explanation structs as P * 14 uint32 words -> the dict ``Engine.explain`` returns (views of ``raw``)"""
+    w = raw.reshape(-1, EXPLAIN_WORDS)
+    return {"n_feasible": w[:, 0], "n_unoffered": w[:, 1], "n_fail": w[:, 2:6], "n_only": w[:, 6:10],
+            "nearest": w[:, 10:14].view(np.int32)}
+
+
 class Engine:
     """One ``rpk_ctx``.  ``n_gpus > 1`` = one process driving several GPUs (the Go kubelet's shape)."""
 
@@ -234,6 +244,30 @@ class Engine:
             self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(best, np.int32, n, "best"),
             _np_ptr(top5, np.int32, n * 5, "top5") if top5 is not None else None))
         return best, top5
+
+    # -- explaining an empty gpuTypeIds list ----------------------------------------------------------------
+    def explain(self, pods: dict, out=None):
+        """Host columns in (as ``select`` takes them), what rules out each offer per row out (rpk_explain): a dict of numpy
+        arrays ``n_feasible[P]``, ``n_unoffered[P]``, ``n_fail[P,4]``, ``n_only[P,4]``, ``nearest[P,4]`` (requirement
+        order RPK_REQ_PRICE, _MEM, _VCPU, _RAM).  ``out``: optional uint32 array of P * 14 words the call writes into (the
+        C structs, row after row); the returned arrays are views of it."""
+        P = int(pods["req_mem_gb"].shape[0])
+        raw = out if out is not None else np.empty(P * EXPLAIN_WORDS, np.uint32)
+        self._check(self._lib.rpk_explain(
+            self._ctx, P, _np_ptr(pods["req_mem_gb"], np.int32, P, "req_mem_gb"), _np_ptr(pods.get("req_vcpu"), np.int32, P, "req_vcpu"),
+            _np_ptr(pods.get("req_ram_gb"), np.int32, P, "req_ram_gb"), _np_ptr(pods.get("max_price"), np.float64, P, "max_price"),
+            _np_ptr(pods.get("cloud"), np.uint8, P, "cloud"), _np_ptr(raw, np.uint32, P * EXPLAIN_WORDS, "out")))
+        return explanation_fields(raw)
+
+    def explain_slots(self, slots: np.ndarray, out=None):
+        """``explain`` over rows of the pod table: the rows held at ``slots`` (any order, repeats allowed;
+        rpk_explain_slots)."""
+        slots = np.ascontiguousarray(slots, np.uint32)  # keep the converted array alive across the call
+        n = int(slots.size)
+        raw = out if out is not None else np.empty(n * EXPLAIN_WORDS, np.uint32)
+        self._check(self._lib.rpk_explain_slots(
+            self._ctx, n, _np_ptr(slots, np.uint32, n, "slots"), _np_ptr(raw, np.uint32, n * EXPLAIN_WORDS, "out")))
+        return explanation_fields(raw)
 
     def pods_mark_pending(self, slots: np.ndarray, pending: np.ndarray):
         """Pending flag of slot slots[i] := pending[i] != 0 (slots strictly ascending; rpk_pods_mark_pending)."""

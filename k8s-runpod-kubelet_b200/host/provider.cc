@@ -4,6 +4,7 @@
 #include <cctype>
 #include <cerrno>
 #include <climits>
+#include <cstdio>
 #include <cstdlib>
 #include <chrono>
 #include <cstring>
@@ -770,6 +771,78 @@ void Provider::ProcessPendingPods() {
         }
         Notify(failed);
     }
+}
+
+std::string UnschedulableMessage(const rpk_explanation& why, uint32_t G, const PodColumns& row, const std::vector<GPUType>& offers) {
+    const bool community = row.cloud == RPK_CLOUD_COMMUNITY;
+    char buf[160];
+    std::string parts;
+    auto part = [&](uint32_t n, const char* fmt, auto v) {
+        if (n == 0) return;
+        snprintf(buf, sizeof(buf), fmt, n, v);
+        parts += (parts.empty() ? "" : ", ") + std::string(buf);
+    };
+    part(why.n_unoffered, "%u not offered in %s cloud", community ? "COMMUNITY" : "SECURE");
+    part(why.n_fail[RPK_REQ_PRICE], "%u at or above $%.2f/hr", row.max_price);
+    part(why.n_fail[RPK_REQ_MEM], "%u under %d GB GPU memory", row.req_mem_gb);
+    part(why.n_fail[RPK_REQ_VCPU], "%u under %d vCPUs", row.req_vcpu);
+    part(why.n_fail[RPK_REQ_RAM], "%u under %d GB RAM", row.req_ram_gb);
+    snprintf(buf, sizeof(buf), "0/%u GPU types fit: ", G);
+    std::string msg = buf + parts + ".";
+    std::string hints;
+    for (int r = 0; r < 4; ++r) {
+        const int32_t g = why.nearest[r];
+        if (g < 0 || (size_t)g >= offers.size()) continue;
+        const GPUType& t = offers[(size_t)g];
+        if (r == RPK_REQ_PRICE) snprintf(buf, sizeof(buf), " needs a max price above $%.2f/hr", community ? t.CommunityPrice : t.SecurePrice);
+        if (r == RPK_REQ_MEM) snprintf(buf, sizeof(buf), " has %d GB GPU memory", t.MemoryInGb);
+        if (r == RPK_REQ_VCPU) snprintf(buf, sizeof(buf), " has %d vCPUs", t.VCPU);
+        if (r == RPK_REQ_RAM) snprintf(buf, sizeof(buf), " has %d GB RAM", t.RAMGb);
+        hints += (hints.empty() ? "" : "; ") + t.ID + buf;
+    }
+    if (!hints.empty()) msg += " Nearest: " + hints + ".";
+    return msg;
+}
+
+// The pods the last pending tick left without a GPU type: flagged slots whose mirrored list is empty.  The slots are
+// read under pods_mutex_, explained and resolved against offers_ under engine_mutex_ (never both at once), and a pod
+// whose slot was taken over meanwhile, or that is no longer pending, is dropped.
+std::vector<Unschedulable> Provider::ExplainUnschedulable() {
+    std::vector<std::pair<uint32_t, std::string>> tracked;  // (slot, key)
+    {
+        std::lock_guard<std::mutex> g(pods_mutex_);
+        for (const auto& kv : pods_) tracked.emplace_back(kv.second.slot, kv.first);
+    }
+    std::sort(tracked.begin(), tracked.end());
+    std::vector<Unschedulable> out;
+    std::vector<std::string> keys;
+    std::vector<uint32_t> slots;
+    {
+        std::lock_guard<std::mutex> g(engine_mutex_);
+        for (const auto& t : tracked) {
+            if ((size_t)t.first >= marked_.size() || !marked_[t.first] || lists_[(size_t)t.first * RPK_TOPK] >= 0) continue;
+            slots.push_back(t.first); keys.push_back(t.second);
+        }
+        if (slots.empty()) return out;
+        std::vector<rpk_explanation> why(slots.size());
+        if (rpk_explain_slots(ctx_, (uint32_t)slots.size(), slots.data(), why.data()) != RPK_OK) return out;
+        for (size_t i = 0; i < slots.size(); ++i) {
+            const uint32_t s = slots[i];
+            const PodColumns row{seeded_.req_mem_gb[s], seeded_.req_vcpu[s], seeded_.req_ram_gb[s], seeded_.max_price[s], seeded_.cloud[s], ""};
+            out.push_back(Unschedulable{"", "", why[i], UnschedulableMessage(why[i], (uint32_t)offers_.size(), row, offers_)});
+        }
+    }
+    std::vector<Unschedulable> kept;
+    std::lock_guard<std::mutex> g(pods_mutex_);
+    for (size_t i = 0; i < out.size(); ++i) {
+        auto it = pods_.find(keys[i]);
+        // still that pod, and still pending: the flags and lists only catch up at the next tick, so a pod failed at 15
+        // minutes, deployed, or replaced in a reused slot since the last tick is not listed
+        if (it == pods_.end() || it->second.slot != slots[i] || slot_key_[slots[i]] != keys[i] || !IsPending(*it->second.pod)) continue;
+        out[i].ns = it->second.pod->ns; out[i].name = it->second.pod->name;
+        kept.push_back(std::move(out[i]));
+    }
+    return kept;
 }
 
 // Re-encode every tracked slot at a wider stride (a status string longer than the slot appeared).  Called with

@@ -154,6 +154,19 @@ struct PodColumnsSoA {
 // the GPU -- is what a tick costs: see host_test --bench-columns and DESIGN.md section 8.
 void PrepareColumnsBatch(const std::vector<PodPtr>& pods, PodColumnsSoA* out, int n_threads = 0);
 
+// ---- explaining unschedulable pods --------------------------------------------------------------------------
+// A pending pod that no GPU type fits, and why (rpk_explain_slots on its pod-table row)
+struct Unschedulable {
+    std::string ns, name;
+    rpk_explanation why;
+    std::string message;  // UnschedulableMessage
+};
+// The scheduler-style message of one explanation: "0/{G} GPU types fit: " and the counts of the requirements that rule
+// offers out (joined by ", ", each only when non-zero), then "."; then, if any nearest[r] >= 0, " Nearest: " and one
+// hint per such r in requirement order (joined by "; "), then ".".  Counts name the row's cloud and requirements; hints
+// name the GPUType (offers[nearest[r]]) and its price in the row's cloud, memory, vCPUs or RAM.
+std::string UnschedulableMessage(const rpk_explanation& why, uint32_t G, const PodColumns& row, const std::vector<GPUType>& offers);
+
 // ---- Provider ----------------------------------------------------------------------------------------------
 struct ProviderOptions {
     // The reference drives itself: NewProvider starts a 30 s status poll and a 30 s pending-pod processor
@@ -184,6 +197,11 @@ public:
     // the two ticker bodies, batched
     void ProcessPendingPods();     // kubelet.go:747-814
     void UpdateAllPodStatuses();   // kubelet.go:816-974
+    // Every tracked pod that is still pending, whose slot the last pending tick flagged and whose gpuTypeIds list came back
+    // empty, ascending by slot, with what rules out each GPU type for it (one rpk_explain_slots over those slots).  Changes nothing: the
+    // ticks, deploys, statuses and notifications are those of a Provider that never calls it.  What to do with the
+    // explanations (k8s Events, logs) is the embedding process's choice.
+    std::vector<Unschedulable> ExplainUnschedulable();
 
     // observability for tests / the benchmark harness
     const InstanceInfo* Info(const std::string& ns, const std::string& name);

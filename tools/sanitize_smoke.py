@@ -37,6 +37,15 @@ if not ONLY_MULTI:
         best, t5 = eng.select_slots(sl, want_top5=True)
         ob, ot = oracle.select(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, n_threads=8)
         assert np.array_equal(best, ob) and np.array_equal(t5, ot), n
+    # explain (k_explain): rows of both clouds and of neither, a partial last tile, columns and slots
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tests"))
+    import explain_model  # noqa: E402
+    few = {k: v[:3001].copy() for k, v in pods.items()}  # a copy: the checks below still read the seeded rows
+    few["cloud"][::97] = 2
+    explain_model.assert_same(eng.explain(few), explain_model.explain(offers, few, 8), "explain")
+    sl = np.random.default_rng(3).integers(0, 200_000, 37).astype(np.uint32)
+    explain_model.assert_same(eng.explain_slots(sl), explain_model.explain(offers, {k: np.ascontiguousarray(v[sl]) for k, v in pods.items()}, 8),
+                              "explain_slots")
     # the pending set: mark, then the select over the list the device builds (k_pod_mark, k_pod_pending: latency path
     # and pipelined path)
     for n in (37, 140_000):
