@@ -189,30 +189,34 @@ bool slots_below(const uint32_t* slots, uint32_t n, uint32_t N) {
 // The buffers of lane ln that a select of `rows` rows from src writes: the pod columns it uploads or gathers, a host list's
 // slot ids, the top-5 lists.  Allocates only when one grows, so a device call stays capturable after a call of its size.
 void reserve_lane(DeviceState::Lane& ln, size_t rows, const RowSource& src, bool top5) {
-    if (src.kind != RowSource::DevCols) {
-        const bool all = src.kind != RowSource::HostCols;  // a list's gather writes all five
-        ln.p_req_mem.reserve(rows);
-        if (all || src.cols.req_vcpu) ln.p_req_vcpu.reserve(rows);
-        if (all || src.cols.req_ram) ln.p_req_ram.reserve(rows);
-        if (all || src.cols.max_price) ln.p_max_price.reserve(rows);
-        if (all || src.cols.cloud) ln.p_cloud.reserve(rows);
-    }
+    // a list's gather writes all five columns, host columns only the ones passed
+    if (src.kind != RowSource::DevCols) ln.cols.reserve(rows, src.kind == RowSource::HostCols ? &src.cols : nullptr);
     if (src.kind == RowSource::HostList) ln.p_slots.reserve(rows);
     if (top5) ln.top5.reserve(rows * RPK_TOPK);
+}
+
+// SelectArgs keeps its pod columns flat for the kernels: set them to c from row b0 on (null stays null), and read them back
+void set_pod_cols(SelectArgs& a, const PodCols& c, uint32_t b0 = 0) {
+    const auto at = [b0](auto* col) { return col ? col + b0 : nullptr; };
+    a.req_mem = at(c.req_mem); a.req_vcpu = at(c.req_vcpu); a.req_ram = at(c.req_ram); a.max_price = at(c.max_price); a.cloud = at(c.cloud);
+}
+PodCols pod_cols(const SelectArgs& a) { return PodCols{a.req_mem, a.req_vcpu, a.req_ram, a.max_price, a.cloud}; }
+
+// Host columns c on the device: put(col, to.x) copies each passed column col to to.x (a lane's buffer, a staging offset)
+template <typename To, typename Put> PodCols to_device(const PodCols& c, To& to, Put&& put) {
+    const auto at = [&](const auto* col, auto& dst) -> decltype(col) { return col ? (decltype(col))put(col, dst) : nullptr; };
+    return PodCols{at(c.req_mem, to.mem), at(c.req_vcpu, to.vcpu), at(c.req_ram, to.ram), at(c.max_price, to.max_price), at(c.cloud, to.cloud)};
 }
 
 // a's pod columns: rows [b0, b0 + n) of the device source src.  Columns go in as pointers; a list is gathered from the
 // pod table into lane ln's columns on st.  Returns the kernels launched.
 int pod_columns(DeviceState& ds, DeviceState::Lane& ln, const RowSource& src, uint32_t b0, uint32_t n, SelectArgs& a, cudaStream_t st) {
     if (src.kind == RowSource::DevCols) {
-        const PodCols& c = src.cols;
-        auto at = [b0](auto* col) { return col ? col + b0 : nullptr; };  // null stays null
-        a.req_mem = at(c.req_mem); a.req_vcpu = at(c.req_vcpu); a.req_ram = at(c.req_ram); a.max_price = at(c.max_price); a.cloud = at(c.cloud);
+        set_pod_cols(a, src.cols, b0);
         return 0;
     }
-    const PodRows out{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
-    a.req_mem = out.mem; a.req_vcpu = out.vcpu; a.req_ram = out.ram; a.max_price = out.max_price; a.cloud = out.cloud;
-    return launch_pod_gather(ds.pods_table(), ds.podsN, n, src.slots + b0, out, st);
+    set_pod_cols(a, ln.cols.cols());
+    return launch_pod_gather(ds.pods_table(), ds.podsN, n, src.slots + b0, ln.cols.rows(), st);
 }
 
 // One select on ds in lane ln's scratch: `a` holds the pod columns, P and the outputs; this adds the offer views and the
@@ -332,6 +336,13 @@ inline uint32_t sub_batch_cap(RowSource::Kind kind, uint32_t Ps) {  // largest s
     return cap ? cap : 1;
 }
 
+// Where n pod rows go in a staging block from byte `base` on: [mem][vcpu][ram][max_price, 8-byte aligned][cloud], then its end
+struct PodBlock { size_t mem, vcpu, ram, max_price, cloud, end; };
+PodBlock pod_block(size_t n, size_t base) {
+    const size_t price = (base + 12 * n + 7) & ~(size_t)7;
+    return PodBlock{base, base + 4 * n, base + 8 * n, price, price + 8 * n, price + 9 * n};
+}
+
 // Latency path of the host entry point (micro-batches, one GPU): the five pod columns -- or, from the pod table, the
 // slot ids -- are packed into one pinned block -> ONE H2D (then the gather, for slots); best and top5 come back in ONE
 // D2H; one stream synchronise.  Same kernels.  Slot ids are in range here.  Returns the kernels launched.
@@ -352,18 +363,10 @@ int select_small(DeviceState& ds, uint32_t P, const RowSource& src, int32_t* bes
         memcpy(h, src.slots, bytes);
         dev = RowSource{RowSource::DevList, PodCols{}, (const uint32_t*)d};
     } else if (src.kind == RowSource::HostCols) {
-        const PodCols& pods = src.cols;
-        const size_t o_mem = 0, o_vcpu = (size_t)P * 4, o_ram = (size_t)P * 8, o_price = ((size_t)P * 12 + 7) & ~(size_t)7,
-                     o_cloud = o_price + (size_t)P * 8;
-        bytes = o_cloud + P;
-        // a column into the block at offset o; null stays null
-        auto pack = [&](const auto* col, size_t o) -> decltype(col) {
-            if (!col) return nullptr;
-            memcpy(h + o, col, (size_t)P * sizeof(*col));
-            return (decltype(col))(d + o);
-        };
-        dev = RowSource{RowSource::DevCols, PodCols{pack(pods.req_mem, o_mem), pack(pods.req_vcpu, o_vcpu), pack(pods.req_ram, o_ram),
-                                                    pack(pods.max_price, o_price), pack(pods.cloud, o_cloud)}, nullptr};
+        const PodBlock blk = pod_block(P, 0);
+        bytes = blk.end;
+        const auto pack = [&](const auto* col, size_t o) { memcpy(h + o, col, (size_t)P * sizeof(*col)); return d + o; };
+        dev = RowSource{RowSource::DevCols, to_device(src.cols, blk, pack), nullptr};
     }
     reserve_lane(ln, kSmallBatch, dev, false);
     if (bytes) RPK_CUDA(cudaMemcpyAsync(d, h, bytes, cudaMemcpyHostToDevice, st));
@@ -418,16 +421,11 @@ RowSource upload_rows(DeviceState::Lane& ln, const RowSource& src, uint32_t b0, 
         return RowSource{RowSource::DevList, PodCols{}, ln.p_slots.p};
     }
     if (src.kind == RowSource::HostCols) {
-        const PodCols& pods = src.cols;
-        // rows [b0, b0 + nb) of a column into the lane's buffer; null stays null
-        auto upload = [&](auto& buf, const auto* col) -> decltype(buf.p) {
-            if (!col) return nullptr;
+        const auto upload = [&](const auto* col, auto& buf) {  // rows [b0, b0 + nb) into the lane's buffer
             RPK_CUDA(cudaMemcpyAsync(buf.p, col + b0, (size_t)nb * sizeof(*col), cudaMemcpyHostToDevice, st));
             return buf.p;
         };
-        return RowSource{RowSource::DevCols,
-                         PodCols{upload(ln.p_req_mem, pods.req_mem), upload(ln.p_req_vcpu, pods.req_vcpu), upload(ln.p_req_ram, pods.req_ram),
-                                 upload(ln.p_max_price, pods.max_price), upload(ln.p_cloud, pods.cloud)}, nullptr};
+        return RowSource{RowSource::DevCols, to_device(src.cols, ln.cols, upload), nullptr};
     }
     *at = b0;
     return src;
@@ -743,7 +741,7 @@ int explain_host(rpk_ctx* ctx, uint32_t P, const RowSource& src, rpk_explanation
             SelectArgs a{};
             launches[(size_t)s] += (uint64_t)pod_columns(ds, ln, dev, at, hi - lo, a, ln.stream);
             ExplainArgs e{};
-            e.rows = PodCols{a.req_mem, a.req_vcpu, a.req_ram, a.max_price, a.cloud}; e.P = hi - lo;
+            e.rows = pod_cols(a); e.P = hi - lo;
             for (int c = 0; c < 2; ++c) { e.wide[c] = ds.v_wide[c].p; e.price[c] = ds.v_price[c].p; }
             e.G = ds.G; e.out = ds.explain_out.p;
             launches[(size_t)s] += (uint64_t)launch_explain(e, ln.stream);
@@ -753,6 +751,40 @@ int explain_host(rpk_ctx* ctx, uint32_t P, const RowSource& src, rpk_explanation
         for (uint64_t l : launches) ctx->launches += l;
         return RPK_OK;
     });
+}
+
+struct SlotRange { uint32_t lo, hi; };
+
+// Columns sharded by slot range move from the old ranges `was` to the new ones `now`.  grow(s) is GPU s's Grow of them (a
+// buffer or a PodBufs; a slot is per_slot elements of each column): every slot of was[s] is copied from s's old column
+// into the new one of the shard d whose new range holds it, on d's stream (a peer copy between GPUs).  A shard whose
+// column is the one it had (same buffer, same first slot) keeps its slots in place; its new range then holds all of
+// them, as a range with the same first slot only grows.
+template <typename GrowOf>
+void move_slots(rpk_ctx* ctx, const std::vector<SlotRange>& was, const std::vector<SlotRange>& now, GrowOf&& grow, size_t per_slot) {
+    const size_t n = ctx->devs.size();
+    for (size_t d = 0; d < n; ++d) {
+        DeviceState& dd = ctx->devs[d];
+        RPK_CUDA(cudaSetDevice(dd.dev));
+        for (size_t s = 0; s < n; ++s) {
+            const uint32_t lo = std::max(was[s].lo, now[d].lo), hi = std::min(was[s].hi, now[d].hi);
+            grow(s).each([&](auto& src, auto*, auto& to, auto& to_fresh) {
+                auto* dst = to_fresh.p ? to_fresh.p : to.p;
+                const size_t bytes = per_slot * sizeof(*dst);
+                if (lo >= hi || src.p == dst) return;
+                RPK_CUDA(cudaMemcpyPeerAsync(reinterpret_cast<char*>(dst) + (size_t)(lo - now[d].lo) * bytes, dd.dev,
+                                             reinterpret_cast<const char*>(src.p) + (size_t)(lo - was[s].lo) * bytes, ctx->devs[s].dev,
+                                             (size_t)(hi - lo) * bytes, dd.stream));
+            }, *grow(d).b, grow(d).fresh);
+        }
+    }
+}
+
+void sync_all(rpk_ctx* ctx) {
+    for (auto& ds : ctx->devs) {
+        RPK_CUDA(cudaSetDevice(ds.dev));
+        RPK_CUDA(cudaStreamSynchronize(ds.stream));
+    }
 }
 
 }  // namespace
@@ -904,6 +936,7 @@ int install_offers(rpk_ctx* ctx, const char* who, bool refresh, uint32_t G, cons
     if (G > (1u << 26)) return fail(ctx, RPK_EINVAL, std::string(who) + ": G above 2^26 offers is not supported");
     if (has_int32_max(mem_gb, G) || has_int32_max(vcpu, G) || has_int32_max(ram_gb, G))
         return fail(ctx, RPK_EINVAL, std::string(who) + ": offer columns must be < INT32_MAX (requests saturate there)");
+    const OfferIngest host{G, mem_gb, vcpu, ram_gb, secure_price, community_price, flags};
     bool diff = refresh;
     for (const auto& ds : ctx->devs) diff = diff && ds.offers_ready && ds.G == G;
     if (!diff) invalidate_results(ctx);
@@ -921,22 +954,12 @@ int install_offers(rpk_ctx* ctx, const char* who, bool refresh, uint32_t G, cons
                 else if (!strcmp(fk, "bitmap_grouped")) ds.force_kind = 5;  // every batch size through the persistent kernel
                 else if (!strcmp(fk, "bitmap_price")) ds.force_kind = 6;    // ... through the persistent kernel, table staged by price
             }
-            const size_t n = G ? G : 1;
-            // the new columns go to raw_* (upload) or new_* (diff); after the diff new_* become raw_*
-            DevBuf<int32_t>& c_mem = diff ? ds.new_mem : ds.raw_mem; DevBuf<int32_t>& c_vcpu = diff ? ds.new_vcpu : ds.raw_vcpu;
-            DevBuf<int32_t>& c_ram = diff ? ds.new_ram : ds.raw_ram; DevBuf<double>& c_sp = diff ? ds.new_sp : ds.raw_sp;
-            DevBuf<double>& c_cp = diff ? ds.new_cp : ds.raw_cp; DevBuf<uint8_t>& c_flags = diff ? ds.new_flags : ds.raw_flags;
-            c_mem.reserve(n); c_vcpu.reserve(n); c_ram.reserve(n); c_sp.reserve(n); c_cp.reserve(n); c_flags.reserve(n);
-            if (G) {
-                RPK_CUDA(cudaMemcpyAsync(c_mem.p, mem_gb, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
-                if (vcpu) RPK_CUDA(cudaMemcpyAsync(c_vcpu.p, vcpu, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
-                else RPK_CUDA(cudaMemsetAsync(c_vcpu.p, 0, (size_t)G * 4, ds.stream));
-                if (ram_gb) RPK_CUDA(cudaMemcpyAsync(c_ram.p, ram_gb, (size_t)G * 4, cudaMemcpyHostToDevice, ds.stream));
-                else RPK_CUDA(cudaMemsetAsync(c_ram.p, 0, (size_t)G * 4, ds.stream));
-                RPK_CUDA(cudaMemcpyAsync(c_sp.p, secure_price, (size_t)G * 8, cudaMemcpyHostToDevice, ds.stream));
-                RPK_CUDA(cudaMemcpyAsync(c_cp.p, community_price, (size_t)G * 8, cudaMemcpyHostToDevice, ds.stream));
-                RPK_CUDA(cudaMemcpyAsync(c_flags.p, flags, (size_t)G, cudaMemcpyHostToDevice, ds.stream));
-            }
+            OfferBufs& c = diff ? ds.raw_next : ds.raw;  // after the diff, raw_next becomes raw
+            OfferBufs::each(c, [G](auto& b) { b.reserve(G ? G : 1); });
+            if (G) OfferBufs::each(c, [&](auto& b, const auto* col) {  // the caller's columns; vcpu and ram: zeros when not passed
+                if (col) RPK_CUDA(cudaMemcpyAsync(b.p, col, (size_t)G * sizeof(*col), cudaMemcpyHostToDevice, ds.stream));
+                else RPK_CUDA(cudaMemsetAsync(b.p, 0, (size_t)G * sizeof(*col), ds.stream));
+            }, host);
             if (diff) {
                 if (!ds.delta_state.p) {  // zero between calls: the diff's last CTA clears it again
                     ds.delta_state.reserve(2); ds.delta_idx.reserve(RPK_OFFERS_DELTA_MAX);
@@ -944,15 +967,11 @@ int install_offers(rpk_ctx* ctx, const char* who, bool refresh, uint32_t G, cons
                 }
                 ds.h_delta.reserve(4 * (1 + RPK_OFFERS_DELTA_MAX));
                 *reinterpret_cast<volatile uint32_t*>(ds.h_delta.h) = 0u;
-                const OfferDiffArgs da{OfferIngest{G, ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p},
-                                       OfferIngest{G, c_mem.p, c_vcpu.p, c_ram.p, c_sp.p, c_cp.p, c_flags.p},
-                                       ds.delta_state.p, ds.delta_idx.p, reinterpret_cast<uint32_t*>(ds.h_delta.d)};
+                const OfferDiffArgs da{ds.raw.view(G), c.view(G), ds.delta_state.p, ds.delta_idx.p, reinterpret_cast<uint32_t*>(ds.h_delta.d)};
                 ctx->launches += (uint64_t)launch_offer_diff(da, ds.stream);
-                ds.raw_mem.swap(ds.new_mem); ds.raw_vcpu.swap(ds.new_vcpu); ds.raw_ram.swap(ds.new_ram);
-                ds.raw_sp.swap(ds.new_sp); ds.raw_cp.swap(ds.new_cp); ds.raw_flags.swap(ds.new_flags);
+                ds.raw.swap(ds.raw_next);
             }
-            OfferIngest in{G, ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p};
-            ctx->launches += (uint64_t)launch_offer_ingest(ds, in, ds.stream);
+            ctx->launches += (uint64_t)launch_offer_ingest(ds, ds.raw.view(G), ds.stream);
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
         }
         if (diff) changed = merge_window(ctx);
@@ -1022,7 +1041,7 @@ int rpk_pods_reset(rpk_ctx* ctx, uint32_t N) {
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();  // a device select may still gather from the table
             const size_t cap = N ? N : 1;
-            ds.pt_mem.reserve(cap); ds.pt_vcpu.reserve(cap); ds.pt_ram.reserve(cap); ds.pt_max_price.reserve(cap); ds.pt_cloud.reserve(cap);
+            ds.pt_cols.reserve(cap);
             ds.pt_pending.reserve(cap);
             ctx->launches += (uint64_t)launch_pod_fill(ds.pods_table(), ds.pt_pending.p, N, ds.sm_count, ds.stream);
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
@@ -1051,23 +1070,17 @@ int rpk_pods_seed_slots(rpk_ctx* ctx, uint32_t n_slots, const uint32_t* slots, c
     if (int rc = check_select_ready(ctx, "rpk_pods_seed_slots", true, -1, false)) return rc;
     if (int rc = check_slots(ctx, n_slots, slots, ctx->devs[0].podsN, true, "rpk_pods_seed_slots", "pod table")) return rc;
     return guarded(ctx, [&]() -> int {
-        // staging block: [slots : 4n][mem : 4n][vcpu : 4n][ram : 4n][max_price : 8n, 8-byte aligned][cloud : n]
-        const size_t n = n_slots, o_mem = 4 * n, o_vcpu = 8 * n, o_ram = 12 * n, o_price = (16 * n + 7) & ~(size_t)7,
-                     o_cloud = o_price + 8 * n;
+        // staging block: [slots : 4n], then the rows
+        const size_t n = n_slots;
+        const PodBlock blk = pod_block(n, 4 * n);
         for (auto& ds : ctx->devs) {  // the table is replicated: every GPU gets every row
             RPK_CUDA(cudaSetDevice(ds.dev));
             ds.sel_scope.host_wait();  // after a device select's gather
-            ds.pt_seed.reserve(o_cloud + n);
+            ds.pt_seed.reserve(blk.end);
             unsigned char* d = ds.pt_seed.p;
-            auto up = [&](size_t off, const void* col, size_t bytes) -> const unsigned char* {
-                if (!col) return nullptr;
-                RPK_CUDA(cudaMemcpyAsync(d + off, col, bytes, cudaMemcpyHostToDevice, ds.stream));
-                return d + off;
-            };
-            const uint32_t* d_slots = (const uint32_t*)up(0, slots, 4 * n);
-            const PodCols in{(const int32_t*)up(o_mem, req_mem_gb, 4 * n), (const int32_t*)up(o_vcpu, req_vcpu, 4 * n),
-                             (const int32_t*)up(o_ram, req_ram_gb, 4 * n), (const double*)up(o_price, max_price, 8 * n),
-                             (const uint8_t*)up(o_cloud, cloud, n)};
+            const auto up = [&](const auto* col, size_t o) { RPK_CUDA(cudaMemcpyAsync(d + o, col, n * sizeof(*col), cudaMemcpyHostToDevice, ds.stream)); return d + o; };
+            const uint32_t* d_slots = (const uint32_t*)up(slots, 0);
+            const PodCols in = to_device(PodCols{req_mem_gb, req_vcpu, req_ram_gb, max_price, cloud}, blk, up);
             ctx->launches += (uint64_t)launch_pod_seed(ds.pods_table(), ds.podsN, n_slots, d_slots, in, ds.stream);
             RPK_CUDA(cudaStreamSynchronize(ds.stream));
         }
@@ -1246,7 +1259,7 @@ void result_range(uint32_t N, int n, int s, uint32_t* lo, uint32_t* hi) {
 void reserve_results(DeviceState& ds, uint32_t lo, uint32_t hi, int n_ranks, int my_rank) {
     if (ds.res_ready) return;
     const size_t n = ((size_t)(hi - lo) + 15) / 16 * 16 + 16;  // whole units: k_pod_stale loads 16 slots at a time
-    ds.r_mem.reserve(n); ds.r_vcpu.reserve(n); ds.r_ram.reserve(n); ds.r_max_price.reserve(n); ds.r_cloud.reserve(n);
+    ds.r_cols.reserve(n);
     ds.r_gen.reserve(n); ds.r_top5.reserve(n * RPK_TOPK); ds.r_list.reserve(n); ds.r_mask.reserve(n / 16 + 1); ds.r_dn.reserve(2);
     reserve_lane(ds.r_lane, std::max<uint32_t>(hi - lo, 1u), RowSource{RowSource::DevList, PodCols{}, ds.r_list.p}, true);
     ds.r_out.reserve(n * (2 + RPK_TOPK)); ds.h_res.reserve(64 + ds.r_out.cap * 4);  // result_rows: the same layout
@@ -1289,8 +1302,9 @@ int enqueue_stale(const rpk_ctx* ctx, DeviceState& ds, uint32_t lo, uint32_t hi,
     a.mask = ds.r_mask.p; a.out = ds.r_list.p; a.n_out = ds.r_dn.p + 1; a.n_pending = ds.r_dn.p;
     a.tile_state = ds.pt_state.p; a.ticket = ds.pt_ticket.p;
     if (ctx->window.empty()) return launch_pod_stale(a, (hi - lo + 15) / 16, ds.sm_count, st);
+    const OfferIngest o = ds.raw.view(ds.G);
     const StaleReachArgs x{a, ctx->offer_floor, ds.win.p, (uint32_t)ctx->window.size(),
-                           ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p, ds.raw_cp.p, ds.raw_flags.p};
+                           o.mem, o.vcpu, o.ram, o.secure_price, o.community_price, o.flags};
     return launch_pod_stale_reach(x, (hi - lo + 15) / 16, ds.sm_count, st);
 }
 
@@ -1308,7 +1322,7 @@ void copy_stale_counts(DeviceState& ds, cudaStream_t st) {
 int enqueue_reselect(DeviceState& ds, uint32_t n_max, bool host_count, uint32_t lo, uint32_t gen, ResultXchgArgs& x,
                      uint32_t* d_counts, cudaStream_t st) {
     const DeviceState::Lane& ln = ds.r_lane;
-    const PodRows cols{ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p};
+    const PodRows cols = ln.cols.rows();
     int launches = 0;
     if (n_max || !host_count) {
         ReselectArgs r{};
@@ -1518,37 +1532,6 @@ int rpk_select_pending_changed_device_gather(rpk_ctx* ctx, int shard, int n_rank
 
 // ---- growing the tables ---------------------------------------------------------------------------------------
 
-namespace {
-struct SlotRange { uint32_t lo, hi; };
-
-// A column sharded by slot range (`bytes` per slot) moves from the old ranges `was` to the new ones `now`: every slot
-// of was[s] is copied from src[s] into dst[d] of the shard d whose new range holds it, on d's stream (a peer copy
-// between GPUs).  A shard whose column is the one it had (same buffer, same first slot) keeps its slots in place; its
-// new range then holds all of them, as a range with the same first slot only grows.
-void move_slots(rpk_ctx* ctx, const std::vector<SlotRange>& was, const std::vector<SlotRange>& now,
-                const std::vector<const void*>& src, const std::vector<void*>& dst, size_t bytes) {
-    const size_t n = ctx->devs.size();
-    for (size_t d = 0; d < n; ++d) {
-        DeviceState& dd = ctx->devs[d];
-        RPK_CUDA(cudaSetDevice(dd.dev));
-        for (size_t s = 0; s < n; ++s) {
-            const uint32_t lo = std::max(was[s].lo, now[d].lo), hi = std::min(was[s].hi, now[d].hi);
-            if (lo >= hi || src[s] == dst[d]) continue;
-            RPK_CUDA(cudaMemcpyPeerAsync(static_cast<char*>(dst[d]) + (size_t)(lo - now[d].lo) * bytes, dd.dev,
-                                         static_cast<const char*>(src[s]) + (size_t)(lo - was[s].lo) * bytes, ctx->devs[s].dev,
-                                         (size_t)(hi - lo) * bytes, dd.stream));
-        }
-    }
-}
-
-void sync_all(rpk_ctx* ctx) {
-    for (auto& ds : ctx->devs) {
-        RPK_CUDA(cudaSetDevice(ds.dev));
-        RPK_CUDA(cudaStreamSynchronize(ds.stream));
-    }
-}
-}  // namespace
-
 int rpk_pods_grow(rpk_ctx* ctx, uint32_t N) {
     static const char* who = "rpk_pods_grow";
     if (!ctx) return RPK_EINVAL;
@@ -1571,10 +1554,8 @@ int rpk_pods_grow(rpk_ctx* ctx, uint32_t N) {
         result_range(N, n, s, &now[(size_t)s].lo, &now[(size_t)s].hi);
     }
     struct Bufs {
-        Grow<int32_t> mem, vcpu, ram; Grow<double> max_price; Grow<uint8_t> cloud, pending; Grow<uint32_t> list;
-        Grow<int32_t> r_mem, r_vcpu, r_ram, r_top5; Grow<double> r_max_price; Grow<uint8_t> r_cloud; Grow<uint32_t> r_gen;
-        Grow<uint32_t> r_list; Grow<uint16_t> r_mask; Grow<int32_t> r_out;
-        Grow<int32_t> l_mem, l_vcpu, l_ram, l_top5; Grow<double> l_max_price; Grow<uint8_t> l_cloud;
+        Grow<PodBufs> rows, r_cols, l_cols; Grow<DevBuf<uint8_t>> pending; Grow<DevBuf<uint32_t>> list, r_gen, r_list;
+        Grow<DevBuf<int32_t>> r_top5, r_out, l_top5; Grow<DevBuf<uint16_t>> r_mask;
         PinnedBuf h_res;
     };
     std::vector<std::unique_ptr<Bufs>> g;
@@ -1586,21 +1567,16 @@ int rpk_pods_grow(rpk_ctx* ctx, uint32_t N) {
             ds.sel_scope.host_wait();  // a device select may still gather from the table
             g.emplace_back(new Bufs());
             Bufs& b = *g.back();
-            b.mem.alloc(ds.pt_mem, N); b.vcpu.alloc(ds.pt_vcpu, N); b.ram.alloc(ds.pt_ram, N);
-            b.max_price.alloc(ds.pt_max_price, N); b.cloud.alloc(ds.pt_cloud, N); b.pending.alloc(ds.pt_pending, N);
+            b.rows.alloc(ds.pt_cols, N); b.pending.alloc(ds.pt_pending, N);
             b.list.alloc(ds.pt_list, ds.pt_list.p ? N : 0);
             if (!move_results) continue;
             // the sizes reserve_results gives a range; a range whose first slot moves gets new columns
             const SlotRange r = now[(size_t)s];
             const bool moved = r.lo != was[(size_t)s].lo;
             const size_t m = ((size_t)(r.hi - r.lo) + 15) / 16 * 16 + 16, rows = std::max<uint32_t>(r.hi - r.lo, 1u);
-            b.r_mem.alloc(ds.r_mem, m, moved); b.r_vcpu.alloc(ds.r_vcpu, m, moved); b.r_ram.alloc(ds.r_ram, m, moved);
-            b.r_max_price.alloc(ds.r_max_price, m, moved); b.r_cloud.alloc(ds.r_cloud, m, moved);
-            b.r_gen.alloc(ds.r_gen, m, moved); b.r_top5.alloc(ds.r_top5, m * RPK_TOPK, moved);
+            b.r_cols.alloc(ds.r_cols, m, moved); b.r_gen.alloc(ds.r_gen, m, moved); b.r_top5.alloc(ds.r_top5, m * RPK_TOPK, moved);
             b.r_list.alloc(ds.r_list, m); b.r_mask.alloc(ds.r_mask, m / 16 + 1);
-            DeviceState::Lane& ln = ds.r_lane;
-            b.l_mem.alloc(ln.p_req_mem, rows); b.l_vcpu.alloc(ln.p_req_vcpu, rows); b.l_ram.alloc(ln.p_req_ram, rows);
-            b.l_max_price.alloc(ln.p_max_price, rows); b.l_cloud.alloc(ln.p_cloud, rows); b.l_top5.alloc(ln.top5, rows * RPK_TOPK);
+            b.l_cols.alloc(ds.r_lane.cols, rows); b.l_top5.alloc(ds.r_lane.top5, rows * RPK_TOPK);
             b.r_out.alloc(ds.r_out, m * (2 + RPK_TOPK));
             if (64 + b.r_out.dst_cap() * 4 > ds.h_res.cap) b.h_res.reserve(64 + b.r_out.dst_cap() * 4);
         }
@@ -1610,35 +1586,29 @@ int rpk_pods_grow(rpk_ctx* ctx, uint32_t N) {
             DeviceState& ds = ctx->devs[(size_t)s];
             Bufs& b = *g[(size_t)s];
             RPK_CUDA(cudaSetDevice(ds.dev));
-            b.mem.keep(N0, ds.stream); b.vcpu.keep(N0, ds.stream); b.ram.keep(N0, ds.stream);
-            b.max_price.keep(N0, ds.stream); b.cloud.keep(N0, ds.stream); b.pending.keep(N0, ds.stream);
-            const PodRows fresh_rows{b.mem.dst() + N0, b.vcpu.dst() + N0, b.ram.dst() + N0, b.max_price.dst() + N0, b.cloud.dst() + N0};
+            b.rows.keep(N0, ds.stream); b.pending.keep(N0, ds.stream);
+            PodRows fresh_rows{};
+            b.rows.each([N0](auto&, auto* dst, auto*& row) { row = dst + N0; }, fresh_rows);
             ctx->launches += (uint64_t)launch_pod_fill(fresh_rows, b.pending.dst() + N0, N - N0, ds.sm_count, ds.stream);
             if (!move_results) continue;
             const size_t kept = b.r_gen.dst() == ds.r_gen.p ? was[(size_t)s].hi - was[(size_t)s].lo : 0;
             RPK_CUDA(cudaMemsetAsync(b.r_gen.dst() + kept, 0, (b.r_gen.dst_cap() - kept) * sizeof(uint32_t), ds.stream));
         }
         if (move_results) {
-            std::vector<const void*> src((size_t)n);
-            std::vector<void*> dst((size_t)n);
-            const auto column = [&](auto buf, size_t bytes) {  // buf: a Grow member of Bufs
-                for (int s = 0; s < n; ++s) { src[(size_t)s] = ((*g[(size_t)s]).*buf).b->p; dst[(size_t)s] = ((*g[(size_t)s]).*buf).dst(); }
-                move_slots(ctx, was, now, src, dst, bytes);
-            };
-            column(&Bufs::r_mem, 4); column(&Bufs::r_vcpu, 4); column(&Bufs::r_ram, 4); column(&Bufs::r_max_price, 8);
-            column(&Bufs::r_cloud, 1); column(&Bufs::r_gen, 4); column(&Bufs::r_top5, 4 * RPK_TOPK);
+            const auto of = [&g](auto Bufs::*m) { return [&g, m](size_t s) -> auto& { return (*g[s]).*m; }; };
+            move_slots(ctx, was, now, of(&Bufs::r_cols), 1); move_slots(ctx, was, now, of(&Bufs::r_gen), 1);
+            move_slots(ctx, was, now, of(&Bufs::r_top5), RPK_TOPK);
         }
         sync_all(ctx);
         // 3. the new buffers and sizes take effect together
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
             Bufs& b = *g[(size_t)s];
-            b.mem.commit(); b.vcpu.commit(); b.ram.commit(); b.max_price.commit(); b.cloud.commit(); b.pending.commit(); b.list.commit();
+            b.rows.commit(); b.pending.commit(); b.list.commit();
             ds.podsN = N;
             if (!move_results) { ds.res_ready = ds.res_bound = false; continue; }
-            b.r_mem.commit(); b.r_vcpu.commit(); b.r_ram.commit(); b.r_max_price.commit(); b.r_cloud.commit(); b.r_gen.commit();
-            b.r_top5.commit(); b.r_list.commit(); b.r_mask.commit(); b.r_out.commit();
-            b.l_mem.commit(); b.l_vcpu.commit(); b.l_ram.commit(); b.l_max_price.commit(); b.l_cloud.commit(); b.l_top5.commit();
+            b.r_cols.commit(); b.r_gen.commit(); b.r_top5.commit(); b.r_list.commit(); b.r_mask.commit(); b.r_out.commit();
+            b.l_cols.commit(); b.l_top5.commit();
             if (b.h_res.h) ds.h_res.swap(b.h_res);
             ds.res_lo = now[(size_t)s].lo; ds.res_hi = now[(size_t)s].hi;
         }
@@ -1751,9 +1721,11 @@ int rpk_test_capture_buffers(const rpk_ctx* ctx, int shard, const void** ptrs, s
     if (!ctx || bad_shard(ctx, shard) || !n || (cap > 0 && !ptrs)) return RPK_EINVAL;
     const DeviceState& ds = ctx->devs[(size_t)shard];
     std::vector<const void*> v;
-    const auto lane = [&v](const DeviceState::Lane& ln) {
-        v.insert(v.end(), {ln.p_req_mem.p, ln.p_req_vcpu.p, ln.p_req_ram.p, ln.p_max_price.p, ln.p_cloud.p, ln.p_slots.p, ln.top5.p,
-                           ln.rw.p, ln.order.p, ln.pos.p, ln.ctrs.p, ln.key.p, ln.ord_rw.p, ln.hist.p, ln.k0_base.p, ln.hdr.p});
+    const auto add = [&v](const auto& b) { v.push_back(b.p); };
+    const auto lane = [&](const DeviceState::Lane& ln) {
+        PodBufs::each(ln.cols, add);
+        v.insert(v.end(), {ln.p_slots.p, ln.top5.p, ln.rw.p, ln.order.p, ln.pos.p, ln.ctrs.p, ln.key.p, ln.ord_rw.p, ln.hist.p,
+                           ln.k0_base.p, ln.hdr.p});
     };
     lane(ds.dev_lane);
     const DeviceState::SweepScratch& w = ds.dev_sweep;
@@ -1761,11 +1733,11 @@ int rpk_test_capture_buffers(const rpk_ctx* ctx, int shard, const void** ptrs, s
     for (int c = 0; c < 2; ++c)
         v.insert(v.end(), {ds.v_packed[c].p, ds.v_bitmap[c].p, ds.v_bitmapT[c].p, ds.v_bitmapM[c].p, ds.v_wide[c].p, ds.v_price[c].p,
                            ds.v_perm[c].p});
-    v.insert(v.end(), {ds.distinct[0].p, ds.distinct[1].p, ds.distinct[2].p, ds.raw_mem.p, ds.raw_vcpu.p, ds.raw_ram.p, ds.raw_sp.p,
-                       ds.raw_cp.p, ds.raw_flags.p, ds.win.p});
-    v.insert(v.end(), {ds.pt_mem.p, ds.pt_vcpu.p, ds.pt_ram.p, ds.pt_max_price.p, ds.pt_cloud.p, ds.pt_pending.p, ds.pt_state.p, ds.pt_ticket.p});
-    v.insert(v.end(), {ds.r_mem.p, ds.r_vcpu.p, ds.r_ram.p, ds.r_max_price.p, ds.r_cloud.p, ds.r_gen.p, ds.r_top5.p, ds.r_list.p,
-                       ds.r_mask.p, ds.r_dn.p});
+    for (const auto& d : ds.distinct) add(d);
+    OfferBufs::each(ds.raw, add); add(ds.win);
+    PodBufs::each(ds.pt_cols, add); v.insert(v.end(), {ds.pt_pending.p, ds.pt_state.p, ds.pt_ticket.p});
+    PodBufs::each(ds.r_cols, add); v.insert(v.end(), {ds.r_gen.p, ds.r_top5.p, ds.r_list.p, ds.r_mask.p, ds.r_dn.p});
+
     lane(ds.r_lane);
     *n = v.size();
     for (size_t i = 0; i < v.size() && i < cap; ++i) ptrs[i] = v[i];
@@ -1809,28 +1781,25 @@ int rpk_status_grow(rpk_ctx* ctx, uint32_t N) {
         shard_range(N0, n, s, &was[(size_t)s].lo, &was[(size_t)s].hi);
         shard_range(N, n, s, &now[(size_t)s].lo, &now[(size_t)s].hi);
     }
-    std::vector<std::unique_ptr<Grow<uint64_t>>> g;
+    std::vector<std::unique_ptr<Grow<DevBuf<uint64_t>>>> g;
     const int rc = guarded(ctx, [&]() -> int {
         // 1. every GPU's new column, before anything changes; a shard whose first slot moves gets a new one
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
             RPK_CUDA(cudaSetDevice(ds.dev));
-            g.emplace_back(new Grow<uint64_t>());
+            g.emplace_back(new Grow<DevBuf<uint64_t>>());
             g.back()->alloc(ds.s_hash_prev, std::max<uint32_t>(now[(size_t)s].hi - now[(size_t)s].lo, 1u), now[(size_t)s].lo != was[(size_t)s].lo);
         }
         // 2. every new slot is never seen (hash 0), the hashes of [0, N0) go to their new shards
-        std::vector<const void*> src((size_t)n);
-        std::vector<void*> dst((size_t)n);
         for (int s = 0; s < n; ++s) {
             DeviceState& ds = ctx->devs[(size_t)s];
-            const Grow<uint64_t>& b = *g[(size_t)s];
+            const Grow<DevBuf<uint64_t>>& b = *g[(size_t)s];
             RPK_CUDA(cudaSetDevice(ds.dev));
             const size_t kept = b.dst() == ds.s_hash_prev.p ? was[(size_t)s].hi - was[(size_t)s].lo : 0;
             const size_t m = std::max<uint32_t>(now[(size_t)s].hi - now[(size_t)s].lo, 1u);
             RPK_CUDA(cudaMemsetAsync(b.dst() + kept, 0, (m - kept) * sizeof(uint64_t), ds.stream));
-            src[(size_t)s] = ds.s_hash_prev.p; dst[(size_t)s] = b.dst();
         }
-        move_slots(ctx, was, now, src, dst, sizeof(uint64_t));
+        move_slots(ctx, was, now, [&g](size_t s) -> auto& { return *g[s]; }, 1);
         sync_all(ctx);
         // 3. the new columns and the size take effect together
         for (int s = 0; s < n; ++s) { g[(size_t)s]->commit(); ctx->devs[(size_t)s].statusN = N; }

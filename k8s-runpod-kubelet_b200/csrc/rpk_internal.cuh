@@ -394,24 +394,56 @@ struct DevBuf {  // grow-only device buffer, freed by its destructor
         cap = want;
     }
     void swap(DevBuf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
+    template <typename S, typename F, typename... O> static void each(S& s, F&& f, O&... o) { f(s, o...); }  // a set of one (Grow)
 };
 
-// One buffer of a grow (rpk_pods_grow, rpk_status_grow).  The replacement of a buffer whose capacity is short (with
-// `always`: of the buffer whatever its capacity) is allocated for every GPU before anything is copied or resized, so a
-// refused allocation frees what was allocated and leaves the ctx as it was.  commit() puts it in place once every copy
-// is done; the old buffer is freed with the Grow.
-template <typename T>
-struct Grow {
-    DevBuf<T>* b = nullptr;
-    DevBuf<T> fresh;
-    void alloc(DevBuf<T>& buf, size_t n, bool always = false) { b = &buf; if (always || n > buf.cap) fresh.reserve(n); }
-    T* dst() const { return fresh.p ? fresh.p : b->p; }
-    size_t dst_cap() const { return fresh.p ? fresh.cap : b->cap; }
-    // the first n elements stay as they are
-    void keep(size_t n, cudaStream_t st) const {
-        if (fresh.p && n) RPK_CUDA(cudaMemcpyAsync(fresh.p, b->p, n * sizeof(T), cudaMemcpyDeviceToDevice, st));
+// The five pod columns of a lane, of the pod table or of the stored results, each an allocation of its own: a column that
+// grows moves alone (rpk.h, "Graph capture").  each: f(s.c, o.c...) for each column c in order; o...: PodBufs or PodRows.
+struct PodBufs {
+    DevBuf<int32_t> mem, vcpu, ram; DevBuf<double> max_price; DevBuf<uint8_t> cloud;
+    template <typename S, typename F, typename... O> static void each(S& s, F&& f, O&... o) {
+        f(s.mem, o.mem...); f(s.vcpu, o.vcpu...); f(s.ram, o.ram...); f(s.max_price, o.max_price...); f(s.cloud, o.cloud...);
     }
-    void commit() { if (fresh.p) b->swap(fresh); }
+    PodRows rows() const { return PodRows{mem.p, vcpu.p, ram.p, max_price.p, cloud.p}; }
+    PodCols cols() const { return PodCols{mem.p, vcpu.p, ram.p, max_price.p, cloud.p}; }
+    void reserve(size_t n, const PodCols* only = nullptr) {  // n rows; with `only` (host columns): in the passed ones only
+        mem.reserve(n);
+        if (!only || only->req_vcpu) vcpu.reserve(n);
+        if (!only || only->req_ram) ram.reserve(n);
+        if (!only || only->max_price) max_price.reserve(n);
+        if (!only || only->cloud) cloud.reserve(n);
+    }
+};
+
+// The six columns of an offer table as uploaded, each its own allocation.  each: f(s.c, o.c...) for each column c in order.
+struct OfferBufs {
+    DevBuf<int32_t> mem, vcpu, ram; DevBuf<double> secure_price, community_price; DevBuf<uint8_t> flags;
+    template <typename S, typename F, typename... O> static void each(S& s, F&& f, O&... o) {
+        f(s.mem, o.mem...); f(s.vcpu, o.vcpu...); f(s.ram, o.ram...); f(s.secure_price, o.secure_price...);
+        f(s.community_price, o.community_price...); f(s.flags, o.flags...);
+    }
+    void swap(OfferBufs& o) { each(*this, [](auto& a, auto& b) { a.swap(b); }, o); }
+    OfferIngest view(uint32_t G) const { return OfferIngest{G, mem.p, vcpu.p, ram.p, secure_price.p, community_price.p, flags.p}; }
+};
+
+// One buffer, or one PodBufs, of a grow (rpk_pods_grow, rpk_status_grow).  The replacement of a column whose capacity is
+// short (with `always`: of every column whatever its capacity) is allocated for every GPU before anything is copied or
+// resized, so a refused allocation frees what was allocated and leaves the ctx as it was.  commit() puts the
+// replacements in place once every copy is done; the old columns are freed with the Grow.
+template <typename S>
+struct Grow {
+    S* b = nullptr;
+    S fresh;
+    void alloc(S& set, size_t n, bool always = false) { b = &set; S::each(set, [&](auto& old, auto& f) { if (always || n > old.cap) f.reserve(n); }, fresh); }
+    template <typename F, typename... O> void each(F&& f, O&... o) const {  // f(old, dst, o.c...): column c now, after commit()
+        S::each(*b, [&](auto& old, const auto& fr, auto&... x) { f(old, fr.p ? fr.p : old.p, x...); }, fresh, o...);
+    }
+    auto dst() const { return fresh.p ? fresh.p : b->p; }  // a buffer's address and capacity after commit()
+    size_t dst_cap() const { return fresh.p ? fresh.cap : b->cap; }
+    void keep(size_t n, cudaStream_t st) const {  // the first n rows stay as they are
+        each([&](auto& old, auto* dst) { if (dst != old.p && n) RPK_CUDA(cudaMemcpyAsync(dst, old.p, n * sizeof(*dst), cudaMemcpyDeviceToDevice, st)); });
+    }
+    void commit() { S::each(*b, [](auto& old, auto& f) { if (f.p) old.swap(f); }, fresh); }
 };
 
 struct PinnedBuf {  // grow-only pinned host block, mapped: the device reaches it at d
@@ -467,10 +499,9 @@ struct DeviceState {
     // offer table
     uint32_t G = 0, Gpad = 0;
     bool offers_ready = false;
-    DevBuf<int32_t> raw_mem, raw_vcpu, raw_ram; DevBuf<double> raw_sp, raw_cp; DevBuf<uint8_t> raw_flags;
-    // rpk_offers_refresh: the new columns land here next to the resident ones and take their place after the diff; the
-    // diff's state words and index list, its mapped output, and the change window's device copy
-    DevBuf<int32_t> new_mem, new_vcpu, new_ram; DevBuf<double> new_sp, new_cp; DevBuf<uint8_t> new_flags;
+    // raw: the table's columns.  rpk_offers_refresh: the new columns land in raw_next next to them and take their place
+    // after the diff; the diff's state words and index list, its mapped output, and the change window's device copy
+    OfferBufs raw, raw_next;
     DevBuf<uint32_t> delta_state, delta_idx; PinnedBuf h_delta; DevBuf<uint2> win;
     DevBuf<unsigned long long> sort_keys; DevBuf<uint32_t> sort_vals;
     DevBuf<uint32_t> v_packed[2]; DevBuf<uint32_t> v_bitmap[2]; DevBuf<uint32_t> v_bitmapT[2]; DevBuf<uint32_t> v_bitmapM[2]; uint32_t nsub = 0; DevBuf<int4> v_wide[2]; DevBuf<double> v_price[2]; DevBuf<int32_t> v_perm[2];
@@ -485,8 +516,7 @@ struct DeviceState {
     struct Lane {
         cudaStream_t stream = nullptr;
         cudaEvent_t done = nullptr;
-        DevBuf<int32_t> p_req_mem, p_req_vcpu, p_req_ram; DevBuf<double> p_max_price; DevBuf<uint8_t> p_cloud;
-        DevBuf<uint32_t> p_slots;  // rpk_select_slots: the sub-batch's slot ids, gathered into the five p_* columns
+        PodBufs cols; DevBuf<uint32_t> p_slots;  // rpk_select_slots: the sub-batch's slot ids, gathered into cols
         DevBuf<int32_t> top5;
         DevBuf<uint32_t> rw, order, pos, ctrs;
         DevBuf<uint16_t> key; DevBuf<uint2> ord_rw; DevBuf<uint32_t> hist, k0_base, hdr;  // persistent path
@@ -519,7 +549,7 @@ struct DeviceState {
     ScratchScope sel_scope, status_scope;  // the offer views, the pod table and dev_lane; dev_sweep
     uint32_t statusN = 0; bool status_sized = false;
     // pod-requirement table (rpk_pods_reset): the five columns of podsN slots, the whole table on every GPU of the ctx
-    DevBuf<int32_t> pt_mem, pt_vcpu, pt_ram; DevBuf<double> pt_max_price; DevBuf<uint8_t> pt_cloud;
+    PodBufs pt_cols;
     DevBuf<unsigned char> pt_seed;         // rpk_pods_seed_slots: the slot ids and the columns of one seed
     // pending set: one flag byte per slot, the list k_pod_pending makes of it, and that kernel's look-back state and
     // tickets (zero between calls by construction, zeroed when allocated)
@@ -533,8 +563,7 @@ struct DeviceState {
     // pointing at them), the host call's changed rows (r_out: [slots : cap][best : cap][top5 : 5 cap]) and their host
     // copy behind the counts (h_res: [r_dn's copy, the changed count : 64 bytes][the r_out layout]).  res_ready:
     // allocated for this table and not cleared since (rpk_pods_reset, a failed call)
-    DevBuf<int32_t> r_mem, r_vcpu, r_ram, r_top5, r_out; DevBuf<double> r_max_price; DevBuf<uint8_t> r_cloud;
-    DevBuf<uint32_t> r_gen, r_list; DevBuf<uint16_t> r_mask;
+    PodBufs r_cols; DevBuf<uint32_t> r_gen, r_list; DevBuf<int32_t> r_top5, r_out; DevBuf<uint16_t> r_mask;
     DevBuf<uint32_t> r_dn; Lane r_lane;
     PinnedBuf h_res;
     bool res_ready = false;
@@ -542,8 +571,8 @@ struct DeviceState {
     // (res_bound), and the (n_ranks, my_rank) it was computed from (rpk_select_pending_changed: the ctx's GPUs and the
     // shard); a call over another range is refused
     bool res_bound = false; uint32_t res_lo = 0, res_hi = 0; int res_ranks = 0, res_rank = 0;
-    StoredResults results() { return StoredResults{r_mem.p, r_vcpu.p, r_ram.p, r_max_price.p, r_cloud.p, r_gen.p, r_top5.p}; }
-    PodRows pods_table() { return PodRows{pt_mem.p, pt_vcpu.p, pt_ram.p, pt_max_price.p, pt_cloud.p}; }
+    StoredResults results() const { const PodRows c = r_cols.rows(); return StoredResults{c.mem, c.vcpu, c.ram, c.max_price, c.cloud, r_gen.p, r_top5.p}; }
+    PodRows pods_table() const { return pt_cols.rows(); }
     ~DeviceState();
 };
 

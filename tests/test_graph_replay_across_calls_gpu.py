@@ -24,13 +24,15 @@ import status_slots_model
 pytestmark = pytest.mark.gpu
 
 # rpk_test_capture_buffers' order
-LANE = ["p_req_mem", "p_req_vcpu", "p_req_ram", "p_max_price", "p_cloud", "p_slots", "top5", "rw", "order", "pos", "ctrs",
+POD_COLS = ("mem", "vcpu", "ram", "max_price", "cloud")
+LANE = ["cols.mem", "cols.vcpu", "cols.ram", "cols.max_price", "cols.cloud", "p_slots", "top5", "rw", "order", "pos", "ctrs",
         "key", "ord_rw", "hist", "k0_base", "hdr"]
 NAMES = ([f"dev_lane.{b}" for b in LANE] + [f"dev_sweep.{b}" for b in ("tile_state", "misc", "stage_idx", "stage_code", "unit_cnt")]
          + [f"view{c}.{b}" for c in (0, 1) for b in ("packed", "bitmap", "bitmapT", "bitmapM", "wide", "price", "perm")]
-         + ["distinct_mem", "distinct_vcpu", "distinct_ram", "raw_mem", "raw_vcpu", "raw_ram", "raw_sp", "raw_cp", "raw_flags", "win"]
-         + ["pt_mem", "pt_vcpu", "pt_ram", "pt_max_price", "pt_cloud", "pt_pending", "pt_state", "pt_ticket"]
-         + ["r_mem", "r_vcpu", "r_ram", "r_max_price", "r_cloud", "r_gen", "r_top5", "r_list", "r_mask", "r_dn"]
+         + ["distinct_mem", "distinct_vcpu", "distinct_ram", "raw.mem", "raw.vcpu", "raw.ram", "raw.secure_price",
+            "raw.community_price", "raw.flags", "win"]
+         + [f"pt_cols.{c}" for c in POD_COLS] + ["pt_pending", "pt_state", "pt_ticket"]
+         + [f"r_cols.{c}" for c in POD_COLS] + ["r_gen", "r_top5", "r_list", "r_mask", "r_dn"]
          + [f"r_lane.{b}" for b in LANE])
 
 C = 20_000         # rows of a captured select: above the fused kernel's 16 384, so the persistent path's buffers exist
@@ -518,8 +520,8 @@ def check_allocated(w, ptrs):
     need = ["dev_lane.rw", "dev_lane.order", "dev_lane.pos", "dev_lane.ctrs"]
     need += [f"dev_sweep.{b}" for b in ("tile_state", "misc", "stage_idx", "stage_code", "unit_cnt")]
     need += [f"view{c}.{b}" for c in (0, 1) for b in ("price", "perm")]
-    need += ["pt_mem", "pt_vcpu", "pt_ram", "pt_max_price", "pt_cloud", "pt_pending", "pt_state", "pt_ticket", "r_gen", "r_list",
-             "r_dn", "r_lane.p_req_mem", "r_lane.top5"]
+    need += [f"pt_cols.{c}" for c in POD_COLS] + ["pt_pending", "pt_state", "pt_ticket", "r_gen", "r_list", "r_dn",
+                                                   "r_lane.cols.mem", "r_lane.top5"]
     if any(e.startswith("slots") for e in w.entries):  # the slot selects gather all five pod columns into the lane
         need += [f"dev_lane.{b}" for b in LANE[:5]]
     if w.eng.stats()["select_kernel_kind"] == 4:  # bit-sliced view: the captured C rows take the persistent path

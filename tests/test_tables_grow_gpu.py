@@ -22,7 +22,7 @@ from test_shared_device_ctx_gpu import shared_engine
 pytestmark = pytest.mark.gpu
 
 EINVAL, ENOMEM, ESTATE = rpk._ffi.RPK_EINVAL, rpk._ffi.RPK_ENOMEM, rpk._ffi.RPK_ESTATE
-PT = ["pt_mem", "pt_vcpu", "pt_ram", "pt_max_price", "pt_cloud", "pt_pending"]
+PT = ["pt_cols.mem", "pt_cols.vcpu", "pt_cols.ram", "pt_cols.max_price", "pt_cols.cloud", "pt_pending"]
 PT_BYTES = [4, 4, 4, 8, 1, 1]
 RESET_ROW = [np.int32(16), np.int32(0), np.int32(0), np.float64(0.5), np.uint8(0), np.uint8(0)]  # rpk_pods_reset's row
 SCHEDULE = [15, 16, 17, 33, 1000, 100_003, 100_019, 110_000, 2**20 + 5]  # 110 000: inside the 25 % slack of 100 019
